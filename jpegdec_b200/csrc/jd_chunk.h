@@ -148,6 +148,9 @@ JD_HD uint32_t jd_chunk_parse(const JDScanIn &sc, const uint16_t *lut, uint32_t 
         }
     }
     *nstart = n; *first = fst;
+    /* fewer than 8 bits before the end: the 1-bit padding of the scan's last byte (T.81 F.1.2.3), read as the start of one
+     * more block.  Whether that is an invalid code depends on the tables; either way the stream ends here. */
+    if (invalid && endbits - rel < 8u) return JD_CS_NONE;
     if (invalid) {
         /* an invalid code under a guessed entry state only says the guess was wrong: let the right neighbour keep
          * speculating from its own first bit (a truly corrupt stream is reported through the flag in `bad`) */

@@ -753,9 +753,11 @@ __device__ __forceinline__ uint32_t jd_pack_sat(int a, int b, uint32_t c)
     return d;
 }
 
-/* x / B for x < 4096 without a high multiply (IMAD.HI is a slow instruction on this part) */
+/* x / B for x < 4096 and B <= 256 without a high multiply (IMAD.HI is a slow instruction on this part).  A 20-bit reciprocal
+ * is exact there (x * B < 2^20); a 16-bit one is not: 719 / 120 came out as 6, and phase C then skipped the last item of
+ * rows 5-7 of every 480-pixel RGB8888 strip (4:2:2, SSE2-build arithmetic) and stored it at x = -1. */
 template <int B>
-__device__ __forceinline__ uint32_t jd_div_small(uint32_t x) { return (x * (uint32_t)(65536 / B + 1)) >> 16; }
+__device__ __forceinline__ uint32_t jd_div_small(uint32_t x) { return (x * (uint32_t)((1u << 20) / B + 1)) >> 20; }
 
 __device__ __forceinline__ uint32_t jd_byte(uint32_t w, int i) { return (w >> (8 * i)) & 0xFFu; }
 
