@@ -96,6 +96,26 @@ int JPEGB200_digestDevice(JPEGB200_CTX *ctx, const void *const *dev_ptrs, const 
  * is JPEG_UNSUPPORTED_FEATURE. */
 JPEGB200_BATCH *JPEGB200_batchCreate(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes,
                                      int n, int pixel_type, int options);
+/* Region-of-interest decode (crop-then-train data loading).  rois: n x {x, y, w, h} in pixels of the OUTPUT image (after
+ * scaling, EXIF thumbnail selection and LUMA_ONLY folding), or NULL = whole images (= JPEGB200_batchCreate).  Image i's
+ * output is exactly rows y..y+h-1, columns x..x+w-1 of what the same call without rois produces; tight pitch = w * bytes
+ * per pixel.
+ *   - Any x, y (no MCU or even-pixel alignment); requires 0 <= x, 0 <= y, w >= 1, h >= 1, x + w <= out_w, y + h <= out_h.
+ *     An image whose rectangle breaks this gets status JPEG_INVALID_PARAMETER; the others decode normally.
+ *   - JPEGB200_batchImageInfo reports out_w, out_h = w, h; JPEGB200_batchOutputBytes, the device arena and
+ *     JPEGB200_C_OUTPUT_BYTES follow from that.
+ *   - Dithered pixel types: returns NULL (error diffusion runs across the whole image, so the dither of a rectangle is
+ *     not a rectangle of the dither).  Every other pixel type, scale and sampling is supported.
+ *   - Work: only the MCUs the rectangle touches are transformed and only its pixels are stored; restart intervals that
+ *     start below its last MCU row are not walked (JPEGB200_C_SEGMENTS counts the walked ones).  Intervals above it are:
+ *     the reference's bit-window phase carries from interval to interval.
+ *   - Status follows the reference's crop decode, which parses every MCU row down to the rectangle's last one and no
+ *     further: JPEG_DECODE_ERROR exactly when the full decode's first undecodable MCU lies in an MCU row at or above the
+ *     last MCU row the rectangle touches; JPEGB200_batchErrMcu then returns that full-image MCU index.  Otherwise the
+ *     status is JPEG_SUCCESS and JPEGB200_batchErrMcu returns -1, even if the scan is corrupt further down.  The same
+ *     holds for scans without restart markers. */
+JPEGB200_BATCH *JPEGB200_batchCreateROI(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes,
+                                        int n, int pixel_type, int options, const int32_t *rois);
 void JPEGB200_batchDestroy(JPEGB200_BATCH *b);
 int JPEGB200_batchCount(JPEGB200_BATCH *b);
 /* per-image facts after batchCreate: status is JPEG_SUCCESS or the open() error the reference would give */
@@ -131,6 +151,11 @@ void *JPEGB200_batchStream(JPEGB200_BATCH *b);          /* cudaStream_t the job 
 int JPEGB200_decodeBatch(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
                          int pixel_type, int options, void *const *outs, const int64_t *pitches,
                          int flags, int32_t *status);
+/* The same with a region of interest per image (rois: n x {x, y, w, h}, semantics of JPEGB200_batchCreateROI; NULL = whole
+ * images).  outs[i] receives h rows of w pixels. */
+int JPEGB200_decodeBatchROI(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                            int pixel_type, int options, const int32_t *rois, void *const *outs,
+                            const int64_t *pitches, int flags, int32_t *status);
 /* JPEGB200_NUM_COUNTERS counters summed over the jobs of the last JPEGB200_decodeBatch on this context */
 int JPEGB200_lastCallCounters(JPEGB200_CTX *ctx, int64_t *counters);
 /* CUDA-event stage times (JPEGB200_NUM_TIMINGS, ms) summed over those jobs, and how many jobs there were.  Jobs overlap

@@ -91,6 +91,8 @@ def lib():
     L.JPEGB200_hostFree.restype = None
     L.JPEGB200_batchCreate.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int]
     L.JPEGB200_batchCreate.restype = vp
+    L.JPEGB200_batchCreateROI.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p]
+    L.JPEGB200_batchCreateROI.restype = vp
     L.JPEGB200_batchDestroy.argtypes = [vp]
     L.JPEGB200_batchDestroy.restype = None
     L.JPEGB200_batchCount.argtypes = [vp]
@@ -101,6 +103,7 @@ def lib():
     L.JPEGB200_batchAllocDeviceOutput.argtypes = [vp]
     L.JPEGB200_batchGetDeviceOutput.argtypes = [vp, C.c_int, C.POINTER(vp), C.POINTER(C.c_int64)]
     L.JPEGB200_batchReadOutput.argtypes = [vp, C.c_int, vp]
+    L.JPEGB200_batchErrMcu.argtypes = [vp, C.c_int]
     L.JPEGB200_batchUpload.argtypes = [vp]
     L.JPEGB200_batchDecode.argtypes = [vp, C.c_int]
     L.JPEGB200_batchDownload.argtypes = [vp]
@@ -111,6 +114,8 @@ def lib():
     L.JPEGB200_batchStream.restype = vp
     L.JPEGB200_decodeBatch.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int,
                                        C.POINTER(vp), C.POINTER(C.c_int64), C.c_int, i32p]
+    L.JPEGB200_decodeBatchROI.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p,
+                                          C.POINTER(vp), C.POINTER(C.c_int64), C.c_int, i32p]
     L.JPEGB200_lastCallCounters.argtypes = [vp, C.POINTER(C.c_int64)]
     L.JPEGB200_lastCallTimings.argtypes = [vp, C.POINTER(C.c_float), ip]
     L.JPEGB200_setPipelineDepth.argtypes = [vp, C.c_int]
@@ -283,16 +288,28 @@ def digest_host(a):
         return int(z.sum(dtype=np.uint64))
 
 
-class Batch:
-    """A decode job over n JPEG files that live in host memory at (ptr, size) pairs."""
+def _roi_array(rois, n):
+    """n (x, y, w, h) rectangles -> int32[4n] for the C ABI (None stays None = whole images)"""
+    if rois is None:
+        return None
+    flat = [int(v) for r in rois for v in r]
+    if len(flat) != 4 * n:
+        raise ValueError("rois: one (x, y, w, h) per image")
+    return (C.c_int32 * (4 * n))(*flat)
 
-    def __init__(self, ctx, ptrs, sizes, pixel_type, options=0):
+
+class Batch:
+    """A decode job over n JPEG files that live in host memory at (ptr, size) pairs.  rois: one (x, y, w, h) rectangle
+    in output pixels per image (JPEGB200_batchCreateROI), or None for whole images."""
+
+    def __init__(self, ctx, ptrs, sizes, pixel_type, options=0, rois=None):
         n = len(ptrs)
         self.n = n
         self._ptrs = (C.c_void_p * n)(*ptrs)
         self._sizes = (C.c_int32 * n)(*sizes)
+        self._rois = _roi_array(rois, n)
         self.ctx = ctx
-        self.h = lib().JPEGB200_batchCreate(ctx.h, self._ptrs, self._sizes, n, pixel_type, options)
+        self.h = lib().JPEGB200_batchCreateROI(ctx.h, self._ptrs, self._sizes, n, pixel_type, options, self._rois)
         if not self.h:
             raise RuntimeError("batchCreate failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
 
@@ -328,6 +345,10 @@ class Batch:
         self._ck(lib().JPEGB200_batchReadOutput(self.h, i, o.ctypes.data), "batchReadOutput")
         return o.reshape(-1, pitch)
 
+    def err_mcu(self, i):
+        """first undecodable MCU of image i after wait(), -1 if none"""
+        return lib().JPEGB200_batchErrMcu(self.h, i)
+
     def upload(self): self._ck(lib().JPEGB200_batchUpload(self.h), "batchUpload")
     def decode(self, flags=0): self._ck(lib().JPEGB200_batchDecode(self.h, flags), "batchDecode")
     def download(self): self._ck(lib().JPEGB200_batchDownload(self.h), "batchDownload")
@@ -353,26 +374,28 @@ class Batch:
             self.h = None
 
 
-def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flags=0):
-    """JPEGB200_decodeBatch: one call for n files (host pointers) -> n outputs (host pointers, or device pointers with
-    JPEGB200_OUT_DEVICE).  Returns (rc, per-image status list, counters summed over the internal jobs)."""
+def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flags=0, rois=None):
+    """JPEGB200_decodeBatch(ROI): one call for n files (host pointers) -> n outputs (host pointers, or device pointers with
+    JPEGB200_OUT_DEVICE); rois: one (x, y, w, h) per image or None.  Returns (rc, per-image status list, counters summed
+    over the internal jobs)."""
     n = len(ptrs)
     pa = (C.c_void_p * n)(*ptrs)
     sa = (C.c_int32 * n)(*sizes)
     oa = (C.c_void_p * n)(*outs)
     pi = (C.c_int64 * n)(*pitches) if pitches is not None else None
     st = (C.c_int32 * n)()
-    rc = lib().JPEGB200_decodeBatch(ctx.h, pa, sa, n, pixel_type, options, oa, pi, flags, st)
+    rc = lib().JPEGB200_decodeBatchROI(ctx.h, pa, sa, n, pixel_type, options, _roi_array(rois, n), oa, pi, flags, st)
     cnt = (C.c_int64 * len(COUNTER_NAMES))()
     lib().JPEGB200_lastCallCounters(ctx.h, cnt)
     return rc, list(st), dict(zip(COUNTER_NAMES, list(cnt)))
 
 
-def decode_batch_to_host(ctx, jpegs, pixel_type, options=0):
+def decode_batch_to_host(ctx, jpegs, pixel_type, options=0, rois=None):
     """Convenience: list of bytes -> list of numpy arrays [out_h, pitch_bytes] (uint8).
-    One public-API call per batch with HOST buffers on both sides."""
+    One public-API call per batch with HOST buffers on both sides.  rois: one (x, y, w, h) per image (the arrays are then
+    h rows of w pixels), or None."""
     bufs = [np.frombuffer(j, dtype=np.uint8) for j in jpegs]
-    b = Batch(ctx, [x.ctypes.data for x in bufs], [len(x) for x in bufs], pixel_type, options)
+    b = Batch(ctx, [x.ctypes.data for x in bufs], [len(x) for x in bufs], pixel_type, options, rois)
     try:
         outs = []
         for i in range(b.n):

@@ -126,6 +126,9 @@ struct JPEGB200_BATCH {
     int pixel_type, options, sshift, ptclass, dither_bits;
     bool gray_out;
     bool padded; /* write the whole MCU-aligned frame (single-image API: callbacks deliver whole MCUs) */
+    bool roi;    /* created with regions of interest (JPEGB200_batchCreateROI) */
+    std::vector<JDRoiPlan> plans;   /* per image, with roi */
+    uint32_t nseg_walk;             /* restart intervals the entropy stage walks (JPEGB200_C_SEGMENTS) */
     cudaStream_t stream;
     std::vector<JDInfo> infos;
     std::vector<int32_t> parse_status;
@@ -445,9 +448,23 @@ static int bytes_per_pixel_class(int ptclass) { return ptclass == JD_PT_565 ? 2 
 extern "C" JPEGB200_BATCH *JPEGB200_batchCreate(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes,
                                                 int n, int pixel_type, int options)
 {
+    return JPEGB200_batchCreateROI(ctx, datas, sizes, n, pixel_type, options, nullptr);
+}
+
+extern "C" JPEGB200_BATCH *JPEGB200_batchCreateROI(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes,
+                                                   int n, int pixel_type, int options, const int32_t *rois)
+{
     if (!ctx || n <= 0 || pixel_type < 0 || pixel_type >= INVALID_PIXEL_TYPE) { snprintf(g_err, sizeof(g_err), "invalid parameter"); return nullptr; }
+    if (rois && pixel_type >= FOUR_BIT_DITHERED && pixel_type <= ONE_BIT_DITHERED) {
+        /* error diffusion runs across the whole image: a rectangle of the dithered image is not the dither of the rectangle */
+        snprintf(g_err, sizeof(g_err), "regions of interest are not supported with dithered pixel types");
+        return nullptr;
+    }
+    if (rois && (options & 0x10000)) { snprintf(g_err, sizeof(g_err), "regions of interest are not supported with padded output"); return nullptr; }
     JPEGB200_BATCH *b = new (std::nothrow) JPEGB200_BATCH();
     if (!b) return nullptr;
+    b->roi = rois != nullptr;
+    if (b->roi) b->plans.assign(n, JDRoiPlan{});
     b->ctx = ctx;
     b->n = n;
     if ((options & JPEG_LUMA_ONLY) && pixel_type < EIGHT_BIT_GRAYSCALE) pixel_type = EIGHT_BIT_GRAYSCALE; /* jpeg.inl:4991 */
@@ -499,6 +516,7 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreate(JPEGB200_CTX *ctx, const uint8_t
     std::vector<uint64_t> lut_hash;
     std::vector<int> lut_owner;      /* first image that defined each LUT set: a hash match is confirmed on the DHT bytes */
     uint32_t seg = 0;
+    b->nseg_walk = 0;
     uint64_t blk = 0, rec_total = 0;
     size_t out_total = 0, gray_total = 0;
     for (int i = 0; i < n; i++) {
@@ -523,6 +541,9 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreate(JPEGB200_CTX *ctx, const uint8_t
         if (ok && !inf.tables_ok) { ok = 0; st = JPEG_DECODE_ERROR; }           /* jpeg.inl:2166 */
         if (ok && inf.ncomp == 1 && pixel_type == RGB8888) { ok = 0; st = JPEG_INVALID_PARAMETER; }
         if (ok && (uint64_t)sizes[i] >= (512ull << 20)) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }   /* image-relative record indices are 32-bit */
+        if (ok && b->roi && !jd_roi_plan(inf.width, inf.height, inf.subsample, inf.restart_interval, b->sshift, rois + 4 * (size_t)i, &b->plans[i])) {
+            ok = 0; st = JPEG_INVALID_PARAMETER;   /* the rectangle does not lie inside the output image */
+        }
         b->parse_status[i] = st;
         if (!ok) { /* keep a harmless empty descriptor */
             d.nseg = 0; d.seg_base = seg; d.blk_base = (uint32_t)blk; d.status = (uint32_t)st;
@@ -556,6 +577,7 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreate(JPEGB200_CTX *ctx, const uint8_t
         d.subsample = (uint8_t)inf.subsample; d.ncomp = (uint8_t)inf.ncomp; d.bpm = (uint8_t)inf.bpm; d.tsel = (uint8_t)inf.tsel;
         d.mcus_per_seg = mps;
         d.nseg = (total_mcus + mps - 1) / mps;
+        d.nseg_walk = b->roi ? (uint32_t)b->plans[i].nseg_walk : d.nseg;
         d.chunk_base = 0; d.nch = 0;
         d.prog = prog ? (1u | ((uint32_t)(inf.approx & 15) << 8)) : 0u;
         if (!prog && inf.restart_interval == 0 && d.nseg == 1 && sizes[i] - inf.scan_offset >= 4096) {
@@ -581,6 +603,13 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreate(JPEGB200_CTX *ctx, const uint8_t
             d.out_w = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> s);
             d.out_h = (uint32_t)inf.mcus_y * (uint32_t)(inf.mcu_h >> s);
         }
+        if (b->roi) {
+            const JDRoiPlan &pl = b->plans[i];
+            d.out_w = (uint32_t)pl.out_w; d.out_h = (uint32_t)pl.out_h;
+            d.roi_x = (uint16_t)rois[4 * (size_t)i]; d.roi_y = (uint16_t)rois[4 * (size_t)i + 1];
+            d.mcu_x0 = (uint16_t)pl.mcu_x0; d.mcu_y0 = (uint16_t)pl.mcu_y0;
+            d.roi_mcu_end = (uint32_t)pl.mcu_end;
+        }
         size_t pitch;
         if (b->dither_bits) {
             const uint32_t pw = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> s);
@@ -592,6 +621,7 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreate(JPEGB200_CTX *ctx, const uint8_t
         b->arena_off[i] = out_total;
         out_total += (pitch * d.out_h + 255) & ~(size_t)255;
         seg += d.nseg;
+        b->nseg_walk += d.nseg_walk;
         blk += (uint64_t)total_mcus * inf.bpm;
         if (blk >= (1ull << 32)) { snprintf(g_err, sizeof(g_err), "batch too large (block count)"); delete b; return nullptr; }
     }
@@ -603,13 +633,19 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreate(JPEGB200_CTX *ctx, const uint8_t
         return nullptr;
     }
     b->out_total = out_total; b->gray_total = gray_total;
-    /* work list: CTAs of 128 segments sharing one LUT set */
+    /* work list: CTAs of 128 segments sharing one LUT set.  With a region of interest the restart intervals that start
+     * below its last MCU row are left out, but every interval above it stays in: the reference's bit-window phase is
+     * carried from one interval to the next (SURVEY.md fact 4, A.2), so the pixels inside the rectangle depend on the walk
+     * of every interval before them. */
     b->seg_img.resize(seg ? seg : 1);
     for (uint32_t li = 0; li < (b->nlut ? b->nlut : 1); li++) {
         for (int i = 0; i < n; i++) {
             const JDImageDesc &d = b->descs[i];
             if (d.nseg == 0 || b->parse_status[i] != JPEG_SUCCESS || d.lutset != li) continue;
-            for (uint32_t s2 = 0; s2 < d.nseg; s2++) { b->seg_img[d.seg_base + s2] = (uint32_t)i; if (d.nch == 0) b->work.push_back(d.seg_base + s2); }
+            for (uint32_t s2 = 0; s2 < d.nseg; s2++) {
+                b->seg_img[d.seg_base + s2] = (uint32_t)i;
+                if (d.nch == 0 && s2 < d.nseg_walk) b->work.push_back(d.seg_base + s2);
+            }
         }
         while (b->work.size() % JD_ENTROPY_THREADS) b->work.push_back(JD_NONE);
         while (b->cta_lut.size() < b->work.size() / JD_ENTROPY_THREADS) b->cta_lut.push_back(li);
@@ -779,12 +815,20 @@ template <int HS, int VS, int NC, int MPB, int PT>
 static void launch_idct_pt(const JDIdctArgs &a, dim3 grid, int arith, bool half, cudaStream_t st)
 {
     using G = JDGeo<HS, VS, NC, MPB>;
-    if (arith == JPEG_ARITH_SSE2) {
-        if (half) jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, true><<<grid, G::THREADS, 0, st>>>(a);
-        else jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, false><<<grid, G::THREADS, 0, st>>>(a);
+    if (a.roi) {
+        if (arith == JPEG_ARITH_SSE2) {
+            if (half) jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, true, true><<<grid, G::THREADS, 0, st>>>(a);
+            else jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, false, true><<<grid, G::THREADS, 0, st>>>(a);
+        } else {
+            if (half) jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, true, true><<<grid, G::THREADS, 0, st>>>(a);
+            else jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, false, true><<<grid, G::THREADS, 0, st>>>(a);
+        }
+    } else if (arith == JPEG_ARITH_SSE2) {
+        if (half) jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, true, false><<<grid, G::THREADS, 0, st>>>(a);
+        else jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, false, false><<<grid, G::THREADS, 0, st>>>(a);
     } else {
-        if (half) jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, true><<<grid, G::THREADS, 0, st>>>(a);
-        else jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, false><<<grid, G::THREADS, 0, st>>>(a);
+        if (half) jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, true, false><<<grid, G::THREADS, 0, st>>>(a);
+        else jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, false, false><<<grid, G::THREADS, 0, st>>>(a);
     }
 }
 
@@ -798,12 +842,17 @@ static void launch_idct_tb(const JDIdctArgs &a, uint32_t mcus_x, uint32_t mcus_y
     dim3 grid((mcus_x + MPB - 1) / MPB, mcus_y, nimg);
     static bool carveout_set = false;   /* 10 CTAs of ~17-21 KB static shared memory per SM need the large carveout */
     if (!carveout_set) {
-        cudaFuncSetAttribute(jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        cudaFuncSetAttribute(jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         carveout_set = true;
     }
-    if (arith == JPEG_ARITH_SSE2) jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2><<<grid, G::THREADS, 0, st>>>(a);
-    else jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR><<<grid, G::THREADS, 0, st>>>(a);
+    if (a.roi) {
+        if (arith == JPEG_ARITH_SSE2) jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, true><<<grid, G::THREADS, 0, st>>>(a);
+        else jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, true><<<grid, G::THREADS, 0, st>>>(a);
+    } else if (arith == JPEG_ARITH_SSE2) jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, false><<<grid, G::THREADS, 0, st>>>(a);
+    else jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, false><<<grid, G::THREADS, 0, st>>>(a);
 }
 
 /* SSE2-build arithmetic: the packed thread-per-block kernel for every sampling / pixel type, full and half size */
@@ -813,12 +862,17 @@ static void launch_idct_p(const JDIdctArgs &a, uint32_t mcus_x, uint32_t mcus_y,
     dim3 grid((mcus_x + MPB - 1) / MPB, mcus_y, nimg);
     static bool carveout_set = false;   /* 7-8 CTAs of ~27 KB static shared memory per SM need the large carveout */
     if (!carveout_set) {
-        cudaFuncSetAttribute(jdk_idct_p<HS, VS, NC, MPB, PT, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        cudaFuncSetAttribute(jdk_idct_p<HS, VS, NC, MPB, PT, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_p<HS, VS, NC, MPB, PT, false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_p<HS, VS, NC, MPB, PT, true, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_p<HS, VS, NC, MPB, PT, false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_p<HS, VS, NC, MPB, PT, true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         carveout_set = true;
     }
-    if (half) jdk_idct_p<HS, VS, NC, MPB, PT, true><<<grid, 128, 0, st>>>(a);
-    else jdk_idct_p<HS, VS, NC, MPB, PT, false><<<grid, 128, 0, st>>>(a);
+    if (a.roi) {
+        if (half) jdk_idct_p<HS, VS, NC, MPB, PT, true, true><<<grid, 128, 0, st>>>(a);
+        else jdk_idct_p<HS, VS, NC, MPB, PT, false, true><<<grid, 128, 0, st>>>(a);
+    } else if (half) jdk_idct_p<HS, VS, NC, MPB, PT, true, false><<<grid, 128, 0, st>>>(a);
+    else jdk_idct_p<HS, VS, NC, MPB, PT, false, false><<<grid, 128, 0, st>>>(a);
 }
 
 template <int HS, int VS>
@@ -1094,13 +1148,23 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
             i1++;
         }
         const uint32_t nimg = (uint32_t)(i1 - i0);
+        if (b->roi) {
+            /* the grid covers the largest box of MCUs a rectangle of the group touches, from each image's first MCU column / row */
+            max_mx = max_my = 0;
+            for (int i = i0; i < i1; i++) {
+                const JDRoiPlan &pl = b->plans[i];
+                if ((uint32_t)(pl.mcu_x1 - pl.mcu_x0 + 1) > max_mx) max_mx = (uint32_t)(pl.mcu_x1 - pl.mcu_x0 + 1);
+                if ((uint32_t)(pl.mcu_y1 - pl.mcu_y0 + 1) > max_my) max_my = (uint32_t)(pl.mcu_y1 - pl.mcu_y0 + 1);
+            }
+        }
         if (b->sshift >= 2) {
             JDScaledArgs sa;
             sa.imgs = b->d_descs.p; sa.blk_hdr = b->d_blk_hdr.p; sa.rec = b->d_rec.p; sa.quant = b->d_quant.p;
             sa.out = stage_out; sa.img0 = (uint32_t)i0; sa.pixel_type = (uint32_t)b->pixel_type; sa.eighth = (b->sshift == 3);
             sa.padded = (b->dither_bits || b->padded) ? 1u : 0u;
             dim3 grid((max_mx * max_my + 127) / 128, nimg);
-            jdk_scaled<<<grid, 128, 0, st>>>(sa);
+            if (b->roi) jdk_scaled<true><<<grid, 128, 0, st>>>(sa);
+            else jdk_scaled<false><<<grid, 128, 0, st>>>(sa);
         } else {
             JDIdctArgs ia;
             ia.imgs = b->d_descs.p; ia.blk_hdr = b->d_blk_hdr.p; ia.rec = b->d_rec.p; ia.quant = b->d_quant.p;
@@ -1109,6 +1173,7 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
             ia.padded = (b->dither_bits || b->padded) ? 1u : 0u;
             ia.mcus_x = (uint32_t)f.mcus_x; ia.mcus_y = (uint32_t)f.mcus_y; ia.width = (uint32_t)f.width; ia.height = (uint32_t)f.height;
             ia.bpm = (uint32_t)f.bpm;
+            ia.roi = b->roi ? 1u : 0u;
             int ok = 0;
             const int ar = b->ctx->arith;
             static int use_packed = -1;   /* JPEGDEC_B200_IDCT=lanes|tb: the round-1 kernels also for the SSE2-build arithmetic (A/B) */
@@ -1154,7 +1219,7 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
     CK(cudaEventRecord(b->ev[7], st));
     CK(cudaGetLastError());
     b->counters[JPEGB200_C_LAUNCHES] = launches;
-    b->counters[JPEGB200_C_SEGMENTS] = b->nseg;
+    b->counters[JPEGB200_C_SEGMENTS] = b->nseg_walk;
     b->counters[JPEGB200_C_BLOCKS] = (int64_t)b->nblk;
     b->counters[JPEGB200_C_COMPRESSED_BYTES] = (int64_t)b->comp_total;
     int64_t ob = 0;
@@ -1295,6 +1360,13 @@ extern "C" int JPEGB200_decodeBatch(JPEGB200_CTX *ctx, const uint8_t *const *dat
                                     int pixel_type, int options, void *const *outs, const int64_t *pitches,
                                     int flags, int32_t *status)
 {
+    return JPEGB200_decodeBatchROI(ctx, datas, sizes, n, pixel_type, options, nullptr, outs, pitches, flags, status);
+}
+
+extern "C" int JPEGB200_decodeBatchROI(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                       int pixel_type, int options, const int32_t *rois, void *const *outs,
+                                       const int64_t *pitches, int flags, int32_t *status)
+{
     if (!ctx || n <= 0) return 0;
     const bool dev_out = (flags & JPEGB200_OUT_DEVICE) != 0;
     if (dev_out && !outs) { snprintf(g_err, sizeof(g_err), "JPEGB200_decodeBatch with JPEGB200_OUT_DEVICE needs the caller's device pointers"); return 0; }
@@ -1338,7 +1410,7 @@ extern "C" int JPEGB200_decodeBatch(JPEGB200_CTX *ctx, const uint8_t *const *dat
             if (cnt > 0 && cb + sz > limit) break;
             cb += sz; cnt++;
         }
-        JPEGB200_BATCH *b = JPEGB200_batchCreate(ctx, datas + i0, sizes + i0, cnt, pixel_type, options);
+        JPEGB200_BATCH *b = JPEGB200_batchCreateROI(ctx, datas + i0, sizes + i0, cnt, pixel_type, options, rois ? rois + 4 * (size_t)i0 : nullptr);
         if (!b) { rc = 0; break; }
         if (!dev_out && i0 + cnt < n && cnt == JD_PIPE_IMAGES) {
             int64_t ob = 0;
@@ -1354,7 +1426,7 @@ extern "C" int JPEGB200_decodeBatch(JPEGB200_CTX *ctx, const uint8_t *const *dat
                 if (cnt2 > cnt) {
                     JPEGB200_batchDestroy(b);
                     cnt = cnt2;
-                    b = JPEGB200_batchCreate(ctx, datas + i0, sizes + i0, cnt, pixel_type, options);
+                    b = JPEGB200_batchCreateROI(ctx, datas + i0, sizes + i0, cnt, pixel_type, options, rois ? rois + 4 * (size_t)i0 : nullptr);
                     if (!b) { rc = 0; break; }
                 }
             }

@@ -438,3 +438,32 @@ uint64_t jd_tables_hash(const JDInfo *info)
     }
     return h;
 }
+
+/* Region of interest -> MCU range, walked restart intervals and output size (JPEGB200_batchCreateROI).  rect is in output
+ * pixels, i.e. after scaling by 2^-sshift; an MCU covers (mcu_w >> sshift) x (mcu_h >> sshift) of them.  Every restart
+ * interval that starts at or before the last MCU of the rectangle's last MCU row is walked, including those above the
+ * rectangle: the reference's bit-window phase is carried from interval to interval, so the pixels inside the rectangle
+ * depend on the walk of every interval before them (SURVEY.md fact 4, A.2). */
+int jd_roi_plan(int width, int height, int subsample, int restart_interval, int sshift, const int32_t *rect, JDRoiPlan *plan)
+{
+    const int mcu_w = (subsample == 0x21 || subsample == 0x22) ? 16 : 8;
+    const int mcu_h = (subsample == 0x12 || subsample == 0x22) ? 16 : 8;
+    const int out_w = (width + (1 << sshift) - 1) >> sshift, out_h = (height + (1 << sshift) - 1) >> sshift;
+    const int64_t x = rect[0], y = rect[1], w = rect[2], h = rect[3];
+    if (x < 0 || y < 0 || w < 1 || h < 1 || x + w > out_w || y + h > out_h) return 0;
+    const int mw = mcu_w >> sshift, mh = mcu_h >> sshift;
+    const int mcus_x = (width + mcu_w - 1) / mcu_w, mcus_y = (height + mcu_h - 1) / mcu_h;
+    plan->mcu_x0 = (int32_t)(x / mw);
+    plan->mcu_x1 = (int32_t)((x + w - 1) / mw);
+    plan->mcu_y0 = (int32_t)(y / mh);
+    plan->mcu_y1 = (int32_t)((y + h - 1) / mh);
+    plan->mcu_end = (plan->mcu_y1 + 1) * mcus_x;
+    const int total = mcus_x * mcus_y;
+    const int mps = restart_interval > 0 ? restart_interval : total;
+    const int nseg = (total + mps - 1) / mps;
+    const int walk = (plan->mcu_end - 1) / mps + 1;        /* intervals whose first MCU is < mcu_end */
+    plan->nseg_walk = walk < nseg ? walk : nseg;
+    plan->out_w = (int32_t)w;
+    plan->out_h = (int32_t)h;
+    return 1;
+}

@@ -67,10 +67,29 @@ typedef struct {
     uint32_t chunk_base;    /* restart-free scans decoded in parallel chunks: first global chunk index ... */
     uint32_t nch;           /* ... and number of chunks (0 = the scan is decoded per restart segment) */
     uint32_t comp_off;      /* offset of this file's first byte in the batch buffer */
-    uint32_t pad_;
+    uint32_t nseg_walk;     /* restart intervals the entropy stage walks: nseg, or with a region of interest those that
+                             * start at or above the rectangle's last MCU row (jd_roi_plan) */
     uint64_t rec_base;      /* index of this image's first coefficient record: block headers hold record indices relative
                              * to it (jd_core.h JD_REC_INDEX with byte offsets relative to comp_off and image-local slots) */
+    /* region of interest (JPEGB200_batchCreateROI); out_w / out_h above are then its size */
+    uint16_t roi_x, roi_y;  /* its origin in output pixels (0, 0 without one) */
+    uint16_t mcu_x0, mcu_y0;/* first MCU column / row it touches: the IDCT grid starts there */
+    uint32_t roi_mcu_end;   /* 1 + the last MCU (full-image raster index) of the last MCU row it touches; 0 = no rectangle.
+                             * An error at or past this MCU is not reported (the reference's crop decode stops above it). */
+    uint32_t pad_;
 } JDImageDesc;
+
+/* What a region of interest (in output pixels: after scaling) means for one image: the MCUs it touches, the restart
+ * intervals that must be walked to reach them and the output size.  jd_roi_plan returns 0 for a rectangle that does not
+ * lie inside the output image. */
+typedef struct {
+    int32_t mcu_x0, mcu_y0, mcu_x1, mcu_y1;  /* MCU columns / rows touched, inclusive */
+    int32_t nseg_walk;                       /* restart intervals walked (intervals below the last touched row are skipped) */
+    int32_t mcu_end;                         /* (mcu_y1 + 1) * MCUs per row */
+    int32_t out_w, out_h;                    /* = the rectangle's w, h */
+} JDRoiPlan;
+int jd_roi_plan(int width, int height, int subsample, int restart_interval, int sshift, const int32_t *rect /* x, y, w, h */,
+                JDRoiPlan *plan);
 
 #ifdef __cplusplus
 }

@@ -60,9 +60,12 @@ __global__ void __launch_bounds__(256) jdk_prescan(const uint8_t *__restrict__ d
     if (nseg <= 1) return;
     __syncthreads();
     const uint32_t lo = im.scan_off, hi = im.scan_end;
+    /* markers needed: the start of every walked interval and the end of the last one (a region of interest leaves the
+     * intervals below it unwalked) */
+    const uint32_t nfind = (im.nseg_walk < nseg) ? im.nseg_walk + 1u : nseg;
     uint32_t found = 0; /* markers found so far (block-uniform) */
     int buf = 0;
-    for (uint32_t p0 = lo & ~15u; p0 < hi && found + 1 < nseg; p0 += 256 * 64) {
+    for (uint32_t p0 = lo & ~15u; p0 < hi && found + 1 < nfind; p0 += 256 * 64) {
         const uint32_t p = p0 + tid * 64;
         unsigned long long m = 0;
         if (p < hi) {
@@ -242,6 +245,7 @@ __global__ void __launch_bounds__(JD_UNSTUFF_WARPS * 32) jdk_unstuff_segs(const 
     const JDImageDesc &im = imgs[seg_img[seg]];
     if (im.nch != 0u || im.nseg == 0u) return;           /* restart-free scans take the chunk path; rejected headers own nothing */
     const uint32_t sl = seg - im.seg_base;
+    if (sl >= im.nseg_walk) return;                      /* below a region of interest: not walked */
     const uint32_t start = seg_start[seg];
     if (start == JD_NONE || start < im.scan_off || start > im.scan_end) { if (lane == 0) seg_clen[seg] = 0; return; }
     const uint32_t next = (sl + 1 < im.nseg) ? seg_start[seg + 1] : JD_NONE;
@@ -337,7 +341,8 @@ __global__ void jdk_stitch(JDImageDesc *imgs, uint32_t nimg, const uint32_t *__r
     JDImageDesc &im = imgs[i];
     uint32_t c = 0, status = 0, err_mcu = 0;
     unsigned long long nrec = 0;
-    for (uint32_t s = 0; s < im.nseg; s++) {
+    /* the walked intervals only: with a region of interest the work list stops at the interval that holds its last MCU row */
+    for (uint32_t s = 0; s < im.nseg_walk; s++) {
         if (im.nch == 0u) nrec += seg_nrec[im.seg_base + s];
         const uint32_t g = im.seg_base + s;
         seg_phase[g] = c;
@@ -346,6 +351,9 @@ __global__ void jdk_stitch(JDImageDesc *imgs, uint32_t nimg, const uint32_t *__r
         const uint32_t st = seg_status[g];
         if (st != 0u && status == 0u) { status = st >> 28; err_mcu = s * im.mcus_per_seg + (st & 0x0FFFFFFFu); }
     }
+    /* a region of interest reports an error only above or in its last MCU row, as the reference's crop decode, which stops
+     * parsing after that row (the chunk path's error MCU is judged the same way, wherever its chunk lies) */
+    if (im.roi_mcu_end != 0u && err_mcu >= im.roi_mcu_end) { status = 0; err_mcu = 0; }
     im.status = status;
     im.err_mcu = err_mcu;
     if (nrec) atomicAdd(rec_count, nrec);
@@ -723,6 +731,7 @@ struct JDIdctArgs {
     uint32_t img0;          /* first image of this launch (blockIdx.z offset) */
     uint32_t big_endian;    /* RGB565_BIG_ENDIAN requested */
     uint32_t padded;        /* 1: write the whole MCU-aligned area (dither intermediate / callback replay) */
+    uint32_t roi;           /* host side: launch the ROI instantiations (grid over each image's rectangle) */
 };
 
 template <int HS, int VS, int NC, int MPB>
@@ -791,12 +800,15 @@ __device__ __forceinline__ uint32_t jd_pixel_scalar(int Y12, int cb, int cr, boo
 }
 
 /* Phase C of the fused kernels (full size): colour conversion of the staged planes + coalesced 16-byte scanline stores.
- * s_y: (VS*8) rows x YSTRIDE luma bytes, s_cb/s_cr: 8 rows x CSTRIDE chroma bytes, covering WCTA pixels of MCU row `my`. */
-template <int HS, int VS, int NC, int PT, int ARITH, int WCTA, int YSTRIDE, int CSTRIDE, int NTHREADS, bool INTERIOR = false>
+ * s_y: (VS*8) rows x YSTRIDE luma bytes, s_cb/s_cr: 8 rows x CSTRIDE chroma bytes, covering WCTA pixels from x = x0 of MCU
+ * row `my`.  ROI: only pixels in [rx, W) x [ry, H) are stored, at (x - rx, y - ry); every value is still computed in
+ * full-image coordinates, so a pixel does not depend on the rectangle. */
+template <int HS, int VS, int NC, int PT, int ARITH, int WCTA, int YSTRIDE, int CSTRIDE, int NTHREADS, bool INTERIOR = false, bool ROI = false>
 __device__ __forceinline__ void jd_phase_c_full(const JDIdctArgs &a, const uint8_t *s_y, const uint8_t *s_cb, const uint8_t *s_cr,
-                                                uint32_t strip, uint32_t my, uint32_t tid, uint32_t W, uint32_t H,
-                                                uint8_t *outbase, uint32_t pitch)
+                                                uint32_t x0, uint32_t my, uint32_t tid, uint32_t W, uint32_t H,
+                                                uint8_t *outbase, uint32_t pitch, uint32_t rx = 0u, uint32_t ry = 0u)
 {
+    static_assert(!(ROI && INTERIOR), "a rectangle is always clipped");
     constexpr int BYPP = (PT == JD_PT_565) ? 2 : (PT == JD_PT_8888 ? 4 : 1);
     /* one item = PXI pixels (OWN 16-byte stores) in each of the VS rows that share chroma */
 #ifndef JD_PXI_8888
@@ -809,9 +821,10 @@ __device__ __forceinline__ void jd_phase_c_full(const JDIdctArgs &a, const uint8
     constexpr bool SSE_PATH = (ARITH == JPEG_ARITH_SSE2) && (HS == VS); /* jpeg.inl:3409-3517, :4006-4308 */
     /* item (rg, xg): PXI pixels at x = xg * PXI in the VS rows of row group rg */
     auto item = [&](const uint32_t rg, const uint32_t xg) {
-        const uint32_t gx = strip * WCTA + xg * PXI;
+        const uint32_t gx = x0 + xg * PXI;
         if (!INTERIOR && gx >= W) return;
-        const bool full = INTERIOR || (gx + PXI <= W);
+        if (ROI && gx + PXI <= rx) return;
+        const bool full = INTERIOR || (gx + PXI <= W && (!ROI || gx >= rx));
         /* chroma samples covering these PXI pixels: PXI / HS of each */
         uint32_t cbw[2] = {0, 0}, crw[2] = {0, 0};
         if (NC == 3 && PT != JD_PT_GRAY) {
@@ -843,6 +856,7 @@ __device__ __forceinline__ void jd_phase_c_full(const JDIdctArgs &a, const uint8
             const uint32_t row = rg * VS + vr;
             const uint32_t gy = my * (VS * 8) + row;
             if (!INTERIOR && gy >= H) continue;
+            if (ROI && gy < ry) continue;
             uint32_t yw[4];
             {
                 const uint8_t *py = s_y + row * YSTRIDE + xg * PXI;
@@ -902,12 +916,15 @@ __device__ __forceinline__ void jd_phase_c_full(const JDIdctArgs &a, const uint8
                 }
                 }
             }
-            uint8_t *dst = outbase + (size_t)gy * pitch + (size_t)gx * BYPP;
+            /* with a rectangle dst may point left of the row for an item that straddles x = rx: only i >= rx - gx is stored */
+            uint8_t *dst = ROI ? outbase + (size_t)(gy - ry) * pitch + (ptrdiff_t)((int)gx - (int)rx) * BYPP
+                               : outbase + (size_t)gy * pitch + (size_t)gx * BYPP;
             if (INTERIOR || (full && ((reinterpret_cast<uintptr_t>(dst) & 15u) == 0))) {
 #pragma unroll
                 for (int q = 0; q < OWN; q++) reinterpret_cast<uint4 *>(dst)[q] = make_uint4(ow[4 * q], ow[4 * q + 1], ow[4 * q + 2], ow[4 * q + 3]);
             } else {
                 for (uint32_t i = 0; i < (uint32_t)PXI && gx + i < W; i++) {
+                    if (ROI && gx + i < rx) continue;
                     if (BYPP == 4) reinterpret_cast<uint32_t *>(dst)[i] = ow[i % (4 * OWN)];
                     else if (BYPP == 2) reinterpret_cast<uint16_t *>(dst)[i] = (uint16_t)(ow[(i >> 1) & 3] >> ((i & 1) * 16));
                     else dst[i] = (uint8_t)(ow[(i >> 2) & 3] >> ((i & 3) * 8));
@@ -924,22 +941,24 @@ __device__ __forceinline__ void jd_phase_c_full(const JDIdctArgs &a, const uint8
     }
 }
 
-/* Phase C at 1/2 scale: 2x2 luma sums; scalar colour code in both builds (jpeg.inl:3297-3322, :3577-3626) */
-template <int HS, int VS, int NC, int PT, int WCTA, int HCTA, int YSTRIDE, int CSTRIDE, int NTHREADS>
+/* Phase C at 1/2 scale: 2x2 luma sums; scalar colour code in both builds (jpeg.inl:3297-3322, :3577-3626).  ox0: output x
+ * of the CTA's first column.  ROI: W, H are the rectangle's right / bottom edge in OUTPUT pixels and (rx, ry) its origin. */
+template <int HS, int VS, int NC, int PT, int WCTA, int HCTA, int YSTRIDE, int CSTRIDE, int NTHREADS, bool ROI = false>
 __device__ __forceinline__ void jd_phase_c_half(const JDIdctArgs &a, const uint8_t *s_y, const uint8_t *s_cb, const uint8_t *s_cr,
-                                                uint32_t strip, uint32_t my, uint32_t tid, uint32_t W, uint32_t H,
-                                                uint8_t *outbase, uint32_t pitch)
+                                                uint32_t ox0, uint32_t my, uint32_t tid, uint32_t W, uint32_t H,
+                                                uint8_t *outbase, uint32_t pitch, uint32_t rx = 0u, uint32_t ry = 0u)
 {
     constexpr int BYPP = (PT == JD_PT_565) ? 2 : (PT == JD_PT_8888 ? 4 : 1);
-    const uint32_t OW = (W + 1) >> 1, OH = (H + 1) >> 1;
+    const uint32_t OW = ROI ? W : (W + 1) >> 1, OH = ROI ? H : (H + 1) >> 1;
     constexpr int OWC = WCTA / 2, OHC = HCTA / 2;
     for (uint32_t it = tid; it < (uint32_t)(OWC * OHC); it += NTHREADS) {
         const uint32_t oy = it / OWC, ox = it - oy * OWC;
-        const uint32_t gy = my * OHC + oy, gx = strip * OWC + ox;
+        const uint32_t gy = my * OHC + oy, gx = ox0 + ox;
         if (gy >= OH || gx >= OW) continue;
+        if (ROI && (gy < ry || gx < rx)) continue;
         const uint8_t *yp = s_y + (2 * oy) * YSTRIDE + 2 * ox;
         const int sum = yp[0] + yp[1] + yp[YSTRIDE] + yp[YSTRIDE + 1];
-        uint8_t *dst = outbase + (size_t)gy * pitch + (size_t)gx * BYPP;
+        uint8_t *dst = outbase + (size_t)(gy - ry) * pitch + (size_t)(gx - rx) * BYPP;
         if (PT == JD_PT_GRAY) {
             *dst = (uint8_t)((sum + 2) >> 2);
         } else if (NC == 1) {
@@ -968,7 +987,17 @@ __device__ __forceinline__ void jd_phase_c_half(const JDIdctArgs &a, const uint8
     }
 }
 
-template <int HS, int VS, int NC, int MPB, int PT, int ARITH, bool HALF>
+/* ROI: a CTA whose first MCU column or whose MCU row lies right of / below the image's rectangle has nothing to store (the
+ * grid is sized for the largest rectangle of the launch).  Exact: MCU row my is needed iff its first output row is above the
+ * rectangle's bottom edge. */
+template <int HS, int VS, bool HALF>
+__device__ __forceinline__ bool jd_roi_cta_outside(const JDImageDesc &im, uint32_t mx0, uint32_t my)
+{
+    constexpr uint32_t SH = HALF ? 1u : 0u;
+    return ((mx0 * HS * 8u) >> SH) >= (uint32_t)im.roi_x + im.out_w || ((my * VS * 8u) >> SH) >= (uint32_t)im.roi_y + im.out_h;
+}
+
+template <int HS, int VS, int NC, int MPB, int PT, int ARITH, bool HALF, bool ROI>
 __global__ void __launch_bounds__(JDGeo<HS, VS, NC, MPB>::THREADS)
 jdk_idct_color(const JDIdctArgs a)
 {
@@ -979,13 +1008,16 @@ jdk_idct_color(const JDIdctArgs a)
 
     const uint32_t img_i = a.img0 + blockIdx.z;
     const JDImageDesc &im = a.imgs[img_i];
-    const uint32_t strip = blockIdx.x, my = blockIdx.y;
+    /* ROI: the grid covers the group's largest rectangle from each image's first MCU column / row */
+    const uint32_t my = ROI ? im.mcu_y0 + blockIdx.y : blockIdx.y;
+    const uint32_t mx0 = (ROI ? (uint32_t)im.mcu_x0 : 0u) + blockIdx.x * MPB;
+    if (ROI && jd_roi_cta_outside<HS, VS, HALF>(im, mx0, my)) return;
     const uint32_t tid = threadIdx.x;
 
     /* ---- phase A: expand this block's records into a column-major coefficient tile ---- */
     const uint32_t gb = tid >> 3, c = tid & 7;           /* block within CTA, lane within block */
     const uint32_t ml = jd_div_small<G::BPMEFF>(gb), blk = gb - ml * G::BPMEFF;
-    const uint32_t mx = strip * MPB + ml;
+    const uint32_t mx = mx0 + ml;
     const uint32_t comp = (blk < (uint32_t)(HS * VS)) ? 0u : blk - HS * VS + 1u;
     jd_u64 h = 0;
     /* (block order inside an MCU in the stream = luma blocks, Cb, Cr = our blk numbering) */
@@ -1065,10 +1097,14 @@ jdk_idct_color(const JDIdctArgs a)
     const uint32_t pitch = im.out_pitch;
     constexpr int BYPP = (PT == JD_PT_565) ? 2 : (PT == JD_PT_8888 ? 4 : 1);
 
-    if (!HALF) {
-        jd_phase_c_full<HS, VS, NC, PT, ARITH, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS>(a, s_y, s_cb, s_cr, strip, my, tid, W, H, outbase, pitch);
+    if (ROI) {
+        const uint32_t rx = im.roi_x, ry = im.roi_y, rxe = rx + im.out_w, rye = ry + im.out_h;
+        if (!HALF) jd_phase_c_full<HS, VS, NC, PT, ARITH, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, false, true>(a, s_y, s_cb, s_cr, mx0 * HS * 8, my, tid, rxe, rye, outbase, pitch, rx, ry);
+        else jd_phase_c_half<HS, VS, NC, PT, G::WCTA, G::HCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, true>(a, s_y, s_cb, s_cr, mx0 * HS * 4, my, tid, rxe, rye, outbase, pitch, rx, ry);
+    } else if (!HALF) {
+        jd_phase_c_full<HS, VS, NC, PT, ARITH, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS>(a, s_y, s_cb, s_cr, mx0 * HS * 8, my, tid, W, H, outbase, pitch);
     } else {
-        jd_phase_c_half<HS, VS, NC, PT, G::WCTA, G::HCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS>(a, s_y, s_cb, s_cr, strip, my, tid, W, H, outbase, pitch);
+        jd_phase_c_half<HS, VS, NC, PT, G::WCTA, G::HCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS>(a, s_y, s_cb, s_cr, mx0 * HS * 4, my, tid, W, H, outbase, pitch);
     }
 }
 
@@ -1114,7 +1150,7 @@ __device__ __forceinline__ uint2 jd_row_finish_packed(const int t[8])
 #ifndef JD_TB_MINB
 #define JD_TB_MINB 10   /* 48 registers: 10 CTAs per SM measured faster than 56 registers / 9 CTAs and than 40 / 12 */
 #endif
-template <int HS, int VS, int NC, int MPB, int PT, int ARITH>
+template <int HS, int VS, int NC, int MPB, int PT, int ARITH, bool ROI>
 __global__ void __launch_bounds__(JDGeoTB<HS, VS, NC, MPB>::THREADS, JD_TB_MINB)
 jdk_idct_tb(const JDIdctArgs a)
 {
@@ -1129,7 +1165,9 @@ jdk_idct_tb(const JDIdctArgs a)
 
     const uint32_t img_i = a.img0 + blockIdx.z;
     const JDImageDesc &im = a.imgs[img_i];
-    const uint32_t strip = blockIdx.x, my = blockIdx.y;
+    const uint32_t my = ROI ? im.mcu_y0 + blockIdx.y : blockIdx.y;
+    const uint32_t mx0 = (ROI ? (uint32_t)im.mcu_x0 : 0u) + blockIdx.x * MPB;
+    if (ROI && jd_roi_cta_outside<HS, VS, false>(im, mx0, my)) return;
     const uint32_t tid = threadIdx.x, lane = tid & 31u, wid = tid >> 5;
     const uint16_t *const irec = a.rec + im.rec_base;
 
@@ -1139,7 +1177,7 @@ jdk_idct_tb(const JDIdctArgs a)
     uint32_t cls = 3;
     if (tid < (uint32_t)G::NB) {
         const uint32_t ml = jd_div_small<G::BPMEFF>(tid), blk = tid - ml * G::BPMEFF;
-        const uint32_t mx = strip * MPB + ml;
+        const uint32_t mx = mx0 + ml;
         if (mx < a.mcus_x) {
             const jd_u64 h = __ldg(a.blk_hdr + im.blk_base + (my * a.mcus_x + mx) * a.bpm + blk);
             s_hdr[tid] = h;
@@ -1345,10 +1383,14 @@ jdk_idct_tb(const JDIdctArgs a)
     const uint32_t H = a.padded ? a.mcus_y * VS * 8 : a.height;
     uint8_t *outbase = a.out + im.out_off;
     const uint32_t pitch = im.out_pitch;
-    if ((strip + 1) * G::WCTA <= W && (my + 1) * G::HCTA <= H && ((reinterpret_cast<uintptr_t>(outbase) | pitch) & 15u) == 0u)
-        jd_phase_c_full<HS, VS, NC, PT, ARITH, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, true>(a, s_y, s_c, s_c + 8 * G::CSTRIDE, strip, my, tid, W, H, outbase, pitch);
+    const uint32_t x0 = mx0 * HS * 8;
+    if (ROI)
+        jd_phase_c_full<HS, VS, NC, PT, ARITH, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, false, true>(a, s_y, s_c, s_c + 8 * G::CSTRIDE, x0, my, tid,
+            (uint32_t)im.roi_x + im.out_w, (uint32_t)im.roi_y + im.out_h, outbase, pitch, im.roi_x, im.roi_y);
+    else if (x0 + G::WCTA <= W && (my + 1) * G::HCTA <= H && ((reinterpret_cast<uintptr_t>(outbase) | pitch) & 15u) == 0u)
+        jd_phase_c_full<HS, VS, NC, PT, ARITH, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, true>(a, s_y, s_c, s_c + 8 * G::CSTRIDE, x0, my, tid, W, H, outbase, pitch);
     else
-        jd_phase_c_full<HS, VS, NC, PT, ARITH, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, false>(a, s_y, s_c, s_c + 8 * G::CSTRIDE, strip, my, tid, W, H, outbase, pitch);
+        jd_phase_c_full<HS, VS, NC, PT, ARITH, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, false>(a, s_y, s_c, s_c + 8 * G::CSTRIDE, x0, my, tid, W, H, outbase, pitch);
 }
 
 /* ------------------------------------------------------------------------------------ */
@@ -1383,7 +1425,7 @@ struct JDGeoP {
 #ifndef JD_P_MINB
 #define JD_P_MINB 7
 #endif
-template <int HS, int VS, int NC, int MPB, int PT, bool HALF>
+template <int HS, int VS, int NC, int MPB, int PT, bool HALF, bool ROI>
 __global__ void __launch_bounds__(128, JD_P_MINB)
 jdk_idct_p(const JDIdctArgs a)
 {
@@ -1399,7 +1441,9 @@ jdk_idct_p(const JDIdctArgs a)
 
     const uint32_t img_i = a.img0 + blockIdx.z;
     const JDImageDesc &im = a.imgs[img_i];
-    const uint32_t strip = blockIdx.x, my = blockIdx.y;
+    const uint32_t my = ROI ? im.mcu_y0 + blockIdx.y : blockIdx.y;
+    const uint32_t mx0 = (ROI ? (uint32_t)im.mcu_x0 : 0u) + blockIdx.x * MPB;
+    if (ROI && jd_roi_cta_outside<HS, VS, HALF>(im, mx0, my)) return;
     const uint32_t tid = threadIdx.x, lane = tid & 31u, wid = tid >> 5;
     const uint16_t *const irec = a.rec + im.rec_base;
 
@@ -1409,7 +1453,7 @@ jdk_idct_p(const JDIdctArgs a)
     uint32_t key = 4;
     if (tid < (uint32_t)G::NB) {
         const uint32_t ml = jd_div_small<G::BPMEFF>(tid), blk = tid - ml * G::BPMEFF;
-        const uint32_t mx = strip * MPB + ml;
+        const uint32_t mx = mx0 + ml;
         if (mx < a.mcus_x) {
             const jd_u64 h = __ldg(a.blk_hdr + im.blk_base + (my * a.mcus_x + mx) * a.bpm + blk);
             s_hdr[tid] = h;
@@ -1527,12 +1571,17 @@ jdk_idct_p(const JDIdctArgs a)
     uint8_t *outbase = a.out + im.out_off;
     const uint32_t pitch = im.out_pitch;
     const uint8_t *s_cb = s_c, *s_cr = s_c + 8 * G::CSTRIDE;
-    if (HALF) {
-        jd_phase_c_half<HS, VS, NC, PT, G::WCTA, G::HCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS>(a, s_y, s_cb, s_cr, strip, my, tid, W, H, outbase, pitch);
-    } else if ((strip + 1) * G::WCTA <= W && (my + 1) * G::HCTA <= H && ((reinterpret_cast<uintptr_t>(outbase) | pitch) & 15u) == 0u) {
-        jd_phase_c_full<HS, VS, NC, PT, JPEG_ARITH_SSE2, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, true>(a, s_y, s_cb, s_cr, strip, my, tid, W, H, outbase, pitch);
+    const uint32_t x0 = mx0 * HS * 8;
+    if (ROI) {
+        const uint32_t rx = im.roi_x, ry = im.roi_y, rxe = rx + im.out_w, rye = ry + im.out_h;
+        if (HALF) jd_phase_c_half<HS, VS, NC, PT, G::WCTA, G::HCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, true>(a, s_y, s_cb, s_cr, x0 / 2, my, tid, rxe, rye, outbase, pitch, rx, ry);
+        else jd_phase_c_full<HS, VS, NC, PT, JPEG_ARITH_SSE2, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, false, true>(a, s_y, s_cb, s_cr, x0, my, tid, rxe, rye, outbase, pitch, rx, ry);
+    } else if (HALF) {
+        jd_phase_c_half<HS, VS, NC, PT, G::WCTA, G::HCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS>(a, s_y, s_cb, s_cr, x0 / 2, my, tid, W, H, outbase, pitch);
+    } else if (x0 + G::WCTA <= W && (my + 1) * G::HCTA <= H && ((reinterpret_cast<uintptr_t>(outbase) | pitch) & 15u) == 0u) {
+        jd_phase_c_full<HS, VS, NC, PT, JPEG_ARITH_SSE2, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, true>(a, s_y, s_cb, s_cr, x0, my, tid, W, H, outbase, pitch);
     } else {
-        jd_phase_c_full<HS, VS, NC, PT, JPEG_ARITH_SSE2, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, false>(a, s_y, s_cb, s_cr, strip, my, tid, W, H, outbase, pitch);
+        jd_phase_c_full<HS, VS, NC, PT, JPEG_ARITH_SSE2, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, false>(a, s_y, s_cb, s_cr, x0, my, tid, W, H, outbase, pitch);
     }
 }
 
@@ -1577,17 +1626,28 @@ __device__ __forceinline__ void jd_scaled_block(const uint16_t *irec, jd_u64 h, 
     px[0] = jd_range(t0 + t1); px[1] = jd_range(t0 - t1); px[2] = jd_range(t2 + t3); px[3] = jd_range(t2 - t3);
 }
 
+/* ROI: one thread per MCU of the box of MCUs the image's rectangle touches (the grid covers the launch's largest box) */
+template <bool ROI>
 __global__ void __launch_bounds__(128) jdk_scaled(const JDScaledArgs a)
 {
     const uint32_t img_i = a.img0 + blockIdx.y;
     const JDImageDesc &im = a.imgs[img_i];
-    const uint32_t m = blockIdx.x * blockDim.x + threadIdx.x;
-    if (m >= (uint32_t)im.mcus_x * im.mcus_y) return;
-    const uint32_t mx = m % im.mcus_x, my = m / im.mcus_x;
     const uint32_t hs = (im.subsample >> 4) ? (im.subsample >> 4) : 1, vs = (im.subsample & 15) ? (im.subsample & 15) : 1;
-    const uint32_t nluma = hs * vs;
     const bool eighth = a.eighth != 0;
     const uint32_t bs = eighth ? 1u : 2u; /* block edge in output pixels */
+    const uint32_t ow = hs * bs, oh = vs * bs; /* output pixels per MCU */
+    uint32_t m = blockIdx.x * blockDim.x + threadIdx.x, mx, my;
+    if (ROI) {
+        const uint32_t ncols = ((uint32_t)im.roi_x + im.out_w - 1u) / ow - im.mcu_x0 + 1u;
+        const uint32_t nrows = ((uint32_t)im.roi_y + im.out_h - 1u) / oh - im.mcu_y0 + 1u;
+        if (m >= ncols * nrows) return;
+        my = im.mcu_y0 + m / ncols; mx = im.mcu_x0 + m % ncols;
+        m = my * im.mcus_x + mx;
+    } else {
+        if (m >= (uint32_t)im.mcus_x * im.mcus_y) return;
+        mx = m % im.mcus_x; my = m / im.mcus_x;
+    }
+    const uint32_t nluma = hs * vs;
     const int32_t *q = a.quant + (size_t)img_i * 192;
     const jd_u64 *hdr = a.blk_hdr + im.blk_base + (size_t)m * im.bpm;
     uint32_t ypx[4][4], cb[4], cr[4];
@@ -1603,11 +1663,14 @@ __global__ void __launch_bounds__(128) jdk_scaled(const JDScaledArgs a)
     const uint32_t W = a.padded ? (uint32_t)im.mcus_x * hs * bs : (((uint32_t)im.width + (1u << shift) - 1u) >> shift);
     const uint32_t H = a.padded ? (uint32_t)im.mcus_y * vs * bs : (((uint32_t)im.height + (1u << shift) - 1u) >> shift);
     uint8_t *outbase = a.out + im.out_off;
-    const uint32_t ow = hs * bs, oh = vs * bs; /* output pixels per MCU */
+    /* stores clipped to [x_lo, x_hi) x [y_lo, y_hi) and shifted to its origin */
+    const uint32_t x_lo = ROI ? im.roi_x : 0u, y_lo = ROI ? im.roi_y : 0u;
+    const uint32_t x_hi = ROI ? x_lo + im.out_w : W, y_hi = ROI ? y_lo + im.out_h : H;
     for (uint32_t y = 0; y < oh; y++) {
         for (uint32_t x = 0; x < ow; x++) {
-            const uint32_t gx = mx * ow + x, gy = my * oh + y;
-            if (gx >= W || gy >= H) continue;
+            const uint32_t fx = mx * ow + x, fy = my * oh + y;
+            if (fx >= x_hi || fy >= y_hi || fx < x_lo || fy < y_lo) continue;
+            const uint32_t gx = fx - x_lo, gy = fy - y_lo;
             const uint32_t bx = x / bs, by = y / bs;
             const uint32_t lb = (hs == 2 && vs == 2) ? by * 2 + bx : (hs == 2 ? bx : by);
             const uint32_t Y = ypx[lb][(y % bs) * bs + (x % bs)];
