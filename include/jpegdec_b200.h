@@ -124,7 +124,12 @@ int JPEGB200_batchImageInfo(JPEGB200_BATCH *b, int i, int32_t *width, int32_t *h
 /* bytes needed for a tightly packed output of image i (out_h rows of out_pitch bytes) */
 int64_t JPEGB200_batchOutputBytes(JPEGB200_BATCH *b, int i, int64_t *pitch_bytes);
 /* Destination for image i.  Device pointer if the batch is decoded with JPEGB200_OUT_DEVICE, else host
- * (pinned recommended).  pitch_bytes = 0 -> tight. */
+ * (pinned recommended).  pitch_bytes <= 0 -> tight (the row bytes of JPEGB200_batchOutputBytes).  Returns 0, with a message
+ * and nothing changed, for a pitch below the row bytes or above 2^32 - 1.  The decode writes out_h rows of row bytes at
+ * out + y * pitch and nothing else: not the pitch padding, not the slot of a rejected image.  (For 1-bit dither with a
+ * padded width that is not a multiple of 8, the half-covered last byte of a row is not stored and is not defined.)
+ * Device outputs: pointer and pitch must be multiples of the pixel store size (2 RGB565, 4 RGB8888, 1 gray / dithered);
+ * JPEGB200_batchDecode returns 0 before enqueueing anything otherwise. */
 int JPEGB200_batchSetOutput(JPEGB200_BATCH *b, int i, void *out, int64_t pitch_bytes);
 /* Let the library own a device output arena (tight images back to back, 256-B aligned). */
 int JPEGB200_batchAllocDeviceOutput(JPEGB200_BATCH *b);
@@ -147,6 +152,11 @@ void *JPEGB200_batchStream(JPEGB200_BATCH *b);          /* cudaStream_t the job 
  * next job's kernels run; with device outputs a job holds at most 192 MiB of compressed bytes, which bounds the transient
  * device memory however large the batch is (the reference equivalent is a loop of JPEG_openRAM + JPEG_decode,
  * src/JPEGDEC.cpp:157-224, which streams any input through a 2 KB window, src/jpeg.inl:1544-1566).
+ * Destinations follow JPEGB200_batchSetOutput: pitch at least the row bytes and below 2^32; device pointers and pitches
+ * multiples of the pixel store size.  A destination that breaks this fails the call (0) with a message naming the image
+ * index (in this call), the pitch and the row bytes.  Only each image's rows are written, except that host buffers laid out
+ * like the device arena (image i at outs[0] + its 256-byte-aligned arena offset, tight pitches) are filled by one copy that
+ * also writes the gaps between images.
  * Returns 1 = all images decoded, 2 = some images failed (see status[]), 0 = call failed. */
 int JPEGB200_decodeBatch(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
                          int pixel_type, int options, void *const *outs, const int64_t *pitches,

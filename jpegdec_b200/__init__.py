@@ -329,7 +329,8 @@ class Batch:
         return b, p.value
 
     def set_output(self, i, ptr, pitch=0):
-        lib().JPEGB200_batchSetOutput(self.h, i, ptr, pitch)
+        """pitch 0 = tight; a pitch below the row bytes or above 2^32 - 1 raises (the image keeps its destination)"""
+        self._ck(lib().JPEGB200_batchSetOutput(self.h, i, ptr, pitch), "batchSetOutput")
 
     def alloc_device_output(self):
         self._ck(lib().JPEGB200_batchAllocDeviceOutput(self.h), "batchAllocDeviceOutput")

@@ -141,6 +141,7 @@ struct JPEGB200_BATCH {
     std::vector<uint64_t> comp_off; /* offset of each file in the device blob */
     std::vector<void *> outs;
     std::vector<int64_t> pitches;
+    int index_base;                 /* index of image 0 in the caller's list (JPEGB200_decodeBatch jobs): error messages */
     std::vector<uint16_t> errinit;  /* dither: initial error line per image (reference quirk), value | 0xFF00 (tag of "the band above band 0") */
     size_t comp_total, out_total, gray_total;
     uint32_t nseg, nlut;
@@ -149,7 +150,7 @@ struct JPEGB200_BATCH {
     bool uploaded, out_device, arena_owned;
     DevBuf<uint8_t> d_comp, d_out, d_gray;
     DevBuf<uint16_t> d_errline;
-    DevBuf<uint64_t> d_gray_off; /* [0,n): gray-stage offsets, [n,2n): packed output offsets */
+    DevBuf<uint64_t> d_gray_off; /* [0,n): gray-stage offsets, [n,2n): packed output offsets, [2n,3n): output pitches */
     DevBuf<uint32_t> d_err_off, d_dprog;
     DevBuf<uint8_t> d_clean;       /* un-stuffed restart segments (jdk_unstuff_segs) */
     DevBuf<uint32_t> d_seg_clen;
@@ -467,6 +468,7 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateROI(JPEGB200_CTX *ctx, const uint
     if (b->roi) b->plans.assign(n, JDRoiPlan{});
     b->ctx = ctx;
     b->n = n;
+    b->index_base = 0;
     if ((options & JPEG_LUMA_ONLY) && pixel_type < EIGHT_BIT_GRAYSCALE) pixel_type = EIGHT_BIT_GRAYSCALE; /* jpeg.inl:4991 */
     b->pixel_type = pixel_type;
     b->padded = (options & 0x10000) != 0; /* JPEGB200_OPT_PADDED (internal, jd_api.c) */
@@ -706,6 +708,8 @@ extern "C" int64_t JPEGB200_batchOutputBytes(JPEGB200_BATCH *b, int i, int64_t *
 extern "C" int JPEGB200_batchSetOutput(JPEGB200_BATCH *b, int i, void *out, int64_t pitch_bytes)
 {
     if (!b || i < 0 || i >= b->n) return 0;
+    if (!jd_check_output(b->index_base + i, b->pixel_type, (int64_t)b->descs[i].out_pitch, out, pitch_bytes, 0, g_err, (int)sizeof(g_err)))
+        return 0;   /* nothing changes: the image keeps its previous destination and pitch */
     b->outs[i] = out;
     if (pitch_bytes > 0) b->pitches[i] = pitch_bytes;
     return 1;
@@ -971,7 +975,14 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         bool any_ptr = false;
         for (int i = 0; i < n; i++) if (b->outs[i]) any_ptr = true;
         if (!user_dev_out && any_ptr) { snprintf(g_err, sizeof(g_err), "device output pointers given for some images only"); return 0; }
+        /* the kernels store through these pointers: refuse misaligned ones before anything is enqueued */
+        for (int i = 0; i < n; i++)
+            if (b->outs[i] && !jd_check_output(b->index_base + i, b->pixel_type, (int64_t)b->descs[i].out_pitch, b->outs[i], b->pitches[i], 1,
+                                               g_err, (int)sizeof(g_err)))
+                return 0;
     }
+    /* the descriptors the kernels read: b->descs keeps the tight pitch (JPEGB200_batchOutputBytes, the arena) */
+    std::vector<JDImageDesc> descs_stage = b->descs;
     uint8_t *out_base = nullptr;
     if (user_dev_out) {
         /* user device pointers: offsets relative to the lowest pointer */
@@ -979,27 +990,27 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         for (int i = 0; i < n; i++) if (b->outs[i] && (uintptr_t)b->outs[i] < lo) lo = (uintptr_t)b->outs[i];
         out_base = (uint8_t *)lo;
         for (int i = 0; i < n; i++) {
-            b->descs[i].out_off = b->outs[i] ? (uint64_t)((uintptr_t)b->outs[i] - lo) : 0;
-            b->descs[i].out_pitch = (uint32_t)b->pitches[i];
+            descs_stage[i].out_off = b->outs[i] ? (uint64_t)((uintptr_t)b->outs[i] - lo) : 0;
+            descs_stage[i].out_pitch = (uint32_t)b->pitches[i];
         }
     } else {
         if (!b->d_out.p) { CK(b->d_out.alloc(&b->ctx->pool, b->out_total + 256)); b->arena_owned = true; }
         out_base = b->d_out.p;
-        for (int i = 0; i < n; i++) b->descs[i].out_off = b->arena_off[i];
+        for (int i = 0; i < n; i++) descs_stage[i].out_off = b->arena_off[i];
     }
     /* dither: the IDCT stage writes an MCU-aligned 8-bit image first */
     std::vector<uint64_t> gray_off;
     std::vector<uint32_t> err_off;
-    std::vector<JDImageDesc> descs_stage = b->descs;
     if (b->dither_bits) {
         CK(b->d_gray.alloc(&b->ctx->pool, b->gray_total + 256));
         size_t go = 0, eo = 0;
-        gray_off.resize(2 * (size_t)n); err_off.resize(n);
+        gray_off.resize(3 * (size_t)n); err_off.resize(n);
         b->errinit.clear();
         for (int i = 0; i < n; i++) {
             const JDInfo &inf = b->infos[i];
             gray_off[i] = go; err_off[i] = (uint32_t)eo;
-            gray_off[(size_t)n + i] = b->descs[i].out_off;
+            gray_off[(size_t)n + i] = descs_stage[i].out_off;         /* where jdk_dither writes the packed rows ... */
+            gray_off[2 * (size_t)n + i] = descs_stage[i].out_pitch;   /* ... and their pitch: the caller's, or tight in the arena */
             if (b->parse_status[i] != JPEG_SUCCESS) continue;
             const uint32_t pw = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> b->sshift);
             const uint32_t ph = (uint32_t)inf.mcus_y * (uint32_t)(inf.mcu_h >> b->sshift);
@@ -1016,9 +1027,9 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         }
         CK(b->d_errline.alloc(&b->ctx->pool, eo + 16));
         CK(cudaMemcpyAsync(b->d_errline.p, b->errinit.data(), eo * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
-        CK(b->d_gray_off.alloc(&b->ctx->pool, 2 * (size_t)n)); CK(b->d_err_off.alloc(&b->ctx->pool, n));
+        CK(b->d_gray_off.alloc(&b->ctx->pool, 3 * (size_t)n)); CK(b->d_err_off.alloc(&b->ctx->pool, n));
         /* pageable sources: the runtime stages them before returning, so the vectors may go out of scope */
-        CK(cudaMemcpyAsync(b->d_gray_off.p, gray_off.data(), (size_t)n * 16, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(b->d_gray_off.p, gray_off.data(), (size_t)n * 24, cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(b->d_err_off.p, err_off.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
         /* one warp per band of 32 rows, band-major (band k of every image, then band k + 1): a band's producer is always
          * launched before it, and the warps resident at any time are bands that can actually run (a band may start ~113
@@ -1432,9 +1443,11 @@ extern "C" int JPEGB200_decodeBatchROI(JPEGB200_CTX *ctx, const uint8_t *const *
             }
         }
         jobs.push_back(b); first.push_back(i0);
+        b->index_base = i0;
         const double t1 = trace ? now_ms() : 0.0;
-        for (int i = 0; i < cnt; i++) JPEGB200_batchSetOutput(b, i, outs ? outs[i0 + i] : nullptr, pitches ? pitches[i0 + i] : 0);
-        rc = JPEGB200_batchUpload(b);
+        /* a refused pitch fails the call with batchSetOutput's message (nothing of this job is enqueued) */
+        for (int i = 0; i < cnt && rc; i++) rc = JPEGB200_batchSetOutput(b, i, outs ? outs[i0 + i] : nullptr, pitches ? pitches[i0 + i] : 0);
+        rc = rc && JPEGB200_batchUpload(b);
         const double t2 = trace ? now_ms() : 0.0;
         rc = rc && JPEGB200_batchDecode(b, flags);
         const double t3 = trace ? now_ms() : 0.0;
@@ -1536,7 +1549,7 @@ jdk_dither(const JDImageDesc *imgs, uint32_t nimg, const uint8_t *gray, const ui
     uint16_t *S = errlines + err_off[i];
     const uint32_t tag_mine = (bi & 0xFFu) << 8, tag_above = ((bi - 1u) & 0xFFu) * 0x01000100u;
     uint8_t *o = out + gray_off[nimg + i];
-    const uint32_t dpitch = ((uint32_t)W * bits + 7) / 8;
+    const size_t opitch = (size_t)gray_off[2 * nimg + i];       /* the caller's pitch, or the tight packed width in the arena */
     const int mask = (bits == 4) ? 0xF0 : (bits == 2 ? 0xC0 : 0x80);
     const uint32_t xmask = (bits == 4) ? 1u : (bits == 2 ? 3u : 7u);
     const bool vec = ((W & 15) == 0);
@@ -1570,7 +1583,7 @@ jdk_dither(const JDImageDesc *imgs, uint32_t nimg, const uint8_t *gray, const ui
         const bool live = y < rows;
         const bool mcu_first = (y % mcu_h) == 0;        /* errors[0..2] are cleared at each JPEGDither call */
         const uint8_t *p = src + (size_t)(live ? y : 0) * W;
-        uint8_t *d = o + (size_t)(live ? y : 0) * dpitch;
+        uint8_t *d = o + (size_t)(live ? y : 0) * opitch;
         int fwd = 0;                 /* lFErr: e1 of the previous pixel + error arriving from above */
         int e2_prev = 0;             /* e2(x-1) */
         int down_m1 = 0;             /* partial outgoing error for pixel x-1: e2(x-2) + e3(x-1) */

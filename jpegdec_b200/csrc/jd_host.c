@@ -7,6 +7,7 @@
  * whole-file buffer (the reference walks a 2 KB window); behaviour that decides
  * open()'s return value / error code is kept, reads are bounds-checked.
  */
+#include <stdio.h>
 #include <string.h>
 #include <stdlib.h>
 #include "jd_internal.h"
@@ -465,5 +466,36 @@ int jd_roi_plan(int width, int height, int subsample, int restart_interval, int 
     plan->nseg_walk = walk < nseg ? walk : nseg;
     plan->out_w = (int32_t)w;
     plan->out_h = (int32_t)h;
+    return 1;
+}
+
+/* A caller's output for one image.  Host and device: a pitch below the row bytes would make rows overlap (and the last
+ * rows run past a buffer of out_h * pitch bytes); the descriptors hold the pitch in 32 bits.  Device outputs are written by
+ * the kernels, whose narrowest stores are per pixel (jd_phase_c_full's per-pixel fallback, jd_phase_c_half, jdk_scaled:
+ * uint16_t for RGB565, uint32_t for RGB8888, bytes for gray and jdk_dither); their 16-byte stores are only taken where
+ * the address is 16-byte aligned.  So a device pointer and pitch must be multiples of that store size, and nothing more.
+ * The host-output copy is a cudaMemcpy2DAsync, which needs no alignment. */
+int jd_check_output(int index, int pixel_type, int64_t row_bytes, const void *out, int64_t pitch, int device,
+                    char *msg, int msg_len)
+{
+    if (pitch > 0 && pitch < row_bytes) {
+        snprintf(msg, (size_t)msg_len, "output of image %d: pitch %lld is below its row size of %lld bytes", index,
+                 (long long)pitch, (long long)row_bytes);
+        return 0;
+    }
+    if (pitch > (int64_t)UINT32_MAX) {
+        snprintf(msg, (size_t)msg_len, "output of image %d: pitch %lld is above the largest supported pitch (%lld bytes)",
+                 index, (long long)pitch, (long long)UINT32_MAX);
+        return 0;
+    }
+    if (device) {
+        const int64_t store = pixel_type == RGB565_LITTLE_ENDIAN || pixel_type == RGB565_BIG_ENDIAN ? 2 : pixel_type == RGB8888 ? 4 : 1;
+        const int64_t p = pitch > 0 ? pitch : row_bytes;
+        if ((uintptr_t)out % (uintptr_t)store != 0 || p % store != 0) {
+            snprintf(msg, (size_t)msg_len, "output of image %d: device pointer %p and pitch %lld must be multiples of %lld bytes "
+                     "(the pixel store size of pixel type %d)", index, out, (long long)p, (long long)store, pixel_type);
+            return 0;
+        }
+    }
     return 1;
 }

@@ -91,6 +91,12 @@ typedef struct {
 int jd_roi_plan(int width, int height, int subsample, int restart_interval, int sshift, const int32_t *rect /* x, y, w, h */,
                 JDRoiPlan *plan);
 
+/* A caller's destination for image `index` (only named in the message): row_bytes is the tight pitch
+ * (JPEGB200_batchOutputBytes), pitch <= 0 means tight.  device != 0: `out` is written by the kernels.  Returns 1, or 0 with
+ * a message in msg[msg_len] (see JPEGB200_batchSetOutput / JPEGB200_decodeBatch for the rules). */
+int jd_check_output(int index, int pixel_type, int64_t row_bytes, const void *out, int64_t pitch, int device,
+                    char *msg, int msg_len);
+
 #ifdef __cplusplus
 }
 #endif
