@@ -205,7 +205,18 @@ typedef struct {
     uint32_t status; /* JD_SEG_* */
     uint32_t nrec;
     uint32_t nblk_done; /* blocks decoded (== blocks asked for unless status != 0) */
+#ifdef JD_ENTROPY_PROBE
+    long long probe[4]; /* clock64() cycles of the walk spent in: ring top-up, DC symbol, AC loop, block header */
+    uint32_t probe_sym; /* AC loop iterations (this lane's own AC symbols) */
+#endif
 } JDSegOut;
+
+/* JD_ENTROPY_PROBE (development build, tools/build_variant.sh + tools/entropy_probe.py): per-section cycle counters of the walk */
+#if defined(JD_ENTROPY_PROBE) && defined(__CUDA_ARCH__)
+#define JD_PROBE(...) __VA_ARGS__
+#else
+#define JD_PROBE(...)
+#endif
 
 /* status codes written per segment */
 #define JD_SEG_OK 0
@@ -328,6 +339,7 @@ JD_HD void jd_decode_segment(const JDSegIn &in, const uint16_t *lut /* JD_LUT_EN
      * A block that swallows more than the ring holds (> ~100 bytes: rare) tops up on the spot. ---- */
     const uint32_t *words = (const uint32_t *)in.data;
     const uint32_t endw = (in.end + 3u) >> 2;    /* first word index past the data */
+    const uint32_t wlast = in.end >> 2;          /* word holding the first byte past the data (if any) */
     uint32_t wi = in.start >> 2;                 /* index of the next word to consume */
     uint32_t wnext = (!CLEAN && wi < endw) ? words[wi] : 0u;
     uint32_t skip = CLEAN ? 0u : (in.start & 3u); /* bytes of the first word that precede the segment */
@@ -390,7 +402,9 @@ JD_HD void jd_decode_segment(const JDSegIn &in, const uint16_t *lut /* JD_LUT_EN
             const uint32_t w = wnext;
             wi++;
             wnext = (wi < endw) ? words[wi] : 0u;
-            if ((((((~w) - 0x01010101u) & w & 0x80808080u)) | skip | ffp | eos) == 0u) {
+            /* fast path: four data bytes, no 0xFF among them, and the whole word before the end of the data (the bytes past
+             * the end belong to whatever follows the file in the batch buffer: the byte path stops there) */
+            if ((((((~w) - 0x01010101u) & w & 0x80808080u)) | skip | ffp | eos | (uint32_t)(wi > wlast)) == 0u) {
                 bb |= (jd_u64)jd_bswap32(w) << (32 - nb);
                 nb += 32;
             } else if (eos) {
@@ -489,9 +503,13 @@ JD_HD void jd_decode_segment(const JDSegIn &in, const uint16_t *lut /* JD_LUT_EN
     constexpr uint32_t LIMIT = (MODE == JD_MODE_STORE_LOW) ? 5u : 64u;
     uint32_t b = 0;                              /* blocks finished */
 
+    JD_PROBE(long long pt[4] = {0, 0, 0, 0}; long long pc0 = clock64(), pc1; uint32_t nsym = 0;)
+#define JD_PROBE_MARK(s) JD_PROBE(pc1 = clock64(); pt[s] += pc1 - pc0; pc0 = pc1;)
     for (; b < nblk_total; b++) {
         const uint32_t cur = (sched >> bsh) & 15u;
+        JD_PROBE_MARK(3)
         if (CLEAN) topup();                      /* the warp is converged here */
+        JD_PROBE_MARK(0)
         /* ---- DC symbol (jpeg.inl:2128-2165) ---- */
         refill();
         jw = jd_jw_ckpt(jw);                     /* R1 at block entry (also the previous block's R4) */
@@ -520,6 +538,7 @@ JD_HD void jd_decode_segment(const JDSegIn &in, const uint16_t *lut /* JD_LUT_EN
             pred2 = (comp >= 2u) ? pv : pred2;
             dcval = pv;
         }
+        JD_PROBE_MARK(1)
         const uint32_t r0 = ro;                  /* this block's first record */
         uint32_t bflags = 0, bigm = 0;           /* OR of the tposw words; JD_ACF_RARE once the block's records are pairs */
         if (MODE != JD_MODE_DC_SCAN) {
@@ -531,6 +550,7 @@ JD_HD void jd_decode_segment(const JDSegIn &in, const uint16_t *lut /* JD_LUT_EN
 #endif
             uint32_t k = 1;                      /* zigzag index of the next coefficient */
             do {
+                JD_PROBE(nsym++;)
                 refill();
                 jw = jd_jw_ckpt(jw);             /* R3 at the loop top (also the previous symbol's R4) */
                 const uint32_t hi = (uint32_t)(bb >> 32);
@@ -620,6 +640,7 @@ JD_HD void jd_decode_segment(const JDSegIn &in, const uint16_t *lut /* JD_LUT_EN
             if (err >= 0) break;
             last_was_eob = (k >= 128u);
         }
+        JD_PROBE_MARK(2)
         /* ---- block finished: header = first record | dc << 32 | count << 48 | BIG << 54 | rows-4..7 << 55 | columns << 56 ---- */
         {
             const uint32_t nrec = ro - r0;
@@ -631,6 +652,9 @@ JD_HD void jd_decode_segment(const JDSegIn &in, const uint16_t *lut /* JD_LUT_EN
         bsh += 4u;
         if (bsh == bsh_end) bsh = 0u;
     }
+    JD_PROBE_MARK(3)
+    JD_PROBE(for (int i = 0; i < 4; i++) out.probe[i] = pt[i]; out.probe_sym = nsym;)
+#undef JD_PROBE_MARK
     if (!direct && (ro & 7u) != 0u) flush_chunk(ro & ~7u);   /* the last, partly filled chunk (its tail lies in the slot's slack) */
     if (err >= 0) {
         /* undecodable from here: later stages must still find well-formed (empty) headers */

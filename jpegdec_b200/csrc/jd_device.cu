@@ -1066,24 +1066,45 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         ea.seg_jmap = b->d_seg_jmap.p; ea.seg_status = b->d_seg_status.p; ea.seg_nrec = b->d_seg_nrec.p;
         ea.events = b->d_events.p; ea.event_count = b->d_counters.p; ea.event_cap = JD_EVENT_CAP;
         ea.nwork = (uint32_t)b->work.size(); ea.dc_output = (b->sshift == 3) ? 1u : (b->sshift == 2) ? 2u : 0u;
-        /* JPEGDEC_B200_ENTROPY=raw: the entropy kernel un-stuffs in its bit reader; default ("clean"): jdk_unstuff_segs
-         * first, so that the reader is a plain word stream */
+        /* default ("raw"): the entropy kernel un-stuffs in its bit reader, 64-thread CTAs.  JPEGDEC_B200_ENTROPY=clean:
+         * jdk_unstuff_segs first, so that the reader is a plain word stream (128-thread CTAs).  On the H100 the raw walk is
+         * the faster one (DESIGN.md 4.1). */
         static int use_clean = -1;
-        if (use_clean < 0) { const char *e = getenv("JPEGDEC_B200_ENTROPY"); use_clean = (e && strcmp(e, "raw") == 0) ? 0 : 1; }
+        if (use_clean < 0) { const char *e = getenv("JPEGDEC_B200_ENTROPY"); use_clean = (e && strcmp(e, "clean") == 0) ? 1 : 0; }
         const unsigned egrid = (unsigned)(b->work.size() / JD_ENTROPY_THREADS);
+#ifdef JD_ENTROPY_PROBE
+        /* development build: time the un-stuffing (clean pipeline) and the walk apart; the walk's warps print their own lines */
+        cudaEvent_t pev[3];
+        for (auto &e : pev) CK(cudaEventCreate(&e));
+        CK(cudaEventRecord(pev[0], st));
+#endif
         if (use_clean) {
             CK(b->d_clean.alloc(&b->ctx->pool, b->comp_total + 32 * (size_t)b->nseg + 4096));
             CK(b->d_seg_clen.alloc(&b->ctx->pool, b->nseg ? b->nseg : 1));
             jdk_unstuff_segs<<<(b->nseg * 32u + JD_UNSTUFF_WARPS * 32u - 1u) / (JD_UNSTUFF_WARPS * 32u), JD_UNSTUFF_WARPS * 32, 0, st>>>(
                 b->d_comp.p, b->d_descs.p, b->d_seg_img.p, b->d_seg_start.p, b->nseg, b->d_clean.p, b->d_seg_clen.p);
             ea.clean = b->d_clean.p; ea.seg_clen = b->d_seg_clen.p;
-            jdk_entropy<true><<<egrid, JD_ENTROPY_THREADS, 0, st>>>(ea);
-            launches += 2;
         } else {
             ea.clean = nullptr; ea.seg_clen = nullptr;
-            jdk_entropy<false><<<egrid, JD_ENTROPY_THREADS, 0, st>>>(ea);
-            launches++;
         }
+#ifdef JD_ENTROPY_PROBE
+        CK(cudaEventRecord(pev[1], st));
+#endif
+        const unsigned ecta = use_clean ? jd_entropy_cta_threads(true) : jd_entropy_cta_threads(false);
+        const unsigned egrid_walk = egrid * (JD_ENTROPY_THREADS / ecta);
+        if (use_clean) jdk_entropy<true><<<egrid_walk, ecta, 0, st>>>(ea);
+        else jdk_entropy<false><<<egrid_walk, ecta, 0, st>>>(ea);
+        launches += use_clean ? 2 : 1;
+#ifdef JD_ENTROPY_PROBE
+        CK(cudaEventRecord(pev[2], st));
+        CK(cudaStreamSynchronize(st));
+        float ms_u = 0.f, ms_w = 0.f;
+        CK(cudaEventElapsedTime(&ms_u, pev[0], pev[1]));
+        CK(cudaEventElapsedTime(&ms_w, pev[1], pev[2]));
+        printf("JDP_LAUNCH nwork %u ctas %u unstuff_ms %.4f walk_ms %.4f\n", (unsigned)b->work.size(), egrid_walk, ms_u, ms_w);
+        fflush(stdout);
+        for (auto &e : pev) CK(cudaEventDestroy(e));
+#endif
     }
     if (b->nchunks) {
         /* restart-free scans: un-stuff, iterate the chunk entry states to their fix point, then emit */

@@ -33,6 +33,14 @@
 #ifndef JD_ENTROPY_THREADS
 #define JD_ENTROPY_THREADS 128
 #endif
+#ifndef JD_ENTROPY_RAW_THREADS
+/* the raw-reader walk runs 64-thread CTAs: 1024 HD images = 1088 of them, 8 or 9 per SM (16 or 18 warps) where 128-thread
+ * CTAs put 4 or 5 per SM (16 or 20 warps); the walk is bound by a per-SM limit, so the most loaded SMs set its time
+ * (DESIGN.md 4.1).  The work list keeps its 128-item LUT groups (JD_ENTROPY_THREADS). */
+#define JD_ENTROPY_RAW_THREADS 64
+#endif
+static_assert(JD_ENTROPY_THREADS % JD_ENTROPY_RAW_THREADS == 0, "a raw-walk CTA must lie inside one LUT group of the work list");
+__host__ __device__ constexpr unsigned jd_entropy_cta_threads(bool clean) { return clean ? JD_ENTROPY_THREADS : JD_ENTROPY_RAW_THREADS; }
 #define JD_RING_STRIDE 36   /* words between two walkers' rings: 32 + 4 keeps 16-byte alignment and spreads the banks */
 
 __constant__ uint8_t c_tpos[64] = JD_TPOS_INIT;
@@ -155,7 +163,11 @@ __host__ __device__ __forceinline__ uint32_t jd_clean_off(uint32_t start, uint32
 template <bool CLEAN>
 __device__ __forceinline__ void jd_entropy_body(const JDEntropyArgs &a, const uint16_t *s_lut, const uint32_t *s_tpos, uint32_t *s_ring, uint16_t *s_stage)
 {
-    const uint32_t wi = blockIdx.x * JD_ENTROPY_THREADS + threadIdx.x;
+#ifdef JD_ENTROPY_PROBE
+    uint64_t g0;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g0));
+#endif
+    const uint32_t wi = blockIdx.x * jd_entropy_cta_threads(CLEAN) + threadIdx.x;
     if (wi >= a.nwork) return;
     const uint32_t seg = a.work[wi];
     if (seg == JD_NONE) return;
@@ -208,20 +220,34 @@ __device__ __forceinline__ void jd_entropy_body(const JDEntropyArgs &a, const ui
     a.seg_jmap[seg] = so.jmap;
     a.seg_status[seg] = (so.err_mcu < 0) ? 0u : (((uint32_t)so.status << 28) | ((uint32_t)so.err_mcu & 0x0FFFFFFFu));
     a.seg_nrec[seg] = so.nrec;
+#ifdef JD_ENTROPY_PROBE
+    /* one line per warp, from its lane 0 (tools/entropy_probe.py aggregates them) */
+    if ((threadIdx.x & 31u) == 0u) {
+        uint64_t g1;
+        uint32_t smid;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g1));
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+        printf("JDP %u %u %u %llu %llu %u %lld %lld %lld %lld %u\n", smid, blockIdx.x, threadIdx.x >> 5, (unsigned long long)g0,
+               (unsigned long long)g1, so.nblk_done, so.probe[0], so.probe[1], so.probe[2], so.probe[3], so.probe_sym);
+    }
+#endif
 }
 
 template <bool CLEAN>
-__global__ void __launch_bounds__(JD_ENTROPY_THREADS) jdk_entropy(const JDEntropyArgs a)
+__global__ void __launch_bounds__(jd_entropy_cta_threads(CLEAN)) jdk_entropy(const JDEntropyArgs a)
 {
+    constexpr int NT = (int)jd_entropy_cta_threads(CLEAN);
     __shared__ __align__(16) uint16_t s_lut[JD_LUT_ENTRIES];
     __shared__ uint32_t s_tpos[64];
-    __shared__ __align__(16) uint32_t s_ring[CLEAN ? JD_ENTROPY_THREADS * JD_RING_STRIDE : 4];   /* per-walker stream rings (jd_core.h) */
-    __shared__ __align__(16) uint16_t s_stage[JD_ENTROPY_THREADS * 8];                           /* per-walker record staging chunks */
-    for (int i = threadIdx.x; i < 64; i += JD_ENTROPY_THREADS) s_tpos[i] = jd_tposw(c_tpos[i]);
+    __shared__ __align__(16) uint32_t s_ring[CLEAN ? NT * JD_RING_STRIDE : 4];   /* per-walker stream rings (jd_core.h) */
+    __shared__ __align__(16) uint16_t s_stage[NT * 8];                           /* per-walker record staging chunks */
+    for (int i = threadIdx.x; i < 64; i += NT) s_tpos[i] = jd_tposw(c_tpos[i]);
     {
-        const uint4 *src = reinterpret_cast<const uint4 *>(a.luts + (size_t)a.cta_lut[blockIdx.x] * JD_LUT_ENTRIES);
+        /* cta_lut has one LUT set per JD_ENTROPY_THREADS work items */
+        const uint32_t grp = blockIdx.x / (uint32_t)(JD_ENTROPY_THREADS / NT);
+        const uint4 *src = reinterpret_cast<const uint4 *>(a.luts + (size_t)a.cta_lut[grp] * JD_LUT_ENTRIES);
         uint4 *dst = reinterpret_cast<uint4 *>(s_lut);
-        for (int i = threadIdx.x; i < JD_LUT_ENTRIES * 2 / 16; i += JD_ENTROPY_THREADS) dst[i] = src[i];
+        for (int i = threadIdx.x; i < JD_LUT_ENTRIES * 2 / 16; i += NT) dst[i] = src[i];
     }
     __syncthreads();
     jd_entropy_body<CLEAN>(a, s_lut, s_tpos, s_ring, s_stage);
