@@ -116,6 +116,27 @@ JPEGB200_BATCH *JPEGB200_batchCreate(JPEGB200_CTX *ctx, const uint8_t *const *da
  *     holds for scans without restart markers. */
 JPEGB200_BATCH *JPEGB200_batchCreateROI(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes,
                                         int n, int pixel_type, int options, const int32_t *rois);
+/* Oriented decode: image i's output is D = T_k(S), S being what the same call without orients produces (after scaling,
+ * thumbnail selection and LUMA_ONLY folding, progressive files at 1/8 included), k one of the 8 EXIF transforms:
+ *   1 identity, 2 mirror x, 3 rotate 180, 4 mirror y, 5 transpose, 6 rotate 90 clockwise, 7 transverse,
+ *   8 rotate 90 counter-clockwise.  For 5-8 out_w and out_h swap.
+ * orients[i]: 0 = from the file (JPEG_getOrientation's tag if it is 1-8, identity otherwise: no tag, 0, 9, 255, ...);
+ * 1-8 = that transform whatever the file says (a loader composes the EXIF transform with its own random flip);
+ * anything else gives that image JPEG_INVALID_PARAMETER.  orients = NULL is JPEGB200_batchCreateROI.
+ *   - rois are in the OUTPUT (upright) frame: image i's output is D[y:y+h, x:x+w].  The work skipped and the status rule are
+ *     those of JPEGB200_batchCreateROI for the same rectangle in the stored frame (where the scan's MCU rows are): with k = 3
+ *     a rectangle at the top of the upright image lies at the bottom of the scan, so almost every restart interval is
+ *     walked and an error near the end of the scan is reported.
+ *   - Pixels are those of the unrotated decode, bit for bit: the transform is applied by the kernels' stores.
+ *   - JPEGB200_batchImageInfo, JPEGB200_batchOutputBytes, the device arena and JPEGB200_C_OUTPUT_BYTES follow the output
+ *     frame; the destination rules of JPEGB200_batchSetOutput apply to it unchanged.
+ *   - Dithered pixel types and padded output: returns NULL.
+ *   - The JPEG_AUTO_ROTATE option bit stays ignored here and in JPEG_decode, as in the reference.
+ * Upright sizes before choosing rectangles: create a plain batch (header parse only, no GPU work), read
+ * JPEGB200_batchOrientation and JPEGB200_batchImageInfo (swap out_w / out_h for tags 5-8), destroy it, then create the
+ * oriented batch. */
+JPEGB200_BATCH *JPEGB200_batchCreateOriented(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes,
+                                             int n, int pixel_type, int options, const int32_t *rois, const uint8_t *orients);
 void JPEGB200_batchDestroy(JPEGB200_BATCH *b);
 int JPEGB200_batchCount(JPEGB200_BATCH *b);
 /* per-image facts after batchCreate: status is JPEG_SUCCESS or the open() error the reference would give */
@@ -136,6 +157,9 @@ int JPEGB200_batchAllocDeviceOutput(JPEGB200_BATCH *b);
 int JPEGB200_batchGetDeviceOutput(JPEGB200_BATCH *b, int i, void **devptr, int64_t *pitch_bytes);
 int JPEGB200_batchReadOutput(JPEGB200_BATCH *b, int i, void *host_dst); /* synchronous D2H of one image from the arena */
 int JPEGB200_batchErrMcu(JPEGB200_BATCH *b, int i);                      /* first undecodable MCU of image i, -1 if none */
+/* Any batch, right after creation: exif_tag = the file's EXIF Orientation tag (0 if it has none), applied = the transform
+ * the decode applies (1-8; 1 for a batch created without orients). */
+int JPEGB200_batchOrientation(JPEGB200_BATCH *b, int i, int32_t *exif_tag, int32_t *applied);
 /* dither needs no extra buffers from the caller: packed rows are written to the output. */
 
 int JPEGB200_batchUpload(JPEGB200_BATCH *b);            /* H2D: compressed bytes + descriptors (async) */
@@ -166,6 +190,11 @@ int JPEGB200_decodeBatch(JPEGB200_CTX *ctx, const uint8_t *const *datas, const i
 int JPEGB200_decodeBatchROI(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
                             int pixel_type, int options, const int32_t *rois, void *const *outs,
                             const int64_t *pitches, int flags, int32_t *status);
+/* The same with an orientation per image (orients: n entries, semantics of JPEGB200_batchCreateOriented; NULL = none).
+ * outs[i] receives the output-frame image (or rectangle of it). */
+int JPEGB200_decodeBatchOriented(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                 int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
+                                 void *const *outs, const int64_t *pitches, int flags, int32_t *status);
 /* JPEGB200_NUM_COUNTERS counters summed over the jobs of the last JPEGB200_decodeBatch on this context */
 int JPEGB200_lastCallCounters(JPEGB200_CTX *ctx, int64_t *counters);
 /* CUDA-event stage times (JPEGB200_NUM_TIMINGS, ms) summed over those jobs, and how many jobs there were.  Jobs overlap

@@ -26,6 +26,7 @@ JPEG_LE_PIXELS, JPEG_EXIF_THUMBNAIL, JPEG_LUMA_ONLY, JPEG_USES_DMA = 16, 32, 64,
  JPEG_INVALID_FILE, JPEG_ERROR_MEMORY) = range(6)
 JPEG_ARITH_SSE2, JPEG_ARITH_SCALAR = 0, 1
 JPEGB200_OUT_DEVICE = 1
+ORIENT_FROM_EXIF = 0   # orients[i]: use the file's EXIF Orientation tag (1-8 force that EXIF transform)
 TIMING_NAMES = ["h2d", "prescan", "entropy", "stitch", "idct", "dither", "d2h", "total"]
 COUNTER_NAMES = ["launches", "segments", "blocks", "events", "compressed_bytes", "output_bytes",
                  "record_bytes", "h2d_bytes", "d2h_bytes", "event_candidates"]
@@ -93,6 +94,9 @@ def lib():
     L.JPEGB200_batchCreate.restype = vp
     L.JPEGB200_batchCreateROI.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p]
     L.JPEGB200_batchCreateROI.restype = vp
+    L.JPEGB200_batchCreateOriented.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8)]
+    L.JPEGB200_batchCreateOriented.restype = vp
+    L.JPEGB200_batchOrientation.argtypes = [vp, C.c_int, i32p, i32p]
     L.JPEGB200_batchDestroy.argtypes = [vp]
     L.JPEGB200_batchDestroy.restype = None
     L.JPEGB200_batchCount.argtypes = [vp]
@@ -116,6 +120,8 @@ def lib():
                                        C.POINTER(vp), C.POINTER(C.c_int64), C.c_int, i32p]
     L.JPEGB200_decodeBatchROI.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p,
                                           C.POINTER(vp), C.POINTER(C.c_int64), C.c_int, i32p]
+    L.JPEGB200_decodeBatchOriented.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
+                                               C.POINTER(vp), C.POINTER(C.c_int64), C.c_int, i32p]
     L.JPEGB200_lastCallCounters.argtypes = [vp, C.POINTER(C.c_int64)]
     L.JPEGB200_lastCallTimings.argtypes = [vp, C.POINTER(C.c_float), ip]
     L.JPEGB200_setPipelineDepth.argtypes = [vp, C.c_int]
@@ -298,18 +304,34 @@ def _roi_array(rois, n):
     return (C.c_int32 * (4 * n))(*flat)
 
 
+def _orient_array(orients, n):
+    """n EXIF transforms (0 = from the file, 1-8) -> uint8[n] for the C ABI (None stays None = no orientation)"""
+    if orients is None:
+        return None
+    v = [int(k) for k in orients]
+    if len(v) != n:
+        raise ValueError("orients: one value per image")
+    if any(k < 0 or k > 255 for k in v):
+        raise ValueError("orients: values are bytes (0 = from the file, 1-8 = EXIF transform)")
+    return (C.c_uint8 * n)(*v)
+
+
 class Batch:
     """A decode job over n JPEG files that live in host memory at (ptr, size) pairs.  rois: one (x, y, w, h) rectangle
-    in output pixels per image (JPEGB200_batchCreateROI), or None for whole images."""
+    in output pixels per image (JPEGB200_batchCreateROI), or None for whole images.  orients: one EXIF transform per
+    image (ORIENT_FROM_EXIF = the file's tag, 1-8 = that transform; JPEGB200_batchCreateOriented), or None; rois are
+    then in the upright frame."""
 
-    def __init__(self, ctx, ptrs, sizes, pixel_type, options=0, rois=None):
+    def __init__(self, ctx, ptrs, sizes, pixel_type, options=0, rois=None, orients=None):
         n = len(ptrs)
         self.n = n
         self._ptrs = (C.c_void_p * n)(*ptrs)
         self._sizes = (C.c_int32 * n)(*sizes)
         self._rois = _roi_array(rois, n)
+        self._orients = _orient_array(orients, n)
         self.ctx = ctx
-        self.h = lib().JPEGB200_batchCreateROI(ctx.h, self._ptrs, self._sizes, n, pixel_type, options, self._rois)
+        self.h = lib().JPEGB200_batchCreateOriented(ctx.h, self._ptrs, self._sizes, n, pixel_type, options, self._rois,
+                                                    self._orients)
         if not self.h:
             raise RuntimeError("batchCreate failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
 
@@ -346,6 +368,12 @@ class Batch:
         self._ck(lib().JPEGB200_batchReadOutput(self.h, i, o.ctypes.data), "batchReadOutput")
         return o.reshape(-1, pitch)
 
+    def orientation(self, i):
+        """(the file's EXIF Orientation tag or 0, the transform this batch applies: 1-8)"""
+        t, k = C.c_int32(), C.c_int32()
+        self._ck(lib().JPEGB200_batchOrientation(self.h, i, C.byref(t), C.byref(k)), "batchOrientation")
+        return t.value, k.value
+
     def err_mcu(self, i):
         """first undecodable MCU of image i after wait(), -1 if none"""
         return lib().JPEGB200_batchErrMcu(self.h, i)
@@ -375,9 +403,10 @@ class Batch:
             self.h = None
 
 
-def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flags=0, rois=None):
-    """JPEGB200_decodeBatch(ROI): one call for n files (host pointers) -> n outputs (host pointers, or device pointers with
-    JPEGB200_OUT_DEVICE); rois: one (x, y, w, h) per image or None.  Returns (rc, per-image status list, counters summed
+def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flags=0, rois=None, orients=None):
+    """JPEGB200_decodeBatch(ROI / Oriented): one call for n files (host pointers) -> n outputs (host pointers, or device
+    pointers with JPEGB200_OUT_DEVICE); rois: one (x, y, w, h) per image or None; orients: one EXIF transform per image
+    (0 = from the file) or None.  Returns (rc, per-image status list, counters summed
     over the internal jobs)."""
     n = len(ptrs)
     pa = (C.c_void_p * n)(*ptrs)
@@ -385,18 +414,19 @@ def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flag
     oa = (C.c_void_p * n)(*outs)
     pi = (C.c_int64 * n)(*pitches) if pitches is not None else None
     st = (C.c_int32 * n)()
-    rc = lib().JPEGB200_decodeBatchROI(ctx.h, pa, sa, n, pixel_type, options, _roi_array(rois, n), oa, pi, flags, st)
+    rc = lib().JPEGB200_decodeBatchOriented(ctx.h, pa, sa, n, pixel_type, options, _roi_array(rois, n),
+                                            _orient_array(orients, n), oa, pi, flags, st)
     cnt = (C.c_int64 * len(COUNTER_NAMES))()
     lib().JPEGB200_lastCallCounters(ctx.h, cnt)
     return rc, list(st), dict(zip(COUNTER_NAMES, list(cnt)))
 
 
-def decode_batch_to_host(ctx, jpegs, pixel_type, options=0, rois=None):
+def decode_batch_to_host(ctx, jpegs, pixel_type, options=0, rois=None, orients=None):
     """Convenience: list of bytes -> list of numpy arrays [out_h, pitch_bytes] (uint8).
     One public-API call per batch with HOST buffers on both sides.  rois: one (x, y, w, h) per image (the arrays are then
-    h rows of w pixels), or None."""
+    h rows of w pixels), or None.  orients: one EXIF transform per image (0 = from the file), or None."""
     bufs = [np.frombuffer(j, dtype=np.uint8) for j in jpegs]
-    b = Batch(ctx, [x.ctypes.data for x in bufs], [len(x) for x in bufs], pixel_type, options, rois)
+    b = Batch(ctx, [x.ctypes.data for x in bufs], [len(x) for x in bufs], pixel_type, options, rois, orients)
     try:
         outs = []
         for i in range(b.n):

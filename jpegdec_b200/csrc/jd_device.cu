@@ -126,8 +126,10 @@ struct JPEGB200_BATCH {
     int pixel_type, options, sshift, ptclass, dither_bits;
     bool gray_out;
     bool padded; /* write the whole MCU-aligned frame (single-image API: callbacks deliver whole MCUs) */
-    bool roi;    /* created with regions of interest (JPEGB200_batchCreateROI) */
+    bool roi;    /* created with regions of interest or orientations (JPEGB200_batchCreateOriented) */
     std::vector<JDRoiPlan> plans;   /* per image, with roi */
+    std::vector<int32_t> exif_tag;  /* per image: the file's EXIF Orientation tag (0 = none) */
+    std::vector<uint8_t> orient;    /* per image: the transform applied, 1-8 (1 without orients) */
     uint32_t nseg_walk;             /* restart intervals the entropy stage walks (JPEGB200_C_SEGMENTS) */
     cudaStream_t stream;
     std::vector<JDInfo> infos;
@@ -455,17 +457,32 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreate(JPEGB200_CTX *ctx, const uint8_t
 extern "C" JPEGB200_BATCH *JPEGB200_batchCreateROI(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes,
                                                    int n, int pixel_type, int options, const int32_t *rois)
 {
+    return JPEGB200_batchCreateOriented(ctx, datas, sizes, n, pixel_type, options, rois, nullptr);
+}
+
+extern "C" JPEGB200_BATCH *JPEGB200_batchCreateOriented(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes,
+                                                        int n, int pixel_type, int options, const int32_t *rois,
+                                                        const uint8_t *orients)
+{
     if (!ctx || n <= 0 || pixel_type < 0 || pixel_type >= INVALID_PIXEL_TYPE) { snprintf(g_err, sizeof(g_err), "invalid parameter"); return nullptr; }
     if (rois && pixel_type >= FOUR_BIT_DITHERED && pixel_type <= ONE_BIT_DITHERED) {
         /* error diffusion runs across the whole image: a rectangle of the dithered image is not the dither of the rectangle */
         snprintf(g_err, sizeof(g_err), "regions of interest are not supported with dithered pixel types");
         return nullptr;
     }
+    if (orients && pixel_type >= FOUR_BIT_DITHERED && pixel_type <= ONE_BIT_DITHERED) {
+        /* likewise: the dither of a rotated image is not the rotation of the dither */
+        snprintf(g_err, sizeof(g_err), "orientations are not supported with dithered pixel types");
+        return nullptr;
+    }
     if (rois && (options & 0x10000)) { snprintf(g_err, sizeof(g_err), "regions of interest are not supported with padded output"); return nullptr; }
+    if (orients && (options & 0x10000)) { snprintf(g_err, sizeof(g_err), "orientations are not supported with padded output"); return nullptr; }
     JPEGB200_BATCH *b = new (std::nothrow) JPEGB200_BATCH();
     if (!b) return nullptr;
-    b->roi = rois != nullptr;
+    b->roi = rois != nullptr || orients != nullptr;
     if (b->roi) b->plans.assign(n, JDRoiPlan{});
+    b->exif_tag.assign(n, 0);
+    b->orient.assign(n, 1);
     b->ctx = ctx;
     b->n = n;
     b->index_base = 0;
@@ -543,8 +560,21 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateROI(JPEGB200_CTX *ctx, const uint
         if (ok && !inf.tables_ok) { ok = 0; st = JPEG_DECODE_ERROR; }           /* jpeg.inl:2166 */
         if (ok && inf.ncomp == 1 && pixel_type == RGB8888) { ok = 0; st = JPEG_INVALID_PARAMETER; }
         if (ok && (uint64_t)sizes[i] >= (512ull << 20)) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }   /* image-relative record indices are 32-bit */
-        if (ok && b->roi && !jd_roi_plan(inf.width, inf.height, inf.subsample, inf.restart_interval, b->sshift, rois + 4 * (size_t)i, &b->plans[i])) {
-            ok = 0; st = JPEG_INVALID_PARAMETER;   /* the rectangle does not lie inside the output image */
+        b->exif_tag[i] = inf.orientation;
+        int32_t srect[4] = {0, 0, 0, 0};
+        if (orients) {
+            /* 0: the file's tag (none or out of range: identity); 1-8: that transform; anything else is refused below */
+            const int k = orients[i] == 0 ? ((inf.orientation >= 1 && inf.orientation <= 8) ? inf.orientation : 1) : orients[i];
+            if (k <= 8) b->orient[i] = (uint8_t)k;
+            if (ok && !jd_orient_plan(inf.width, inf.height, inf.subsample, inf.restart_interval, b->sshift, k,
+                                      rois ? rois + 4 * (size_t)i : nullptr, srect, &b->plans[i])) {
+                ok = 0; st = JPEG_INVALID_PARAMETER;   /* no such transform, or the rectangle does not lie inside the output */
+            }
+        } else if (ok && b->roi) {
+            if (!jd_roi_plan(inf.width, inf.height, inf.subsample, inf.restart_interval, b->sshift, rois + 4 * (size_t)i, &b->plans[i])) {
+                ok = 0; st = JPEG_INVALID_PARAMETER;   /* the rectangle does not lie inside the output image */
+            }
+            srect[0] = rois[4 * (size_t)i]; srect[1] = rois[4 * (size_t)i + 1];
         }
         b->parse_status[i] = st;
         if (!ok) { /* keep a harmless empty descriptor */
@@ -608,9 +638,10 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateROI(JPEGB200_CTX *ctx, const uint
         if (b->roi) {
             const JDRoiPlan &pl = b->plans[i];
             d.out_w = (uint32_t)pl.out_w; d.out_h = (uint32_t)pl.out_h;
-            d.roi_x = (uint16_t)rois[4 * (size_t)i]; d.roi_y = (uint16_t)rois[4 * (size_t)i + 1];
+            d.roi_x = (uint16_t)srect[0]; d.roi_y = (uint16_t)srect[1];
             d.mcu_x0 = (uint16_t)pl.mcu_x0; d.mcu_y0 = (uint16_t)pl.mcu_y0;
             d.roi_mcu_end = (uint32_t)pl.mcu_end;
+            d.orient = orients ? b->orient[i] : 0u;
         }
         size_t pitch;
         if (b->dither_bits) {
@@ -819,7 +850,15 @@ template <int HS, int VS, int NC, int MPB, int PT>
 static void launch_idct_pt(const JDIdctArgs &a, dim3 grid, int arith, bool half, cudaStream_t st)
 {
     using G = JDGeo<HS, VS, NC, MPB>;
-    if (a.roi) {
+    if (a.roi > 1u) {
+        /* oriented stores: one instantiation per transform class */
+#define JD_COLOR_ORC(ARITH_, HALF_)                                                                                            \
+        if (a.roi == 1u + JD_ORC_FLIP) jdk_idct_color<HS, VS, NC, MPB, PT, ARITH_, HALF_, true, JD_ORC_FLIP><<<grid, G::THREADS, 0, st>>>(a); \
+        else jdk_idct_color<HS, VS, NC, MPB, PT, ARITH_, HALF_, true, JD_ORC_TRANSPOSE><<<grid, G::THREADS, 0, st>>>(a);
+        if (arith == JPEG_ARITH_SSE2) { if (half) { JD_COLOR_ORC(JPEG_ARITH_SSE2, true) } else { JD_COLOR_ORC(JPEG_ARITH_SSE2, false) } }
+        else { if (half) { JD_COLOR_ORC(JPEG_ARITH_SCALAR, true) } else { JD_COLOR_ORC(JPEG_ARITH_SCALAR, false) } }
+#undef JD_COLOR_ORC
+    } else if (a.roi) {
         if (arith == JPEG_ARITH_SSE2) {
             if (half) jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, true, true><<<grid, G::THREADS, 0, st>>>(a);
             else jdk_idct_color<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, false, true><<<grid, G::THREADS, 0, st>>>(a);
@@ -850,9 +889,19 @@ static void launch_idct_tb(const JDIdctArgs &a, uint32_t mcus_x, uint32_t mcus_y
         cudaFuncSetAttribute(jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         cudaFuncSetAttribute(jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         cudaFuncSetAttribute(jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, true, JD_ORC_FLIP>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, true, JD_ORC_FLIP>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, true, JD_ORC_TRANSPOSE>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, true, JD_ORC_TRANSPOSE>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         carveout_set = true;
     }
-    if (a.roi) {
+    if (a.roi == 1u + JD_ORC_FLIP) {
+        if (arith == JPEG_ARITH_SSE2) jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, true, JD_ORC_FLIP><<<grid, G::THREADS, 0, st>>>(a);
+        else jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, true, JD_ORC_FLIP><<<grid, G::THREADS, 0, st>>>(a);
+    } else if (a.roi == 1u + JD_ORC_TRANSPOSE) {
+        if (arith == JPEG_ARITH_SSE2) jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, true, JD_ORC_TRANSPOSE><<<grid, G::THREADS, 0, st>>>(a);
+        else jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, true, JD_ORC_TRANSPOSE><<<grid, G::THREADS, 0, st>>>(a);
+    } else if (a.roi) {
         if (arith == JPEG_ARITH_SSE2) jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, true><<<grid, G::THREADS, 0, st>>>(a);
         else jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SCALAR, true><<<grid, G::THREADS, 0, st>>>(a);
     } else if (arith == JPEG_ARITH_SSE2) jdk_idct_tb<HS, VS, NC, MPB, PT, JPEG_ARITH_SSE2, false><<<grid, G::THREADS, 0, st>>>(a);
@@ -870,9 +919,19 @@ static void launch_idct_p(const JDIdctArgs &a, uint32_t mcus_x, uint32_t mcus_y,
         cudaFuncSetAttribute(jdk_idct_p<HS, VS, NC, MPB, PT, true, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         cudaFuncSetAttribute(jdk_idct_p<HS, VS, NC, MPB, PT, false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         cudaFuncSetAttribute(jdk_idct_p<HS, VS, NC, MPB, PT, true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_p<HS, VS, NC, MPB, PT, false, true, JD_ORC_FLIP>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_p<HS, VS, NC, MPB, PT, true, true, JD_ORC_FLIP>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_p<HS, VS, NC, MPB, PT, false, true, JD_ORC_TRANSPOSE>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(jdk_idct_p<HS, VS, NC, MPB, PT, true, true, JD_ORC_TRANSPOSE>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         carveout_set = true;
     }
-    if (a.roi) {
+    if (a.roi == 1u + JD_ORC_FLIP) {
+        if (half) jdk_idct_p<HS, VS, NC, MPB, PT, true, true, JD_ORC_FLIP><<<grid, 128, 0, st>>>(a);
+        else jdk_idct_p<HS, VS, NC, MPB, PT, false, true, JD_ORC_FLIP><<<grid, 128, 0, st>>>(a);
+    } else if (a.roi == 1u + JD_ORC_TRANSPOSE) {
+        if (half) jdk_idct_p<HS, VS, NC, MPB, PT, true, true, JD_ORC_TRANSPOSE><<<grid, 128, 0, st>>>(a);
+        else jdk_idct_p<HS, VS, NC, MPB, PT, false, true, JD_ORC_TRANSPOSE><<<grid, 128, 0, st>>>(a);
+    } else if (a.roi) {
         if (half) jdk_idct_p<HS, VS, NC, MPB, PT, true, true><<<grid, 128, 0, st>>>(a);
         else jdk_idct_p<HS, VS, NC, MPB, PT, false, true><<<grid, 128, 0, st>>>(a);
     } else if (half) jdk_idct_p<HS, VS, NC, MPB, PT, true, false><<<grid, 128, 0, st>>>(a);
@@ -1189,13 +1248,30 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
                 if ((uint32_t)(pl.mcu_y1 - pl.mcu_y0 + 1) > max_my) max_my = (uint32_t)(pl.mcu_y1 - pl.mcu_y0 + 1);
             }
         }
+        /* Orientations: one instantiation per transform class.  Runs are not split by class (a loader's mix of k would cut
+         * them into many small launches): each class's launch covers the whole run and its CTAs of the other class's
+         * images exit at once.  The mirror kernel also stores k = 1 (no mirror); a run of k = 1 only takes the ROI kernel. */
+        bool any_id = false, any_mir = false, any_tr = false;
+        for (int i = i0; i < i1 && b->roi; i++) {
+            const uint32_t k = b->descs[i].orient;
+            if (k >= 5u) any_tr = true; else if (k >= 2u) any_mir = true; else any_id = true;
+        }
+        uint32_t classes[2] = {JD_ORC_NONE, JD_ORC_NONE};
+        int nclass = 0;
+        if (any_mir || (any_tr && any_id)) classes[nclass++] = JD_ORC_FLIP;
+        else if (!any_tr) classes[nclass++] = JD_ORC_NONE;
+        if (any_tr) classes[nclass++] = JD_ORC_TRANSPOSE;
+        for (int ci = 0; ci < nclass; ci++) {
+        const uint32_t orc = classes[ci];
         if (b->sshift >= 2) {
             JDScaledArgs sa;
             sa.imgs = b->d_descs.p; sa.blk_hdr = b->d_blk_hdr.p; sa.rec = b->d_rec.p; sa.quant = b->d_quant.p;
             sa.out = stage_out; sa.img0 = (uint32_t)i0; sa.pixel_type = (uint32_t)b->pixel_type; sa.eighth = (b->sshift == 3);
             sa.padded = (b->dither_bits || b->padded) ? 1u : 0u;
             dim3 grid((max_mx * max_my + 127) / 128, nimg);
-            if (b->roi) jdk_scaled<true><<<grid, 128, 0, st>>>(sa);
+            if (orc == JD_ORC_FLIP) jdk_scaled<true, JD_ORC_FLIP><<<grid, 128, 0, st>>>(sa);
+            else if (orc == JD_ORC_TRANSPOSE) jdk_scaled<true, JD_ORC_TRANSPOSE><<<grid, 128, 0, st>>>(sa);
+            else if (b->roi) jdk_scaled<true><<<grid, 128, 0, st>>>(sa);
             else jdk_scaled<false><<<grid, 128, 0, st>>>(sa);
         } else {
             JDIdctArgs ia;
@@ -1205,7 +1281,7 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
             ia.padded = (b->dither_bits || b->padded) ? 1u : 0u;
             ia.mcus_x = (uint32_t)f.mcus_x; ia.mcus_y = (uint32_t)f.mcus_y; ia.width = (uint32_t)f.width; ia.height = (uint32_t)f.height;
             ia.bpm = (uint32_t)f.bpm;
-            ia.roi = b->roi ? 1u : 0u;
+            ia.roi = b->roi ? 1u + orc : 0u;
             int ok = 0;
             const int ar = b->ctx->arith;
             static int use_packed = -1;   /* JPEGDEC_B200_IDCT=lanes|tb: the round-1 kernels also for the SSE2-build arithmetic (A/B) */
@@ -1233,6 +1309,7 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
             if (!ok) { snprintf(g_err, sizeof(g_err), "no kernel for subsample 0x%02x / pixel type %d", f.subsample, b->pixel_type); return 0; }
         }
         launches++;
+        }
         i0 = i1;
     }
     CK(cudaEventRecord(b->ev[6], st));
@@ -1362,6 +1439,14 @@ extern "C" int JPEGB200_batchErrMcu(JPEGB200_BATCH *b, int i)
     return b->descs_dl[i].status ? (int)b->descs_dl[i].err_mcu : -1;
 }
 
+extern "C" int JPEGB200_batchOrientation(JPEGB200_BATCH *b, int i, int32_t *exif_tag, int32_t *applied)
+{
+    if (!b || i < 0 || i >= b->n) return 0;
+    if (exif_tag) *exif_tag = b->exif_tag[i];
+    if (applied) *applied = b->orient[i];
+    return 1;
+}
+
 extern "C" int JPEGB200_batchGetTimings(JPEGB200_BATCH *b, float *ms)
 {
     if (!b) return 0;
@@ -1398,6 +1483,13 @@ extern "C" int JPEGB200_decodeBatch(JPEGB200_CTX *ctx, const uint8_t *const *dat
 extern "C" int JPEGB200_decodeBatchROI(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
                                        int pixel_type, int options, const int32_t *rois, void *const *outs,
                                        const int64_t *pitches, int flags, int32_t *status)
+{
+    return JPEGB200_decodeBatchOriented(ctx, datas, sizes, n, pixel_type, options, rois, nullptr, outs, pitches, flags, status);
+}
+
+extern "C" int JPEGB200_decodeBatchOriented(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                            int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
+                                            void *const *outs, const int64_t *pitches, int flags, int32_t *status)
 {
     if (!ctx || n <= 0) return 0;
     const bool dev_out = (flags & JPEGB200_OUT_DEVICE) != 0;
@@ -1442,7 +1534,8 @@ extern "C" int JPEGB200_decodeBatchROI(JPEGB200_CTX *ctx, const uint8_t *const *
             if (cnt > 0 && cb + sz > limit) break;
             cb += sz; cnt++;
         }
-        JPEGB200_BATCH *b = JPEGB200_batchCreateROI(ctx, datas + i0, sizes + i0, cnt, pixel_type, options, rois ? rois + 4 * (size_t)i0 : nullptr);
+        JPEGB200_BATCH *b = JPEGB200_batchCreateOriented(ctx, datas + i0, sizes + i0, cnt, pixel_type, options, rois ? rois + 4 * (size_t)i0 : nullptr,
+                                               orients ? orients + i0 : nullptr);
         if (!b) { rc = 0; break; }
         if (!dev_out && i0 + cnt < n && cnt == JD_PIPE_IMAGES) {
             int64_t ob = 0;
@@ -1458,7 +1551,8 @@ extern "C" int JPEGB200_decodeBatchROI(JPEGB200_CTX *ctx, const uint8_t *const *
                 if (cnt2 > cnt) {
                     JPEGB200_batchDestroy(b);
                     cnt = cnt2;
-                    b = JPEGB200_batchCreateROI(ctx, datas + i0, sizes + i0, cnt, pixel_type, options, rois ? rois + 4 * (size_t)i0 : nullptr);
+                    b = JPEGB200_batchCreateOriented(ctx, datas + i0, sizes + i0, cnt, pixel_type, options, rois ? rois + 4 * (size_t)i0 : nullptr,
+                                               orients ? orients + i0 : nullptr);
                     if (!b) { rc = 0; break; }
                 }
             }

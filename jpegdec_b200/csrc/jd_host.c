@@ -469,6 +469,30 @@ int jd_roi_plan(int width, int height, int subsample, int restart_interval, int 
     return 1;
 }
 
+/* Oriented output D = T_k(S) of the scaled image S (sw x sh).  Per transform: mirror x (2, 3, 7, 8), mirror y (3, 4, 6, 7),
+ * then transpose (5-8).  Stored pixel (sx, sy) lands at ex = mirror x ? sw - 1 - sx : sx, ey likewise, D(ey, ex) when
+ * transposed and D(ex, ey) otherwise; an upright rectangle is therefore one rectangle in the stored frame too. */
+int jd_orient_plan(int width, int height, int subsample, int restart_interval, int sshift, int k, const int32_t *rect,
+                   int32_t *srect, JDRoiPlan *plan)
+{
+    if (k < 1 || k > 8) return 0;
+    const int64_t sw = (width + (1 << sshift) - 1) >> sshift, sh = (height + (1 << sshift) - 1) >> sshift;
+    const int tr = k >= 5;
+    const int64_t dw = tr ? sh : sw, dh = tr ? sw : sh;
+    const int64_t x = rect ? rect[0] : 0, y = rect ? rect[1] : 0, w = rect ? rect[2] : dw, h = rect ? rect[3] : dh;
+    if (x < 0 || y < 0 || w < 1 || h < 1 || x + w > dw || y + h > dh) return 0;
+    /* the rectangle in the mirrored stored frame (ex, ey), then un-mirrored */
+    const int64_t ex0 = tr ? y : x, exn = tr ? h : w, ey0 = tr ? x : y, eyn = tr ? w : h;
+    srect[0] = (int32_t)(((JD_ORIENT_MX >> k) & 1u) ? sw - ex0 - exn : ex0);
+    srect[1] = (int32_t)(((JD_ORIENT_MY >> k) & 1u) ? sh - ey0 - eyn : ey0);
+    srect[2] = (int32_t)exn;
+    srect[3] = (int32_t)eyn;
+    if (!jd_roi_plan(width, height, subsample, restart_interval, sshift, srect, plan)) return 0;
+    plan->out_w = (int32_t)w;
+    plan->out_h = (int32_t)h;
+    return 1;
+}
+
 /* A caller's output for one image.  Host and device: a pitch below the row bytes would make rows overlap (and the last
  * rows run past a buffer of out_h * pitch bytes); the descriptors hold the pitch in 32 bits.  Device outputs are written by
  * the kernels, whose narrowest stores are per pixel (jd_phase_c_full's per-pixel fallback, jd_phase_c_half, jdk_scaled:

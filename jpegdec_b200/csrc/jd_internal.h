@@ -76,7 +76,9 @@ typedef struct {
     uint16_t mcu_x0, mcu_y0;/* first MCU column / row it touches: the IDCT grid starts there */
     uint32_t roi_mcu_end;   /* 1 + the last MCU (full-image raster index) of the last MCU row it touches; 0 = no rectangle.
                              * An error at or past this MCU is not reported (the reference's crop decode stops above it). */
-    uint32_t pad_;
+    uint32_t orient;        /* EXIF transform 1-8 applied by the stores (JPEGB200_batchCreateOriented; 0 / 1 = none).  With
+                             * it, roi_x / roi_y and the MCU box are those of the rectangle in the STORED frame, while out_w /
+                             * out_h stay the output (upright) size: swapped against the stored rectangle for 5-8. */
 } JDImageDesc;
 
 /* What a region of interest (in output pixels: after scaling) means for one image: the MCUs it touches, the restart
@@ -90,6 +92,17 @@ typedef struct {
 } JDRoiPlan;
 int jd_roi_plan(int width, int height, int subsample, int restart_interval, int sshift, const int32_t *rect /* x, y, w, h */,
                 JDRoiPlan *plan);
+/* EXIF transform k as mirrors of the stored frame followed by an optional transpose (k >= 5): bit k of these masks says
+ * whether k mirrors x (stored column sx -> sw - 1 - sx) and y.  2 = mirror x, 3 = both, 4 = y, 5 = transpose, 6 = y then
+ * transpose (90 degrees clockwise), 7 = both then transpose, 8 = x then transpose (90 degrees counter-clockwise). */
+#define JD_ORIENT_MX 0x18Cu
+#define JD_ORIENT_MY 0x0D8u
+/* The same for an oriented image.  k: EXIF transform 1-8.  rect: x, y, w, h in the OUTPUT (upright) frame, whose size is the
+ * scaled image's with width and height swapped for k = 5-8; NULL = the whole image.  srect receives the rectangle in the
+ * stored frame (where the MCUs are), plan is jd_roi_plan's for srect except that out_w / out_h are the output size (w, h).
+ * Returns 0 for a k outside 1-8 or a rectangle that does not lie inside the output image. */
+int jd_orient_plan(int width, int height, int subsample, int restart_interval, int sshift, int k, const int32_t *rect,
+                   int32_t *srect /* x, y, w, h */, JDRoiPlan *plan);
 
 /* A caller's destination for image `index` (only named in the message): row_bytes is the tight pitch
  * (JPEGB200_batchOutputBytes), pitch <= 0 means tight.  device != 0: `out` is written by the kernels.  Returns 1, or 0 with

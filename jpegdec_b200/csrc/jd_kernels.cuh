@@ -746,6 +746,28 @@ __global__ void __launch_bounds__(128) jdk_chunk_stitch(const JDChunkArgs a)
 #define JD_PT_8888 1
 #define JD_PT_GRAY 2
 
+/* transform classes of the oriented stores (JDImageDesc.orient), one kernel instantiation each */
+#define JD_ORC_NONE 0       /* EXIF 1 (and no orientation) */
+#define JD_ORC_FLIP 1       /* 2, 3, 4: mirrors only -- the store item is reversed in registers, rows are re-addressed */
+#define JD_ORC_TRANSPOSE 2  /* 5-8: a stored row becomes an output column -- the strip is staged in shared memory */
+__host__ __device__ __forceinline__ uint32_t jd_orient_class(uint32_t k) { return k >= 5u ? JD_ORC_TRANSPOSE : (k >= 2u ? JD_ORC_FLIP : JD_ORC_NONE); }
+
+/* with a rectangle: its size in the stored frame (out_w / out_h are the output's, swapped by a transpose) */
+template <int ORC> __device__ __forceinline__ uint32_t jd_roi_sw(const JDImageDesc &im) { return ORC == JD_ORC_TRANSPOSE ? im.out_h : im.out_w; }
+template <int ORC> __device__ __forceinline__ uint32_t jd_roi_sh(const JDImageDesc &im) { return ORC == JD_ORC_TRANSPOSE ? im.out_w : im.out_h; }
+
+/* shared staging of the transposed stores, only in the instantiations that use it */
+template <int BYTES> __device__ __forceinline__ uint8_t *jd_orient_stage()
+{
+    __shared__ __align__(16) uint8_t s_stage[BYTES];
+    return s_stage;
+}
+/* passes in which a transposed strip of wcta x hcta pixels is staged: as few as keep the stage within 16 KB */
+__host__ __device__ constexpr int jd_orient_npass(int wcta, int hcta, int bypp)
+{
+    return wcta * (hcta * bypp + 4) <= 16384 ? 1 : (wcta * (hcta / 2 * bypp + 4) <= 16384 ? 2 : 4);
+}
+
 struct JDIdctArgs {
     const JDImageDesc *imgs;
     const jd_u64 *blk_hdr;
@@ -757,7 +779,7 @@ struct JDIdctArgs {
     uint32_t img0;          /* first image of this launch (blockIdx.z offset) */
     uint32_t big_endian;    /* RGB565_BIG_ENDIAN requested */
     uint32_t padded;        /* 1: write the whole MCU-aligned area (dither intermediate / callback replay) */
-    uint32_t roi;           /* host side: launch the ROI instantiations (grid over each image's rectangle) */
+    uint32_t roi;           /* host side: launch the ROI instantiations (grid over each image's rectangle); 1 + JD_ORC_* */
 };
 
 template <int HS, int VS, int NC, int MPB>
@@ -828,14 +850,27 @@ __device__ __forceinline__ uint32_t jd_pixel_scalar(int Y12, int cb, int cr, boo
 /* Phase C of the fused kernels (full size): colour conversion of the staged planes + coalesced 16-byte scanline stores.
  * s_y: (VS*8) rows x YSTRIDE luma bytes, s_cb/s_cr: 8 rows x CSTRIDE chroma bytes, covering WCTA pixels from x = x0 of MCU
  * row `my`.  ROI: only pixels in [rx, W) x [ry, H) are stored, at (x - rx, y - ry); every value is still computed in
- * full-image coordinates, so a pixel does not depend on the rectangle. */
-template <int HS, int VS, int NC, int PT, int ARITH, int WCTA, int YSTRIDE, int CSTRIDE, int NTHREADS, bool INTERIOR = false, bool ROI = false>
+ * full-image coordinates, so a pixel does not depend on the rectangle.
+ * Orientation (ORC != JD_ORC_NONE, always with a rectangle: [rx, W) x [ry, H) in the stored frame): only the store address
+ * changes.  JD_ORC_FLIP reverses an item's pixels in registers (byte permutes) for a mirror in x and keeps the 16-byte store
+ * where the mirrored destination is aligned; a mirror in y only changes the row.  JD_ORC_TRANSPOSE stages the converted
+ * strip column-major in s_t (NPASS passes of HCTA / NPASS rows each, WCTA x (HCTA / NPASS * BYPP + 4) bytes), then writes
+ * each stored column as a segment of an output row with 16-byte stores. */
+template <int HS, int VS, int NC, int PT, int ARITH, int WCTA, int YSTRIDE, int CSTRIDE, int NTHREADS, bool INTERIOR = false, bool ROI = false,
+          int ORC = JD_ORC_NONE, int NPASS = 1>
 __device__ __forceinline__ void jd_phase_c_full(const JDIdctArgs &a, const uint8_t *s_y, const uint8_t *s_cb, const uint8_t *s_cr,
                                                 uint32_t x0, uint32_t my, uint32_t tid, uint32_t W, uint32_t H,
-                                                uint8_t *outbase, uint32_t pitch, uint32_t rx = 0u, uint32_t ry = 0u)
+                                                uint8_t *outbase, uint32_t pitch, uint32_t rx = 0u, uint32_t ry = 0u,
+                                                uint32_t orient = 0u, uint8_t *s_t = nullptr)
 {
     static_assert(!(ROI && INTERIOR), "a rectangle is always clipped");
+    static_assert(ORC == JD_ORC_NONE || ROI, "oriented stores run with a rectangle");
     constexpr int BYPP = (PT == JD_PT_565) ? 2 : (PT == JD_PT_8888 ? 4 : 1);
+    constexpr int HCTA = VS * 8, HP = HCTA / NPASS;          /* transposed: stored rows per pass */
+    constexpr int TSB = HP * BYPP + 4;                        /* bytes per staged column (4-byte aligned, spreads banks) */
+    const bool mxf = ORC != JD_ORC_NONE && ((JD_ORIENT_MX >> orient) & 1u);
+    const bool myf = ORC != JD_ORC_NONE && ((JD_ORIENT_MY >> orient) & 1u);
+    uint32_t pass_row0 = 0u;                                  /* transposed: first strip row of the current pass */
     /* one item = PXI pixels (OWN 16-byte stores) in each of the VS rows that share chroma */
 #ifndef JD_PXI_8888
 #define JD_PXI_8888 4   /* 8-pixel items (two stores per row) measured slower */
@@ -942,6 +977,58 @@ __device__ __forceinline__ void jd_phase_c_full(const JDIdctArgs &a, const uint8
                 }
                 }
             }
+            /* pixel i of this row's item as stored bytes */
+            auto pix = [&](uint32_t i) -> uint32_t {
+                if (BYPP == 4) return ow[i % (4 * OWN)];
+                if (BYPP == 2) return (ow[(i >> 1) & 3] >> ((i & 1) * 16)) & 0xFFFFu;
+                return (ow[(i >> 2) & 3] >> ((i & 3) * 8)) & 0xFFu;
+            };
+            auto put = [&](uint8_t *p, uint32_t v) {
+                if (BYPP == 4) *reinterpret_cast<uint32_t *>(p) = v;
+                else if (BYPP == 2) *reinterpret_cast<uint16_t *>(p) = (uint16_t)v;
+                else *p = (uint8_t)v;
+            };
+            if (ORC == JD_ORC_TRANSPOSE) {
+                /* stored column c -> staged column c, stored row -> position j along it (reversed by a mirror in y) */
+                const uint32_t rl = row - pass_row0;
+                const uint32_t j = myf ? (uint32_t)HP - 1u - rl : rl;
+#pragma unroll
+                for (int i = 0; i < PXI; i++) put(s_t + (xg * PXI + i) * TSB + j * BYPP, pix(i));
+                continue;
+            }
+            if (ORC == JD_ORC_FLIP) {
+                const uint32_t dy = myf ? H - 1u - gy : gy - ry;
+                uint8_t *row_p = outbase + (size_t)dy * pitch;
+                if (mxf) {
+                    /* mirrored: pixel i lands at x = W - 1 - (gx + i), so the item starts at W - gx - PXI, reversed */
+                    uint8_t *dm = row_p + (ptrdiff_t)((int)W - (int)gx - PXI) * BYPP;
+                    if (full && ((reinterpret_cast<uintptr_t>(dm) & 15u) == 0)) {
+                        uint32_t rv[4 * OWN];
+#pragma unroll
+                        for (int q = 0; q < 4 * OWN; q++)
+                            rv[q] = BYPP == 4 ? ow[4 * OWN - 1 - q] : __byte_perm(ow[3 - q], 0u, BYPP == 2 ? 0x1032 : 0x0123);
+#pragma unroll
+                        for (int q = 0; q < OWN; q++) reinterpret_cast<uint4 *>(dm)[q] = make_uint4(rv[4 * q], rv[4 * q + 1], rv[4 * q + 2], rv[4 * q + 3]);
+                    } else {
+                        for (uint32_t i = 0; i < (uint32_t)PXI && gx + i < W; i++) {
+                            if (gx + i < rx) continue;
+                            put(row_p + (size_t)(W - 1u - gx - i) * BYPP, pix(i));
+                        }
+                    }
+                    continue;
+                }
+                uint8_t *dn = row_p + (ptrdiff_t)((int)gx - (int)rx) * BYPP;
+                if (full && ((reinterpret_cast<uintptr_t>(dn) & 15u) == 0)) {
+#pragma unroll
+                    for (int q = 0; q < OWN; q++) reinterpret_cast<uint4 *>(dn)[q] = make_uint4(ow[4 * q], ow[4 * q + 1], ow[4 * q + 2], ow[4 * q + 3]);
+                } else {
+                    for (uint32_t i = 0; i < (uint32_t)PXI && gx + i < W; i++) {
+                        if (gx + i < rx) continue;
+                        put(dn + (size_t)i * BYPP, pix(i));
+                    }
+                }
+                continue;
+            }
             /* with a rectangle dst may point left of the row for an item that straddles x = rx: only i >= rx - gx is stored */
             uint8_t *dst = ROI ? outbase + (size_t)(gy - ry) * pitch + (ptrdiff_t)((int)gx - (int)rx) * BYPP
                                : outbase + (size_t)gy * pitch + (size_t)gx * BYPP;
@@ -958,7 +1045,46 @@ __device__ __forceinline__ void jd_phase_c_full(const JDIdctArgs &a, const uint8
             }
         }
         };
-    if (NTHREADS % IPR == 0) {
+    if (ORC == JD_ORC_TRANSPOSE) {
+        /* per pass: stage HP stored rows of the strip, then write stored column c as output row dy, HP pixels from dx0 on.
+         * Units of 16 bytes (or the whole column when it is shorter) so that a 64-byte RGB8888 segment of a 16-row strip
+         * is four 16-byte stores where the destination is aligned. */
+        constexpr int SEGB = HP * BYPP, CH = SEGB >= 16 ? 16 : SEGB, PPU = CH / BYPP, NU = SEGB / CH;
+        constexpr int RGP = 8 / NPASS;                       /* row groups per pass */
+        const int sh = (int)H - (int)ry;
+        for (int pass = 0; pass < NPASS; pass++) {
+            pass_row0 = (uint32_t)(pass * HP);
+            for (uint32_t it = tid; it < (uint32_t)(IPR * RGP); it += NTHREADS) {
+                const uint32_t rg = jd_div_small<IPR>(it);
+                item(pass * RGP + rg, it - rg * IPR);
+            }
+            __syncthreads();
+            const int y0p = (int)(my * HCTA) + pass * HP;
+            const int dxbase = myf ? (int)H - y0p - HP : y0p - (int)ry;   /* output x of staged position 0 */
+            for (uint32_t it = tid; it < (uint32_t)(WCTA * NU); it += NTHREADS) {
+                const uint32_t c = it / NU, u = it % NU;
+                const uint32_t gx = x0 + c;
+                if (gx < rx || gx >= W) continue;
+                const uint32_t dy = mxf ? W - 1u - gx : gx - rx;
+                const int dx0 = dxbase + (int)(u * PPU);
+                uint8_t *orow = outbase + (size_t)dy * pitch;
+                const uint8_t *src = s_t + c * TSB + u * CH;
+                if (CH == 16 && dx0 >= 0 && dx0 + PPU <= sh && ((reinterpret_cast<uintptr_t>(orow + dx0 * BYPP) & 15u) == 0)) {
+                    const uint32_t *s4 = reinterpret_cast<const uint32_t *>(src);
+                    *reinterpret_cast<uint4 *>(orow + dx0 * BYPP) = make_uint4(s4[0], s4[1], s4[2], s4[3]);
+                } else {
+                    for (int p = 0; p < PPU; p++) {
+                        const int dx = dx0 + p;
+                        if (dx < 0 || dx >= sh) continue;
+                        if (BYPP == 4) *reinterpret_cast<uint32_t *>(orow + dx * 4) = *reinterpret_cast<const uint32_t *>(src + p * 4);
+                        else if (BYPP == 2) *reinterpret_cast<uint16_t *>(orow + dx * 2) = *reinterpret_cast<const uint16_t *>(src + p * 2);
+                        else orow[dx] = src[p];
+                    }
+                }
+            }
+            if (pass + 1 < NPASS) __syncthreads();
+        }
+    } else if (NTHREADS % IPR == 0) {
         /* the thread keeps its x position; only the row group advances (no division, x addressing hoisted) */
         const uint32_t xg = tid % IPR;
         for (uint32_t rg = tid / IPR; rg < 8u; rg += NTHREADS / IPR) item(rg, xg);
@@ -968,15 +1094,19 @@ __device__ __forceinline__ void jd_phase_c_full(const JDIdctArgs &a, const uint8
 }
 
 /* Phase C at 1/2 scale: 2x2 luma sums; scalar colour code in both builds (jpeg.inl:3297-3322, :3577-3626).  ox0: output x
- * of the CTA's first column.  ROI: W, H are the rectangle's right / bottom edge in OUTPUT pixels and (rx, ry) its origin. */
-template <int HS, int VS, int NC, int PT, int WCTA, int HCTA, int YSTRIDE, int CSTRIDE, int NTHREADS, bool ROI = false>
+ * of the CTA's first column.  ROI: W, H are the rectangle's right / bottom edge in OUTPUT pixels and (rx, ry) its origin.
+ * Orientation (ORC != JD_ORC_NONE): the stores are per pixel already, so only their address changes. */
+template <int HS, int VS, int NC, int PT, int WCTA, int HCTA, int YSTRIDE, int CSTRIDE, int NTHREADS, bool ROI = false, int ORC = JD_ORC_NONE>
 __device__ __forceinline__ void jd_phase_c_half(const JDIdctArgs &a, const uint8_t *s_y, const uint8_t *s_cb, const uint8_t *s_cr,
                                                 uint32_t ox0, uint32_t my, uint32_t tid, uint32_t W, uint32_t H,
-                                                uint8_t *outbase, uint32_t pitch, uint32_t rx = 0u, uint32_t ry = 0u)
+                                                uint8_t *outbase, uint32_t pitch, uint32_t rx = 0u, uint32_t ry = 0u, uint32_t orient = 0u)
 {
+    static_assert(ORC == JD_ORC_NONE || ROI, "oriented stores run with a rectangle");
     constexpr int BYPP = (PT == JD_PT_565) ? 2 : (PT == JD_PT_8888 ? 4 : 1);
     const uint32_t OW = ROI ? W : (W + 1) >> 1, OH = ROI ? H : (H + 1) >> 1;
     constexpr int OWC = WCTA / 2, OHC = HCTA / 2;
+    const bool mxf = ORC != JD_ORC_NONE && ((JD_ORIENT_MX >> orient) & 1u);
+    const bool myf = ORC != JD_ORC_NONE && ((JD_ORIENT_MY >> orient) & 1u);
     for (uint32_t it = tid; it < (uint32_t)(OWC * OHC); it += NTHREADS) {
         const uint32_t oy = it / OWC, ox = it - oy * OWC;
         const uint32_t gy = my * OHC + oy, gx = ox0 + ox;
@@ -984,7 +1114,12 @@ __device__ __forceinline__ void jd_phase_c_half(const JDIdctArgs &a, const uint8
         if (ROI && (gy < ry || gx < rx)) continue;
         const uint8_t *yp = s_y + (2 * oy) * YSTRIDE + 2 * ox;
         const int sum = yp[0] + yp[1] + yp[YSTRIDE] + yp[YSTRIDE + 1];
-        uint8_t *dst = outbase + (size_t)(gy - ry) * pitch + (size_t)(gx - rx) * BYPP;
+        uint8_t *dst;
+        if (ORC == JD_ORC_NONE) dst = outbase + (size_t)(gy - ry) * pitch + (size_t)(gx - rx) * BYPP;
+        else {
+            const uint32_t ex = mxf ? OW - 1u - gx : gx - rx, ey = myf ? OH - 1u - gy : gy - ry;
+            dst = ORC == JD_ORC_TRANSPOSE ? outbase + (size_t)ex * pitch + (size_t)ey * BYPP : outbase + (size_t)ey * pitch + (size_t)ex * BYPP;
+        }
         if (PT == JD_PT_GRAY) {
             *dst = (uint8_t)((sum + 2) >> 2);
         } else if (NC == 1) {
@@ -1016,14 +1151,15 @@ __device__ __forceinline__ void jd_phase_c_half(const JDIdctArgs &a, const uint8
 /* ROI: a CTA whose first MCU column or whose MCU row lies right of / below the image's rectangle has nothing to store (the
  * grid is sized for the largest rectangle of the launch).  Exact: MCU row my is needed iff its first output row is above the
  * rectangle's bottom edge. */
-template <int HS, int VS, bool HALF>
+template <int HS, int VS, bool HALF, int ORC = JD_ORC_NONE>
 __device__ __forceinline__ bool jd_roi_cta_outside(const JDImageDesc &im, uint32_t mx0, uint32_t my)
 {
     constexpr uint32_t SH = HALF ? 1u : 0u;
-    return ((mx0 * HS * 8u) >> SH) >= (uint32_t)im.roi_x + im.out_w || ((my * VS * 8u) >> SH) >= (uint32_t)im.roi_y + im.out_h;
+    if (ORC != JD_ORC_NONE && (im.orient >= 5u) != (ORC == JD_ORC_TRANSPOSE)) return true;   /* the other class's launch */
+    return ((mx0 * HS * 8u) >> SH) >= (uint32_t)im.roi_x + jd_roi_sw<ORC>(im) || ((my * VS * 8u) >> SH) >= (uint32_t)im.roi_y + jd_roi_sh<ORC>(im);
 }
 
-template <int HS, int VS, int NC, int MPB, int PT, int ARITH, bool HALF, bool ROI>
+template <int HS, int VS, int NC, int MPB, int PT, int ARITH, bool HALF, bool ROI, int ORC = JD_ORC_NONE>
 __global__ void __launch_bounds__(JDGeo<HS, VS, NC, MPB>::THREADS)
 jdk_idct_color(const JDIdctArgs a)
 {
@@ -1037,7 +1173,7 @@ jdk_idct_color(const JDIdctArgs a)
     /* ROI: the grid covers the group's largest rectangle from each image's first MCU column / row */
     const uint32_t my = ROI ? im.mcu_y0 + blockIdx.y : blockIdx.y;
     const uint32_t mx0 = (ROI ? (uint32_t)im.mcu_x0 : 0u) + blockIdx.x * MPB;
-    if (ROI && jd_roi_cta_outside<HS, VS, HALF>(im, mx0, my)) return;
+    if (ROI && jd_roi_cta_outside<HS, VS, HALF, ORC>(im, mx0, my)) return;
     const uint32_t tid = threadIdx.x;
 
     /* ---- phase A: expand this block's records into a column-major coefficient tile ---- */
@@ -1123,7 +1259,14 @@ jdk_idct_color(const JDIdctArgs a)
     const uint32_t pitch = im.out_pitch;
     constexpr int BYPP = (PT == JD_PT_565) ? 2 : (PT == JD_PT_8888 ? 4 : 1);
 
-    if (ROI) {
+    if (ROI && ORC != JD_ORC_NONE) {
+        const uint32_t rx = im.roi_x, ry = im.roi_y, rxe = rx + jd_roi_sw<ORC>(im), rye = ry + jd_roi_sh<ORC>(im);
+        constexpr int NP = jd_orient_npass(G::WCTA, G::HCTA, BYPP);
+        constexpr int STAGE = ORC == JD_ORC_TRANSPOSE ? G::WCTA * (G::HCTA / NP * BYPP + 4) : 16;
+        if (!HALF) jd_phase_c_full<HS, VS, NC, PT, ARITH, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, false, true, ORC, NP>(a, s_y, s_cb, s_cr, mx0 * HS * 8, my, tid, rxe, rye, outbase, pitch, rx, ry,
+                                                                                                                    im.orient, ORC == JD_ORC_TRANSPOSE ? jd_orient_stage<STAGE>() : nullptr);
+        else jd_phase_c_half<HS, VS, NC, PT, G::WCTA, G::HCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, true, ORC>(a, s_y, s_cb, s_cr, mx0 * HS * 4, my, tid, rxe, rye, outbase, pitch, rx, ry, im.orient);
+    } else if (ROI) {
         const uint32_t rx = im.roi_x, ry = im.roi_y, rxe = rx + im.out_w, rye = ry + im.out_h;
         if (!HALF) jd_phase_c_full<HS, VS, NC, PT, ARITH, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, false, true>(a, s_y, s_cb, s_cr, mx0 * HS * 8, my, tid, rxe, rye, outbase, pitch, rx, ry);
         else jd_phase_c_half<HS, VS, NC, PT, G::WCTA, G::HCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, true>(a, s_y, s_cb, s_cr, mx0 * HS * 4, my, tid, rxe, rye, outbase, pitch, rx, ry);
@@ -1176,7 +1319,7 @@ __device__ __forceinline__ uint2 jd_row_finish_packed(const int t[8])
 #ifndef JD_TB_MINB
 #define JD_TB_MINB 10   /* 48 registers: 10 CTAs per SM measured faster than 56 registers / 9 CTAs and than 40 / 12 */
 #endif
-template <int HS, int VS, int NC, int MPB, int PT, int ARITH, bool ROI>
+template <int HS, int VS, int NC, int MPB, int PT, int ARITH, bool ROI, int ORC = JD_ORC_NONE>
 __global__ void __launch_bounds__(JDGeoTB<HS, VS, NC, MPB>::THREADS, JD_TB_MINB)
 jdk_idct_tb(const JDIdctArgs a)
 {
@@ -1193,7 +1336,7 @@ jdk_idct_tb(const JDIdctArgs a)
     const JDImageDesc &im = a.imgs[img_i];
     const uint32_t my = ROI ? im.mcu_y0 + blockIdx.y : blockIdx.y;
     const uint32_t mx0 = (ROI ? (uint32_t)im.mcu_x0 : 0u) + blockIdx.x * MPB;
-    if (ROI && jd_roi_cta_outside<HS, VS, false>(im, mx0, my)) return;
+    if (ROI && jd_roi_cta_outside<HS, VS, false, ORC>(im, mx0, my)) return;
     const uint32_t tid = threadIdx.x, lane = tid & 31u, wid = tid >> 5;
     const uint16_t *const irec = a.rec + im.rec_base;
 
@@ -1410,7 +1553,15 @@ jdk_idct_tb(const JDIdctArgs a)
     uint8_t *outbase = a.out + im.out_off;
     const uint32_t pitch = im.out_pitch;
     const uint32_t x0 = mx0 * HS * 8;
-    if (ROI)
+    if (ROI && ORC != JD_ORC_NONE) {
+        /* transposes stage the strip in two passes of half its rows: 32-byte RGB8888 / 16-byte RGB565 output segments, and
+         * half the shared memory of a whole-strip stage (this kernel runs 10 CTAs per SM) */
+        constexpr int BYPP = (PT == JD_PT_565) ? 2 : (PT == JD_PT_8888 ? 4 : 1);
+        constexpr int STAGE = ORC == JD_ORC_TRANSPOSE ? G::WCTA * (G::HCTA / 2 * BYPP + 4) : 16;
+        jd_phase_c_full<HS, VS, NC, PT, ARITH, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, false, true, ORC, 2>(a, s_y, s_c, s_c + 8 * G::CSTRIDE, x0, my, tid,
+            (uint32_t)im.roi_x + jd_roi_sw<ORC>(im), (uint32_t)im.roi_y + jd_roi_sh<ORC>(im), outbase, pitch, im.roi_x, im.roi_y,
+            im.orient, ORC == JD_ORC_TRANSPOSE ? jd_orient_stage<STAGE>() : nullptr);
+    } else if (ROI)
         jd_phase_c_full<HS, VS, NC, PT, ARITH, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, false, true>(a, s_y, s_c, s_c + 8 * G::CSTRIDE, x0, my, tid,
             (uint32_t)im.roi_x + im.out_w, (uint32_t)im.roi_y + im.out_h, outbase, pitch, im.roi_x, im.roi_y);
     else if (x0 + G::WCTA <= W && (my + 1) * G::HCTA <= H && ((reinterpret_cast<uintptr_t>(outbase) | pitch) & 15u) == 0u)
@@ -1451,7 +1602,7 @@ struct JDGeoP {
 #ifndef JD_P_MINB
 #define JD_P_MINB 7
 #endif
-template <int HS, int VS, int NC, int MPB, int PT, bool HALF, bool ROI>
+template <int HS, int VS, int NC, int MPB, int PT, bool HALF, bool ROI, int ORC = JD_ORC_NONE>
 __global__ void __launch_bounds__(128, JD_P_MINB)
 jdk_idct_p(const JDIdctArgs a)
 {
@@ -1469,7 +1620,7 @@ jdk_idct_p(const JDIdctArgs a)
     const JDImageDesc &im = a.imgs[img_i];
     const uint32_t my = ROI ? im.mcu_y0 + blockIdx.y : blockIdx.y;
     const uint32_t mx0 = (ROI ? (uint32_t)im.mcu_x0 : 0u) + blockIdx.x * MPB;
-    if (ROI && jd_roi_cta_outside<HS, VS, HALF>(im, mx0, my)) return;
+    if (ROI && jd_roi_cta_outside<HS, VS, HALF, ORC>(im, mx0, my)) return;
     const uint32_t tid = threadIdx.x, lane = tid & 31u, wid = tid >> 5;
     const uint16_t *const irec = a.rec + im.rec_base;
 
@@ -1598,7 +1749,15 @@ jdk_idct_p(const JDIdctArgs a)
     const uint32_t pitch = im.out_pitch;
     const uint8_t *s_cb = s_c, *s_cr = s_c + 8 * G::CSTRIDE;
     const uint32_t x0 = mx0 * HS * 8;
-    if (ROI) {
+    if (ROI && ORC != JD_ORC_NONE) {
+        const uint32_t rx = im.roi_x, ry = im.roi_y, rxe = rx + jd_roi_sw<ORC>(im), rye = ry + jd_roi_sh<ORC>(im);
+        constexpr int BYPP = (PT == JD_PT_565) ? 2 : (PT == JD_PT_8888 ? 4 : 1);
+        constexpr int NP = jd_orient_npass(G::WCTA, G::HCTA, BYPP);
+        constexpr int STAGE = ORC == JD_ORC_TRANSPOSE ? G::WCTA * (G::HCTA / NP * BYPP + 4) : 16;
+        if (HALF) jd_phase_c_half<HS, VS, NC, PT, G::WCTA, G::HCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, true, ORC>(a, s_y, s_cb, s_cr, x0 / 2, my, tid, rxe, rye, outbase, pitch, rx, ry, im.orient);
+        else jd_phase_c_full<HS, VS, NC, PT, JPEG_ARITH_SSE2, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, false, true, ORC, NP>(a, s_y, s_cb, s_cr, x0, my, tid, rxe, rye, outbase, pitch, rx, ry,
+                                                                                                                          im.orient, ORC == JD_ORC_TRANSPOSE && !HALF ? jd_orient_stage<STAGE>() : nullptr);
+    } else if (ROI) {
         const uint32_t rx = im.roi_x, ry = im.roi_y, rxe = rx + im.out_w, rye = ry + im.out_h;
         if (HALF) jd_phase_c_half<HS, VS, NC, PT, G::WCTA, G::HCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, true>(a, s_y, s_cb, s_cr, x0 / 2, my, tid, rxe, rye, outbase, pitch, rx, ry);
         else jd_phase_c_full<HS, VS, NC, PT, JPEG_ARITH_SSE2, G::WCTA, G::YSTRIDE, G::CSTRIDE, G::THREADS, false, true>(a, s_y, s_cb, s_cr, x0, my, tid, rxe, rye, outbase, pitch, rx, ry);
@@ -1652,20 +1811,23 @@ __device__ __forceinline__ void jd_scaled_block(const uint16_t *irec, jd_u64 h, 
     px[0] = jd_range(t0 + t1); px[1] = jd_range(t0 - t1); px[2] = jd_range(t2 + t3); px[3] = jd_range(t2 - t3);
 }
 
-/* ROI: one thread per MCU of the box of MCUs the image's rectangle touches (the grid covers the launch's largest box) */
-template <bool ROI>
+/* ROI: one thread per MCU of the box of MCUs the image's rectangle touches (the grid covers the launch's largest box).
+ * ORC: oriented stores (per pixel, so only the address changes; the rectangle is then in the stored frame). */
+template <bool ROI, int ORC = JD_ORC_NONE>
 __global__ void __launch_bounds__(128) jdk_scaled(const JDScaledArgs a)
 {
+    static_assert(ORC == JD_ORC_NONE || ROI, "oriented stores run with a rectangle");
     const uint32_t img_i = a.img0 + blockIdx.y;
     const JDImageDesc &im = a.imgs[img_i];
+    if (ORC != JD_ORC_NONE && (im.orient >= 5u) != (ORC == JD_ORC_TRANSPOSE)) return;   /* the other class's launch */
     const uint32_t hs = (im.subsample >> 4) ? (im.subsample >> 4) : 1, vs = (im.subsample & 15) ? (im.subsample & 15) : 1;
     const bool eighth = a.eighth != 0;
     const uint32_t bs = eighth ? 1u : 2u; /* block edge in output pixels */
     const uint32_t ow = hs * bs, oh = vs * bs; /* output pixels per MCU */
     uint32_t m = blockIdx.x * blockDim.x + threadIdx.x, mx, my;
     if (ROI) {
-        const uint32_t ncols = ((uint32_t)im.roi_x + im.out_w - 1u) / ow - im.mcu_x0 + 1u;
-        const uint32_t nrows = ((uint32_t)im.roi_y + im.out_h - 1u) / oh - im.mcu_y0 + 1u;
+        const uint32_t ncols = ((uint32_t)im.roi_x + jd_roi_sw<ORC>(im) - 1u) / ow - im.mcu_x0 + 1u;
+        const uint32_t nrows = ((uint32_t)im.roi_y + jd_roi_sh<ORC>(im) - 1u) / oh - im.mcu_y0 + 1u;
         if (m >= ncols * nrows) return;
         my = im.mcu_y0 + m / ncols; mx = im.mcu_x0 + m % ncols;
         m = my * im.mcus_x + mx;
@@ -1691,12 +1853,20 @@ __global__ void __launch_bounds__(128) jdk_scaled(const JDScaledArgs a)
     uint8_t *outbase = a.out + im.out_off;
     /* stores clipped to [x_lo, x_hi) x [y_lo, y_hi) and shifted to its origin */
     const uint32_t x_lo = ROI ? im.roi_x : 0u, y_lo = ROI ? im.roi_y : 0u;
-    const uint32_t x_hi = ROI ? x_lo + im.out_w : W, y_hi = ROI ? y_lo + im.out_h : H;
+    const uint32_t x_hi = ROI ? x_lo + jd_roi_sw<ORC>(im) : W, y_hi = ROI ? y_lo + jd_roi_sh<ORC>(im) : H;
+    const bool mxf = ORC != JD_ORC_NONE && ((JD_ORIENT_MX >> im.orient) & 1u);
+    const bool myf = ORC != JD_ORC_NONE && ((JD_ORIENT_MY >> im.orient) & 1u);
     for (uint32_t y = 0; y < oh; y++) {
         for (uint32_t x = 0; x < ow; x++) {
             const uint32_t fx = mx * ow + x, fy = my * oh + y;
             if (fx >= x_hi || fy >= y_hi || fx < x_lo || fy < y_lo) continue;
-            const uint32_t gx = fx - x_lo, gy = fy - y_lo;
+            uint32_t gx = fx - x_lo, gy = fy - y_lo;
+            if (ORC != JD_ORC_NONE) {
+                /* output column / row of this pixel: mirrored in the stored frame, then transposed */
+                const uint32_t ex = mxf ? x_hi - 1u - fx : gx, ey = myf ? y_hi - 1u - fy : gy;
+                gx = ORC == JD_ORC_TRANSPOSE ? ey : ex;
+                gy = ORC == JD_ORC_TRANSPOSE ? ex : ey;
+            }
             const uint32_t bx = x / bs, by = y / bs;
             const uint32_t lb = (hs == 2 && vs == 2) ? by * 2 + bx : (hs == 2 ? bx : by);
             const uint32_t Y = ypx[lb][(y % bs) * bs + (x % bs)];
