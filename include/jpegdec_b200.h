@@ -42,7 +42,7 @@ enum {
     JPEGB200_T_ENTROPY,
     JPEGB200_T_STITCH,
     JPEGB200_T_IDCT,
-    JPEGB200_T_DITHER,
+    JPEGB200_T_DITHER,         /* the pixel pass after the IDCT: dither, or resize (the two never occur together) */
     JPEGB200_T_D2H,
     JPEGB200_T_TOTAL,
     JPEGB200_NUM_TIMINGS
@@ -137,6 +137,31 @@ JPEGB200_BATCH *JPEGB200_batchCreateROI(JPEGB200_CTX *ctx, const uint8_t *const 
  * oriented batch. */
 JPEGB200_BATCH *JPEGB200_batchCreateOriented(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes,
                                              int n, int pixel_type, int options, const int32_t *rois, const uint8_t *orients);
+/* Resized decode (a loader's crop -> flip -> resize in one call).  S_i = what JPEGB200_batchCreateOriented produces for
+ * image i with the same rois / orients (after scaling, thumbnail selection and LUMA_ONLY folding); out_sizes[2i], [2i+1] =
+ * W, H.  Image i's output is Pillow's Image.resize((W, H), filter) of every byte plane of S_i viewed as [rows, cols, bytes
+ * per pixel], bit for bit (PIL/libImaging/Resample.c: double coefficients rounded to 22-bit integers, a horizontal pass
+ * into a uint8 intermediate holding only the source rows the vertical pass reads, then the vertical pass; a pass along an
+ * axis whose size does not change is skipped, so W, H = S's size gives S).  Crop, then orient, then resize: torchvision's
+ * resized_crop on PIL images.  out_sizes = NULL is JPEGB200_batchCreateOriented (filter ignored).
+ *   - filter: JPEGB200_RESIZE_BILINEAR, _BICUBIC or _BOX (PIL.Image.Resampling's numbers).  NEAREST is another algorithm
+ *     in Pillow; HAMMING and LANCZOS need sin(), whose device rounding is not libm's.
+ *   - Pixel types: RGB8888 (in the SSE2-build byte order B,G,R,A too: planes are independent, the 0xFF alpha plane stays
+ *     0xFF) and EIGHT_BIT_GRAYSCALE, LUMA_ONLY folding included; every scale, progressive at 1/8, EXIF thumbnails.
+ *   - Returns NULL with a message for RGB565 (a 5/6/5 word has no byte planes), dithered types, padded output and any
+ *     other filter.  A W or H outside 1..65535 gives that image JPEG_INVALID_PARAMETER; the others decode.
+ *   - Status, JPEGB200_batchErrMcu and the restart intervals walked are those of the same ROI / orient plan; an image with
+ *     JPEG_DECODE_ERROR gets the resize of what the unresized call stores for it.
+ *   - JPEGB200_batchImageInfo reports out_w, out_h = W, H; JPEGB200_batchOutputBytes, the device arena,
+ *     JPEGB200_C_OUTPUT_BYTES, the D2H bytes and the destination rules of JPEGB200_batchSetOutput follow W x H.
+ *   - Device work: the IDCT stage writes S into library scratch (pooled device memory: S plus the intermediate per image),
+ *     then jdk_resize_coeffs / _h / _v; timed in the JPEGB200_T_DITHER slot. */
+#define JPEGB200_RESIZE_BILINEAR 2
+#define JPEGB200_RESIZE_BICUBIC  3
+#define JPEGB200_RESIZE_BOX      4
+JPEGB200_BATCH *JPEGB200_batchCreateResized(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                            int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
+                                            const int32_t *out_sizes /* n x {W, H}; NULL = no resize */, int filter);
 void JPEGB200_batchDestroy(JPEGB200_BATCH *b);
 int JPEGB200_batchCount(JPEGB200_BATCH *b);
 /* per-image facts after batchCreate: status is JPEG_SUCCESS or the open() error the reference would give */
@@ -195,6 +220,15 @@ int JPEGB200_decodeBatchROI(JPEGB200_CTX *ctx, const uint8_t *const *datas, cons
 int JPEGB200_decodeBatchOriented(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
                                  int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
                                  void *const *outs, const int64_t *pitches, int flags, int32_t *status);
+/* The same with a resize per image (out_sizes: n x {W, H}, filter: semantics of JPEGB200_batchCreateResized; NULL = none).
+ * outs[i] receives H rows of W pixels.  Each job also holds at most 1 GiB of resize scratch (the unresized outputs plus
+ * the intermediates), or one image if a single image needs more, so the transient device memory of the call stays
+ * bounded however many images it decodes: each job in flight holds at most that scratch plus, with device outputs, 192 MiB
+ * of compressed bytes and their coefficient records. */
+int JPEGB200_decodeBatchResized(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
+                                const int32_t *out_sizes, int filter, void *const *outs, const int64_t *pitches,
+                                int flags, int32_t *status);
 /* JPEGB200_NUM_COUNTERS counters summed over the jobs of the last JPEGB200_decodeBatch on this context */
 int JPEGB200_lastCallCounters(JPEGB200_CTX *ctx, int64_t *counters);
 /* CUDA-event stage times (JPEGB200_NUM_TIMINGS, ms) summed over those jobs, and how many jobs there were.  Jobs overlap

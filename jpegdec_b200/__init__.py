@@ -27,6 +27,8 @@ JPEG_LE_PIXELS, JPEG_EXIF_THUMBNAIL, JPEG_LUMA_ONLY, JPEG_USES_DMA = 16, 32, 64,
 JPEG_ARITH_SSE2, JPEG_ARITH_SCALAR = 0, 1
 JPEGB200_OUT_DEVICE = 1
 ORIENT_FROM_EXIF = 0   # orients[i]: use the file's EXIF Orientation tag (1-8 force that EXIF transform)
+# resize filters: PIL.Image.Resampling's numbers, so Pillow's constants can be passed as they are
+RESIZE_BILINEAR, RESIZE_BICUBIC, RESIZE_BOX = 2, 3, 4
 TIMING_NAMES = ["h2d", "prescan", "entropy", "stitch", "idct", "dither", "d2h", "total"]
 COUNTER_NAMES = ["launches", "segments", "blocks", "events", "compressed_bytes", "output_bytes",
                  "record_bytes", "h2d_bytes", "d2h_bytes", "event_candidates"]
@@ -96,6 +98,9 @@ def lib():
     L.JPEGB200_batchCreateROI.restype = vp
     L.JPEGB200_batchCreateOriented.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8)]
     L.JPEGB200_batchCreateOriented.restype = vp
+    L.JPEGB200_batchCreateResized.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
+                                              i32p, C.c_int]
+    L.JPEGB200_batchCreateResized.restype = vp
     L.JPEGB200_batchOrientation.argtypes = [vp, C.c_int, i32p, i32p]
     L.JPEGB200_batchDestroy.argtypes = [vp]
     L.JPEGB200_batchDestroy.restype = None
@@ -122,6 +127,8 @@ def lib():
                                           C.POINTER(vp), C.POINTER(C.c_int64), C.c_int, i32p]
     L.JPEGB200_decodeBatchOriented.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
                                                C.POINTER(vp), C.POINTER(C.c_int64), C.c_int, i32p]
+    L.JPEGB200_decodeBatchResized.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
+                                              i32p, C.c_int, C.POINTER(vp), C.POINTER(C.c_int64), C.c_int, i32p]
     L.JPEGB200_lastCallCounters.argtypes = [vp, C.POINTER(C.c_int64)]
     L.JPEGB200_lastCallTimings.argtypes = [vp, C.POINTER(C.c_float), ip]
     L.JPEGB200_setPipelineDepth.argtypes = [vp, C.c_int]
@@ -316,22 +323,35 @@ def _orient_array(orients, n):
     return (C.c_uint8 * n)(*v)
 
 
+def _size_array(out_sizes, n):
+    """n (W, H) resize targets -> int32[2n] for the C ABI (None stays None = no resize)"""
+    if out_sizes is None:
+        return None
+    flat = [int(v) for s in out_sizes for v in s]
+    if len(flat) != 2 * n:
+        raise ValueError("out_sizes: one (W, H) per image")
+    return (C.c_int32 * (2 * n))(*flat)
+
+
 class Batch:
     """A decode job over n JPEG files that live in host memory at (ptr, size) pairs.  rois: one (x, y, w, h) rectangle
     in output pixels per image (JPEGB200_batchCreateROI), or None for whole images.  orients: one EXIF transform per
     image (ORIENT_FROM_EXIF = the file's tag, 1-8 = that transform; JPEGB200_batchCreateOriented), or None; rois are
-    then in the upright frame."""
+    then in the upright frame.  out_sizes: one (W, H) per image, each output then being Pillow's resize of that size
+    with `filter` (RESIZE_BILINEAR / _BICUBIC / _BOX) of the upright crop (JPEGB200_batchCreateResized), or None."""
 
-    def __init__(self, ctx, ptrs, sizes, pixel_type, options=0, rois=None, orients=None):
+    def __init__(self, ctx, ptrs, sizes, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
+                 filter=RESIZE_BILINEAR):
         n = len(ptrs)
         self.n = n
         self._ptrs = (C.c_void_p * n)(*ptrs)
         self._sizes = (C.c_int32 * n)(*sizes)
         self._rois = _roi_array(rois, n)
         self._orients = _orient_array(orients, n)
+        self._out_sizes = _size_array(out_sizes, n)
         self.ctx = ctx
-        self.h = lib().JPEGB200_batchCreateOriented(ctx.h, self._ptrs, self._sizes, n, pixel_type, options, self._rois,
-                                                    self._orients)
+        self.h = lib().JPEGB200_batchCreateResized(ctx.h, self._ptrs, self._sizes, n, pixel_type, options, self._rois,
+                                                   self._orients, self._out_sizes, int(filter))
         if not self.h:
             raise RuntimeError("batchCreate failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
 
@@ -403,30 +423,34 @@ class Batch:
             self.h = None
 
 
-def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flags=0, rois=None, orients=None):
-    """JPEGB200_decodeBatch(ROI / Oriented): one call for n files (host pointers) -> n outputs (host pointers, or device
-    pointers with JPEGB200_OUT_DEVICE); rois: one (x, y, w, h) per image or None; orients: one EXIF transform per image
-    (0 = from the file) or None.  Returns (rc, per-image status list, counters summed
-    over the internal jobs)."""
+def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flags=0, rois=None, orients=None,
+                 out_sizes=None, filter=RESIZE_BILINEAR):
+    """JPEGB200_decodeBatch(ROI / Oriented / Resized): one call for n files (host pointers) -> n outputs (host pointers,
+    or device pointers with JPEGB200_OUT_DEVICE); rois: one (x, y, w, h) per image or None; orients: one EXIF transform
+    per image (0 = from the file) or None; out_sizes: one (W, H) per image (resized with `filter`) or None.  Returns (rc,
+    per-image status list, counters summed over the internal jobs)."""
     n = len(ptrs)
     pa = (C.c_void_p * n)(*ptrs)
     sa = (C.c_int32 * n)(*sizes)
     oa = (C.c_void_p * n)(*outs)
     pi = (C.c_int64 * n)(*pitches) if pitches is not None else None
     st = (C.c_int32 * n)()
-    rc = lib().JPEGB200_decodeBatchOriented(ctx.h, pa, sa, n, pixel_type, options, _roi_array(rois, n),
-                                            _orient_array(orients, n), oa, pi, flags, st)
+    rc = lib().JPEGB200_decodeBatchResized(ctx.h, pa, sa, n, pixel_type, options, _roi_array(rois, n),
+                                           _orient_array(orients, n), _size_array(out_sizes, n), int(filter), oa, pi, flags, st)
     cnt = (C.c_int64 * len(COUNTER_NAMES))()
     lib().JPEGB200_lastCallCounters(ctx.h, cnt)
     return rc, list(st), dict(zip(COUNTER_NAMES, list(cnt)))
 
 
-def decode_batch_to_host(ctx, jpegs, pixel_type, options=0, rois=None, orients=None):
+def decode_batch_to_host(ctx, jpegs, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
+                         filter=RESIZE_BILINEAR):
     """Convenience: list of bytes -> list of numpy arrays [out_h, pitch_bytes] (uint8).
     One public-API call per batch with HOST buffers on both sides.  rois: one (x, y, w, h) per image (the arrays are then
-    h rows of w pixels), or None.  orients: one EXIF transform per image (0 = from the file), or None."""
+    h rows of w pixels), or None.  orients: one EXIF transform per image (0 = from the file), or None.  out_sizes: one
+    (W, H) per image (the arrays are then H rows of W pixels, resized with `filter`), or None."""
     bufs = [np.frombuffer(j, dtype=np.uint8) for j in jpegs]
-    b = Batch(ctx, [x.ctypes.data for x in bufs], [len(x) for x in bufs], pixel_type, options, rois, orients)
+    b = Batch(ctx, [x.ctypes.data for x in bufs], [len(x) for x in bufs], pixel_type, options, rois, orients, out_sizes,
+              filter)
     try:
         outs = []
         for i in range(b.n):

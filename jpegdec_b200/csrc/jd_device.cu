@@ -131,6 +131,18 @@ struct JPEGB200_BATCH {
     std::vector<int32_t> exif_tag;  /* per image: the file's EXIF Orientation tag (0 = none) */
     std::vector<uint8_t> orient;    /* per image: the transform applied, 1-8 (1 without orients) */
     uint32_t nseg_walk;             /* restart intervals the entropy stage walks (JPEGB200_C_SEGMENTS) */
+    /* resize (JPEGB200_batchCreateResized): descs hold the resized size; the IDCT stage writes S (the unresized output,
+     * rs_src_w x rs_src_h) into d_rs, the resize passes write the destination */
+    bool resize;
+    int rs_filter;
+    std::vector<JDResizePlan> rs_plans;
+    std::vector<uint32_t> rs_src_w, rs_src_h;
+    std::vector<int64_t> rs_scratch;    /* per image: S + intermediate bytes in d_rs (256-byte aligned each) */
+    int64_t rs_scratch_total;
+    std::vector<JDResizeDesc> rs_desc;
+    DevBuf<uint8_t> d_rs;
+    DevBuf<int32_t> d_rs_coef;
+    DevBuf<JDResizeDesc> d_rs_desc;
     cudaStream_t stream;
     std::vector<JDInfo> infos;
     std::vector<int32_t> parse_status;
@@ -464,7 +476,31 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateOriented(JPEGB200_CTX *ctx, const
                                                         int n, int pixel_type, int options, const int32_t *rois,
                                                         const uint8_t *orients)
 {
+    return JPEGB200_batchCreateResized(ctx, datas, sizes, n, pixel_type, options, rois, orients, nullptr, 0);
+}
+
+extern "C" JPEGB200_BATCH *JPEGB200_batchCreateResized(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes,
+                                                       int n, int pixel_type, int options, const int32_t *rois,
+                                                       const uint8_t *orients, const int32_t *out_sizes, int filter)
+{
     if (!ctx || n <= 0 || pixel_type < 0 || pixel_type >= INVALID_PIXEL_TYPE) { snprintf(g_err, sizeof(g_err), "invalid parameter"); return nullptr; }
+    if (out_sizes) {
+        /* resizing works on byte planes: RGB8888 (either byte order) and 8-bit gray, LUMA_ONLY folding included */
+        const int pt = ((options & JPEG_LUMA_ONLY) && pixel_type < EIGHT_BIT_GRAYSCALE) ? EIGHT_BIT_GRAYSCALE : pixel_type;
+        if (pt == RGB565_LITTLE_ENDIAN || pt == RGB565_BIG_ENDIAN) {
+            snprintf(g_err, sizeof(g_err), "resizing is not supported with RGB565 pixel types (a packed 5/6/5 word has no byte planes)");
+            return nullptr;
+        }
+        if (pt >= FOUR_BIT_DITHERED && pt <= ONE_BIT_DITHERED) {
+            snprintf(g_err, sizeof(g_err), "resizing is not supported with dithered pixel types");
+            return nullptr;
+        }
+        if (options & 0x10000) { snprintf(g_err, sizeof(g_err), "resizing is not supported with padded output"); return nullptr; }
+        if (!jd_rs_filter_ok(filter)) {
+            snprintf(g_err, sizeof(g_err), "resize filter %d is not supported (JPEGB200_RESIZE_BILINEAR 2, BICUBIC 3 or BOX 4)", filter);
+            return nullptr;
+        }
+    }
     if (rois && pixel_type >= FOUR_BIT_DITHERED && pixel_type <= ONE_BIT_DITHERED) {
         /* error diffusion runs across the whole image: a rectangle of the dithered image is not the dither of the rectangle */
         snprintf(g_err, sizeof(g_err), "regions of interest are not supported with dithered pixel types");
@@ -483,6 +519,13 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateOriented(JPEGB200_CTX *ctx, const
     if (b->roi) b->plans.assign(n, JDRoiPlan{});
     b->exif_tag.assign(n, 0);
     b->orient.assign(n, 1);
+    b->resize = out_sizes != nullptr;
+    b->rs_filter = filter;
+    b->rs_scratch_total = 0;
+    if (b->resize) {
+        b->rs_plans.assign(n, JDResizePlan{});
+        b->rs_src_w.assign(n, 0); b->rs_src_h.assign(n, 0); b->rs_scratch.assign(n, 0);
+    }
     b->ctx = ctx;
     b->n = n;
     b->index_base = 0;
@@ -576,6 +619,10 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateOriented(JPEGB200_CTX *ctx, const
             }
             srect[0] = rois[4 * (size_t)i]; srect[1] = rois[4 * (size_t)i + 1];
         }
+        if (ok && out_sizes) {
+            const int32_t rw = out_sizes[2 * (size_t)i], rh = out_sizes[2 * (size_t)i + 1];
+            if (rw < 1 || rw > 65535 || rh < 1 || rh > 65535) { ok = 0; st = JPEG_INVALID_PARAMETER; }
+        }
         b->parse_status[i] = st;
         if (!ok) { /* keep a harmless empty descriptor */
             d.nseg = 0; d.seg_base = seg; d.blk_base = (uint32_t)blk; d.status = (uint32_t)st;
@@ -643,6 +690,19 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateOriented(JPEGB200_CTX *ctx, const
             d.roi_mcu_end = (uint32_t)pl.mcu_end;
             d.orient = orients ? b->orient[i] : 0u;
         }
+        if (b->resize) {
+            /* S = what the same call without out_sizes stores; the descriptor carries the resized size from here on */
+            const int bp = bytes_per_pixel_class(b->ptclass);
+            JDResizePlan &rp = b->rs_plans[i];
+            const int32_t rw = out_sizes[2 * (size_t)i], rh = out_sizes[2 * (size_t)i + 1];
+            if (!jd_resize_plan((int)d.out_w, (int)d.out_h, rw, rh, filter, bp, &rp)) {
+                snprintf(g_err, sizeof(g_err), "resize plan failed for image %d", i); delete b; return nullptr;
+            }
+            b->rs_src_w[i] = d.out_w; b->rs_src_h[i] = d.out_h;
+            b->rs_scratch[i] = (int64_t)(((size_t)d.out_w * d.out_h * bp + 255) & ~(size_t)255) + ((rp.mid_bytes + 255) & ~(int64_t)255);
+            b->rs_scratch_total += b->rs_scratch[i];
+            d.out_w = (uint32_t)rw; d.out_h = (uint32_t)rh;
+        }
         size_t pitch;
         if (b->dither_bits) {
             const uint32_t pw = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> s);
@@ -700,6 +760,7 @@ extern "C" void JPEGB200_batchDestroy(JPEGB200_BATCH *b)
     b->d_work.release(); b->d_cta_lut.release(); b->d_seg_img.release(); b->d_seg_start.release();
     b->d_seg_jmap.release(); b->d_seg_status.release(); b->d_seg_nrec.release(); b->d_seg_phase.release();
     b->d_counters.release(); b->d_blk_hdr.release(); b->d_events.release();
+    b->d_rs.release(); b->d_rs_coef.release(); b->d_rs_desc.release();
     if (b->stream && b->have_ev) {   /* back to the context for the next job */
         JDStreamSet ss;
         ss.stream = b->stream;
@@ -1057,6 +1118,51 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         out_base = b->d_out.p;
         for (int i = 0; i < n; i++) descs_stage[i].out_off = b->arena_off[i];
     }
+    /* resize: the IDCT stage writes S tightly into d_rs; jdk_resize_v writes where the IDCT would have */
+    uint32_t rs_ctas[4] = {0u, 0u, 0u, 0u};
+    if (b->resize) {
+        const int bp = bytes_per_pixel_class(b->ptclass);
+        b->rs_desc.assign(n, JDResizeDesc{});
+        uint64_t so = 0, co = 0, ctas[4] = {0, 0, 0, 0};
+        for (int i = 0; i < n; i++) {
+            JDResizeDesc &r = b->rs_desc[i];
+            r.blk_c = (uint32_t)ctas[0]; r.blk_h = (uint32_t)ctas[1]; r.blk_v = (uint32_t)ctas[2]; r.blk_h2 = (uint32_t)ctas[3];
+            if (b->parse_status[i] != JPEG_SUCCESS) continue;
+            const JDResizePlan &rp = b->rs_plans[i];
+            r.src_w = b->rs_src_w[i]; r.src_h = b->rs_src_h[i]; r.dst_w = b->descs[i].out_w; r.dst_h = b->descs[i].out_h;
+            r.dst_off = descs_stage[i].out_off; r.dst_pitch = descs_stage[i].out_pitch;
+            r.ksize_h = (uint32_t)rp.ksize_h; r.ksize_v = (uint32_t)rp.ksize_v;
+            r.ybox0 = (uint32_t)rp.ybox0; r.rows = (uint32_t)rp.rows;
+            r.flags = (rp.need_h ? 1u : 0u) | (rp.need_v ? 2u : 0u) | (rp.vfirst ? 4u : 0u);
+            r.src_off = so;
+            so += ((uint64_t)r.src_w * r.src_h * bp + 255) & ~(uint64_t)255;
+            r.mid_off = so;
+            so += ((uint64_t)rp.mid_bytes + 255) & ~(uint64_t)255;
+            r.coef_h = co;
+            co += rp.need_h ? (uint64_t)r.dst_w * (r.ksize_h + 2) : 0;
+            r.coef_v = co;
+            co += rp.need_v ? (uint64_t)r.dst_h * (r.ksize_v + 2) : 0;
+            const uint64_t q = ((rp.vfirst ? r.src_w : r.dst_w) + 16 / bp - 1) / (16 / bp);
+            ctas[0] += ((rp.need_h ? r.dst_w : 0u) + (rp.need_v ? r.dst_h : 0u) + JD_RS_THREADS - 1) / JD_RS_THREADS;
+            if (rp.need_h && !rp.vfirst)   /* jdk_resize_h<4, 0>: one thread per pixel; <1, 0>: column chunks x row blocks */
+                ctas[1] += bp == 4 ? ((uint64_t)r.rows * r.dst_w + JD_RS_THREADS - 1) / JD_RS_THREADS
+                                   : (uint64_t)((r.dst_w + JD_RS_HCOLS - 1) / JD_RS_HCOLS) * ((r.rows + JD_RS_HROWS - 1) / JD_RS_HROWS);
+            ctas[2] += (q * r.dst_h + JD_RS_THREADS - 1) / JD_RS_THREADS;
+            ctas[3] += rp.vfirst ? ((uint64_t)r.dst_h * r.dst_w + JD_RS_THREADS - 1) / JD_RS_THREADS : 0;
+            descs_stage[i].out_off = r.src_off;
+            descs_stage[i].out_pitch = r.src_w * (uint32_t)bp;
+            descs_stage[i].out_w = r.src_w; descs_stage[i].out_h = r.src_h;
+        }
+        if (ctas[1] >= (1ull << 31) || ctas[2] >= (1ull << 31) || ctas[3] >= (1ull << 31)) {
+            snprintf(g_err, sizeof(g_err), "resize: too many output pixels in one job");
+            return 0;
+        }
+        for (int c = 0; c < 4; c++) rs_ctas[c] = (uint32_t)ctas[c];
+        CK(b->d_rs.alloc(&b->ctx->pool, so + 256));
+        CK(b->d_rs_coef.alloc(&b->ctx->pool, co + 64));
+        CK(b->d_rs_desc.alloc(&b->ctx->pool, n));
+        CK(cudaMemcpyAsync(b->d_rs_desc.p, b->rs_desc.data(), sizeof(JDResizeDesc) * n, cudaMemcpyHostToDevice, st));
+    }
     /* dither: the IDCT stage writes an MCU-aligned 8-bit image first */
     std::vector<uint64_t> gray_off;
     std::vector<uint32_t> err_off;
@@ -1226,7 +1332,7 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
     CK(cudaEventRecord(b->ev[5], st));
     /* IDCT + colour: one launch per run of images with the same geometry class */
     const bool half = b->sshift == 1;
-    uint8_t *stage_out = b->dither_bits ? b->d_gray.p : out_base;
+    uint8_t *stage_out = b->dither_bits ? b->d_gray.p : b->resize ? b->d_rs.p : out_base;
     for (int i0 = 0; i0 < n;) {
         if (b->parse_status[i0] != JPEG_SUCCESS) { i0++; continue; }
         const JDInfo &f = b->infos[i0];
@@ -1324,6 +1430,28 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
 #undef JD_DITHER_ARGS
             launches++;
         }
+    }
+    if (b->resize) {
+        /* timed in the dither slot (the pixel pass after the IDCT): the two never occur together */
+        const bool gray = b->ptclass == JD_PT_GRAY;
+        if (rs_ctas[0]) { jdk_resize_coeffs<<<rs_ctas[0], JD_RS_THREADS, 0, st>>>(b->d_rs_desc.p, (uint32_t)n, b->d_rs_coef.p, b->rs_filter); launches++; }
+#define JD_RS_ARGS b->d_rs_desc.p, (uint32_t)n, b->d_rs.p, b->d_rs_coef.p, out_base
+        if (rs_ctas[1]) {
+            if (gray) jdk_resize_h<1, 0><<<rs_ctas[1], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
+            else jdk_resize_h<4, 0><<<rs_ctas[1], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
+            launches++;
+        }
+        if (rs_ctas[2]) {
+            if (gray) jdk_resize_v<1><<<rs_ctas[2], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
+            else jdk_resize_v<4><<<rs_ctas[2], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
+            launches++;
+        }
+        if (rs_ctas[3]) {   /* images whose vertical pass ran first (JDResizePlan.vfirst) */
+            if (gray) jdk_resize_h<1, 1><<<rs_ctas[3], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
+            else jdk_resize_h<4, 1><<<rs_ctas[3], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
+            launches++;
+        }
+#undef JD_RS_ARGS
     }
     CK(cudaEventRecord(b->ev[7], st));
     CK(cudaGetLastError());
@@ -1473,6 +1601,7 @@ extern "C" int JPEGB200_batchGetCounters(JPEGB200_BATCH *b, int64_t *counters)
 #define JD_JOB_COMP_BYTES ((int64_t)192 << 20)
 #define JD_JOB_MAX_IMAGES 4096
 #define JD_PIPE_INFLIGHT_DEVICE 3
+#define JD_JOB_RESIZE_SCRATCH ((int64_t)1 << 30)
 extern "C" int JPEGB200_decodeBatch(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
                                     int pixel_type, int options, void *const *outs, const int64_t *pitches,
                                     int flags, int32_t *status)
@@ -1490,6 +1619,14 @@ extern "C" int JPEGB200_decodeBatchROI(JPEGB200_CTX *ctx, const uint8_t *const *
 extern "C" int JPEGB200_decodeBatchOriented(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
                                             int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
                                             void *const *outs, const int64_t *pitches, int flags, int32_t *status)
+{
+    return JPEGB200_decodeBatchResized(ctx, datas, sizes, n, pixel_type, options, rois, orients, nullptr, 0, outs, pitches, flags, status);
+}
+
+extern "C" int JPEGB200_decodeBatchResized(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                           int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
+                                           const int32_t *out_sizes, int filter, void *const *outs, const int64_t *pitches,
+                                           int flags, int32_t *status)
 {
     if (!ctx || n <= 0) return 0;
     const bool dev_out = (flags & JPEGB200_OUT_DEVICE) != 0;
@@ -1534,8 +1671,11 @@ extern "C" int JPEGB200_decodeBatchOriented(JPEGB200_CTX *ctx, const uint8_t *co
             if (cnt > 0 && cb + sz > limit) break;
             cb += sz; cnt++;
         }
-        JPEGB200_BATCH *b = JPEGB200_batchCreateOriented(ctx, datas + i0, sizes + i0, cnt, pixel_type, options, rois ? rois + 4 * (size_t)i0 : nullptr,
-                                               orients ? orients + i0 : nullptr);
+        auto create = [&](int c) {
+            return JPEGB200_batchCreateResized(ctx, datas + i0, sizes + i0, c, pixel_type, options, rois ? rois + 4 * (size_t)i0 : nullptr,
+                                               orients ? orients + i0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)i0 : nullptr, filter);
+        };
+        JPEGB200_BATCH *b = create(cnt);
         if (!b) { rc = 0; break; }
         if (!dev_out && i0 + cnt < n && cnt == JD_PIPE_IMAGES) {
             int64_t ob = 0;
@@ -1551,11 +1691,20 @@ extern "C" int JPEGB200_decodeBatchOriented(JPEGB200_CTX *ctx, const uint8_t *co
                 if (cnt2 > cnt) {
                     JPEGB200_batchDestroy(b);
                     cnt = cnt2;
-                    b = JPEGB200_batchCreateOriented(ctx, datas + i0, sizes + i0, cnt, pixel_type, options, rois ? rois + 4 * (size_t)i0 : nullptr,
-                                               orients ? orients + i0 : nullptr);
+                    b = create(cnt);
                     if (!b) { rc = 0; break; }
                 }
             }
+        }
+        if (b->resize && cnt > 1 && b->rs_scratch_total > JD_JOB_RESIZE_SCRATCH) {
+            /* resize scratch (S + intermediate) of a job: at most JD_JOB_RESIZE_SCRATCH, or one image */
+            int c = 0;
+            int64_t sb = 0;
+            while (c < cnt && (c == 0 || sb + b->rs_scratch[c] <= JD_JOB_RESIZE_SCRATCH)) sb += b->rs_scratch[c++];
+            JPEGB200_batchDestroy(b);
+            cnt = c;
+            b = create(cnt);
+            if (!b) { rc = 0; break; }
         }
         jobs.push_back(b); first.push_back(i0);
         b->index_base = i0;

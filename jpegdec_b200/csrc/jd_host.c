@@ -11,6 +11,7 @@
 #include <string.h>
 #include <stdlib.h>
 #include "jd_internal.h"
+#include "jd_resize.h"
 
 #define HUFF_TABLEN 273 /* reference src/JPEGDEC.h:58: stride of one DHT table in the scratch area */
 
@@ -490,6 +491,28 @@ int jd_orient_plan(int width, int height, int subsample, int restart_interval, i
     if (!jd_roi_plan(width, height, subsample, restart_interval, sshift, srect, plan)) return 0;
     plan->out_w = (int32_t)w;
     plan->out_h = (int32_t)h;
+    return 1;
+}
+
+/* Resize plan (JDResizePlan): ImagingResampleInner's pass choice and row box, without computing the coefficients */
+int jd_resize_plan(int src_w, int src_h, int out_w, int out_h, int filter, int bytes_per_pixel, JDResizePlan *plan)
+{
+    if (!jd_rs_filter_ok(filter) || src_w < 1 || src_h < 1 || src_w > 65535 || src_h > 65535 ||
+        out_w < 1 || out_h < 1 || out_w > 65535 || out_h > 65535) return 0;
+    plan->need_h = out_w != src_w;
+    plan->need_v = out_h != src_h;
+    plan->ksize_h = jd_rs_ksize(src_w, out_w, filter);
+    plan->ksize_v = jd_rs_ksize(src_h, out_h, filter);
+    int32_t y0, n0, y1, n1;
+    jd_rs_bounds(src_h, out_h, filter, 0, &y0, &n0);
+    jd_rs_bounds(src_h, out_h, filter, out_h - 1, &y1, &n1);
+    plan->ybox0 = plan->need_v ? y0 : 0;
+    plan->rows = plan->need_v ? y1 + n1 - y0 : src_h;
+    plan->vfirst = plan->need_h && plan->need_v && out_h < src_h && src_h > 100 * src_w;
+    if (plan->vfirst) plan->mid_bytes = (int64_t)out_h * src_w * bytes_per_pixel;
+    else plan->mid_bytes = plan->need_h ? (int64_t)plan->rows * out_w * bytes_per_pixel : 0;
+    plan->coef_words = (plan->need_h ? (int64_t)out_w * (plan->ksize_h + 2) : 0) +
+                       (plan->need_v ? (int64_t)out_h * (plan->ksize_v + 2) : 0);
     return 1;
 }
 

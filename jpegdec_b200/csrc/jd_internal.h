@@ -104,6 +104,23 @@ int jd_roi_plan(int width, int height, int subsample, int restart_interval, int 
 int jd_orient_plan(int width, int height, int subsample, int restart_interval, int sshift, int k, const int32_t *rect,
                    int32_t *srect /* x, y, w, h */, JDRoiPlan *plan);
 
+/* Resize of one image (JPEGB200_batchCreateResized) from the unresized output S (src_w x src_h) to out_w x out_h: the O(1)
+ * facts that size its scratch; the coefficients themselves are computed on the GPU (jd_resize.h, jdk_resize_coeffs).
+ * A pass runs only along an axis whose size changes (Pillow skips the other).  The horizontal pass reads source rows
+ * ybox0 .. ybox0 + rows - 1 (those the vertical pass's first and last output rows reach) and writes rows x out_w pixels.
+ * Pillow 12 runs the vertical pass first for a tall source that shrinks vertically (src_h > 100 src_w, out_h < src_h,
+ * both passes needed); the intermediate is then out_h x src_w pixels.  The order changes the rounding, so it is kept. */
+typedef struct {
+    int32_t need_h, need_v;
+    int32_t vfirst;             /* vertical pass first */
+    int32_t ksize_h, ksize_v;   /* coefficient table strides (taps of the widest output column / row) */
+    int32_t ybox0, rows;        /* source rows of the horizontal pass (all src_h rows when the height does not change) */
+    int64_t mid_bytes;          /* intermediate: rows x out_w x bytes per pixel (0 without a horizontal pass) */
+    int64_t coef_words;         /* int32 table words: out_w x (ksize_h + 2) and out_h x (ksize_v + 2) for the passes that run */
+} JDResizePlan;
+/* Returns 0 for a filter other than JPEGB200_RESIZE_* or a size outside 1..65535. */
+int jd_resize_plan(int src_w, int src_h, int out_w, int out_h, int filter, int bytes_per_pixel, JDResizePlan *plan);
+
 /* A caller's destination for image `index` (only named in the message): row_bytes is the tight pitch
  * (JPEGB200_batchOutputBytes), pitch <= 0 means tight.  device != 0: `out` is written by the kernels.  Returns 1, or 0 with
  * a message in msg[msg_len] (see JPEGB200_batchSetOutput / JPEGB200_decodeBatch for the rules). */
