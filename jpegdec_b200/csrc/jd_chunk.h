@@ -45,9 +45,9 @@ struct JDBitWin {
     int nb;
     JD_HDM void seek(const JDScanIn &sc, uint32_t rel)                 /* rel = bit position relative to the scan start */
     {
-        const uint32_t ap = sc.f0 * 8u + rel;
+        const jd_u64 ap = (jd_u64)sc.f0 * 8u + rel;   /* 64-bit: a scan may start 512 MiB or more into the batch */
         wp = (const uint32_t *)sc.filt + (ap >> 5);
-        const uint32_t sft = ap & 31u;
+        const uint32_t sft = (uint32_t)ap & 31u;
         bb = (jd_u64)jd_bswap32(*wp++) << (32u + sft);
         nb = 32 - (int)sft;
     }

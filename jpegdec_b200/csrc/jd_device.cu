@@ -460,6 +460,19 @@ extern "C" int JPEGB200_sharedTableHits(JPEGB200_CTX *ctx) { return ctx ? ctx->s
 /* ---- batch ---- */
 static int bytes_per_pixel_class(int ptclass) { return ptclass == JD_PT_565 ? 2 : (ptclass == JD_PT_8888 ? 4 : 1); }
 
+extern "C" uint64_t jd_rec_extent(uint64_t size, uint32_t scan_offset, uint32_t nseg, uint32_t nch)
+{
+    /* restart segment s: JD_REC_INDEX(start, s) + JD_REC_CAP(end - start) <= 6 end + 128 s + 120, and end <= size */
+    uint64_t e = (uint64_t)JD_REC_PER_BYTE * size + (uint64_t)JD_REC_SLOT_SLACK * (nseg ? nseg - 1u : 0u) + JD_REC_SLOT_SLACK - 8u;
+    if (nch) {   /* the last chunk, c = nch - 1 at slot nseg + c: its start is past the data, but its capacity counts */
+        const uint64_t off = (uint64_t)scan_offset + (uint64_t)JD_CHUNK_BYTES * (nch - 1u);
+        const uint64_t c = ((JD_REC_PER_BYTE * off) & ~(uint64_t)7) + (uint64_t)JD_REC_SLOT_SLACK * (nseg + nch - 1u) +
+                           JD_REC_PER_BYTE * JD_CHUNK_BYTES + JD_REC_SLOT_SLACK - 8u;
+        if (c > e) e = c;
+    }
+    return e;
+}
+
 extern "C" JPEGB200_BATCH *JPEGB200_batchCreate(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes,
                                                 int n, int pixel_type, int options)
 {
@@ -623,6 +636,15 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateResized(JPEGB200_CTX *ctx, const 
             const int32_t rw = out_sizes[2 * (size_t)i], rh = out_sizes[2 * (size_t)i + 1];
             if (rw < 1 || rw > 65535 || rh < 1 || rh > 65535) { ok = 0; st = JPEG_INVALID_PARAMETER; }
         }
+        const uint32_t total_mcus = ok ? (uint32_t)inf.mcus_x * inf.mcus_y : 0u;
+        const uint32_t mps = inf.restart_interval ? (uint32_t)inf.restart_interval : total_mcus;
+        const uint32_t nseg = ok ? (total_mcus + mps - 1) / mps : 0u;
+        /* no restart markers: one long dependent stream -> chunk-parallel decode */
+        const uint32_t nch = (ok && !prog && inf.restart_interval == 0 && nseg == 1 && sizes[i] - inf.scan_offset >= 4096)
+                                 ? ((uint32_t)(sizes[i] - inf.scan_offset) + JD_CHUNK_BYTES - 1) / JD_CHUNK_BYTES + 1 : 0u;
+        if (ok && jd_rec_extent((uint64_t)sizes[i], (uint32_t)inf.scan_offset, nseg, nch) > (1ull << 32)) {
+            ok = 0; st = JPEG_UNSUPPORTED_FEATURE;   /* its record indices would wrap onto its own first records */
+        }
         b->parse_status[i] = st;
         if (!ok) { /* keep a harmless empty descriptor */
             d.nseg = 0; d.seg_base = seg; d.blk_base = (uint32_t)blk; d.status = (uint32_t)st;
@@ -647,22 +669,19 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateResized(JPEGB200_CTX *ctx, const 
             else jd_build_lut(&inf, &b->luts[(size_t)li * JD_LUT_ENTRIES]);
         }
         if (shared) ctx->shared_hits++;
-        const uint32_t total_mcus = (uint32_t)inf.mcus_x * inf.mcus_y;
-        const uint32_t mps = inf.restart_interval ? (uint32_t)inf.restart_interval : total_mcus;
         d.scan_off = (uint32_t)(b->comp_off[i] + inf.scan_offset);
         d.scan_end = (uint32_t)(b->comp_off[i] + sizes[i]);
         d.width = (uint16_t)inf.width; d.height = (uint16_t)inf.height;
         d.mcus_x = (uint16_t)inf.mcus_x; d.mcus_y = (uint16_t)inf.mcus_y;
         d.subsample = (uint8_t)inf.subsample; d.ncomp = (uint8_t)inf.ncomp; d.bpm = (uint8_t)inf.bpm; d.tsel = (uint8_t)inf.tsel;
         d.mcus_per_seg = mps;
-        d.nseg = (total_mcus + mps - 1) / mps;
+        d.nseg = nseg;
         d.nseg_walk = b->roi ? (uint32_t)b->plans[i].nseg_walk : d.nseg;
         d.chunk_base = 0; d.nch = 0;
         d.prog = prog ? (1u | ((uint32_t)(inf.approx & 15) << 8)) : 0u;
-        if (!prog && inf.restart_interval == 0 && d.nseg == 1 && sizes[i] - inf.scan_offset >= 4096) {
-            /* no restart markers: one long dependent stream -> chunk-parallel decode */
+        if (nch) {
             d.chunk_base = b->nchunks;
-            d.nch = ((uint32_t)(sizes[i] - inf.scan_offset) + JD_CHUNK_BYTES - 1) / JD_CHUNK_BYTES + 1;
+            d.nch = nch;
             b->nchunks += d.nch;
             if (d.nch > b->max_nch) b->max_nch = d.nch;
             b->cimg_list.push_back((uint32_t)i);

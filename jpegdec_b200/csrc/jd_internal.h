@@ -121,6 +121,14 @@ typedef struct {
 /* Returns 0 for a filter other than JPEGB200_RESIZE_* or a size outside 1..65535. */
 int jd_resize_plan(int src_w, int src_h, int out_w, int out_h, int filter, int bytes_per_pixel, JDResizePlan *plan);
 
+/* Coefficient records an image's entropy walks can address above its record base: the largest JD_REC_INDEX + JD_REC_CAP
+ * (jd_core.h) over its restart segments (slots 0 .. nseg - 1, each ending at or before the file's end) and the chunks of a
+ * restart-free scan (slots nseg .. nseg + nch - 1, 512 bytes each from scan_offset), computed in 64 bits.  Those indices
+ * are 32-bit: JPEGB200_batchCreate refuses an image whose extent passes 2^32, whose last slots would otherwise overwrite
+ * the records of its first ones.  Files under 512 MiB reach it only through the 128 spare records per restart interval.
+ * (jd_device.cu; declared here so that the CPU tests can call it.) */
+uint64_t jd_rec_extent(uint64_t size, uint32_t scan_offset, uint32_t nseg, uint32_t nch);
+
 /* A caller's destination for image `index` (only named in the message): row_bytes is the tight pitch
  * (JPEGB200_batchOutputBytes), pitch <= 0 means tight.  device != 0: `out` is written by the kernels.  Returns 1, or 0 with
  * a message in msg[msg_len] (see JPEGB200_batchSetOutput / JPEGB200_decodeBatch for the rules). */
