@@ -18,6 +18,7 @@
  *   jdk_idct_tb, jdk_idct_color <- JPEGIDCT + DC-only shortcut (:5146-5154) + JPEGPutMCU22/11/12/21/Gray/8BitGray
  *   jdk_scaled         <- the 1/4 and 1/8 paths of the above (:2305-2326, :3323-3396, :3627-3748)
  *   jdk_dither         <- JPEGDither (:4871-4940)
+ *   jdk_resize_*, jdk_tensor <- no reference counterpart: Pillow's resize and torchvision's to_tensor / Normalize
  */
 #ifndef JPEGDEC_B200_H
 #define JPEGDEC_B200_H
@@ -42,7 +43,8 @@ enum {
     JPEGB200_T_ENTROPY,
     JPEGB200_T_STITCH,
     JPEGB200_T_IDCT,
-    JPEGB200_T_DITHER,         /* the pixel pass after the IDCT: dither, or resize (the two never occur together) */
+    JPEGB200_T_DITHER,         /* the pixel passes after the IDCT: dither, or resize and tensor conversion (dither never
+                                  occurs with either) */
     JPEGB200_T_D2H,
     JPEGB200_T_TOTAL,
     JPEGB200_NUM_TIMINGS
@@ -165,6 +167,56 @@ JPEGB200_BATCH *JPEGB200_batchCreateOriented(JPEGB200_CTX *ctx, const uint8_t *c
 JPEGB200_BATCH *JPEGB200_batchCreateResized(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
                                             int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
                                             const int32_t *out_sizes /* n x {W, H}; NULL = no resize */, int filter);
+/* Tensor output (a model's input tensor, straight from the decode).  U_i = what JPEGB200_batchCreateResized stores for image
+ * i with the same rois / orients / out_sizes / filter (crop, orient, resize, every scale, EXIF thumbnail, progressive at
+ * 1/8), W x H pixels.  Image i's output is a tensor of C x H x W elements (CHW) or H x W x C (HWC):
+ *   - C = 3 for RGB8888: output channel 0 is true red (blue with spec->bgr), 1 green, 2 blue (red with bgr); the library
+ *     applies U_i's own byte order (B,G,R,A with the SSE2-build arithmetic at full scale for 4:2:0 and 4:4:4 files, R,G,B,A
+ *     otherwise, decided per image), and the alpha byte is dropped.  C = 1 for EIGHT_BIT_GRAYSCALE and LUMA_ONLY folding;
+ *     only mean[0] and std[0] are used then.
+ *   - Element for byte value x of output channel c: s = (float)x (SCALE_NONE), (float)x / 255.0f (SCALE_DIV255: torchvision
+ *     to_tensor) or (float)x * (float)(1.0 / 255) (SCALE_MUL255: torchvision v2 ToDtype(float32, scale=True)); then
+ *     y = (s - mean[c]) / std[c], each operation one IEEE float32 rounding (torchvision's Normalize), then round to
+ *     nearest even to the dtype (torch's .half() / .bfloat16()).  Bit for bit: the host computes the C x 256 values once per
+ *     batch and the kernel only looks them up.  JPEGB200_DT_U8 is a layout conversion: it needs SCALE_NONE, mean 0, std 1.
+ *   - Returns NULL with a message for RGB565, dithered types, padded output, an unknown dtype / layout / scale, a std that
+ *     is 0 or not finite or a mean that is not finite (over the C channels used), and U8 with any normalization.
+ *   - Destinations are device memory only (JPEGB200_batchSetOutputTensor + JPEGB200_batchDecode with JPEGB200_OUT_DEVICE, or
+ *     the device arena): batchDecode without JPEGB200_OUT_DEVICE, or a destination that is not device memory of the
+ *     context's GPU, fails with a message.  Element (c, y, x) of CHW lies at out + c * plane_stride + y * pitch + x * elt,
+ *     element (y, x, c) of HWC at out + y * pitch + (x * C + c) * elt.  Only the tensor's elements are written: not the
+ *     pitch padding, not the bytes between planes, not the slot of a rejected image.
+ *   - JPEGB200_batchImageInfo reports out_w, out_h = W, H.  JPEGB200_batchOutputBytes = C * H * W * elt with pitch_bytes =
+ *     the row bytes (W * elt for CHW, W * C * elt for HWC); the device arena (each tensor tight, 256-byte aligned),
+ *     JPEGB200_batchGetDeviceOutput, JPEGB200_batchReadOutput and JPEGB200_C_OUTPUT_BYTES follow from that.
+ *   - Status, JPEGB200_batchErrMcu and the restart intervals walked are those of the same call without spec.
+ *   - Device work: the pipeline writes U_i into pooled uint8 staging instead of the destination (the IDCT stage, or the
+ *     resize's last pass), then one jdk_tensor launch converts every image; timed in the JPEGB200_T_DITHER slot with the
+ *     resize.  One launch more than the same call without spec.
+ * spec = NULL is JPEGB200_batchCreateResized. */
+#define JPEGB200_DT_U8   0
+#define JPEGB200_DT_F32  1
+#define JPEGB200_DT_F16  2
+#define JPEGB200_DT_BF16 3
+#define JPEGB200_LAYOUT_CHW 0          /* planar: plane c at out + c * plane_stride, row y at + y * pitch */
+#define JPEGB200_LAYOUT_HWC 1          /* interleaved (torch channels_last): pixel x of row y at out + y * pitch + x * C * elt */
+#define JPEGB200_SCALE_NONE   0        /* s = (float)x */
+#define JPEGB200_SCALE_DIV255 1        /* s = (float)x / 255.0f             (torchvision to_tensor) */
+#define JPEGB200_SCALE_MUL255 2        /* s = (float)x * (float)(1.0 / 255)  (torchvision v2 ToDtype(float32, scale=True)) */
+typedef struct {
+    int32_t dtype, layout, scale, bgr; /* bgr != 0: output channel 0 is blue */
+    float mean[3], std[3];             /* per OUTPUT channel: y = (s - mean[c]) / std[c], each step one IEEE float32
+                                          rounding, then round-to-nearest-even to dtype (torch's .half() / .bfloat16()) */
+} JPEGB200_TensorSpec;
+JPEGB200_BATCH *JPEGB200_batchCreateTensor(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                           int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
+                                           const int32_t *out_sizes, int filter, const JPEGB200_TensorSpec *spec);
+/* Destination of image i of a tensor batch (device memory).  pitch: bytes between rows, <= 0 = tight (the row bytes);
+ * plane_stride: bytes between the planes of CHW, 0 = pitch * H, ignored for HWC.  Pointer, pitch and plane stride must be
+ * multiples of the element size; the pitch must be at least the row bytes and below 2^32, a plane stride at least
+ * pitch * H.  Returns 0 with a message, and nothing changed, otherwise.  JPEGB200_batchSetOutput(b, i, out, pitch) on a
+ * tensor batch is this call with plane_stride 0. */
+int JPEGB200_batchSetOutputTensor(JPEGB200_BATCH *b, int i, void *out, int64_t pitch, int64_t plane_stride);
 void JPEGB200_batchDestroy(JPEGB200_BATCH *b);
 int JPEGB200_batchCount(JPEGB200_BATCH *b);
 /* per-image facts after batchCreate: status is JPEG_SUCCESS or the open() error the reference would give */
@@ -232,6 +284,14 @@ int JPEGB200_decodeBatchResized(JPEGB200_CTX *ctx, const uint8_t *const *datas, 
                                 int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
                                 const int32_t *out_sizes, int filter, void *const *outs, const int64_t *pitches,
                                 int flags, int32_t *status);
+/* The same into tensors (spec: semantics of JPEGB200_batchCreateTensor; NULL = JPEGB200_decodeBatchResized).  With spec,
+ * flags must hold JPEGB200_OUT_DEVICE and outs[i] are device tensors with pitches[i] (NULL or <= 0 = tight) and
+ * plane_strides[i] (NULL or 0 = pitch * H) under the rules of JPEGB200_batchSetOutputTensor.  The 1 GiB of scratch per
+ * job counts the uint8 staging of the tensors too. */
+int JPEGB200_decodeBatchTensor(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                               int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
+                               const int32_t *out_sizes, int filter, const JPEGB200_TensorSpec *spec, void *const *outs,
+                               const int64_t *pitches, const int64_t *plane_strides, int flags, int32_t *status);
 /* JPEGB200_NUM_COUNTERS counters summed over the jobs of the last JPEGB200_decodeBatch on this context */
 int JPEGB200_lastCallCounters(JPEGB200_CTX *ctx, int64_t *counters);
 /* CUDA-event stage times (JPEGB200_NUM_TIMINGS, ms) summed over those jobs, and how many jobs there were.  Jobs overlap

@@ -29,10 +29,20 @@ JPEGB200_OUT_DEVICE = 1
 ORIENT_FROM_EXIF = 0   # orients[i]: use the file's EXIF Orientation tag (1-8 force that EXIF transform)
 # resize filters: PIL.Image.Resampling's numbers, so Pillow's constants can be passed as they are
 RESIZE_BILINEAR, RESIZE_BICUBIC, RESIZE_BOX = 2, 3, 4
+# tensor output (JPEGB200_TensorSpec)
+DT_U8, DT_F32, DT_F16, DT_BF16 = 0, 1, 2, 3
+LAYOUT_CHW, LAYOUT_HWC = 0, 1
+SCALE_NONE, SCALE_DIV255, SCALE_MUL255 = 0, 1, 2
 TIMING_NAMES = ["h2d", "prescan", "entropy", "stitch", "idct", "dither", "d2h", "total"]
 COUNTER_NAMES = ["launches", "segments", "blocks", "events", "compressed_bytes", "output_bytes",
                  "record_bytes", "h2d_bytes", "d2h_bytes", "event_candidates"]
 TABLE_BLOB_BYTES = 10496 * 2 + 3 * 64 * 2 + 16
+
+
+class TensorSpec(C.Structure):
+    """JPEGB200_TensorSpec (include/jpegdec_b200.h)"""
+    _fields_ = [("dtype", C.c_int32), ("layout", C.c_int32), ("scale", C.c_int32), ("bgr", C.c_int32),
+                ("mean", C.c_float * 3), ("std", C.c_float * 3)]
 
 
 class JPEGDRAW(C.Structure):
@@ -101,6 +111,14 @@ def lib():
     L.JPEGB200_batchCreateResized.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
                                               i32p, C.c_int]
     L.JPEGB200_batchCreateResized.restype = vp
+    L.JPEGB200_batchCreateTensor.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
+                                             i32p, C.c_int, C.POINTER(TensorSpec)]
+    L.JPEGB200_batchCreateTensor.restype = vp
+    L.JPEGB200_batchSetOutputTensor.argtypes = [vp, C.c_int, vp, C.c_int64, C.c_int64]
+    L.JPEGB200_decodeBatchTensor.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
+                                             i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(vp), C.POINTER(C.c_int64),
+                                             C.POINTER(C.c_int64), C.c_int, i32p]
+    L.JPEGB200_currentDevice.restype = C.c_int
     L.JPEGB200_batchOrientation.argtypes = [vp, C.c_int, i32p, i32p]
     L.JPEGB200_batchDestroy.argtypes = [vp]
     L.JPEGB200_batchDestroy.restype = None
@@ -226,6 +244,7 @@ class Context:
         self.h = lib().JPEGB200_create(device, arith)
         if not self.h:
             raise RuntimeError("JPEGB200_create failed: " + lib().JPEGB200_lastErrorString(None).decode())
+        self.device = device if device >= 0 else lib().JPEGB200_currentDevice()   # the CUDA device the context decodes on
 
     def close(self):
         if self.h:
@@ -341,7 +360,7 @@ class Batch:
     with `filter` (RESIZE_BILINEAR / _BICUBIC / _BOX) of the upright crop (JPEGB200_batchCreateResized), or None."""
 
     def __init__(self, ctx, ptrs, sizes, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
-                 filter=RESIZE_BILINEAR):
+                 filter=RESIZE_BILINEAR, spec=None):
         n = len(ptrs)
         self.n = n
         self._ptrs = (C.c_void_p * n)(*ptrs)
@@ -350,8 +369,13 @@ class Batch:
         self._orients = _orient_array(orients, n)
         self._out_sizes = _size_array(out_sizes, n)
         self.ctx = ctx
-        self.h = lib().JPEGB200_batchCreateResized(ctx.h, self._ptrs, self._sizes, n, pixel_type, options, self._rois,
-                                                   self._orients, self._out_sizes, int(filter))
+        if spec is None:
+            self.h = lib().JPEGB200_batchCreateResized(ctx.h, self._ptrs, self._sizes, n, pixel_type, options, self._rois,
+                                                       self._orients, self._out_sizes, int(filter))
+        else:   # a TensorSpec: JPEGB200_batchCreateTensor (device outputs only)
+            self._spec = spec
+            self.h = lib().JPEGB200_batchCreateTensor(ctx.h, self._ptrs, self._sizes, n, pixel_type, options, self._rois,
+                                                      self._orients, self._out_sizes, int(filter), C.byref(spec))
         if not self.h:
             raise RuntimeError("batchCreate failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
 
@@ -373,6 +397,10 @@ class Batch:
     def set_output(self, i, ptr, pitch=0):
         """pitch 0 = tight; a pitch below the row bytes or above 2^32 - 1 raises (the image keeps its destination)"""
         self._ck(lib().JPEGB200_batchSetOutput(self.h, i, ptr, pitch), "batchSetOutput")
+
+    def set_output_tensor(self, i, ptr, pitch=0, plane_stride=0):
+        """tensor batches: device destination of image i (JPEGB200_batchSetOutputTensor)"""
+        self._ck(lib().JPEGB200_batchSetOutputTensor(self.h, i, ptr, pitch, plane_stride), "batchSetOutputTensor")
 
     def alloc_device_output(self):
         self._ck(lib().JPEGB200_batchAllocDeviceOutput(self.h), "batchAllocDeviceOutput")
@@ -467,3 +495,104 @@ def decode_batch_to_host(ctx, jpegs, pixel_type, options=0, rois=None, orients=N
         return outs, status, b.timings(), b.counters()
     finally:
         b.close()
+
+
+_SCALES = {"none": SCALE_NONE, "div255": SCALE_DIV255, "mul255": SCALE_MUL255}
+_LAYOUTS = {"CHW": LAYOUT_CHW, "HWC": LAYOUT_HWC}
+
+
+def _torch_dtype_code(dtype):
+    import torch
+    codes = {torch.uint8: DT_U8, torch.float32: DT_F32, torch.float16: DT_F16, torch.bfloat16: DT_BF16}
+    if dtype not in codes:
+        raise ValueError("dtype: torch.float32, float16, bfloat16 or uint8")
+    return codes[dtype]
+
+
+def tensor_spec(dtype, layout="CHW", scale="div255", mean=(0.0, 0.0, 0.0), std=(1.0, 1.0, 1.0), bgr=False):
+    """A TensorSpec from torch-style arguments (dtype: a torch dtype; layout "CHW" / "HWC"; scale "none", "div255"
+    (torchvision to_tensor) or "mul255" (v2 ToDtype(float32, scale=True)); mean / std: 1 or 3 values)."""
+    if layout not in _LAYOUTS:
+        raise ValueError("layout: 'CHW' or 'HWC'")
+    if scale not in _SCALES:
+        raise ValueError("scale: 'none', 'div255' or 'mul255'")
+    mean, std = [float(v) for v in mean], [float(v) for v in std]
+    if len(mean) not in (1, 3) or len(std) not in (1, 3):
+        raise ValueError("mean / std: 1 or 3 values")
+    mean, std = (mean * 3)[:3], (std * 3)[:3]
+    return TensorSpec(_torch_dtype_code(dtype), _LAYOUTS[layout], _SCALES[scale], 1 if bgr else 0,
+                      (C.c_float * 3)(*mean), (C.c_float * 3)(*std))
+
+
+def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, orients=None, out_sizes=None,
+                        filter=RESIZE_BILINEAR, dtype=None, layout="CHW", scale="div255", mean=(0.0, 0.0, 0.0),
+                        std=(1.0, 1.0, 1.0), bgr=False, out=None):
+    """JPEGB200_decodeBatchTensor: list of bytes -> the model's input tensor on the context's GPU, and the status list.
+
+    Image i becomes a C x H x W (layout "CHW") or H x W x C ("HWC") tensor of `dtype` (torch.float32 by default, float16,
+    bfloat16 or uint8): channels in true R, G, B order (B, G, R with bgr=True; C = 1 for gray / LUMA_ONLY), scaled per
+    `scale` and normalized with mean / std bit for bit as torchvision does (include/jpegdec_b200.h).  rois / orients /
+    out_sizes / filter as in decode_batch.  Returns (tensor [N, C, H, W] or [N, H, W, C] when every image has the same
+    size, else a list of per-image tensors, per-image status list).  An image that fails keeps whatever its slot held.
+    out: a CUDA tensor of that shape and dtype on the context's device (any row / plane strides the library accepts), or
+    a list of per-image tensors; else the result is allocated with torch.empty."""
+    import torch
+    dtype = torch.float32 if dtype is None else dtype
+    spec = tensor_spec(dtype, layout, scale, mean, std, bgr)
+    n = len(jpegs)
+    bufs = [np.frombuffer(j, dtype=np.uint8) for j in jpegs]
+    ptrs, sizes = [x.ctypes.data for x in bufs], [len(x) for x in bufs]
+    C_ = 3 if pixel_type == RGB8888 and not (options & JPEG_LUMA_ONLY) else 1
+    if out_sizes is not None:
+        hw = [(int(h), int(w)) for w, h in out_sizes]
+    elif rois is not None:
+        hw = [(int(r[3]), int(r[2])) for r in rois]
+    else:   # sizes from a header-only batch (no GPU work); an image refused there has size 0 x 0
+        b = Batch(ctx, ptrs, sizes, pixel_type, options, rois, orients, out_sizes, filter, spec=spec)
+        try:
+            hw = [(b.info(i)["out_h"], b.info(i)["out_w"]) for i in range(n)]
+        finally:
+            b.close()
+    same = len(set(hw)) == 1
+
+    def shape(h, w):
+        return (C_, h, w) if layout == "CHW" else (h, w, C_)
+
+    dev = torch.device("cuda", ctx.device)
+    if out is None:
+        out = torch.empty((n,) + shape(*hw[0]), dtype=dtype, device=dev) if same else \
+            [torch.empty(shape(h, w), dtype=dtype, device=dev) for h, w in hw]
+    views = list(out) if isinstance(out, (list, tuple)) else None
+    if views is None:
+        if not isinstance(out, torch.Tensor) or not same or tuple(out.shape) != (n,) + shape(*hw[0]):
+            raise ValueError("out: a tensor of shape %s" % (((n,) + shape(*hw[0])) if same else "(per-image sizes differ: pass a list)",))
+        views = [out[i] for i in range(n)]
+    if len(views) != n:
+        raise ValueError("out: one tensor per image")
+    ptr_l, pitch_l, plane_l = [], [], []
+    for i, v in enumerate(views):
+        if not isinstance(v, torch.Tensor) or v.device != dev or v.dtype != dtype or tuple(v.shape) != shape(*hw[i]):
+            raise ValueError("out[%d]: a %s tensor of shape %s on %s" % (i, dtype, shape(*hw[i]), dev))
+        es = dtype.itemsize
+        if layout == "CHW":
+            if v.shape[2] > 1 and v.stride(2) != 1:
+                raise ValueError("out[%d]: rows must be contiguous" % i)
+            pitch_l.append(v.stride(1) * es if v.shape[1] > 1 else hw[i][1] * es)
+            plane_l.append(v.stride(0) * es if v.shape[0] > 1 else 0)
+        else:
+            if (v.shape[2] > 1 and v.stride(2) != 1) or (v.shape[1] > 1 and v.stride(1) != C_):
+                raise ValueError("out[%d]: pixels must be contiguous" % i)
+            pitch_l.append(v.stride(0) * es if v.shape[0] > 1 else hw[i][1] * C_ * es)
+            plane_l.append(0)
+        ptr_l.append(v.data_ptr())
+    pa, sa = (C.c_void_p * n)(*ptrs), (C.c_int32 * n)(*sizes)
+    st = (C.c_int32 * n)()
+    with torch.cuda.device(dev):
+        torch.cuda.current_stream(dev).synchronize()   # the library's streams do not order against torch's
+        rc = lib().JPEGB200_decodeBatchTensor(ctx.h, pa, sa, n, pixel_type, options, _roi_array(rois, n),
+                                              _orient_array(orients, n), _size_array(out_sizes, n), int(filter),
+                                              C.byref(spec), (C.c_void_p * n)(*ptr_l), (C.c_int64 * n)(*pitch_l),
+                                              (C.c_int64 * n)(*plane_l), JPEGB200_OUT_DEVICE, st)
+    if rc == 0:
+        raise RuntimeError("decodeBatchTensor failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
+    return out, list(st)

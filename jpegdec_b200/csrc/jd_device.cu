@@ -143,6 +143,20 @@ struct JPEGB200_BATCH {
     DevBuf<uint8_t> d_rs;
     DevBuf<int32_t> d_rs_coef;
     DevBuf<JDResizeDesc> d_rs_desc;
+    /* tensor output (JPEGB200_batchCreateTensor): descs hold the row bytes as out_pitch; the pipeline (IDCT or resize) writes
+     * U (out_w x out_h, tn_bpp bytes per pixel) tightly into d_tn, jdk_tensor writes the destination */
+    bool tensor;
+    JPEGB200_TensorSpec tn_spec;
+    int tn_elt, tn_nc, tn_bpp, tn_planes;   /* tn_planes: C for CHW (the tensor is tn_planes x out_h rows), 1 for HWC */
+    std::vector<uint8_t> tn_swap;           /* per image: output channel c reads byte 2 - c of a staged pixel */
+    std::vector<int64_t> tn_stage;          /* per image: staging bytes (256-byte aligned) */
+    std::vector<int64_t> tn_plane;          /* per image: the caller's plane stride (0 = pitch * out_h) */
+    int64_t tn_stage_total;
+    std::vector<uint32_t> tn_table;         /* 3 x 256 elements, zero-extended to 32 bits */
+    std::vector<JDTensorDesc> tn_desc;
+    DevBuf<uint8_t> d_tn;
+    DevBuf<uint32_t> d_tn_tab;
+    DevBuf<JDTensorDesc> d_tn_desc;
     cudaStream_t stream;
     std::vector<JDInfo> infos;
     std::vector<int32_t> parse_status;
@@ -496,7 +510,29 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateResized(JPEGB200_CTX *ctx, const 
                                                        int n, int pixel_type, int options, const int32_t *rois,
                                                        const uint8_t *orients, const int32_t *out_sizes, int filter)
 {
+    return JPEGB200_batchCreateTensor(ctx, datas, sizes, n, pixel_type, options, rois, orients, out_sizes, filter, nullptr);
+}
+
+extern "C" JPEGB200_BATCH *JPEGB200_batchCreateTensor(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes,
+                                                      int n, int pixel_type, int options, const int32_t *rois,
+                                                      const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                                      const JPEGB200_TensorSpec *spec)
+{
     if (!ctx || n <= 0 || pixel_type < 0 || pixel_type >= INVALID_PIXEL_TYPE) { snprintf(g_err, sizeof(g_err), "invalid parameter"); return nullptr; }
+    if (spec) {
+        /* tensors are built from byte planes: RGB8888 (either byte order) and 8-bit gray, LUMA_ONLY folding included */
+        const int pt = ((options & JPEG_LUMA_ONLY) && pixel_type < EIGHT_BIT_GRAYSCALE) ? EIGHT_BIT_GRAYSCALE : pixel_type;
+        if (pt == RGB565_LITTLE_ENDIAN || pt == RGB565_BIG_ENDIAN) {
+            snprintf(g_err, sizeof(g_err), "tensor output is not supported with RGB565 pixel types (a packed 5/6/5 word has no byte planes)");
+            return nullptr;
+        }
+        if (pt >= FOUR_BIT_DITHERED && pt <= ONE_BIT_DITHERED) {
+            snprintf(g_err, sizeof(g_err), "tensor output is not supported with dithered pixel types");
+            return nullptr;
+        }
+        if (options & 0x10000) { snprintf(g_err, sizeof(g_err), "tensor output is not supported with padded output"); return nullptr; }
+        if (!jd_tensor_check(spec, pt == RGB8888 ? 3 : 1, g_err, (int)sizeof(g_err))) return nullptr;
+    }
     if (out_sizes) {
         /* resizing works on byte planes: RGB8888 (either byte order) and 8-bit gray, LUMA_ONLY folding included */
         const int pt = ((options & JPEG_LUMA_ONLY) && pixel_type < EIGHT_BIT_GRAYSCALE) ? EIGHT_BIT_GRAYSCALE : pixel_type;
@@ -539,6 +575,17 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateResized(JPEGB200_CTX *ctx, const 
         b->rs_plans.assign(n, JDResizePlan{});
         b->rs_src_w.assign(n, 0); b->rs_src_h.assign(n, 0); b->rs_scratch.assign(n, 0);
     }
+    b->tensor = spec != nullptr;
+    b->tn_stage_total = 0;
+    b->tn_elt = b->tn_nc = b->tn_bpp = b->tn_planes = 0;
+    if (b->tensor) {
+        b->tn_spec = *spec;
+        b->tn_swap.assign(n, 0); b->tn_stage.assign(n, 0); b->tn_plane.assign(n, 0);
+        std::vector<uint8_t> tb(3 * 256 * 4);
+        b->tn_elt = jd_tensor_table(spec, tb.data());
+        b->tn_table.assign(3 * 256, 0u);
+        for (int k = 0; k < 3 * 256; k++) memcpy(&b->tn_table[k], tb.data() + (size_t)k * b->tn_elt, (size_t)b->tn_elt);
+    }
     b->ctx = ctx;
     b->n = n;
     b->index_base = 0;
@@ -550,6 +597,11 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateResized(JPEGB200_CTX *ctx, const 
     b->gray_out = pixel_type >= EIGHT_BIT_GRAYSCALE;
     b->ptclass = (pixel_type == RGB8888) ? JD_PT_8888 : (b->gray_out ? JD_PT_GRAY : JD_PT_565);
     b->dither_bits = (pixel_type == FOUR_BIT_DITHERED) ? 4 : (pixel_type == TWO_BIT_DITHERED) ? 2 : (pixel_type == ONE_BIT_DITHERED) ? 1 : 0;
+    if (b->tensor) {
+        b->tn_nc = b->ptclass == JD_PT_8888 ? 3 : 1;
+        b->tn_bpp = bytes_per_pixel_class(b->ptclass);
+        b->tn_planes = spec->layout == JPEGB200_LAYOUT_CHW ? b->tn_nc : 1;
+    }
     b->stream = nullptr;
     b->descs_dl = nullptr; b->descs_dl_bytes = 0; b->downloaded = false; b->h_counters = nullptr;
     b->nchunks = 0; b->max_nch = 0; b->chunk_iterate = false; b->decode_flags = 0;
@@ -722,8 +774,16 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateResized(JPEGB200_CTX *ctx, const 
             b->rs_scratch_total += b->rs_scratch[i];
             d.out_w = (uint32_t)rw; d.out_h = (uint32_t)rh;
         }
+        if (b->tensor) {
+            /* U = what the same call without spec stores (out_w x out_h); staged, then converted */
+            b->tn_stage[i] = (int64_t)(((size_t)d.out_w * d.out_h * b->tn_bpp + 255) & ~(size_t)255);
+            b->tn_stage_total += b->tn_stage[i];
+            b->tn_swap[i] = (uint8_t)(b->tn_nc == 3 &&
+                                      (jd_rgb8888_is_bgr(ctx->arith, b->sshift, inf.ncomp, inf.subsample) != 0) != (spec->bgr != 0));
+        }
         size_t pitch;
-        if (b->dither_bits) {
+        if (b->tensor) pitch = (size_t)d.out_w * (spec->layout == JPEGB200_LAYOUT_HWC ? b->tn_nc : 1) * b->tn_elt;
+        else if (b->dither_bits) {
             const uint32_t pw = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> s);
             pitch = ((size_t)pw * b->dither_bits + 7) / 8;
             gray_total += (((size_t)pw * (size_t)inf.mcus_y * (size_t)(inf.mcu_h >> s)) + 255) & ~(size_t)255;
@@ -731,7 +791,7 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateResized(JPEGB200_CTX *ctx, const 
         d.out_pitch = (uint32_t)pitch;
         b->pitches[i] = (int64_t)pitch;
         b->arena_off[i] = out_total;
-        out_total += (pitch * d.out_h + 255) & ~(size_t)255;
+        out_total += (pitch * d.out_h * (b->tensor ? (size_t)b->tn_planes : 1u) + 255) & ~(size_t)255;
         seg += d.nseg;
         b->nseg_walk += d.nseg_walk;
         blk += (uint64_t)total_mcus * inf.bpm;
@@ -780,6 +840,7 @@ extern "C" void JPEGB200_batchDestroy(JPEGB200_BATCH *b)
     b->d_seg_jmap.release(); b->d_seg_status.release(); b->d_seg_nrec.release(); b->d_seg_phase.release();
     b->d_counters.release(); b->d_blk_hdr.release(); b->d_events.release();
     b->d_rs.release(); b->d_rs_coef.release(); b->d_rs_desc.release();
+    b->d_tn.release(); b->d_tn_tab.release(); b->d_tn_desc.release();
     if (b->stream && b->have_ev) {   /* back to the context for the next job */
         JDStreamSet ss;
         ss.stream = b->stream;
@@ -813,12 +874,26 @@ extern "C" int64_t JPEGB200_batchOutputBytes(JPEGB200_BATCH *b, int i, int64_t *
 {
     if (!b || i < 0 || i >= b->n) return 0;
     if (pitch_bytes) *pitch_bytes = (int64_t)b->descs[i].out_pitch;
-    return (int64_t)b->descs[i].out_pitch * b->descs[i].out_h;
+    return (int64_t)b->descs[i].out_pitch * b->descs[i].out_h * (b->tensor ? b->tn_planes : 1);
+}
+
+extern "C" int JPEGB200_batchSetOutputTensor(JPEGB200_BATCH *b, int i, void *out, int64_t pitch, int64_t plane_stride)
+{
+    if (!b || i < 0 || i >= b->n) return 0;
+    if (!b->tensor) { snprintf(g_err, sizeof(g_err), "batchSetOutputTensor on a batch created without a tensor spec"); return 0; }
+    if (!jd_check_tensor_output(b->index_base + i, b->tn_elt, (int64_t)b->descs[i].out_pitch, (int64_t)b->descs[i].out_h,
+                                b->tn_spec.layout == JPEGB200_LAYOUT_CHW, out, pitch, plane_stride, g_err, (int)sizeof(g_err)))
+        return 0;   /* nothing changes */
+    b->outs[i] = out;
+    b->pitches[i] = pitch > 0 ? pitch : (int64_t)b->descs[i].out_pitch;
+    b->tn_plane[i] = plane_stride;
+    return 1;
 }
 
 extern "C" int JPEGB200_batchSetOutput(JPEGB200_BATCH *b, int i, void *out, int64_t pitch_bytes)
 {
     if (!b || i < 0 || i >= b->n) return 0;
+    if (b->tensor) return JPEGB200_batchSetOutputTensor(b, i, out, pitch_bytes, 0);
     if (!jd_check_output(b->index_base + i, b->pixel_type, (int64_t)b->descs[i].out_pitch, out, pitch_bytes, 0, g_err, (int)sizeof(g_err)))
         return 0;   /* nothing changes: the image keeps its previous destination and pitch */
     b->outs[i] = out;
@@ -869,7 +944,7 @@ extern "C" int JPEGB200_batchReadOutput(JPEGB200_BATCH *b, int i, void *host_dst
     if (!b || i < 0 || i >= b->n || !b->d_out.p || !host_dst) return 0;
     CK(cudaSetDevice(b->ctx->device));
     if (b->stream) CK(cudaStreamSynchronize(b->stream));
-    CK(cudaMemcpy(host_dst, b->d_out.p + b->arena_off[i], (size_t)b->descs[i].out_pitch * b->descs[i].out_h, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(host_dst, b->d_out.p + b->arena_off[i], (size_t)JPEGB200_batchOutputBytes(b, i, nullptr), cudaMemcpyDeviceToHost));
     return 1;
 }
 
@@ -1105,6 +1180,10 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
     const int n = b->n;
     b->out_device = (flags & JPEGB200_OUT_DEVICE) != 0;
     b->decode_flags = flags;
+    if (b->tensor && !b->out_device) {
+        snprintf(g_err, sizeof(g_err), "tensor output is written to device memory only: decode with JPEGB200_OUT_DEVICE");
+        return 0;
+    }
     int launches = 0;
     /* output placement */
     bool user_dev_out = false;
@@ -1116,9 +1195,21 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         if (!user_dev_out && any_ptr) { snprintf(g_err, sizeof(g_err), "device output pointers given for some images only"); return 0; }
         /* the kernels store through these pointers: refuse misaligned ones before anything is enqueued */
         for (int i = 0; i < n; i++)
-            if (b->outs[i] && !jd_check_output(b->index_base + i, b->pixel_type, (int64_t)b->descs[i].out_pitch, b->outs[i], b->pitches[i], 1,
-                                               g_err, (int)sizeof(g_err)))
+            if (b->outs[i] && !b->tensor && !jd_check_output(b->index_base + i, b->pixel_type, (int64_t)b->descs[i].out_pitch, b->outs[i], b->pitches[i], 1,
+                                                             g_err, (int)sizeof(g_err)))
                 return 0;
+        for (int i = 0; i < n && b->tensor; i++) {
+            /* the kernel stores through these pointers: they must be device memory of this context's GPU */
+            if (!b->outs[i]) continue;
+            cudaPointerAttributes pa;
+            const cudaError_t e = cudaPointerGetAttributes(&pa, b->outs[i]);
+            if (e != cudaSuccess) cudaGetLastError();
+            if (e != cudaSuccess || (pa.type != cudaMemoryTypeDevice && pa.type != cudaMemoryTypeManaged) || pa.device != b->ctx->device) {
+                snprintf(g_err, sizeof(g_err), "tensor output of image %d: %p is not device memory of GPU %d", b->index_base + i,
+                         b->outs[i], b->ctx->device);
+                return 0;
+            }
+        }
     }
     /* the descriptors the kernels read: b->descs keeps the tight pitch (JPEGB200_batchOutputBytes, the arena) */
     std::vector<JDImageDesc> descs_stage = b->descs;
@@ -1136,6 +1227,39 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         if (!b->d_out.p) { CK(b->d_out.alloc(&b->ctx->pool, b->out_total + 256)); b->arena_owned = true; }
         out_base = b->d_out.p;
         for (int i = 0; i < n; i++) descs_stage[i].out_off = b->arena_off[i];
+    }
+    /* tensor: the pipeline below writes U tightly into d_tn (pipe_out) where it would have written the destination;
+     * jdk_tensor then writes the destination */
+    uint8_t *pipe_out = out_base;
+    uint32_t tn_ctas = 0;
+    if (b->tensor) {
+        b->tn_desc.assign(n, JDTensorDesc{});
+        constexpr uint32_t px_per_thread[5] = {0u, 16u, 8u, 0u, 4u};
+        const uint32_t PX = px_per_thread[b->tn_elt];
+        uint64_t so = 0, ctas = 0;
+        for (int i = 0; i < n; i++) {
+            JDTensorDesc &t = b->tn_desc[i];
+            t.blk = (uint32_t)ctas;
+            if (b->parse_status[i] != JPEG_SUCCESS) continue;
+            const JDImageDesc &d = b->descs[i];
+            t.w = d.out_w; t.h = d.out_h; t.swap = b->tn_swap[i];
+            t.src_off = so;
+            so += (uint64_t)b->tn_stage[i];
+            t.dst_off = descs_stage[i].out_off;
+            t.pitch = user_dev_out ? (uint64_t)b->pitches[i] : (uint64_t)d.out_pitch;
+            t.plane = (user_dev_out && b->tn_plane[i]) ? (uint64_t)b->tn_plane[i] : t.pitch * d.out_h;
+            ctas += ((uint64_t)(d.out_w + PX - 1) / PX * d.out_h + JD_TN_THREADS - 1) / JD_TN_THREADS;
+            descs_stage[i].out_off = t.src_off;
+            descs_stage[i].out_pitch = d.out_w * (uint32_t)b->tn_bpp;
+        }
+        if (ctas >= (1ull << 31)) { snprintf(g_err, sizeof(g_err), "tensor output: too many elements in one job"); return 0; }
+        tn_ctas = (uint32_t)ctas;
+        CK(b->d_tn.alloc(&b->ctx->pool, so + 256));
+        CK(b->d_tn_tab.alloc(&b->ctx->pool, 3 * 256));
+        CK(b->d_tn_desc.alloc(&b->ctx->pool, n));
+        CK(cudaMemcpyAsync(b->d_tn_tab.p, b->tn_table.data(), 3 * 256 * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(b->d_tn_desc.p, b->tn_desc.data(), sizeof(JDTensorDesc) * n, cudaMemcpyHostToDevice, st));
+        pipe_out = b->d_tn.p;
     }
     /* resize: the IDCT stage writes S tightly into d_rs; jdk_resize_v writes where the IDCT would have */
     uint32_t rs_ctas[4] = {0u, 0u, 0u, 0u};
@@ -1351,7 +1475,7 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
     CK(cudaEventRecord(b->ev[5], st));
     /* IDCT + colour: one launch per run of images with the same geometry class */
     const bool half = b->sshift == 1;
-    uint8_t *stage_out = b->dither_bits ? b->d_gray.p : b->resize ? b->d_rs.p : out_base;
+    uint8_t *stage_out = b->dither_bits ? b->d_gray.p : b->resize ? b->d_rs.p : pipe_out;
     for (int i0 = 0; i0 < n;) {
         if (b->parse_status[i0] != JPEG_SUCCESS) { i0++; continue; }
         const JDInfo &f = b->infos[i0];
@@ -1454,7 +1578,7 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         /* timed in the dither slot (the pixel pass after the IDCT): the two never occur together */
         const bool gray = b->ptclass == JD_PT_GRAY;
         if (rs_ctas[0]) { jdk_resize_coeffs<<<rs_ctas[0], JD_RS_THREADS, 0, st>>>(b->d_rs_desc.p, (uint32_t)n, b->d_rs_coef.p, b->rs_filter); launches++; }
-#define JD_RS_ARGS b->d_rs_desc.p, (uint32_t)n, b->d_rs.p, b->d_rs_coef.p, out_base
+#define JD_RS_ARGS b->d_rs_desc.p, (uint32_t)n, b->d_rs.p, b->d_rs_coef.p, pipe_out
         if (rs_ctas[1]) {
             if (gray) jdk_resize_h<1, 0><<<rs_ctas[1], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
             else jdk_resize_h<4, 0><<<rs_ctas[1], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
@@ -1472,6 +1596,20 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         }
 #undef JD_RS_ARGS
     }
+    if (b->tensor && tn_ctas) {
+        /* timed in the dither slot too, after the resize */
+        const bool hwc = b->tn_spec.layout == JPEGB200_LAYOUT_HWC;
+#define JD_TN_LAUNCH(ELT_, NC_)                                                                                           \
+        if (hwc) jdk_tensor<ELT_, 1, NC_><<<tn_ctas, JD_TN_THREADS, 0, st>>>(b->d_tn_desc.p, (uint32_t)n, b->d_tn.p, b->d_tn_tab.p, out_base); \
+        else jdk_tensor<ELT_, 0, NC_><<<tn_ctas, JD_TN_THREADS, 0, st>>>(b->d_tn_desc.p, (uint32_t)n, b->d_tn.p, b->d_tn_tab.p, out_base);
+        if (b->tn_nc == 3) {
+            if (b->tn_elt == 4) { JD_TN_LAUNCH(4, 3) } else if (b->tn_elt == 2) { JD_TN_LAUNCH(2, 3) } else { JD_TN_LAUNCH(1, 3) }
+        } else {
+            if (b->tn_elt == 4) { JD_TN_LAUNCH(4, 1) } else if (b->tn_elt == 2) { JD_TN_LAUNCH(2, 1) } else { JD_TN_LAUNCH(1, 1) }
+        }
+#undef JD_TN_LAUNCH
+        launches++;
+    }
     CK(cudaEventRecord(b->ev[7], st));
     CK(cudaGetLastError());
     b->counters[JPEGB200_C_LAUNCHES] = launches;
@@ -1479,7 +1617,9 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
     b->counters[JPEGB200_C_BLOCKS] = (int64_t)b->nblk;
     b->counters[JPEGB200_C_COMPRESSED_BYTES] = (int64_t)b->comp_total;
     int64_t ob = 0;
-    for (int i = 0; i < n; i++) if (b->parse_status[i] == JPEG_SUCCESS) ob += (int64_t)b->pitches[i] * b->descs[i].out_h;
+    for (int i = 0; i < n; i++)
+        if (b->parse_status[i] == JPEG_SUCCESS)
+            ob += b->tensor ? JPEGB200_batchOutputBytes(b, i, nullptr) : (int64_t)b->pitches[i] * b->descs[i].out_h;
     b->counters[JPEGB200_C_OUTPUT_BYTES] = ob;
     return 1;
 }
@@ -1647,8 +1787,21 @@ extern "C" int JPEGB200_decodeBatchResized(JPEGB200_CTX *ctx, const uint8_t *con
                                            const int32_t *out_sizes, int filter, void *const *outs, const int64_t *pitches,
                                            int flags, int32_t *status)
 {
+    return JPEGB200_decodeBatchTensor(ctx, datas, sizes, n, pixel_type, options, rois, orients, out_sizes, filter, nullptr, outs,
+                                      pitches, nullptr, flags, status);
+}
+
+extern "C" int JPEGB200_decodeBatchTensor(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                          int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
+                                          const int32_t *out_sizes, int filter, const JPEGB200_TensorSpec *spec, void *const *outs,
+                                          const int64_t *pitches, const int64_t *plane_strides, int flags, int32_t *status)
+{
     if (!ctx || n <= 0) return 0;
     const bool dev_out = (flags & JPEGB200_OUT_DEVICE) != 0;
+    if (spec && !dev_out) {
+        snprintf(g_err, sizeof(g_err), "tensor output is written to device memory only: call with JPEGB200_OUT_DEVICE");
+        return 0;
+    }
     if (dev_out && !outs) { snprintf(g_err, sizeof(g_err), "JPEGB200_decodeBatch with JPEGB200_OUT_DEVICE needs the caller's device pointers"); return 0; }
     memset(ctx->last_counters, 0, sizeof(ctx->last_counters));
     memset(ctx->last_ms, 0, sizeof(ctx->last_ms));
@@ -1691,8 +1844,8 @@ extern "C" int JPEGB200_decodeBatchResized(JPEGB200_CTX *ctx, const uint8_t *con
             cb += sz; cnt++;
         }
         auto create = [&](int c) {
-            return JPEGB200_batchCreateResized(ctx, datas + i0, sizes + i0, c, pixel_type, options, rois ? rois + 4 * (size_t)i0 : nullptr,
-                                               orients ? orients + i0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)i0 : nullptr, filter);
+            return JPEGB200_batchCreateTensor(ctx, datas + i0, sizes + i0, c, pixel_type, options, rois ? rois + 4 * (size_t)i0 : nullptr,
+                                              orients ? orients + i0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)i0 : nullptr, filter, spec);
         };
         JPEGB200_BATCH *b = create(cnt);
         if (!b) { rc = 0; break; }
@@ -1715,11 +1868,12 @@ extern "C" int JPEGB200_decodeBatchResized(JPEGB200_CTX *ctx, const uint8_t *con
                 }
             }
         }
-        if (b->resize && cnt > 1 && b->rs_scratch_total > JD_JOB_RESIZE_SCRATCH) {
-            /* resize scratch (S + intermediate) of a job: at most JD_JOB_RESIZE_SCRATCH, or one image */
+        if ((b->resize || b->tensor) && cnt > 1 && b->rs_scratch_total + b->tn_stage_total > JD_JOB_RESIZE_SCRATCH) {
+            /* scratch of a job (resize: S + intermediate; tensor: the uint8 staging): at most JD_JOB_RESIZE_SCRATCH, or one image */
+            auto scratch = [&](int c) { return (b->resize ? b->rs_scratch[c] : 0) + (b->tensor ? b->tn_stage[c] : 0); };
             int c = 0;
             int64_t sb = 0;
-            while (c < cnt && (c == 0 || sb + b->rs_scratch[c] <= JD_JOB_RESIZE_SCRATCH)) sb += b->rs_scratch[c++];
+            while (c < cnt && (c == 0 || sb + scratch(c) <= JD_JOB_RESIZE_SCRATCH)) sb += scratch(c++);
             JPEGB200_batchDestroy(b);
             cnt = c;
             b = create(cnt);
@@ -1729,7 +1883,9 @@ extern "C" int JPEGB200_decodeBatchResized(JPEGB200_CTX *ctx, const uint8_t *con
         b->index_base = i0;
         const double t1 = trace ? now_ms() : 0.0;
         /* a refused pitch fails the call with batchSetOutput's message (nothing of this job is enqueued) */
-        for (int i = 0; i < cnt && rc; i++) rc = JPEGB200_batchSetOutput(b, i, outs ? outs[i0 + i] : nullptr, pitches ? pitches[i0 + i] : 0);
+        for (int i = 0; i < cnt && rc; i++)
+            rc = spec ? JPEGB200_batchSetOutputTensor(b, i, outs[i0 + i], pitches ? pitches[i0 + i] : 0, plane_strides ? plane_strides[i0 + i] : 0)
+                      : JPEGB200_batchSetOutput(b, i, outs ? outs[i0 + i] : nullptr, pitches ? pitches[i0 + i] : 0);
         rc = rc && JPEGB200_batchUpload(b);
         const double t2 = trace ? now_ms() : 0.0;
         rc = rc && JPEGB200_batchDecode(b, flags);

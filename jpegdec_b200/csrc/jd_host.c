@@ -10,6 +10,7 @@
 #include <stdio.h>
 #include <string.h>
 #include <stdlib.h>
+#include <math.h>
 #include "jd_internal.h"
 #include "jd_resize.h"
 
@@ -543,6 +544,124 @@ int jd_check_output(int index, int pixel_type, int64_t row_bytes, const void *ou
                      "(the pixel store size of pixel type %d)", index, out, (long long)p, (long long)store, pixel_type);
             return 0;
         }
+    }
+    return 1;
+}
+
+/* ---- tensor output (JPEGB200_batchCreateTensor) ---- */
+int jd_rgb8888_is_bgr(int arith, int sshift, int ncomp, int subsample)
+{
+    return arith == JPEG_ARITH_SSE2 && sshift == 0 && ncomp == 3 && (subsample == 0x22 || subsample == 0x11);
+}
+
+int jd_tensor_elt(int dtype)
+{
+    return dtype == JPEGB200_DT_U8 ? 1 : dtype == JPEGB200_DT_F32 ? 4 : (dtype == JPEGB200_DT_F16 || dtype == JPEGB200_DT_BF16) ? 2 : 0;
+}
+
+int jd_tensor_check(const JPEGB200_TensorSpec *spec, int channels, char *msg, int msg_len)
+{
+    if (!spec) { snprintf(msg, (size_t)msg_len, "tensor output: no spec"); return 0; }
+    if (!jd_tensor_elt(spec->dtype)) { snprintf(msg, (size_t)msg_len, "tensor output: unknown dtype %d", spec->dtype); return 0; }
+    if (spec->layout != JPEGB200_LAYOUT_CHW && spec->layout != JPEGB200_LAYOUT_HWC) {
+        snprintf(msg, (size_t)msg_len, "tensor output: unknown layout %d", spec->layout);
+        return 0;
+    }
+    if (spec->scale < JPEGB200_SCALE_NONE || spec->scale > JPEGB200_SCALE_MUL255) {
+        snprintf(msg, (size_t)msg_len, "tensor output: unknown scale %d", spec->scale);
+        return 0;
+    }
+    for (int c = 0; c < channels; c++) {
+        if (!isfinite(spec->mean[c])) { snprintf(msg, (size_t)msg_len, "tensor output: mean[%d] is not finite", c); return 0; }
+        if (!isfinite(spec->std[c]) || spec->std[c] == 0.0f) {
+            snprintf(msg, (size_t)msg_len, "tensor output: std[%d] = %g (it must be finite and not 0)", c, (double)spec->std[c]);
+            return 0;
+        }
+        if (spec->dtype == JPEGB200_DT_U8 && (spec->mean[c] != 0.0f || spec->std[c] != 1.0f)) {
+            snprintf(msg, (size_t)msg_len, "tensor output: uint8 elements take no normalization (mean 0, std 1)");
+            return 0;
+        }
+    }
+    if (spec->dtype == JPEGB200_DT_U8 && spec->scale != JPEGB200_SCALE_NONE) {
+        snprintf(msg, (size_t)msg_len, "tensor output: uint8 elements take no scale (JPEGB200_SCALE_NONE)");
+        return 0;
+    }
+    return 1;
+}
+
+/* float32 -> IEEE binary16 bits, round to nearest even (overflow to infinity, subnormals kept) */
+static uint16_t jd_f16_bits(float f)
+{
+    uint32_t u;
+    memcpy(&u, &f, 4);
+    const uint32_t sign = (u >> 16) & 0x8000u, a = u & 0x7FFFFFFFu;
+    if (a > 0x7F800000u) return (uint16_t)(sign | 0x7E00u);                 /* NaN */
+    if (a >= 0x477FF000u) return (uint16_t)(sign | 0x7C00u);                /* >= 65520: infinity */
+    if (a >= 0x38800000u)                                                   /* normal: 2^-14 and above */
+        return (uint16_t)(sign | ((a + 0x0FFFu + ((a >> 13) & 1u) - 0x38000000u) >> 13));
+    const uint32_t e = a >> 23;                                             /* subnormal result: units of 2^-24 */
+    if (e < 102u) return (uint16_t)sign;                                    /* below 2^-25: rounds to 0 */
+    const uint32_t mant = (a & 0x7FFFFFu) | 0x800000u, sh = 126u - e;       /* value = mant * 2^(e - 150) */
+    uint32_t q = mant >> sh;
+    const uint32_t rem = mant & ((1u << sh) - 1u), half = 1u << (sh - 1u);
+    if (rem > half || (rem == half && (q & 1u))) q++;
+    return (uint16_t)(sign | q);
+}
+
+/* float32 -> bfloat16 bits, round to nearest even (c10::BFloat16's rule) */
+static uint16_t jd_bf16_bits(float f)
+{
+    uint32_t u;
+    memcpy(&u, &f, 4);
+    if ((u & 0x7FFFFFFFu) > 0x7F800000u) return 0x7FC0u;
+    return (uint16_t)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
+}
+
+int jd_tensor_table(const JPEGB200_TensorSpec *spec, void *out)
+{
+    const int elt = jd_tensor_elt(spec->dtype);
+    if (!elt || spec->scale < JPEGB200_SCALE_NONE || spec->scale > JPEGB200_SCALE_MUL255) return 0;
+    const float inv255 = (float)(1.0 / 255);
+    for (int c = 0; c < 3; c++)
+        for (int x = 0; x < 256; x++) {
+            /* each step rounded to float32 on its own (volatile: no contraction into a fused multiply-add) */
+            volatile float s = (float)x;
+            if (spec->scale == JPEGB200_SCALE_DIV255) s = s / 255.0f;
+            else if (spec->scale == JPEGB200_SCALE_MUL255) s = s * inv255;
+            volatile float d = s - spec->mean[c];
+            volatile float y = d / spec->std[c];
+            const int k = c * 256 + x;
+            if (spec->dtype == JPEGB200_DT_U8) ((uint8_t *)out)[k] = (uint8_t)x;
+            else if (spec->dtype == JPEGB200_DT_F32) { const float v = y; memcpy((uint8_t *)out + 4 * k, &v, 4); }
+            else if (spec->dtype == JPEGB200_DT_F16) ((uint16_t *)out)[k] = jd_f16_bits(y);
+            else ((uint16_t *)out)[k] = jd_bf16_bits(y);
+        }
+    return elt;
+}
+
+int jd_check_tensor_output(int index, int elt, int64_t row_bytes, int64_t rows, int chw, const void *out, int64_t pitch,
+                           int64_t plane_stride, char *msg, int msg_len)
+{
+    const int64_t p = pitch > 0 ? pitch : row_bytes;
+    if ((uintptr_t)out % (uintptr_t)elt != 0 || p % elt != 0 || plane_stride % elt != 0) {
+        snprintf(msg, (size_t)msg_len, "tensor output of image %d: pointer %p, pitch %lld and plane stride %lld must be "
+                 "multiples of the element size (%d bytes)", index, out, (long long)p, (long long)plane_stride, elt);
+        return 0;
+    }
+    if (p < row_bytes) {
+        snprintf(msg, (size_t)msg_len, "tensor output of image %d: pitch %lld is below its row size of %lld bytes", index,
+                 (long long)p, (long long)row_bytes);
+        return 0;
+    }
+    if (p > (int64_t)UINT32_MAX) {
+        snprintf(msg, (size_t)msg_len, "tensor output of image %d: pitch %lld is above the largest supported pitch (%lld bytes)",
+                 index, (long long)p, (long long)UINT32_MAX);
+        return 0;
+    }
+    if (chw && plane_stride != 0 && (plane_stride < 0 || plane_stride < p * rows)) {
+        snprintf(msg, (size_t)msg_len, "tensor output of image %d: plane stride %lld is below pitch x rows = %lld bytes", index,
+                 (long long)plane_stride, (long long)(p * rows));
+        return 0;
     }
     return 1;
 }

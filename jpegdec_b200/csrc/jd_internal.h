@@ -135,6 +135,23 @@ uint64_t jd_rec_extent(uint64_t size, uint32_t scan_offset, uint32_t nseg, uint3
 int jd_check_output(int index, int pixel_type, int64_t row_bytes, const void *out, int64_t pitch, int device,
                     char *msg, int msg_len);
 
+/* Tensor output (JPEGB200_batchCreateTensor).  The byte order of an RGB8888 output: 1 = B,G,R,A, 0 = R,G,B,A.  The
+ * SSE2-build arithmetic stores B,G,R,A at full scale for 3-component 4:2:0 and 4:4:4 files (its SIMD colour paths);
+ * every other case takes the scalar colour code, which stores R,G,B,A.  Depends on the image, so it is asked per image. */
+int jd_rgb8888_is_bgr(int arith, int sshift, int ncomp, int subsample);
+/* Element size of a JPEGB200_DT_* (0 = unknown). */
+int jd_tensor_elt(int dtype);
+/* 1 if spec is usable with `channels` output channels (1 or 3), else 0 with a message. */
+int jd_tensor_check(const JPEGB200_TensorSpec *spec, int channels, char *msg, int msg_len);
+/* The 3 x 256 output elements (channel-major, jd_tensor_elt(spec->dtype) bytes each, little-endian bit patterns) of byte
+ * value x in output channel c, in plain IEEE float32 arithmetic (JPEGB200_batchCreateTensor's formula).  The kernel only
+ * looks these up.  Returns the element size, 0 for an unknown dtype or scale. */
+int jd_tensor_table(const JPEGB200_TensorSpec *spec, void *out);
+/* A caller's tensor destination (device memory): see JPEGB200_batchSetOutputTensor.  row_bytes: the tight row, rows: H,
+ * chw: planar layout.  Returns 1, or 0 with a message. */
+int jd_check_tensor_output(int index, int elt, int64_t row_bytes, int64_t rows, int chw, const void *out, int64_t pitch,
+                           int64_t plane_stride, char *msg, int msg_len);
+
 #ifdef __cplusplus
 }
 #endif

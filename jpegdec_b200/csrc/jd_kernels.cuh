@@ -2077,3 +2077,116 @@ __global__ void __launch_bounds__(JD_RS_THREADS) jdk_resize_v(const JDResizeDesc
         }
     }
 }
+
+/* ------------------------------------------------------------------------------------ */
+/* Tensor output (JPEGB200_batchCreateTensor): the pipeline has written each image's uint8  */
+/* output U tightly into the staging buffer; jdk_tensor looks every byte up in the C x 256  */
+/* table the host computed (jd_tensor_table) and stores the elements in CHW or HWC order.   */
+/* One launch covers every image; a CTA finds its image by a binary search over the images' */
+/* first CTA indices.                                                                        */
+/* ------------------------------------------------------------------------------------ */
+#define JD_TN_THREADS 128
+struct JDTensorDesc {
+    uint64_t src_off;          /* U in the staging buffer: h rows of w * bpp bytes (tight) */
+    uint64_t dst_off;          /* the tensor, from the output base */
+    uint64_t pitch;            /* bytes between rows */
+    uint64_t plane;            /* bytes between planes (CHW) */
+    uint32_t w, h;
+    uint32_t swap;             /* output channel c reads byte 2 - c of a pixel (else byte c) */
+    uint32_t blk;              /* first CTA of this image */
+};
+
+__device__ __forceinline__ uint32_t jd_tn_find(const JDTensorDesc *td, uint32_t n, uint32_t b)
+{
+    uint32_t lo = 0, hi = n - 1;   /* the last image whose first CTA is <= b (images without CTAs share the next one's) */
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (td[mid].blk <= b) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+/* One thread per 16 / ELT pixels of a row: one 16-byte store per plane (CHW) or NC of them (HWC) where the destination
+ * is 16-byte aligned and the run is whole, else one store per element.  ELT: element bytes (1 uint8, 2 fp16 / bf16,
+ * 4 fp32; the table holds the bit patterns, so the two 16-bit types share code).  NC: 3 (RGB8888 staging, 4 bytes per
+ * pixel) or 1 (gray). */
+template <int ELT, int HWC, int NC>
+__global__ void __launch_bounds__(JD_TN_THREADS) jdk_tensor(const JDTensorDesc *td, uint32_t n, const uint8_t *stage,
+                                                            const uint32_t *table, uint8_t *out)
+{
+    constexpr uint32_t PX = 16 / ELT;
+    constexpr uint32_t SB = NC == 3 ? 4 : 1;   /* staging bytes per pixel */
+    __shared__ uint32_t tab[NC * 256];
+    for (uint32_t k = threadIdx.x; k < NC * 256; k += JD_TN_THREADS) tab[k] = table[k];
+    __syncthreads();
+    const JDTensorDesc &d = td[jd_tn_find(td, n, blockIdx.x)];
+    const uint32_t q = (d.w + PX - 1) / PX;
+    const uint64_t item = (uint64_t)(blockIdx.x - d.blk) * JD_TN_THREADS + threadIdx.x;
+    if (item >= (uint64_t)q * d.h) return;
+    const uint32_t y = (uint32_t)(item / q), x0 = (uint32_t)(item % q) * PX;
+    const uint32_t npx = d.w - x0 < PX ? d.w - x0 : PX;
+    const uint8_t *src = stage + d.src_off + ((uint64_t)y * d.w + x0) * SB;
+    uint32_t px[PX];
+    if (NC == 3 && npx == PX && ((uintptr_t)src & 15u) == 0) {
+#pragma unroll
+        for (uint32_t g = 0; g < PX / 4; g++) {
+            const uint4 v = reinterpret_cast<const uint4 *>(src)[g];
+            px[4 * g] = v.x; px[4 * g + 1] = v.y; px[4 * g + 2] = v.z; px[4 * g + 3] = v.w;
+        }
+    } else {
+#pragma unroll
+        for (uint32_t p = 0; p < PX; p++)
+            px[p] = p < npx ? (NC == 3 ? reinterpret_cast<const uint32_t *>(src)[p] : (uint32_t)src[p]) : 0u;
+    }
+    uint32_t sh[NC];
+#pragma unroll
+    for (uint32_t c = 0; c < NC; c++) sh[c] = 8u * (d.swap ? 2u - c : c);
+    /* element e of this thread's run: CHW plane c holds e = p, HWC holds e = p * NC + c in one run of NC x 16 bytes */
+    uint32_t wv[NC][4];
+#pragma unroll
+    for (uint32_t c = 0; c < NC; c++) wv[c][0] = wv[c][1] = wv[c][2] = wv[c][3] = 0u;
+#pragma unroll
+    for (uint32_t p = 0; p < PX; p++) {
+#pragma unroll
+        for (uint32_t c = 0; c < NC; c++) {
+            const uint32_t v = tab[c * 256u + ((px[p] >> sh[c]) & 0xFFu)];
+            const uint32_t byte = (HWC ? p * NC + c : p) * ELT;
+            uint32_t &wd = wv[HWC ? byte / 16u : c][(byte / 4u) & 3u];
+            wd |= ELT == 4 ? v : v << (8u * (byte & 3u));
+        }
+    }
+    uint8_t *row = out + d.dst_off + (uint64_t)y * d.pitch;
+    if (HWC) {
+        uint8_t *dst = row + (uint64_t)x0 * NC * ELT;
+        if (npx == PX && ((uintptr_t)dst & 15u) == 0) {
+#pragma unroll
+            for (uint32_t c = 0; c < NC; c++) reinterpret_cast<uint4 *>(dst)[c] = make_uint4(wv[c][0], wv[c][1], wv[c][2], wv[c][3]);
+            return;
+        }
+#pragma unroll
+        for (uint32_t e = 0; e < PX * NC; e++) {
+            if (e >= npx * NC) break;
+            const uint32_t byte = e * ELT, wd = wv[byte / 16u][(byte / 4u) & 3u];
+            if (ELT == 4) reinterpret_cast<uint32_t *>(dst)[e] = wd;
+            else if (ELT == 2) reinterpret_cast<uint16_t *>(dst)[e] = (uint16_t)(wd >> (8u * (byte & 3u)));
+            else dst[e] = (uint8_t)(wd >> (8u * (byte & 3u)));
+        }
+        return;
+    }
+#pragma unroll
+    for (uint32_t c = 0; c < NC; c++) {
+        uint8_t *dst = row + c * d.plane + (uint64_t)x0 * ELT;
+        if (npx == PX && ((uintptr_t)dst & 15u) == 0) {
+            *reinterpret_cast<uint4 *>(dst) = make_uint4(wv[c][0], wv[c][1], wv[c][2], wv[c][3]);
+            continue;
+        }
+#pragma unroll
+        for (uint32_t p = 0; p < PX; p++) {
+            if (p >= npx) break;
+            const uint32_t byte = p * ELT, wd = wv[c][(byte / 4u) & 3u];
+            if (ELT == 4) reinterpret_cast<uint32_t *>(dst)[p] = wd;
+            else if (ELT == 2) reinterpret_cast<uint16_t *>(dst)[p] = (uint16_t)(wd >> (8u * (byte & 3u)));
+            else dst[p] = (uint8_t)(wd >> (8u * (byte & 3u)));
+        }
+    }
+}
