@@ -217,6 +217,33 @@ JPEGB200_BATCH *JPEGB200_batchCreateTensor(JPEGB200_CTX *ctx, const uint8_t *con
  * pitch * H.  Returns 0 with a message, and nothing changed, otherwise.  JPEGB200_batchSetOutput(b, i, out, pitch) on a
  * tensor batch is this call with plane_stride 0. */
 int JPEGB200_batchSetOutputTensor(JPEGB200_BATCH *b, int i, void *out, int64_t pitch, int64_t plane_stride);
+/* Several views of each file from one entropy walk (multi-crop loaders: SimCLR / MoCo pairs, DINO's global and local crops,
+ * FiveCrop / TenCrop).  views[i] >= 1 is the number of views of file i; V = the sum.  The views of file i are the consecutive
+ * view indices starting at views[0] + ... + views[i-1].  rois (V x 4), orients (V), out_sizes (V x 2) hold one entry per VIEW,
+ * and so do the batch's images from here on: JPEGB200_batchCount returns V and every per-image call (batchImageInfo,
+ * batchOutputBytes, batchSetOutput / _Tensor, batchGetDeviceOutput, batchReadOutput, batchErrMcu, batchOrientation, the
+ * status of batchWait) takes a view index.  views = NULL is JPEGB200_batchCreateTensor (one view per file).
+ *   - The result is that of JPEGB200_batchCreateTensor on the EXPANDED file list (file i repeated views[i] times, in order)
+ *     with the same per-view arrays: every output byte (and the bytes left alone), status, batchErrMcu, batchOrientation,
+ *     batchImageInfo and batchOutputBytes value, destination rule and refusal.
+ *   - Paid once per file: the upload of its bytes, jdk_prescan, the entropy walk (restart intervals down to the deepest last
+ *     MCU row among its valid views, or the chunk path of a restart-free scan), jdk_stitch / jdk_patch, the block headers and
+ *     coefficient records.  Paid per view: the IDCT / colour stores of its MCU box, the resize and the tensor conversion.
+ *   - Counted once per file: JPEGB200_C_COMPRESSED_BYTES, _H2D_BYTES (the per-view descriptors and quantisation tables are
+ *     still per view), _SEGMENTS, _BLOCKS, _RECORD_BYTES, _EVENTS and _EVENT_CANDIDATES; the status read-back in
+ *     _D2H_BYTES is one descriptor per file.  _OUTPUT_BYTES counts per view.  The window-event overflow of a job
+ *     (batchWait) is judged on the candidates counted once per file.
+ *   - Status: a file that fails to parse gives its status to all of its views.  A view whose own arguments are invalid
+ *     (rectangle outside the output, orientation outside 0-8, W or H outside 1..65535) gets JPEG_INVALID_PARAMETER alone;
+ *     the file's other views still decode, and a file without a valid view is not walked.  The file's walk reports its
+ *     first undecodable MCU m (no rectangle rule); a view gets JPEG_DECODE_ERROR with batchErrMcu = m when it has no
+ *     rectangle or m lies above the end of its last MCU row, else JPEG_SUCCESS and -1 -- the rule of
+ *     JPEGB200_batchCreateROI, since a view's walk is a prefix of its file's.
+ *   - Returns NULL with a message for any views[i] < 1, V above INT32_MAX, dithered pixel types and padded output. */
+JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                          const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                          const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                          const JPEGB200_TensorSpec *spec);
 void JPEGB200_batchDestroy(JPEGB200_BATCH *b);
 int JPEGB200_batchCount(JPEGB200_BATCH *b);
 /* per-image facts after batchCreate: status is JPEG_SUCCESS or the open() error the reference would give */
@@ -292,6 +319,16 @@ int JPEGB200_decodeBatchTensor(JPEGB200_CTX *ctx, const uint8_t *const *datas, c
                                int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
                                const int32_t *out_sizes, int filter, const JPEGB200_TensorSpec *spec, void *const *outs,
                                const int64_t *pitches, const int64_t *plane_strides, int flags, int32_t *status);
+/* The same with several views per file (views: n per-file counts, semantics of JPEGB200_batchCreateViews; NULL =
+ * JPEGB200_decodeBatchTensor).  rois, orients, out_sizes, outs, pitches, plane_strides and status hold one entry per view.
+ * Jobs are cut at file boundaries only: the views of one file are always decoded by one job.  The per-job image cap, the
+ * host-output job re-plan for small images and the 1 GiB of scratch per job count views; a file whose views alone need more
+ * scratch gets a job of its own.  Error messages name the view index in this call. */
+int JPEGB200_decodeBatchViews(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                              const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                              const uint8_t *orients, const int32_t *out_sizes, int filter,
+                              const JPEGB200_TensorSpec *spec, void *const *outs, const int64_t *pitches,
+                              const int64_t *plane_strides, int flags, int32_t *status);
 /* JPEGB200_NUM_COUNTERS counters summed over the jobs of the last JPEGB200_decodeBatch on this context */
 int JPEGB200_lastCallCounters(JPEGB200_CTX *ctx, int64_t *counters);
 /* CUDA-event stage times (JPEGB200_NUM_TIMINGS, ms) summed over those jobs, and how many jobs there were.  Jobs overlap

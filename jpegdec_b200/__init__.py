@@ -114,6 +114,12 @@ def lib():
     L.JPEGB200_batchCreateTensor.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
                                              i32p, C.c_int, C.POINTER(TensorSpec)]
     L.JPEGB200_batchCreateTensor.restype = vp
+    L.JPEGB200_batchCreateViews.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, i32p, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
+                                            i32p, C.c_int, C.POINTER(TensorSpec)]
+    L.JPEGB200_batchCreateViews.restype = vp
+    L.JPEGB200_decodeBatchViews.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, i32p, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
+                                            i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(vp), C.POINTER(C.c_int64),
+                                            C.POINTER(C.c_int64), C.c_int, i32p]
     L.JPEGB200_batchSetOutputTensor.argtypes = [vp, C.c_int, vp, C.c_int64, C.c_int64]
     L.JPEGB200_decodeBatchTensor.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
                                              i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(vp), C.POINTER(C.c_int64),
@@ -320,6 +326,18 @@ def digest_host(a):
         return int(z.sum(dtype=np.uint64))
 
 
+def _views_array(views, nfiles):
+    """per-file view counts -> (int32[nfiles] for the C ABI, number of views); None = one view per file"""
+    if views is None:
+        return None, nfiles
+    v = [int(k) for k in views]
+    if len(v) != nfiles:
+        raise ValueError("views: one count per file")
+    if any(k < 1 for k in v):
+        raise ValueError("views: every file needs at least one view")
+    return (C.c_int32 * nfiles)(*v), sum(v)
+
+
 def _roi_array(rois, n):
     """n (x, y, w, h) rectangles -> int32[4n] for the C ABI (None stays None = whole images)"""
     if rois is None:
@@ -357,25 +375,30 @@ class Batch:
     in output pixels per image (JPEGB200_batchCreateROI), or None for whole images.  orients: one EXIF transform per
     image (ORIENT_FROM_EXIF = the file's tag, 1-8 = that transform; JPEGB200_batchCreateOriented), or None; rois are
     then in the upright frame.  out_sizes: one (W, H) per image, each output then being Pillow's resize of that size
-    with `filter` (RESIZE_BILINEAR / _BICUBIC / _BOX) of the upright crop (JPEGB200_batchCreateResized), or None."""
+    with `filter` (RESIZE_BILINEAR / _BICUBIC / _BOX) of the upright crop (JPEGB200_batchCreateResized), or None.
+    views: one view count per file (JPEGB200_batchCreateViews: file i's views come next to each other and share one
+    entropy walk), or None for one per file; rois / orients / out_sizes and every per-image call are then per view, and
+    self.n is the number of views."""
 
     def __init__(self, ctx, ptrs, sizes, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
-                 filter=RESIZE_BILINEAR, spec=None):
-        n = len(ptrs)
+                 filter=RESIZE_BILINEAR, spec=None, views=None):
+        nf = len(ptrs)
+        self._views, n = _views_array(views, nf)
         self.n = n
-        self._ptrs = (C.c_void_p * n)(*ptrs)
-        self._sizes = (C.c_int32 * n)(*sizes)
+        self._ptrs = (C.c_void_p * nf)(*ptrs)
+        self._sizes = (C.c_int32 * nf)(*sizes)
         self._rois = _roi_array(rois, n)
         self._orients = _orient_array(orients, n)
         self._out_sizes = _size_array(out_sizes, n)
         self.ctx = ctx
-        if spec is None:
+        if spec is None and views is None:
             self.h = lib().JPEGB200_batchCreateResized(ctx.h, self._ptrs, self._sizes, n, pixel_type, options, self._rois,
                                                        self._orients, self._out_sizes, int(filter))
-        else:   # a TensorSpec: JPEGB200_batchCreateTensor (device outputs only)
+        else:   # views and / or a TensorSpec (device outputs only): JPEGB200_batchCreateViews
             self._spec = spec
-            self.h = lib().JPEGB200_batchCreateTensor(ctx.h, self._ptrs, self._sizes, n, pixel_type, options, self._rois,
-                                                      self._orients, self._out_sizes, int(filter), C.byref(spec))
+            self.h = lib().JPEGB200_batchCreateViews(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
+                                                     self._rois, self._orients, self._out_sizes, int(filter),
+                                                     C.byref(spec) if spec is not None else None)
         if not self.h:
             raise RuntimeError("batchCreate failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
 
@@ -452,33 +475,44 @@ class Batch:
 
 
 def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flags=0, rois=None, orients=None,
-                 out_sizes=None, filter=RESIZE_BILINEAR):
-    """JPEGB200_decodeBatch(ROI / Oriented / Resized): one call for n files (host pointers) -> n outputs (host pointers,
-    or device pointers with JPEGB200_OUT_DEVICE); rois: one (x, y, w, h) per image or None; orients: one EXIF transform
-    per image (0 = from the file) or None; out_sizes: one (W, H) per image (resized with `filter`) or None.  Returns (rc,
+                 out_sizes=None, filter=RESIZE_BILINEAR, views=None):
+    """JPEGB200_decodeBatch(ROI / Oriented / Resized / Views): one call for n files (host pointers) -> n outputs (host
+    pointers, or device pointers with JPEGB200_OUT_DEVICE); rois: one (x, y, w, h) per image or None; orients: one EXIF
+    transform per image (0 = from the file) or None; out_sizes: one (W, H) per image (resized with `filter`) or None.
+    views: one view count per file, or None; outs, pitches and the per-image lists are then per view.  Returns (rc,
     per-image status list, counters summed over the internal jobs)."""
-    n = len(ptrs)
-    pa = (C.c_void_p * n)(*ptrs)
-    sa = (C.c_int32 * n)(*sizes)
+    nf = len(ptrs)
+    va, n = _views_array(views, nf)
+    pa = (C.c_void_p * nf)(*ptrs)
+    sa = (C.c_int32 * nf)(*sizes)
+    if len(outs) != n:
+        raise ValueError("outs: one destination per image (view)")
     oa = (C.c_void_p * n)(*outs)
     pi = (C.c_int64 * n)(*pitches) if pitches is not None else None
     st = (C.c_int32 * n)()
-    rc = lib().JPEGB200_decodeBatchResized(ctx.h, pa, sa, n, pixel_type, options, _roi_array(rois, n),
-                                           _orient_array(orients, n), _size_array(out_sizes, n), int(filter), oa, pi, flags, st)
+    if views is None:
+        rc = lib().JPEGB200_decodeBatchResized(ctx.h, pa, sa, n, pixel_type, options, _roi_array(rois, n),
+                                               _orient_array(orients, n), _size_array(out_sizes, n), int(filter), oa, pi, flags,
+                                               st)
+    else:
+        rc = lib().JPEGB200_decodeBatchViews(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
+                                             _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None, oa, pi,
+                                             None, flags, st)
     cnt = (C.c_int64 * len(COUNTER_NAMES))()
     lib().JPEGB200_lastCallCounters(ctx.h, cnt)
     return rc, list(st), dict(zip(COUNTER_NAMES, list(cnt)))
 
 
 def decode_batch_to_host(ctx, jpegs, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
-                         filter=RESIZE_BILINEAR):
+                         filter=RESIZE_BILINEAR, views=None):
     """Convenience: list of bytes -> list of numpy arrays [out_h, pitch_bytes] (uint8).
     One public-API call per batch with HOST buffers on both sides.  rois: one (x, y, w, h) per image (the arrays are then
     h rows of w pixels), or None.  orients: one EXIF transform per image (0 = from the file), or None.  out_sizes: one
-    (W, H) per image (the arrays are then H rows of W pixels, resized with `filter`), or None."""
+    (W, H) per image (the arrays are then H rows of W pixels, resized with `filter`), or None.  views: one view count
+    per file, or None; the lists (and rois / orients / out_sizes) are then per view."""
     bufs = [np.frombuffer(j, dtype=np.uint8) for j in jpegs]
     b = Batch(ctx, [x.ctypes.data for x in bufs], [len(x) for x in bufs], pixel_type, options, rois, orients, out_sizes,
-              filter)
+              filter, views=views)
     try:
         outs = []
         for i in range(b.n):
@@ -526,7 +560,7 @@ def tensor_spec(dtype, layout="CHW", scale="div255", mean=(0.0, 0.0, 0.0), std=(
 
 def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, orients=None, out_sizes=None,
                         filter=RESIZE_BILINEAR, dtype=None, layout="CHW", scale="div255", mean=(0.0, 0.0, 0.0),
-                        std=(1.0, 1.0, 1.0), bgr=False, out=None):
+                        std=(1.0, 1.0, 1.0), bgr=False, out=None, views=None):
     """JPEGB200_decodeBatchTensor: list of bytes -> the model's input tensor on the context's GPU, and the status list.
 
     Image i becomes a C x H x W (layout "CHW") or H x W x C ("HWC") tensor of `dtype` (torch.float32 by default, float16,
@@ -535,11 +569,14 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     out_sizes / filter as in decode_batch.  Returns (tensor [N, C, H, W] or [N, H, W, C] when every image has the same
     size, else a list of per-image tensors, per-image status list).  An image that fails keeps whatever its slot held.
     out: a CUDA tensor of that shape and dtype on the context's device (any row / plane strides the library accepts), or
-    a list of per-image tensors; else the result is allocated with torch.empty."""
+    a list of per-image tensors; else the result is allocated with torch.empty.
+    views: one view count per file (JPEGB200_decodeBatchViews: the views of a file share one entropy walk), or None; the
+    images are then the views: rois / orients / out_sizes / out and the result ([V, C, H, W], or a list) are per view."""
     import torch
     dtype = torch.float32 if dtype is None else dtype
     spec = tensor_spec(dtype, layout, scale, mean, std, bgr)
-    n = len(jpegs)
+    nf = len(jpegs)
+    va, n = _views_array(views, nf)
     bufs = [np.frombuffer(j, dtype=np.uint8) for j in jpegs]
     ptrs, sizes = [x.ctypes.data for x in bufs], [len(x) for x in bufs]
     C_ = 3 if pixel_type == RGB8888 and not (options & JPEG_LUMA_ONLY) else 1
@@ -548,7 +585,7 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     elif rois is not None:
         hw = [(int(r[3]), int(r[2])) for r in rois]
     else:   # sizes from a header-only batch (no GPU work); an image refused there has size 0 x 0
-        b = Batch(ctx, ptrs, sizes, pixel_type, options, rois, orients, out_sizes, filter, spec=spec)
+        b = Batch(ctx, ptrs, sizes, pixel_type, options, rois, orients, out_sizes, filter, spec=spec, views=views)
         try:
             hw = [(b.info(i)["out_h"], b.info(i)["out_w"]) for i in range(n)]
         finally:
@@ -562,15 +599,15 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     if out is None:
         out = torch.empty((n,) + shape(*hw[0]), dtype=dtype, device=dev) if same else \
             [torch.empty(shape(h, w), dtype=dtype, device=dev) for h, w in hw]
-    views = list(out) if isinstance(out, (list, tuple)) else None
-    if views is None:
+    dst = list(out) if isinstance(out, (list, tuple)) else None
+    if dst is None:
         if not isinstance(out, torch.Tensor) or not same or tuple(out.shape) != (n,) + shape(*hw[0]):
             raise ValueError("out: a tensor of shape %s" % (((n,) + shape(*hw[0])) if same else "(per-image sizes differ: pass a list)",))
-        views = [out[i] for i in range(n)]
-    if len(views) != n:
+        dst = [out[i] for i in range(n)]
+    if len(dst) != n:
         raise ValueError("out: one tensor per image")
     ptr_l, pitch_l, plane_l = [], [], []
-    for i, v in enumerate(views):
+    for i, v in enumerate(dst):
         if not isinstance(v, torch.Tensor) or v.device != dev or v.dtype != dtype or tuple(v.shape) != shape(*hw[i]):
             raise ValueError("out[%d]: a %s tensor of shape %s on %s" % (i, dtype, shape(*hw[i]), dev))
         es = dtype.itemsize
@@ -585,14 +622,14 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
             pitch_l.append(v.stride(0) * es if v.shape[0] > 1 else hw[i][1] * C_ * es)
             plane_l.append(0)
         ptr_l.append(v.data_ptr())
-    pa, sa = (C.c_void_p * n)(*ptrs), (C.c_int32 * n)(*sizes)
+    pa, sa = (C.c_void_p * nf)(*ptrs), (C.c_int32 * nf)(*sizes)
     st = (C.c_int32 * n)()
     with torch.cuda.device(dev):
         torch.cuda.current_stream(dev).synchronize()   # the library's streams do not order against torch's
-        rc = lib().JPEGB200_decodeBatchTensor(ctx.h, pa, sa, n, pixel_type, options, _roi_array(rois, n),
-                                              _orient_array(orients, n), _size_array(out_sizes, n), int(filter),
-                                              C.byref(spec), (C.c_void_p * n)(*ptr_l), (C.c_int64 * n)(*pitch_l),
-                                              (C.c_int64 * n)(*plane_l), JPEGB200_OUT_DEVICE, st)
+        rc = lib().JPEGB200_decodeBatchViews(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
+                                             _orient_array(orients, n), _size_array(out_sizes, n), int(filter),
+                                             C.byref(spec), (C.c_void_p * n)(*ptr_l), (C.c_int64 * n)(*pitch_l),
+                                             (C.c_int64 * n)(*plane_l), JPEGB200_OUT_DEVICE, st)
     if rc == 0:
-        raise RuntimeError("decodeBatchTensor failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
+        raise RuntimeError("decodeBatchViews failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
     return out, list(st)

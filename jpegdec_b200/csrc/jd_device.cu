@@ -122,7 +122,15 @@ struct DevBuf {
 
 struct JPEGB200_BATCH {
     JPEGB200_CTX *ctx;
-    int n;
+    int n;                          /* images (views with JPEGB200_batchCreateViews): everything per image is per view */
+    /* views (JPEGB200_batchCreateViews): nf files, each walked once through its entropy-facing descriptor fdescs[f]
+     * (d_fdescs); descs[i] is view i's descriptor for the IDCT and after it, carrying its file's seg / blk / rec bases.
+     * Without views nf = n and descs serves both (fdescs and vfile stay empty). */
+    int nf;
+    bool views;
+    std::vector<int32_t> vfile;     /* per view: its file */
+    std::vector<JDImageDesc> fdescs;
+    DevBuf<JDImageDesc> d_fdescs;
     int pixel_type, options, sshift, ptclass, dither_bits;
     bool gray_out;
     bool padded; /* write the whole MCU-aligned frame (single-image API: callbacks deliver whole MCUs) */
@@ -212,6 +220,11 @@ struct JPEGB200_BATCH {
 };
 
 static char *ctx_err() { return g_err; }
+
+/* the file of image (view) i, and the entropy-facing descriptors (one per file) on the host and the device */
+static inline int file_of(const JPEGB200_BATCH *b, int i) { return b->views ? b->vfile[i] : i; }
+static inline std::vector<JDImageDesc> &file_descs(JPEGB200_BATCH *b) { return b->views ? b->fdescs : b->descs; }
+static inline JDImageDesc *file_descs_dev(JPEGB200_BATCH *b) { return b->views ? b->d_fdescs.p : b->d_descs.p; }
 
 #define JD_EVENT_CAP (1u << 20)
 #define JD_CHUNK_PASSES 6     /* restart-free scans: entry-state passes per decode (from the third on only moved chunks are parsed; the last one verifies) */
@@ -518,7 +531,31 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateTensor(JPEGB200_CTX *ctx, const u
                                                       const uint8_t *orients, const int32_t *out_sizes, int filter,
                                                       const JPEGB200_TensorSpec *spec)
 {
+    return JPEGB200_batchCreateViews(ctx, datas, sizes, n, nullptr, pixel_type, options, rois, orients, out_sizes, filter, spec);
+}
+
+extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                                     const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                                     const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                                     const JPEGB200_TensorSpec *spec)
+{
     if (!ctx || n <= 0 || pixel_type < 0 || pixel_type >= INVALID_PIXEL_TYPE) { snprintf(g_err, sizeof(g_err), "invalid parameter"); return nullptr; }
+    int64_t nv = n;   /* images of the batch: views */
+    if (views) {
+        nv = 0;
+        for (int f = 0; f < n; f++) {
+            if (views[f] < 1) { snprintf(g_err, sizeof(g_err), "views[%d] = %d: every file needs at least one view", f, views[f]); return nullptr; }
+            nv += views[f];
+        }
+        if (nv > INT32_MAX) { snprintf(g_err, sizeof(g_err), "%lld views: at most %d per batch", (long long)nv, INT32_MAX); return nullptr; }
+        /* like rectangles and orientations: the dither of a view is not a view of the dither; padded output is the
+         * single-image API's */
+        if (pixel_type >= FOUR_BIT_DITHERED && pixel_type <= ONE_BIT_DITHERED) {
+            snprintf(g_err, sizeof(g_err), "views are not supported with dithered pixel types");
+            return nullptr;
+        }
+        if (options & 0x10000) { snprintf(g_err, sizeof(g_err), "views are not supported with padded output"); return nullptr; }
+    }
     if (spec) {
         /* tensors are built from byte planes: RGB8888 (either byte order) and 8-bit gray, LUMA_ONLY folding included */
         const int pt = ((options & JPEG_LUMA_ONLY) && pixel_type < EIGHT_BIT_GRAYSCALE) ? EIGHT_BIT_GRAYSCALE : pixel_type;
@@ -565,29 +602,31 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateTensor(JPEGB200_CTX *ctx, const u
     JPEGB200_BATCH *b = new (std::nothrow) JPEGB200_BATCH();
     if (!b) return nullptr;
     b->roi = rois != nullptr || orients != nullptr;
-    if (b->roi) b->plans.assign(n, JDRoiPlan{});
-    b->exif_tag.assign(n, 0);
-    b->orient.assign(n, 1);
+    b->plans.assign(nv, JDRoiPlan{});   /* read with rois or orients only */
+    b->exif_tag.assign(nv, 0);
+    b->orient.assign(nv, 1);
     b->resize = out_sizes != nullptr;
     b->rs_filter = filter;
     b->rs_scratch_total = 0;
     if (b->resize) {
-        b->rs_plans.assign(n, JDResizePlan{});
-        b->rs_src_w.assign(n, 0); b->rs_src_h.assign(n, 0); b->rs_scratch.assign(n, 0);
+        b->rs_plans.assign(nv, JDResizePlan{});
+        b->rs_src_w.assign(nv, 0); b->rs_src_h.assign(nv, 0); b->rs_scratch.assign(nv, 0);
     }
     b->tensor = spec != nullptr;
     b->tn_stage_total = 0;
     b->tn_elt = b->tn_nc = b->tn_bpp = b->tn_planes = 0;
     if (b->tensor) {
         b->tn_spec = *spec;
-        b->tn_swap.assign(n, 0); b->tn_stage.assign(n, 0); b->tn_plane.assign(n, 0);
+        b->tn_swap.assign(nv, 0); b->tn_stage.assign(nv, 0); b->tn_plane.assign(nv, 0);
         std::vector<uint8_t> tb(3 * 256 * 4);
         b->tn_elt = jd_tensor_table(spec, tb.data());
         b->tn_table.assign(3 * 256, 0u);
         for (int k = 0; k < 3 * 256; k++) memcpy(&b->tn_table[k], tb.data() + (size_t)k * b->tn_elt, (size_t)b->tn_elt);
     }
     b->ctx = ctx;
-    b->n = n;
+    b->n = (int)nv;
+    b->nf = n;
+    b->views = views != nullptr;
     b->index_base = 0;
     if ((options & JPEG_LUMA_ONLY) && pixel_type < EIGHT_BIT_GRAYSCALE) pixel_type = EIGHT_BIT_GRAYSCALE; /* jpeg.inl:4991 */
     b->pixel_type = pixel_type;
@@ -609,15 +648,20 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateTensor(JPEGB200_CTX *ctx, const u
     memset(b->ms, 0, sizeof(b->ms));
     memset(b->counters, 0, sizeof(b->counters));
     b->infos.resize(n);
-    b->parse_status.assign(n, JPEG_SUCCESS);
+    b->parse_status.assign(nv, JPEG_SUCCESS);
     b->datas.assign(datas, datas + n);
     b->sizes.assign(sizes, sizes + n);
-    b->descs.resize(n);
-    b->quant.assign((size_t)n * 192, 0);
-    b->outs.assign(n, nullptr);
-    b->pitches.assign(n, 0);
+    b->descs.resize(nv);
+    if (b->views) {
+        b->fdescs.resize(n);
+        b->vfile.resize(nv);
+        for (int f = 0, i = 0; f < n; f++) for (int k = 0; k < views[f]; k++) b->vfile[i++] = f;
+    }
+    b->quant.assign((size_t)nv * 192, 0);   /* per view: the IDCT kernels index it by their descriptor's index */
+    b->outs.assign(nv, nullptr);
+    b->pitches.assign(nv, 0);
     b->comp_off.assign(n, 0);
-    b->arena_off.assign(n, 0);
+    b->arena_off.assign(nv, 0);
 
     /* input layout: one span if the files already sit back to back in host memory */
     bool contig = true;
@@ -646,15 +690,18 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateTensor(JPEGB200_CTX *ctx, const u
     b->nseg_walk = 0;
     uint64_t blk = 0, rec_total = 0;
     size_t out_total = 0, gray_total = 0;
-    for (int i = 0; i < n; i++) {
-        JDInfo &inf = b->infos[i];
-        JDImageDesc &d = b->descs[i];
+    std::vector<int32_t> srects(4 * (size_t)nv, 0), vok((size_t)nv, 0);
+    std::vector<uint8_t> ks(orients ? (size_t)nv : 0u, 0);
+    for (int f = 0, v0 = 0; f < n; v0 += views ? views[f] : 1, f++) {
+        const int nvf = views ? views[f] : 1;   /* the file's views (images) are v0 .. v0 + nvf - 1 */
+        JDInfo &inf = b->infos[f];
+        JDImageDesc &d = file_descs(b)[f];
         memset(&d, 0, sizeof(d));
-        int ok = jd_parse_header(datas[i], sizes[i], 0, &inf);
+        int ok = jd_parse_header(datas[f], sizes[f], 0, &inf);
         int st = ok ? JPEG_SUCCESS : inf.error;
         if (ok && (options & JPEG_EXIF_THUMBNAIL)) {
             if (inf.thumb_data == 0 || inf.thumb_w == 0) { ok = 0; st = JPEG_INVALID_PARAMETER; }
-            else { ok = jd_parse_header(datas[i], sizes[i], inf.thumb_data, &inf); if (!ok) st = inf.error; }
+            else { ok = jd_parse_header(datas[f], sizes[f], inf.thumb_data, &inf); if (!ok) st = inf.error; }
         }
         bool prog = false;
         if (ok && inf.mode == 0xC2) {
@@ -667,47 +714,55 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateTensor(JPEGB200_CTX *ctx, const u
         } else if (ok && inf.mode != 0xC0) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }
         if (ok && !inf.tables_ok) { ok = 0; st = JPEG_DECODE_ERROR; }           /* jpeg.inl:2166 */
         if (ok && inf.ncomp == 1 && pixel_type == RGB8888) { ok = 0; st = JPEG_INVALID_PARAMETER; }
-        if (ok && (uint64_t)sizes[i] >= (512ull << 20)) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }   /* image-relative record indices are 32-bit */
-        b->exif_tag[i] = inf.orientation;
-        int32_t srect[4] = {0, 0, 0, 0};
-        if (orients) {
-            /* 0: the file's tag (none or out of range: identity); 1-8: that transform; anything else is refused below */
-            const int k = orients[i] == 0 ? ((inf.orientation >= 1 && inf.orientation <= 8) ? inf.orientation : 1) : orients[i];
-            if (k <= 8) b->orient[i] = (uint8_t)k;
-            if (ok && !jd_orient_plan(inf.width, inf.height, inf.subsample, inf.restart_interval, b->sshift, k,
-                                      rois ? rois + 4 * (size_t)i : nullptr, srect, &b->plans[i])) {
-                ok = 0; st = JPEG_INVALID_PARAMETER;   /* no such transform, or the rectangle does not lie inside the output */
+        if (ok && (uint64_t)sizes[f] >= (512ull << 20)) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }   /* image-relative record indices are 32-bit */
+        const int file_ok = ok;
+        for (int i = v0; i < v0 + nvf; i++) {
+            b->exif_tag[i] = inf.orientation;
+            if (orients) {
+                /* 0: the file's tag (none or out of range: identity); 1-8: that transform; anything else is refused below */
+                const int k = orients[i] == 0 ? ((inf.orientation >= 1 && inf.orientation <= 8) ? inf.orientation : 1) : orients[i];
+                if (k <= 8) b->orient[i] = (uint8_t)k;
+                ks[i] = (uint8_t)k;
             }
-        } else if (ok && b->roi) {
-            if (!jd_roi_plan(inf.width, inf.height, inf.subsample, inf.restart_interval, b->sshift, rois + 4 * (size_t)i, &b->plans[i])) {
-                ok = 0; st = JPEG_INVALID_PARAMETER;   /* the rectangle does not lie inside the output image */
-            }
-            srect[0] = rois[4 * (size_t)i]; srect[1] = rois[4 * (size_t)i + 1];
         }
-        if (ok && out_sizes) {
-            const int32_t rw = out_sizes[2 * (size_t)i], rh = out_sizes[2 * (size_t)i + 1];
-            if (rw < 1 || rw > 65535 || rh < 1 || rh > 65535) { ok = 0; st = JPEG_INVALID_PARAMETER; }
+        /* the views' own arguments (no such transform, a rectangle outside the output, a resize target outside 1..65535) and
+         * how deep the file is walked: down to the deepest last MCU row among its valid views */
+        uint32_t walk = 0;
+        if (ok) {
+            walk = (uint32_t)jd_views_plan(inf.width, inf.height, inf.subsample, inf.restart_interval, b->sshift, nvf,
+                                           rois ? rois + 4 * (size_t)v0 : nullptr, orients ? &ks[v0] : nullptr,
+                                           out_sizes ? out_sizes + 2 * (size_t)v0 : nullptr, &b->plans[v0], &srects[4 * (size_t)v0],
+                                           &vok[v0]);
+            if (walk == 0) ok = 0;   /* no valid view: the file is not walked */
         }
         const uint32_t total_mcus = ok ? (uint32_t)inf.mcus_x * inf.mcus_y : 0u;
         const uint32_t mps = inf.restart_interval ? (uint32_t)inf.restart_interval : total_mcus;
         const uint32_t nseg = ok ? (total_mcus + mps - 1) / mps : 0u;
         /* no restart markers: one long dependent stream -> chunk-parallel decode */
-        const uint32_t nch = (ok && !prog && inf.restart_interval == 0 && nseg == 1 && sizes[i] - inf.scan_offset >= 4096)
-                                 ? ((uint32_t)(sizes[i] - inf.scan_offset) + JD_CHUNK_BYTES - 1) / JD_CHUNK_BYTES + 1 : 0u;
-        if (ok && jd_rec_extent((uint64_t)sizes[i], (uint32_t)inf.scan_offset, nseg, nch) > (1ull << 32)) {
+        const uint32_t nch = (ok && !prog && inf.restart_interval == 0 && nseg == 1 && sizes[f] - inf.scan_offset >= 4096)
+                                 ? ((uint32_t)(sizes[f] - inf.scan_offset) + JD_CHUNK_BYTES - 1) / JD_CHUNK_BYTES + 1 : 0u;
+        if (ok && jd_rec_extent((uint64_t)sizes[f], (uint32_t)inf.scan_offset, nseg, nch) > (1ull << 32)) {
             ok = 0; st = JPEG_UNSUPPORTED_FEATURE;   /* its record indices would wrap onto its own first records */
         }
-        b->parse_status[i] = st;
-        if (!ok) { /* keep a harmless empty descriptor */
+        /* a failed parse first, then the view's own arguments, then the record extent */
+        for (int i = v0; i < v0 + nvf; i++) b->parse_status[i] = (file_ok && !vok[i]) ? JPEG_INVALID_PARAMETER : st;
+        if (!ok) { /* keep harmless empty descriptors */
             d.nseg = 0; d.seg_base = seg; d.blk_base = (uint32_t)blk; d.status = (uint32_t)st;
+            for (int i = v0; i < v0 + nvf; i++) {
+                JDImageDesc &vd = b->descs[i];
+                if (b->views) vd = d;
+                vd.status = (uint32_t)b->parse_status[i];
+            }
             continue;
         }
-        {   /* kernels read quant column-major ([c * 8 + r]) so a lane's column is one 16-byte load */
+        {   /* kernels read quant column-major ([c * 8 + r]) so a lane's column is one 16-byte load; one copy per view */
             int16_t qn[192];
             jd_build_quant(&inf, qn);
-            int32_t *qt = &b->quant[(size_t)i * 192];
-            for (int cc = 0; cc < 3; cc++)
-                for (int nn = 0; nn < 64; nn++) qt[cc * 64 + (nn & 7) * 8 + (nn >> 3)] = qn[cc * 64 + nn];
+            for (int i = v0; i < v0 + nvf; i++) {
+                int32_t *qt = &b->quant[(size_t)i * 192];
+                for (int cc = 0; cc < 3; cc++)
+                    for (int nn = 0; nn < 64; nn++) qt[cc * 64 + (nn & 7) * 8 + (nn >> 3)] = qn[cc * 64 + nn];
+            }
         }
         /* Huffman LUT set: dedupe on the raw DHT content */
         const uint64_t h = jd_tables_hash(&inf);
@@ -715,20 +770,20 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateTensor(JPEGB200_CTX *ctx, const u
         for (; li < lut_hash.size(); li++) if (lut_hash[li] == h && jd_tables_equal(&inf, &b->infos[lut_owner[li]])) break;
         const bool shared = ctx->has_shared && ctx->shared_hash == h && ctx->shared_hash2 == jd_tables_hash2(&inf);
         if (li == lut_hash.size()) {
-            lut_hash.push_back(h); lut_owner.push_back(i);
+            lut_hash.push_back(h); lut_owner.push_back(f);
             b->luts.resize((size_t)(li + 1) * JD_LUT_ENTRIES);
             if (shared) memcpy(&b->luts[(size_t)li * JD_LUT_ENTRIES], ctx->shared_lut, JD_LUT_ENTRIES * 2);
             else jd_build_lut(&inf, &b->luts[(size_t)li * JD_LUT_ENTRIES]);
         }
         if (shared) ctx->shared_hits++;
-        d.scan_off = (uint32_t)(b->comp_off[i] + inf.scan_offset);
-        d.scan_end = (uint32_t)(b->comp_off[i] + sizes[i]);
+        d.scan_off = (uint32_t)(b->comp_off[f] + inf.scan_offset);
+        d.scan_end = (uint32_t)(b->comp_off[f] + sizes[f]);
         d.width = (uint16_t)inf.width; d.height = (uint16_t)inf.height;
         d.mcus_x = (uint16_t)inf.mcus_x; d.mcus_y = (uint16_t)inf.mcus_y;
         d.subsample = (uint8_t)inf.subsample; d.ncomp = (uint8_t)inf.ncomp; d.bpm = (uint8_t)inf.bpm; d.tsel = (uint8_t)inf.tsel;
         d.mcus_per_seg = mps;
         d.nseg = nseg;
-        d.nseg_walk = b->roi ? (uint32_t)b->plans[i].nseg_walk : d.nseg;
+        d.nseg_walk = b->roi ? walk : d.nseg;
         d.chunk_base = 0; d.nch = 0;
         d.prog = prog ? (1u | ((uint32_t)(inf.approx & 15) << 8)) : 0u;
         if (nch) {
@@ -736,62 +791,76 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateTensor(JPEGB200_CTX *ctx, const u
             d.nch = nch;
             b->nchunks += d.nch;
             if (d.nch > b->max_nch) b->max_nch = d.nch;
-            b->cimg_list.push_back((uint32_t)i);
+            b->cimg_list.push_back((uint32_t)f);
         }
         d.seg_base = seg;
         d.blk_base = (uint32_t)blk;
         d.lutset = li;
         /* coefficient records: image-relative indices (jd_core.h JD_REC_INDEX), one slot per restart segment and per chunk */
-        d.comp_off = (uint32_t)b->comp_off[i];
+        d.comp_off = (uint32_t)b->comp_off[f];
         d.rec_base = rec_total;
-        rec_total += (uint64_t)JD_REC_PER_BYTE * (uint64_t)(((size_t)sizes[i] + 15) & ~(size_t)15) + (uint64_t)JD_REC_SLOT_SLACK * (d.nseg + d.nch + 1u);
+        rec_total += (uint64_t)JD_REC_PER_BYTE * (uint64_t)(((size_t)sizes[f] + 15) & ~(size_t)15) + (uint64_t)JD_REC_SLOT_SLACK * (d.nseg + d.nch + 1u);
 
+        /* the views: the file's descriptor (its walk, blocks and records) with each view's rectangle, orientation and output.
+         * The file's own descriptor keeps roi_mcu_end = 0: jdk_stitch reports its first error, jd_view_err_mcu judges it
+         * per view. */
         const int s = b->sshift;
-        d.out_w = (uint32_t)((inf.width + (1 << s) - 1) >> s);
-        d.out_h = (uint32_t)((inf.height + (1 << s) - 1) >> s);
+        for (int i = v0; i < v0 + nvf; i++) {
+        JDImageDesc &vd = b->descs[i];
+        if (b->views) {
+            if (b->parse_status[i] != JPEG_SUCCESS) {   /* an invalid view of a walked file: empty, like a refused image */
+                memset(&vd, 0, sizeof(vd));
+                vd.seg_base = seg; vd.blk_base = (uint32_t)blk; vd.status = (uint32_t)b->parse_status[i];
+                continue;
+            }
+            vd = d;
+        }
+        vd.out_w = (uint32_t)((inf.width + (1 << s) - 1) >> s);
+        vd.out_h = (uint32_t)((inf.height + (1 << s) - 1) >> s);
         if (b->padded) {
-            d.out_w = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> s);
-            d.out_h = (uint32_t)inf.mcus_y * (uint32_t)(inf.mcu_h >> s);
+            vd.out_w = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> s);
+            vd.out_h = (uint32_t)inf.mcus_y * (uint32_t)(inf.mcu_h >> s);
         }
         if (b->roi) {
             const JDRoiPlan &pl = b->plans[i];
-            d.out_w = (uint32_t)pl.out_w; d.out_h = (uint32_t)pl.out_h;
-            d.roi_x = (uint16_t)srect[0]; d.roi_y = (uint16_t)srect[1];
-            d.mcu_x0 = (uint16_t)pl.mcu_x0; d.mcu_y0 = (uint16_t)pl.mcu_y0;
-            d.roi_mcu_end = (uint32_t)pl.mcu_end;
-            d.orient = orients ? b->orient[i] : 0u;
+            vd.out_w = (uint32_t)pl.out_w; vd.out_h = (uint32_t)pl.out_h;
+            vd.roi_x = (uint16_t)srects[4 * (size_t)i]; vd.roi_y = (uint16_t)srects[4 * (size_t)i + 1];
+            vd.mcu_x0 = (uint16_t)pl.mcu_x0; vd.mcu_y0 = (uint16_t)pl.mcu_y0;
+            vd.roi_mcu_end = (uint32_t)pl.mcu_end;
+            vd.orient = orients ? b->orient[i] : 0u;
         }
         if (b->resize) {
             /* S = what the same call without out_sizes stores; the descriptor carries the resized size from here on */
             const int bp = bytes_per_pixel_class(b->ptclass);
             JDResizePlan &rp = b->rs_plans[i];
             const int32_t rw = out_sizes[2 * (size_t)i], rh = out_sizes[2 * (size_t)i + 1];
-            if (!jd_resize_plan((int)d.out_w, (int)d.out_h, rw, rh, filter, bp, &rp)) {
+            if (!jd_resize_plan((int)vd.out_w, (int)vd.out_h, rw, rh, filter, bp, &rp)) {
                 snprintf(g_err, sizeof(g_err), "resize plan failed for image %d", i); delete b; return nullptr;
             }
-            b->rs_src_w[i] = d.out_w; b->rs_src_h[i] = d.out_h;
-            b->rs_scratch[i] = (int64_t)(((size_t)d.out_w * d.out_h * bp + 255) & ~(size_t)255) + ((rp.mid_bytes + 255) & ~(int64_t)255);
+            b->rs_src_w[i] = vd.out_w; b->rs_src_h[i] = vd.out_h;
+            b->rs_scratch[i] = (int64_t)(((size_t)vd.out_w * vd.out_h * bp + 255) & ~(size_t)255) + ((rp.mid_bytes + 255) & ~(int64_t)255);
             b->rs_scratch_total += b->rs_scratch[i];
-            d.out_w = (uint32_t)rw; d.out_h = (uint32_t)rh;
+            vd.out_w = (uint32_t)rw; vd.out_h = (uint32_t)rh;
         }
         if (b->tensor) {
             /* U = what the same call without spec stores (out_w x out_h); staged, then converted */
-            b->tn_stage[i] = (int64_t)(((size_t)d.out_w * d.out_h * b->tn_bpp + 255) & ~(size_t)255);
+            b->tn_stage[i] = (int64_t)(((size_t)vd.out_w * vd.out_h * b->tn_bpp + 255) & ~(size_t)255);
             b->tn_stage_total += b->tn_stage[i];
             b->tn_swap[i] = (uint8_t)(b->tn_nc == 3 &&
                                       (jd_rgb8888_is_bgr(ctx->arith, b->sshift, inf.ncomp, inf.subsample) != 0) != (spec->bgr != 0));
         }
         size_t pitch;
-        if (b->tensor) pitch = (size_t)d.out_w * (spec->layout == JPEGB200_LAYOUT_HWC ? b->tn_nc : 1) * b->tn_elt;
+        if (b->tensor) pitch = (size_t)vd.out_w * (spec->layout == JPEGB200_LAYOUT_HWC ? b->tn_nc : 1) * b->tn_elt;
         else if (b->dither_bits) {
             const uint32_t pw = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> s);
             pitch = ((size_t)pw * b->dither_bits + 7) / 8;
             gray_total += (((size_t)pw * (size_t)inf.mcus_y * (size_t)(inf.mcu_h >> s)) + 255) & ~(size_t)255;
-        } else pitch = (size_t)d.out_w * bytes_per_pixel_class(b->ptclass);
-        d.out_pitch = (uint32_t)pitch;
+        } else pitch = (size_t)vd.out_w * bytes_per_pixel_class(b->ptclass);
+        vd.out_pitch = (uint32_t)pitch;
         b->pitches[i] = (int64_t)pitch;
         b->arena_off[i] = out_total;
-        out_total += (pitch * d.out_h * (b->tensor ? (size_t)b->tn_planes : 1u) + 255) & ~(size_t)255;
+        out_total += (pitch * vd.out_h * (b->tensor ? (size_t)b->tn_planes : 1u) + 255) & ~(size_t)255;
+        }
         seg += d.nseg;
         b->nseg_walk += d.nseg_walk;
         blk += (uint64_t)total_mcus * inf.bpm;
@@ -808,12 +877,13 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateTensor(JPEGB200_CTX *ctx, const u
     /* work list: CTAs of 128 segments sharing one LUT set.  With a region of interest the restart intervals that start
      * below its last MCU row are left out, but every interval above it stays in: the reference's bit-window phase is
      * carried from one interval to the next (SURVEY.md fact 4, A.2), so the pixels inside the rectangle depend on the walk
-     * of every interval before them. */
+     * of every interval before them.  One entry per file: its views share the walk. */
     b->seg_img.resize(seg ? seg : 1);
+    const std::vector<JDImageDesc> &fd = file_descs(b);
     for (uint32_t li = 0; li < (b->nlut ? b->nlut : 1); li++) {
         for (int i = 0; i < n; i++) {
-            const JDImageDesc &d = b->descs[i];
-            if (d.nseg == 0 || b->parse_status[i] != JPEG_SUCCESS || d.lutset != li) continue;
+            const JDImageDesc &d = fd[i];
+            if (d.nseg == 0 || d.lutset != li) continue;   /* nseg = 0: a file that is not walked */
             for (uint32_t s2 = 0; s2 < d.nseg; s2++) {
                 b->seg_img[d.seg_base + s2] = (uint32_t)i;
                 if (d.nch == 0 && s2 < d.nseg_walk) b->work.push_back(d.seg_base + s2);
@@ -835,7 +905,7 @@ extern "C" void JPEGB200_batchDestroy(JPEGB200_BATCH *b)
     b->d_clean.release(); b->d_seg_clen.release();
     b->d_filt.release(); b->d_cimg_list.release(); b->d_flen.release(); b->d_E0.release(); b->d_E1.release(); b->d_Ep.release(); b->d_cfirst.release();
     b->d_cn.release(); b->d_cpre.release(); b->d_cjmap.release(); b->d_cstatus.release(); b->d_cnown.release(); b->d_cdcs.release(); b->d_cpe.release();
-    b->d_descs.release(); b->d_quant.release(); b->d_luts.release(); b->d_rec.release();
+    b->d_descs.release(); b->d_fdescs.release(); b->d_quant.release(); b->d_luts.release(); b->d_rec.release();
     b->d_work.release(); b->d_cta_lut.release(); b->d_seg_img.release(); b->d_seg_start.release();
     b->d_seg_jmap.release(); b->d_seg_status.release(); b->d_seg_nrec.release(); b->d_seg_phase.release();
     b->d_counters.release(); b->d_blk_hdr.release(); b->d_events.release();
@@ -860,7 +930,7 @@ extern "C" int JPEGB200_batchImageInfo(JPEGB200_BATCH *b, int i, int32_t *width,
                                        int32_t *out_w, int32_t *out_h, int32_t *status)
 {
     if (!b || i < 0 || i >= b->n) return 0;
-    const JDInfo &inf = b->infos[i];
+    const JDInfo &inf = b->infos[file_of(b, i)];
     if (width) *width = inf.width;
     if (height) *height = inf.height;
     if (subsample) *subsample = inf.subsample;
@@ -952,9 +1022,10 @@ extern "C" int JPEGB200_batchUpload(JPEGB200_BATCH *b)
 {
     if (!b) return 0;
     if (!batch_stream(b)) return 0;
-    const int n = b->n;
+    const int n = b->n, nf = b->nf;
     CK(b->d_comp.alloc(&b->ctx->pool, b->comp_total + 256));
     CK(b->d_descs.alloc(&b->ctx->pool, n));
+    if (b->views) CK(b->d_fdescs.alloc(&b->ctx->pool, nf));
     CK(b->d_quant.alloc(&b->ctx->pool, (size_t)n * 192));
     CK(b->d_luts.alloc(&b->ctx->pool, b->luts.size() ? b->luts.size() : 1));
     CK(b->d_work.alloc(&b->ctx->pool, b->work.size() ? b->work.size() : 1));
@@ -966,7 +1037,7 @@ extern "C" int JPEGB200_batchUpload(JPEGB200_BATCH *b)
     if (b->nchunks) {
         const size_t nc = b->nchunks;
         CK(b->d_filt.alloc(&b->ctx->pool, b->comp_total + 512));
-        CK(b->d_cimg_list.alloc(&b->ctx->pool, b->cimg_list.size())); CK(b->d_flen.alloc(&b->ctx->pool, n));
+        CK(b->d_cimg_list.alloc(&b->ctx->pool, b->cimg_list.size())); CK(b->d_flen.alloc(&b->ctx->pool, nf));
         CK(b->d_E0.alloc(&b->ctx->pool, nc + 1)); CK(b->d_E1.alloc(&b->ctx->pool, nc + 1)); CK(b->d_Ep.alloc(&b->ctx->pool, nc)); CK(b->d_cfirst.alloc(&b->ctx->pool, nc)); CK(b->d_cn.alloc(&b->ctx->pool, nc)); CK(b->d_cpre.alloc(&b->ctx->pool, nc)); CK(b->d_cjmap.alloc(&b->ctx->pool, nc));
         CK(b->d_cstatus.alloc(&b->ctx->pool, nc)); CK(b->d_cnown.alloc(&b->ctx->pool, nc)); CK(b->d_cdcs.alloc(&b->ctx->pool, 3 * nc)); CK(b->d_cpe.alloc(&b->ctx->pool, 3 * nc));
     }
@@ -981,10 +1052,11 @@ extern "C" int JPEGB200_batchUpload(JPEGB200_BATCH *b)
     if (b->contiguous_in) {
         CK(cudaMemcpyAsync(b->d_comp.p, b->datas[0], b->comp_total, cudaMemcpyHostToDevice, st));
     } else {
-        for (int i = 0; i < n; i++)
+        for (int i = 0; i < nf; i++)
             CK(cudaMemcpyAsync(b->d_comp.p + b->comp_off[i], b->datas[i], (size_t)b->sizes[i], cudaMemcpyHostToDevice, st));
     }
-    CK(cudaMemcpyAsync(b->d_descs.p, b->descs.data(), sizeof(JDImageDesc) * n, cudaMemcpyHostToDevice, st));
+    /* the entropy-facing descriptors; view descriptors go up with their output placement in batchDecode */
+    CK(cudaMemcpyAsync(file_descs_dev(b), file_descs(b).data(), sizeof(JDImageDesc) * nf, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(b->d_quant.p, b->quant.data(), sizeof(int32_t) * 192 * n, cudaMemcpyHostToDevice, st));
     if (b->luts.size()) CK(cudaMemcpyAsync(b->d_luts.p, b->luts.data(), b->luts.size() * 2, cudaMemcpyHostToDevice, st));
     if (b->work.size()) CK(cudaMemcpyAsync(b->d_work.p, b->work.data(), b->work.size() * 4, cudaMemcpyHostToDevice, st));
@@ -995,7 +1067,7 @@ extern "C" int JPEGB200_batchUpload(JPEGB200_BATCH *b)
     }
     CK(cudaEventRecord(b->ev[1], st));
     b->uploaded = true;
-    b->counters[JPEGB200_C_H2D_BYTES] = (int64_t)(b->comp_total + sizeof(JDImageDesc) * n + 768 * (size_t)n + b->luts.size() * 2 +
+    b->counters[JPEGB200_C_H2D_BYTES] = (int64_t)(b->comp_total + sizeof(JDImageDesc) * nf + 768 * (size_t)n + b->luts.size() * 2 +
                                                   b->work.size() * 4 + b->cta_lut.size() * 4 + b->seg_img.size() * 4);
     return 1;
 }
@@ -1363,13 +1435,16 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
     CK(cudaMemsetAsync(b->d_counters.p, 0, 32, st));
     if (b->nchunks) CK(cudaMemsetAsync(b->d_blk_hdr.p, 0, (size_t)b->nblk * 8, st)); /* blocks a truncated restart-free scan never reaches stay empty */
 
+    /* prescan, entropy walk, stitch and patch: one entropy-facing descriptor per file (its views share them) */
+    JDImageDesc *const fdev = file_descs_dev(b);
+    const int nf = b->nf;
     CK(cudaEventRecord(b->ev[2], st));
-    jdk_prescan<<<n, 256, 0, st>>>(b->d_comp.p, b->d_descs.p, b->d_seg_start.p);
+    jdk_prescan<<<nf, 256, 0, st>>>(b->d_comp.p, fdev, b->d_seg_start.p);
     launches++;
     CK(cudaEventRecord(b->ev[3], st));
     if (!b->work.empty()) {
         JDEntropyArgs ea;
-        ea.data = b->d_comp.p; ea.imgs = b->d_descs.p; ea.luts = b->d_luts.p; ea.work = b->d_work.p; ea.cta_lut = b->d_cta_lut.p;
+        ea.data = b->d_comp.p; ea.imgs = fdev; ea.luts = b->d_luts.p; ea.work = b->d_work.p; ea.cta_lut = b->d_cta_lut.p;
         ea.seg_img = b->d_seg_img.p; ea.seg_start = b->d_seg_start.p; ea.blk_hdr = b->d_blk_hdr.p; ea.rec = b->d_rec.p;
         ea.seg_jmap = b->d_seg_jmap.p; ea.seg_status = b->d_seg_status.p; ea.seg_nrec = b->d_seg_nrec.p;
         ea.events = b->d_events.p; ea.event_count = b->d_counters.p; ea.event_cap = JD_EVENT_CAP;
@@ -1390,7 +1465,7 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
             CK(b->d_clean.alloc(&b->ctx->pool, b->comp_total + 32 * (size_t)b->nseg + 4096));
             CK(b->d_seg_clen.alloc(&b->ctx->pool, b->nseg ? b->nseg : 1));
             jdk_unstuff_segs<<<(b->nseg * 32u + JD_UNSTUFF_WARPS * 32u - 1u) / (JD_UNSTUFF_WARPS * 32u), JD_UNSTUFF_WARPS * 32, 0, st>>>(
-                b->d_comp.p, b->d_descs.p, b->d_seg_img.p, b->d_seg_start.p, b->nseg, b->d_clean.p, b->d_seg_clen.p);
+                b->d_comp.p, fdev, b->d_seg_img.p, b->d_seg_start.p, b->nseg, b->d_clean.p, b->d_seg_clen.p);
             ea.clean = b->d_clean.p; ea.seg_clen = b->d_seg_clen.p;
         } else {
             ea.clean = nullptr; ea.seg_clen = nullptr;
@@ -1417,7 +1492,7 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
     if (b->nchunks) {
         /* restart-free scans: un-stuff, iterate the chunk entry states to their fix point, then emit */
         JDChunkArgs ca;
-        ca.comp = b->d_comp.p; ca.filt = b->d_filt.p; ca.imgs = b->d_descs.p; ca.luts = b->d_luts.p;
+        ca.comp = b->d_comp.p; ca.filt = b->d_filt.p; ca.imgs = fdev; ca.luts = b->d_luts.p;
         ca.cimg_list = b->d_cimg_list.p; ca.ncimg = (uint32_t)b->cimg_list.size(); ca.flen = b->d_flen.p;
         ca.nchunks = b->nchunks;
         ca.cn = b->d_cn.p; ca.cpre = b->d_cpre.p; ca.cjmap = b->d_cjmap.p; ca.cstatus = b->d_cstatus.p; ca.cnown = b->d_cnown.p;
@@ -1468,9 +1543,9 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         launches += 3;
     }
     CK(cudaEventRecord(b->ev[4], st));
-    jdk_stitch<<<(n + 127) / 128, 128, 0, st>>>(b->d_descs.p, (uint32_t)n, b->d_seg_jmap.p, b->d_seg_status.p, b->d_seg_phase.p, b->d_seg_nrec.p,
+    jdk_stitch<<<(nf + 127) / 128, 128, 0, st>>>(fdev, (uint32_t)nf, b->d_seg_jmap.p, b->d_seg_status.p, b->d_seg_phase.p, b->d_seg_nrec.p,
                                                reinterpret_cast<unsigned long long *>(b->d_counters.p + 4));
-    jdk_patch<<<32, 256, 0, st>>>(b->d_descs.p, b->d_events.p, b->d_counters.p, JD_EVENT_CAP, b->d_seg_phase.p, b->d_blk_hdr.p, b->d_rec.p, b->d_counters.p + 1);
+    jdk_patch<<<32, 256, 0, st>>>(fdev, b->d_events.p, b->d_counters.p, JD_EVENT_CAP, b->d_seg_phase.p, b->d_blk_hdr.p, b->d_rec.p, b->d_counters.p + 1);
     launches += 2;
     CK(cudaEventRecord(b->ev[5], st));
     /* IDCT + colour: one launch per run of images with the same geometry class */
@@ -1478,13 +1553,14 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
     uint8_t *stage_out = b->dither_bits ? b->d_gray.p : b->resize ? b->d_rs.p : pipe_out;
     for (int i0 = 0; i0 < n;) {
         if (b->parse_status[i0] != JPEG_SUCCESS) { i0++; continue; }
-        const JDInfo &f = b->infos[i0];
+        const JDInfo &f = b->infos[file_of(b, i0)];
         int i1 = i0 + 1;
         uint32_t max_mx = f.mcus_x, max_my = f.mcus_y;
-        while (i1 < n && i1 - i0 < 65535 && b->parse_status[i1] == JPEG_SUCCESS && b->infos[i1].subsample == f.subsample &&
-               b->infos[i1].ncomp == f.ncomp && (b->sshift >= 2 || (b->infos[i1].width == f.width && b->infos[i1].height == f.height))) {
-            if ((uint32_t)b->infos[i1].mcus_x > max_mx) max_mx = b->infos[i1].mcus_x;
-            if ((uint32_t)b->infos[i1].mcus_y > max_my) max_my = b->infos[i1].mcus_y;
+        while (i1 < n && i1 - i0 < 65535 && b->parse_status[i1] == JPEG_SUCCESS) {
+            const JDInfo &g = b->infos[file_of(b, i1)];
+            if (g.subsample != f.subsample || g.ncomp != f.ncomp || (b->sshift < 2 && (g.width != f.width || g.height != f.height))) break;
+            if ((uint32_t)g.mcus_x > max_mx) max_mx = g.mcus_x;
+            if ((uint32_t)g.mcus_y > max_my) max_my = g.mcus_y;
             i1++;
         }
         const uint32_t nimg = (uint32_t)(i1 - i0);
@@ -1658,15 +1734,16 @@ extern "C" int JPEGB200_batchDownload(JPEGB200_BATCH *b)
             }
         }
     }
+    /* status and failing MCU: per file (views are judged on the host, jd_view_err_mcu) */
     if (!b->descs_dl) {
-        b->descs_dl = (JDImageDesc *)b->ctx->pinpool.get(sizeof(JDImageDesc) * b->n + 32, &b->descs_dl_bytes);
+        b->descs_dl = (JDImageDesc *)b->ctx->pinpool.get(sizeof(JDImageDesc) * b->nf + 32, &b->descs_dl_bytes);
         if (!b->descs_dl) { snprintf(g_err, sizeof(g_err), "pinned status buffer allocation failed"); return 0; }
-        b->h_counters = (uint32_t *)(b->descs_dl + b->n);
+        b->h_counters = (uint32_t *)(b->descs_dl + b->nf);
     }
-    CK(cudaMemcpyAsync(b->descs_dl, b->d_descs.p, sizeof(JDImageDesc) * b->n, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(b->descs_dl, file_descs_dev(b), sizeof(JDImageDesc) * b->nf, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(b->h_counters, b->d_counters.p, 32, cudaMemcpyDeviceToHost, st));
     b->downloaded = true;
-    bytes += (int64_t)sizeof(JDImageDesc) * b->n + 32;
+    bytes += (int64_t)sizeof(JDImageDesc) * b->nf + 32;
     CK(cudaEventRecord(b->ev[9], st));
     b->counters[JPEGB200_C_D2H_BYTES] = bytes;
     return 1;
@@ -1695,7 +1772,8 @@ extern "C" int JPEGB200_batchWait(JPEGB200_BATCH *b, int32_t *status)
     if (ev_overflow) snprintf(g_err, sizeof(g_err), "%u window-truncation events exceed the event buffer (%u): job rejected", b->h_counters[0], JD_EVENT_CAP);
     for (int i = 0; i < b->n; i++) {
         int st = b->parse_status[i];
-        if (st == JPEG_SUCCESS && b->downloaded && b->descs_dl[i].status != 0) st = JPEG_DECODE_ERROR; /* jpeg.inl:5354 */
+        if (st == JPEG_SUCCESS && b->downloaded && (b->views ? JPEGB200_batchErrMcu(b, i) >= 0 : b->descs_dl[i].status != 0))
+            st = JPEG_DECODE_ERROR; /* jpeg.inl:5354 */
         if (st == JPEG_SUCCESS && ev_overflow) st = JPEG_DECODE_ERROR;
         if (status) status[i] = st;
         if (st != JPEG_SUCCESS) all_ok = 0;
@@ -1723,6 +1801,11 @@ extern "C" int JPEGB200_batchErrMcu(JPEGB200_BATCH *b, int i)
 {
     if (!b || i < 0 || i >= b->n) return -1;
     if (!b->downloaded) return -1;
+    if (b->views) {
+        if (b->parse_status[i] != JPEG_SUCCESS) return -1;
+        const JDImageDesc &fd = b->descs_dl[b->vfile[i]];
+        return jd_view_err_mcu(fd.status, fd.err_mcu, b->descs[i].roi_mcu_end);
+    }
     return b->descs_dl[i].status ? (int)b->descs_dl[i].err_mcu : -1;
 }
 
@@ -1796,7 +1879,26 @@ extern "C" int JPEGB200_decodeBatchTensor(JPEGB200_CTX *ctx, const uint8_t *cons
                                           const int32_t *out_sizes, int filter, const JPEGB200_TensorSpec *spec, void *const *outs,
                                           const int64_t *pitches, const int64_t *plane_strides, int flags, int32_t *status)
 {
+    return JPEGB200_decodeBatchViews(ctx, datas, sizes, n, nullptr, pixel_type, options, rois, orients, out_sizes, filter, spec, outs,
+                                     pitches, plane_strides, flags, status);
+}
+
+extern "C" int JPEGB200_decodeBatchViews(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                         const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                         const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                         const JPEGB200_TensorSpec *spec, void *const *outs, const int64_t *pitches,
+                                         const int64_t *plane_strides, int flags, int32_t *status)
+{
     if (!ctx || n <= 0) return 0;
+    int64_t nv = n;   /* images (views) of the call */
+    if (views) {
+        nv = 0;
+        for (int f = 0; f < n; f++) {
+            if (views[f] < 1) { snprintf(g_err, sizeof(g_err), "views[%d] = %d: every file needs at least one view", f, views[f]); return 0; }
+            nv += views[f];
+        }
+        if (nv > INT32_MAX) { snprintf(g_err, sizeof(g_err), "%lld views: at most %d per call", (long long)nv, INT32_MAX); return 0; }
+    }
     const bool dev_out = (flags & JPEGB200_OUT_DEVICE) != 0;
     if (spec && !dev_out) {
         snprintf(g_err, sizeof(g_err), "tensor output is written to device memory only: call with JPEGB200_OUT_DEVICE");
@@ -1829,74 +1931,70 @@ extern "C" int JPEGB200_decodeBatchTensor(JPEGB200_CTX *ctx, const uint8_t *cons
     if (trace < 0) { const char *e = getenv("JPEGDEC_B200_TRACE"); trace = (e && atoi(e) > 0) ? 1 : 0; }
     auto now_ms = []() { struct timespec ts; clock_gettime(CLOCK_MONOTONIC, &ts); return ts.tv_sec * 1e3 + ts.tv_nsec * 1e-6; };
     const double t_call = trace ? now_ms() : 0.0;
-    for (int i0 = 0; i0 < n && rc;) {
+    for (int i0 = 0, v0 = 0; i0 < n && rc;) {   /* i0: the job's first file, v0: its first view */
         const double t0 = trace ? now_ms() : 0.0;
-        /* how many images the next job takes */
-        int cnt = 0;
-        int64_t cb = 0;
+        /* how many files the next job takes (cnt), with how many views (cv): jobs are cut between files only */
+        int32_t cv = 0, capped = 0;
         const int maxcnt = dev_out ? JD_JOB_MAX_IMAGES : JD_PIPE_IMAGES;
         /* (measured and dropped: ramping the job size up from a small first job and down towards the end of a device-output
          * call was slower than equal jobs; every job pays the full latency of an entropy walk, so fewer, larger jobs win.) */
         const int64_t limit = job_bytes;
-        while (i0 + cnt < n && cnt < maxcnt) {
-            const int64_t sz = sizes[i0 + cnt] > 0 ? sizes[i0 + cnt] : 0;
-            if (cnt > 0 && cb + sz > limit) break;
-            cb += sz; cnt++;
-        }
+        const int32_t *vi = views ? views + i0 : nullptr;
+        int cnt = jd_job_files(n - i0, sizes + i0, vi, maxcnt, limit, nullptr, 0, &cv, &capped);
         auto create = [&](int c) {
-            return JPEGB200_batchCreateTensor(ctx, datas + i0, sizes + i0, c, pixel_type, options, rois ? rois + 4 * (size_t)i0 : nullptr,
-                                              orients ? orients + i0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)i0 : nullptr, filter, spec);
+            return JPEGB200_batchCreateViews(ctx, datas + i0, sizes + i0, c, vi, pixel_type, options, rois ? rois + 4 * (size_t)v0 : nullptr,
+                                             orients ? orients + v0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)v0 : nullptr, filter, spec);
         };
         JPEGB200_BATCH *b = create(cnt);
         if (!b) { rc = 0; break; }
-        if (!dev_out && i0 + cnt < n && cnt == JD_PIPE_IMAGES) {
+        if (!dev_out && capped) {   /* the job stopped at JD_PIPE_IMAGES views with files left */
             int64_t ob = 0;
-            for (int i = 0; i < cnt; i++) { int64_t pb = 0; ob += JPEGB200_batchOutputBytes(b, i, &pb); }
+            for (int i = 0; i < cv; i++) { int64_t pb = 0; ob += JPEGB200_batchOutputBytes(b, i, &pb); }
             if (ob < JD_PIPE_MIN_BYTES) { /* small images: redo with a job big enough to keep the kernels efficient */
-                int64_t per = ob > 0 ? (ob + cnt - 1) / cnt : 1;
+                int64_t per = ob > 0 ? (ob + cv - 1) / cv : 1;
                 int64_t want = (JD_PIPE_MIN_BYTES + per - 1) / per;
-                int cnt2 = (int)(want < (int64_t)(n - i0) ? want : (int64_t)(n - i0));
+                int64_t cnt2 = want < nv - v0 ? want : nv - v0;
                 if (cnt2 > JD_JOB_MAX_IMAGES) cnt2 = JD_JOB_MAX_IMAGES;
-                int64_t cb2 = 0; int c3 = 0;
-                while (c3 < cnt2 && (c3 == 0 || cb2 + sizes[i0 + c3] <= job_bytes)) { cb2 += sizes[i0 + c3] > 0 ? sizes[i0 + c3] : 0; c3++; }
-                cnt2 = c3;
-                if (cnt2 > cnt) {
+                int32_t cv2 = 0, capped2 = 0;
+                const int c3 = jd_job_files(n - i0, sizes + i0, vi, cnt2, job_bytes, nullptr, 0, &cv2, &capped2);
+                if (c3 > cnt) {
                     JPEGB200_batchDestroy(b);
-                    cnt = cnt2;
+                    cnt = c3; cv = cv2;
                     b = create(cnt);
                     if (!b) { rc = 0; break; }
                 }
             }
         }
         if ((b->resize || b->tensor) && cnt > 1 && b->rs_scratch_total + b->tn_stage_total > JD_JOB_RESIZE_SCRATCH) {
-            /* scratch of a job (resize: S + intermediate; tensor: the uint8 staging): at most JD_JOB_RESIZE_SCRATCH, or one image */
-            auto scratch = [&](int c) { return (b->resize ? b->rs_scratch[c] : 0) + (b->tensor ? b->tn_stage[c] : 0); };
-            int c = 0;
-            int64_t sb = 0;
-            while (c < cnt && (c == 0 || sb + scratch(c) <= JD_JOB_RESIZE_SCRATCH)) sb += scratch(c++);
+            /* scratch of a job (resize: S + intermediate; tensor: the uint8 staging): at most JD_JOB_RESIZE_SCRATCH, or one file
+             * with all of its views */
+            std::vector<int64_t> sc(cv);
+            for (int i = 0; i < cv; i++) sc[i] = (b->resize ? b->rs_scratch[i] : 0) + (b->tensor ? b->tn_stage[i] : 0);
+            int32_t cv3 = 0, capped3 = 0;
+            const int c = jd_job_files(cnt, sizes + i0, vi, INT64_MAX, INT64_MAX, sc.data(), JD_JOB_RESIZE_SCRATCH, &cv3, &capped3);
             JPEGB200_batchDestroy(b);
-            cnt = c;
+            cnt = c; cv = cv3;
             b = create(cnt);
             if (!b) { rc = 0; break; }
         }
-        jobs.push_back(b); first.push_back(i0);
-        b->index_base = i0;
+        jobs.push_back(b); first.push_back(v0);
+        b->index_base = v0;
         const double t1 = trace ? now_ms() : 0.0;
         /* a refused pitch fails the call with batchSetOutput's message (nothing of this job is enqueued) */
-        for (int i = 0; i < cnt && rc; i++)
-            rc = spec ? JPEGB200_batchSetOutputTensor(b, i, outs[i0 + i], pitches ? pitches[i0 + i] : 0, plane_strides ? plane_strides[i0 + i] : 0)
-                      : JPEGB200_batchSetOutput(b, i, outs ? outs[i0 + i] : nullptr, pitches ? pitches[i0 + i] : 0);
+        for (int i = 0; i < cv && rc; i++)
+            rc = spec ? JPEGB200_batchSetOutputTensor(b, i, outs[v0 + i], pitches ? pitches[v0 + i] : 0, plane_strides ? plane_strides[v0 + i] : 0)
+                      : JPEGB200_batchSetOutput(b, i, outs ? outs[v0 + i] : nullptr, pitches ? pitches[v0 + i] : 0);
         rc = rc && JPEGB200_batchUpload(b);
         const double t2 = trace ? now_ms() : 0.0;
         rc = rc && JPEGB200_batchDecode(b, flags);
         const double t3 = trace ? now_ms() : 0.0;
         rc = rc && JPEGB200_batchDownload(b);
         const double t4 = trace ? now_ms() : 0.0;
-        i0 += cnt;
+        i0 += cnt; v0 += cv;
         /* bound the device memory of a very large batch: at most `depth` jobs hold buffers at a time */
         while (rc && jobs.size() - retired > depth) retire(retired++);
         if (trace) fprintf(stderr, "[jpegdec_b200] job %zu (%d images) at %.2f ms: create %.2f upload %.2f decode %.2f download %.2f retire %.2f\n",
-                           jobs.size() - 1, cnt, t0 - t_call, t1 - t0, t2 - t1, t3 - t2, t4 - t3, now_ms() - t4);
+                           jobs.size() - 1, cv, t0 - t_call, t1 - t0, t2 - t1, t3 - t2, t4 - t3, now_ms() - t4);
     }
     { const double t5 = trace ? now_ms() : 0.0;
       while (retired < jobs.size()) retire(retired++);

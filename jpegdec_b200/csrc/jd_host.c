@@ -495,6 +495,63 @@ int jd_orient_plan(int width, int height, int subsample, int restart_interval, i
     return 1;
 }
 
+int jd_views_plan(int width, int height, int subsample, int restart_interval, int sshift, int nv, const int32_t *rois,
+                  const uint8_t *ks, const int32_t *out_sizes, JDRoiPlan *plans, int32_t *srects, int32_t *ok)
+{
+    const int mcu_w = (subsample == 0x21 || subsample == 0x22) ? 16 : 8;
+    const int mcu_h = (subsample == 0x12 || subsample == 0x22) ? 16 : 8;
+    const int total = ((width + mcu_w - 1) / mcu_w) * ((height + mcu_h - 1) / mcu_h);
+    const int mps = restart_interval > 0 ? restart_interval : total;
+    const int nseg = (total + mps - 1) / mps;
+    int walk = 0;
+    for (int v = 0; v < nv; v++) {
+        int32_t *sr = srects + 4 * (size_t)v;
+        sr[0] = sr[1] = sr[2] = sr[3] = 0;
+        int good = 1;
+        if (ks) good = jd_orient_plan(width, height, subsample, restart_interval, sshift, ks[v], rois ? rois + 4 * (size_t)v : NULL,
+                                      sr, &plans[v]);
+        else if (rois) {
+            good = jd_roi_plan(width, height, subsample, restart_interval, sshift, rois + 4 * (size_t)v, &plans[v]);
+            sr[0] = rois[4 * (size_t)v]; sr[1] = rois[4 * (size_t)v + 1];
+        }
+        if (good && out_sizes) {
+            const int32_t rw = out_sizes[2 * (size_t)v], rh = out_sizes[2 * (size_t)v + 1];
+            if (rw < 1 || rw > 65535 || rh < 1 || rh > 65535) good = 0;
+        }
+        ok[v] = good;
+        const int w = (ks || rois) ? plans[v].nseg_walk : nseg;
+        if (good && w > walk) walk = w;
+    }
+    return walk;
+}
+
+int32_t jd_view_err_mcu(uint32_t file_status, uint32_t file_err_mcu, uint32_t mcu_end)
+{
+    if (file_status == 0u) return -1;
+    return (mcu_end == 0u || file_err_mcu < mcu_end) ? (int32_t)file_err_mcu : -1;
+}
+
+int jd_job_files(int nf, const int32_t *sizes, const int32_t *views, int64_t max_views, int64_t max_bytes,
+                 const int64_t *scratch, int64_t max_scratch, int32_t *nviews, int32_t *capped)
+{
+    int f = 0;
+    int64_t nv = 0, bytes = 0, sb = 0;
+    *capped = 0;
+    for (; f < nf; f++) {
+        const int64_t v = views ? views[f] : 1;
+        const int64_t sz = sizes[f] > 0 ? sizes[f] : 0;
+        int64_t s = 0;
+        for (int64_t k = 0; scratch && k < v; k++) s += scratch[nv + k];
+        if (f > 0) {
+            if (nv + v > max_views) { *capped = 1; break; }
+            if (bytes + sz > max_bytes || (scratch && sb + s > max_scratch)) break;
+        }
+        nv += v; bytes += sz; sb += s;
+    }
+    *nviews = (int32_t)nv;
+    return f;
+}
+
 /* Resize plan (JDResizePlan): ImagingResampleInner's pass choice and row box, without computing the coefficients */
 int jd_resize_plan(int src_w, int src_h, int out_w, int out_h, int filter, int bytes_per_pixel, JDResizePlan *plan)
 {

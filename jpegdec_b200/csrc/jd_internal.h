@@ -104,6 +104,27 @@ int jd_roi_plan(int width, int height, int subsample, int restart_interval, int 
 int jd_orient_plan(int width, int height, int subsample, int restart_interval, int sshift, int k, const int32_t *rect,
                    int32_t *srect /* x, y, w, h */, JDRoiPlan *plan);
 
+/* The per-image arguments of nv images (or views) of one file, as JPEGB200_batchCreateViews checks them: for view v,
+ * ok[v] = 0 when its rectangle does not lie inside the output, its transform ks[v] is outside 1-8 or its resize target
+ * out_sizes[2v], [2v+1] is outside 1..65535; plans[v] / srects[4v] are jd_orient_plan's (ks given: the resolved EXIF
+ * transforms, 0 = from the file already replaced) or jd_roi_plan's and the rectangle's origin (rois only); rois, ks and
+ * out_sizes may each be NULL.  Returns the restart intervals the file's entropy walk covers: the largest nseg_walk of its
+ * valid views (all nseg intervals for a view of a batch without rois and orients), 0 if no view is valid. */
+int jd_views_plan(int width, int height, int subsample, int restart_interval, int sshift, int nv, const int32_t *rois,
+                  const uint8_t *ks, const int32_t *out_sizes, JDRoiPlan *plans, int32_t *srects, int32_t *ok);
+/* Views (JPEGB200_batchCreateViews): the first undecodable MCU a view reports, -1 for none.  file_status / file_err_mcu:
+ * what jdk_stitch wrote for the view's file, whose walk reaches the deepest view and has no rectangle rule; mcu_end: the
+ * view's JDRoiPlan.mcu_end (0 = no rectangle).  The view reports the file's error when it has no rectangle or the error lies
+ * before mcu_end: the rule jdk_stitch applies to a single-view batch, because a view's walked intervals are a prefix of its
+ * file's and every MCU before its mcu_end lies in that prefix. */
+int32_t jd_view_err_mcu(uint32_t file_status, uint32_t file_err_mcu, uint32_t mcu_end);
+/* How many files, from the first, the next job of JPEGB200_decodeBatchViews takes: always the first, then each next file
+ * while the job keeps at most max_views views, at most max_bytes compressed bytes (a negative size counts 0) and, with
+ * scratch (per view, may be NULL), at most max_scratch scratch bytes.  views NULL = one view per file.  *nviews receives
+ * the job's views; *capped is 1 when the file after the job was left out because of max_views. */
+int jd_job_files(int nf, const int32_t *sizes, const int32_t *views, int64_t max_views, int64_t max_bytes,
+                 const int64_t *scratch, int64_t max_scratch, int32_t *nviews, int32_t *capped);
+
 /* Resize of one image (JPEGB200_batchCreateResized) from the unresized output S (src_w x src_h) to out_w x out_h: the O(1)
  * facts that size its scratch; the coefficients themselves are computed on the GPU (jd_resize.h, jdk_resize_coeffs).
  * A pass runs only along an axis whose size changes (Pillow skips the other).  The horizontal pass reads source rows

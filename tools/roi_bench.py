@@ -25,12 +25,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
-def make_rois(w_img, h_img, n, seed=1000):
+def make_rois(w_img, h_img, n, seed=1000, scale=(0.25, 1.0)):
+    """n seeded RandomResizedCrop rectangles: `scale` is the range of their share of the image's area"""
     rng = np.random.default_rng(seed)
     out = []
     for _ in range(n):
         while True:
-            area = w_img * h_img * rng.uniform(0.25, 1.0)
+            area = w_img * h_img * rng.uniform(*scale)
             ar = np.exp(rng.uniform(np.log(3 / 4), np.log(4 / 3)))
             w, h = int(round(np.sqrt(area * ar))), int(round(np.sqrt(area / ar)))
             if 1 <= w <= w_img and 1 <= h <= h_img:
