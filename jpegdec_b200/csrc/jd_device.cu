@@ -191,7 +191,7 @@ struct JPEGB200_BATCH {
     DevBuf<uint8_t> d_clean;       /* un-stuffed restart segments (jdk_unstuff_segs) */
     DevBuf<uint32_t> d_seg_clen;
     uint64_t rec_total;            /* coefficient records the batch may need (JD_REC_INDEX layout) */
-    DevBuf<uint4> d_dbands;        /* dither: (image, band, list position of the band above, -) per warp */
+    DevBuf<uint4> d_dbands;        /* dither: (image, band, list position of the band above, of band - 255 or ~0) per warp */
     std::vector<uint4> dbands;
     JDImageDesc *descs_dl;             /* descriptors read back (status, err_mcu); pinned, from ctx->pinpool */
     size_t descs_dl_bytes;
@@ -1416,14 +1416,18 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
          * steps after the one above it, so only ~W/113 bands of an image are ever active together) */
         b->dbands.clear();
         {
+            /* .w: the list position of band k - 255 of the same image, which band k >= 256 waits for (jdk_dither), else ~0 */
             uint32_t maxb = 0;
-            std::vector<uint32_t> nb(n, 0), prevpos(n, 0);
+            std::vector<uint32_t> nb(n, 0), prevpos(n, 0), first(n, 0);
             for (int i = 0; i < n; i++) if (b->parse_status[i] == JPEG_SUCCESS) { nb[i] = (b->descs[i].out_h + 31) / 32; if (nb[i] > maxb) maxb = nb[i]; }
+            std::vector<uint32_t> where;                       /* list position of band k of image i at first[i] + k */
+            for (int i = 0; i < n; i++) { first[i] = (uint32_t)where.size(); where.resize(where.size() + nb[i]); }
             for (uint32_t k = 0; k < maxb; k++)
                 for (int i = 0; i < n; i++) {
                     if (k >= nb[i]) continue;
                     const uint32_t pos = (uint32_t)b->dbands.size();
-                    b->dbands.push_back(make_uint4((uint32_t)i, k, prevpos[i], 0u));
+                    where[first[i] + k] = pos;
+                    b->dbands.push_back(make_uint4((uint32_t)i, k, prevpos[i], k >= 256 ? where[first[i] + k - 255] : ~0u));
                     prevpos[i] = pos;
                 }
         }
@@ -2033,7 +2037,13 @@ extern "C" int JPEGB200_lastCallCounters(JPEGB200_CTX *ctx, int64_t *counters)
 /* that wrote it; band b+1 reads 16 entries at a time and asks again until all of them carry    */
 /* band b's number, so value and "ready" arrive in one store and the bands need no counters or  */
 /* fences between them.  Each entry is read by band b+1 before band b+1 overwrites it (64 steps */
-/* later), so one line per image serves all bands, as in the reference.  An image is a chain of  */
+/* later), so one line per image serves all bands, as in the reference -- provided no entry can  */
+/* carry band b's number mod 256 without band b having written it.  Every band is claimed at     */
+/* once, so in an image of more than 256 bands band b+1 may start while the entries still hold    */
+/* band b-256's tag (or, for band 256, the initial line's "band -1"): a band b >= 256 therefore  */
+/* first waits until band b-255 has finished (one flag per band in `progress`, written once with */
+/* a release store at the band's end).  Every entry's last writer is then one of bands           */
+/* b-255 .. b-1, whose numbers mod 256 are distinct.  An image is a chain of                     */
 /* ~(bands x 80 + width) dependent steps whatever the batch size; with fewer than ~500 images    */
 /* that chain, not throughput, sets the kernel's time (DESIGN.md section 4).                     */
 /* ------------------------------------------------------------------------------------ */
@@ -2061,9 +2071,8 @@ jdk_dither(const JDImageDesc *imgs, uint32_t nimg, const uint8_t *gray, const ui
            const uint4 *bands, uint32_t nbands, uint32_t *progress)
 {
     constexpr uint32_t bits = BITS;
-    /* Bands are handed out through a ticket counter (progress[nbands]; the words before it are unused since the bands signal each
-     * other through the error line -- but shrinking this buffer to the one counter measured slower with identical SASS: kept
-     * as it was) in the order in which warps START, not by warp index:
+    /* Bands are handed out through a ticket counter (progress[nbands]; progress[k] is set once band k of the list has
+     * finished, which only bands 256 and later of an image wait for) in the order in which warps START, not by warp index:
      * the list is band-major (band k of every image before band k + 1), so the band a warp waits on was always claimed by a
      * warp that is already running -- forward progress does not depend on the order in which the hardware schedules CTAs. */
     const uint32_t lane = threadIdx.x & 31u;
@@ -2143,6 +2152,16 @@ jdk_dither(const JDImageDesc *imgs, uint32_t nimg, const uint8_t *gray, const ui
             if (live && j >= 0 && j < nchunks) asm volatile("prefetch.global.L1 [%0];" ::"l"(p + 16 * j));
             if (lane == 0 && m < nchunks) asm volatile("prefetch.global.L2 [%0];" ::"l"(S + 16 * m));
         };
+        if (lane == 0 && bd.w != ~0u) {
+            /* band >= 256: wait until band bi - 255 (list position bd.w) has finished before the first read of the line.  It
+             * is ~255 x 80 steps ahead, so this rarely spins. */
+            uint32_t v, ns = 128;
+            for (;;) {
+                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(progress + bd.w) : "memory");
+                if (v) break;
+                __nanosleep(ns); if (ns < 1024u) ns *= 2u;
+            }
+        }
         if (vec) {
             A0 = chunk(-jsh); A1 = chunk(1 - jsh);
             if (lane == 0) {
@@ -2242,5 +2261,8 @@ jdk_dither(const JDImageDesc *imgs, uint32_t nimg, const uint8_t *gray, const ui
                 prefetch_next(m + 1);
             }
         }
+        /* this band is finished: the lane that parked the line (lane 31 in every band but an image's last) publishes it, after
+         * its own stores to the line */
+        if (parks) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(progress + wg), "r"(1u) : "memory");
     }
 }
