@@ -36,6 +36,26 @@ typedef struct JPEGB200_BATCH JPEGB200_BATCH; /* one decode job: n images, one p
 /* batch flags */
 #define JPEGB200_OUT_DEVICE 1   /* output pointers are device pointers (pixels stay in HBM) */
 
+/* Option bit (with the JPEG_* options of JPEGDEC.h; every batch entry point and JPEG_decode take it): decode progressive
+ * (SOF2) files from all of their scans, at every scale, pixel type, rectangle, orientation, resize, tensor spec and view
+ * count.  Image i's output is then what the baseline file B with the same quantised coefficients, quant tables, geometry
+ * and EXIF data decodes to, with B's coefficients exact (no bit-window truncation: a progressive decoder has none) and
+ * the IDCT shortcuts taken from the final coefficients' nonzero positions; at 1/8 scale the DC is the fully refined one.
+ * An AC magnitude of 2048 or more after all refinements is a decode error at its block (the baseline rule).  Baseline
+ * files decode byte for byte as without the bit.  Status: a file that breaks the progression rules (T.81 G.1.1.1) gets
+ * JPEG_DECODE_ERROR; more than 64 scans or more than 2^26 blocks JPEG_UNSUPPORTED_FEATURE; a file whose coefficient plane
+ * (128 bytes per block of device memory) cannot be allocated JPEG_ERROR_MEMORY, and the batch goes on.  A block is
+ * undecodable when it is corrupt or needs bits past its scan's data; with R the lowest MCU row holding a first
+ * undecodable block of any scan, the image gets JPEG_DECODE_ERROR with JPEGB200_batchErrMcu = R x MCUs per row (the
+ * region-of-interest and view rules below apply to that MCU), and every MCU row above R decodes exactly.  Work: one
+ * GPU thread per (file, scan) in waves (jdk_prog_scan, timed as JPEGB200_T_ENTROPY and counted in JPEGB200_C_SEGMENTS),
+ * then jdk_prog_pack writes the baseline walk's block headers and records (JPEGB200_T_STITCH, JPEGB200_C_RECORD_BYTES);
+ * progressive images add nothing to JPEGB200_C_EVENTS.  Dithered types: the error diffusion starts, as for every file,
+ * from the file's own DHT bytes (a reference quirk); they are those of the progressive file, not of B, so the dithered
+ * output equals B's only when B carries the same tables.  Without the bit a progressive file gives the reference's 1/8 DC
+ * thumbnail of its first scan, or JPEG_UNSUPPORTED_FEATURE at other scales. */
+#define JPEGB200_OPT_PROGRESSIVE 0x100
+
 /* stage indices for JPEGB200_batchGetTimings (milliseconds, CUDA events on the batch stream) */
 enum {
     JPEGB200_T_H2D = 0,
@@ -98,7 +118,8 @@ int JPEGB200_digestDevice(JPEGB200_CTX *ctx, const void *const *dev_ptrs, const 
  * other images of the batch still decode.
  * Progressive files are accepted when options has JPEG_SCALE_EIGHTH: like the reference (src/jpeg.inl:4964-4966,
  * JPEGDecodeMCU_P :1819-1884) only the DC coefficients of the first scan are decoded; otherwise that image's status
- * is JPEG_UNSUPPORTED_FEATURE. */
+ * is JPEG_UNSUPPORTED_FEATURE.  With JPEGB200_OPT_PROGRESSIVE in options they are decoded from all of their scans at
+ * every scale instead (see there). */
 JPEGB200_BATCH *JPEGB200_batchCreate(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes,
                                      int n, int pixel_type, int options);
 /* Region-of-interest decode (crop-then-train data loading).  rois: n x {x, y, w, h} in pixels of the OUTPUT image (after
@@ -113,7 +134,8 @@ JPEGB200_BATCH *JPEGB200_batchCreate(JPEGB200_CTX *ctx, const uint8_t *const *da
  *     not a rectangle of the dither).  Every other pixel type, scale and sampling is supported.
  *   - Work: only the MCUs the rectangle touches are transformed and only its pixels are stored; restart intervals that
  *     start below its last MCU row are not walked (JPEGB200_C_SEGMENTS counts the walked ones).  Intervals above it are:
- *     the reference's bit-window phase carries from interval to interval.
+ *     the reference's bit-window phase carries from interval to interval.  (A progressive file decoded with
+ *     JPEGB200_OPT_PROGRESSIVE: each scan stops after the rectangle's last MCU row; with views, after the deepest one's.)
  *   - Status follows the reference's crop decode, which parses every MCU row down to the rectangle's last one and no
  *     further: JPEG_DECODE_ERROR exactly when the full decode's first undecodable MCU lies in an MCU row at or above the
  *     last MCU row the rectangle touches; JPEGB200_batchErrMcu then returns that full-image MCU index.  Otherwise the

@@ -448,7 +448,8 @@ static int decode_common(JPEGIMAGE *p)
 {
     int options = p->iOptions;
     if (!p->pFileData) { p->iError = JPEG_INVALID_PARAMETER; return 0; }
-    if (p->ucMode == 0xc2) options = (p->iOptions |= JPEG_SCALE_EIGHTH); /* progressive: DC-only 1/8 image (jpeg.inl:4964-4966) */
+    /* progressive: DC-only 1/8 image (jpeg.inl:4964-4966), unless decoded from all scans (JPEGB200_OPT_PROGRESSIVE) */
+    if (p->ucMode == 0xc2 && !(options & JPEGB200_OPT_PROGRESSIVE)) options = (p->iOptions |= JPEG_SCALE_EIGHTH);
     if (options & JPEG_EXIF_THUMBNAIL) {
         if (p->iThumbData == 0 || p->iThumbWidth == 0) { p->iError = JPEG_INVALID_PARAMETER; return 0; } /* jpeg.inl:4969 */
     }
@@ -467,7 +468,7 @@ static int decode_common(JPEGIMAGE *p)
     pthread_mutex_lock(ctx_lock);
     const uint8_t *datas[1] = {p->pFileData};
     int32_t sizes[1] = {p->iFileSize};
-    JPEGB200_BATCH *b = JPEGB200_batchCreate(ctx, datas, sizes, 1, pt, (options & 0xFF) | JPEGB200_OPT_PADDED);
+    JPEGB200_BATCH *b = JPEGB200_batchCreate(ctx, datas, sizes, 1, pt, (options & (0xFF | JPEGB200_OPT_PROGRESSIVE)) | JPEGB200_OPT_PADDED);
     if (!b) { pthread_mutex_unlock(ctx_lock); p->iError = JPEG_ERROR_MEMORY; return 0; }
     int32_t w = 0, h = 0, sub = 0, fw = 0, fh = 0, st = 0;
     JPEGB200_batchImageInfo(b, 0, &w, &h, &sub, &fw, &fh, &st);

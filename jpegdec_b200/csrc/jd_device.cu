@@ -9,6 +9,8 @@
 #include <stdlib.h>
 #include <string.h>
 #include <vector>
+#include <algorithm>
+#include <unordered_map>
 #include <time.h>
 #include <new>
 #include <sched.h>
@@ -209,8 +211,23 @@ struct JPEGB200_BATCH {
     DevBuf<uint8_t> d_filt;
     DevBuf<uint32_t> d_cimg_list, d_flen, d_E0, d_E1, d_Ep, d_cfirst, d_cn, d_cpre, d_cjmap, d_cstatus, d_cnown;
     DevBuf<int32_t> d_cdcs, d_cpe;
+    /* progressive files decoded from all their scans (JPEGB200_OPT_PROGRESSIVE, jd_prog.h) */
+    std::vector<JDProgScan> pscans;      /* the walkers: by wave, longest scan first inside a wave */
+    std::vector<uint32_t> pwave_off;     /* wave w: pscans[pwave_off[w] .. pwave_off[w + 1]) */
+    std::vector<JDProgHuff> ptabs;       /* the batch's decoder tables, one per distinct content */
+    std::vector<JDProgFile> pfiles;
+    std::vector<int64_t> pplane;         /* per file: coefficient plane bytes (0: no such plane) */
+    int64_t pplane_total;
+    uint32_t pwalkers;                   /* walkers of files whose plane was allocated (JPEGB200_C_SEGMENTS) */
+    std::vector<DevBuf<int16_t>> d_pplane;
+    std::vector<int16_t *> pplane_ptr;
+    DevBuf<JDProgScan> d_pscans;
+    DevBuf<JDProgHuff> d_ptabs;
+    DevBuf<JDProgFile> d_pfiles;
+    DevBuf<int16_t *> d_pplanes;
+    DevBuf<uint32_t> d_perr;
     uint32_t h_changed;
-    bool chunk_iterate;            /* restart-free scans: iterate the entry states with a host check (fallback mode) */
+    bool chunk_iterate;           /* restart-free scans: iterate the entry states with a host check (fallback mode) */
     int decode_flags;
     cudaEvent_t ev[JPEGB200_NUM_TIMINGS + 2];
     bool have_ev;
@@ -692,19 +709,31 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
     size_t out_total = 0, gray_total = 0;
     std::vector<int32_t> srects(4 * (size_t)nv, 0), vok((size_t)nv, 0);
     std::vector<uint8_t> ks(orients ? (size_t)nv : 0u, 0);
+    const bool prog_scans = (options & JPEGB200_OPT_PROGRESSIVE) != 0;
+    std::vector<JDProgScan> fscans(prog_scans ? JD_PROG_MAX_SCANS : 0);
+    std::vector<JDProgHuff> ftabs(prog_scans ? JD_PROG_MAX_TABS : 0);
+    std::unordered_map<uint64_t, std::vector<uint32_t>> ptab_index;   /* table content hash -> its indices in b->ptabs */
+    b->pplane.assign(n, 0);
+    b->pplane_total = 0;
+    b->pwalkers = 0;
     for (int f = 0, v0 = 0; f < n; v0 += views ? views[f] : 1, f++) {
         const int nvf = views ? views[f] : 1;   /* the file's views (images) are v0 .. v0 + nvf - 1 */
         JDInfo &inf = b->infos[f];
         JDImageDesc &d = file_descs(b)[f];
         memset(&d, 0, sizeof(d));
-        int ok = jd_parse_header(datas[f], sizes[f], 0, &inf);
+        int ok = jd_parse_header_opt(datas[f], sizes[f], 0, &inf, options);
         int st = ok ? JPEG_SUCCESS : inf.error;
         if (ok && (options & JPEG_EXIF_THUMBNAIL)) {
             if (inf.thumb_data == 0 || inf.thumb_w == 0) { ok = 0; st = JPEG_INVALID_PARAMETER; }
-            else { ok = jd_parse_header(datas[f], sizes[f], inf.thumb_data, &inf); if (!ok) st = inf.error; }
+            else { ok = jd_parse_header_opt(datas[f], sizes[f], inf.thumb_data, &inf, options); if (!ok) st = inf.error; }
         }
-        bool prog = false;
-        if (ok && inf.mode == 0xC2) {
+        bool prog = false, full = false;   /* full: a progressive file decoded from all its scans (jd_prog.h) */
+        int nsc = 0, ntb = 0;
+        if (ok && inf.mode == 0xC2 && prog_scans) {
+            nsc = jd_prog_parse(datas[f], sizes[f], (options & JPEG_EXIF_THUMBNAIL) ? inf.thumb_data : 0, &inf, fscans.data(),
+                                ftabs.data(), &ntb);
+            if (nsc <= 0) { ok = 0; st = -nsc; } else full = true;
+        } else if (ok && inf.mode == 0xC2) {
             /* progressive: like the reference, only the DC coefficients of the first scan are decoded and a 1/8-size image
              * is produced (jpeg.inl:4964-4966, JPEGDecodeMCU_P :1819-1884).  That needs a first scan that is the interleaved
              * DC scan of every component (Ss = Se = 0, Ah = 0) -- what every common encoder writes -- and 1/8 scale. */
@@ -712,7 +741,7 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
             if (b->sshift != 3 || inf.p.ncomp_in_scan != inf.ncomp || inf.p.scan_start != 0 || inf.p.scan_end != 0 || (inf.approx >> 4) != 0 ||
                 (inf.approx & 15) > 13) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }
         } else if (ok && inf.mode != 0xC0) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }
-        if (ok && !inf.tables_ok) { ok = 0; st = JPEG_DECODE_ERROR; }           /* jpeg.inl:2166 */
+        if (ok && !full && !inf.tables_ok) { ok = 0; st = JPEG_DECODE_ERROR; }  /* jpeg.inl:2166 */
         if (ok && inf.ncomp == 1 && pixel_type == RGB8888) { ok = 0; st = JPEG_INVALID_PARAMETER; }
         if (ok && (uint64_t)sizes[f] >= (512ull << 20)) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }   /* image-relative record indices are 32-bit */
         const int file_ok = ok;
@@ -737,7 +766,7 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
         }
         const uint32_t total_mcus = ok ? (uint32_t)inf.mcus_x * inf.mcus_y : 0u;
         const uint32_t mps = inf.restart_interval ? (uint32_t)inf.restart_interval : total_mcus;
-        const uint32_t nseg = ok ? (total_mcus + mps - 1) / mps : 0u;
+        const uint32_t nseg = (ok && !full) ? (total_mcus + mps - 1) / mps : 0u;   /* a full progressive file has walkers instead */
         /* no restart markers: one long dependent stream -> chunk-parallel decode */
         const uint32_t nch = (ok && !prog && inf.restart_interval == 0 && nseg == 1 && sizes[f] - inf.scan_offset >= 4096)
                                  ? ((uint32_t)(sizes[f] - inf.scan_offset) + JD_CHUNK_BYTES - 1) / JD_CHUNK_BYTES + 1 : 0u;
@@ -764,9 +793,10 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
                     for (int nn = 0; nn < 64; nn++) qt[cc * 64 + (nn & 7) * 8 + (nn >> 3)] = qn[cc * 64 + nn];
             }
         }
-        /* Huffman LUT set: dedupe on the raw DHT content */
-        const uint64_t h = jd_tables_hash(&inf);
+        /* Huffman LUT set: dedupe on the raw DHT content (a full progressive file uses its scans' own tables instead) */
         uint32_t li = 0;
+        if (!full) {
+        const uint64_t h = jd_tables_hash(&inf);
         for (; li < lut_hash.size(); li++) if (lut_hash[li] == h && jd_tables_equal(&inf, &b->infos[lut_owner[li]])) break;
         const bool shared = ctx->has_shared && ctx->shared_hash == h && ctx->shared_hash2 == jd_tables_hash2(&inf);
         if (li == lut_hash.size()) {
@@ -776,6 +806,7 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
             else jd_build_lut(&inf, &b->luts[(size_t)li * JD_LUT_ENTRIES]);
         }
         if (shared) ctx->shared_hits++;
+        }
         d.scan_off = (uint32_t)(b->comp_off[f] + inf.scan_offset);
         d.scan_end = (uint32_t)(b->comp_off[f] + sizes[f]);
         d.width = (uint16_t)inf.width; d.height = (uint16_t)inf.height;
@@ -783,7 +814,7 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
         d.subsample = (uint8_t)inf.subsample; d.ncomp = (uint8_t)inf.ncomp; d.bpm = (uint8_t)inf.bpm; d.tsel = (uint8_t)inf.tsel;
         d.mcus_per_seg = mps;
         d.nseg = nseg;
-        d.nseg_walk = b->roi ? walk : d.nseg;
+        d.nseg_walk = full ? 0u : b->roi ? walk : d.nseg;   /* a full progressive file has no restart segments to walk */
         d.chunk_base = 0; d.nch = 0;
         d.prog = prog ? (1u | ((uint32_t)(inf.approx & 15) << 8)) : 0u;
         if (nch) {
@@ -799,7 +830,41 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
         /* coefficient records: image-relative indices (jd_core.h JD_REC_INDEX), one slot per restart segment and per chunk */
         d.comp_off = (uint32_t)b->comp_off[f];
         d.rec_base = rec_total;
-        rec_total += (uint64_t)JD_REC_PER_BYTE * (uint64_t)(((size_t)sizes[f] + 15) & ~(size_t)15) + (uint64_t)JD_REC_SLOT_SLACK * (d.nseg + d.nch + 1u);
+        if (full) {
+            /* walkers down to the deepest MCU row a valid view needs; records sized by jd_prog_rec_cap */
+            uint32_t rows = (uint32_t)inf.mcus_y;
+            if (b->roi) {
+                rows = 0;
+                for (int i = v0; i < v0 + nvf; i++) if (vok[i] && (uint32_t)b->plans[i].mcu_y1 + 1u > rows) rows = (uint32_t)b->plans[i].mcu_y1 + 1u;
+            }
+            const uint64_t cap = jd_prog_rec_cap((uint64_t)sizes[f], (uint32_t)nsc);
+            /* whole 16-byte chunks: the entropy walk of the next image stores its records as aligned 16-byte chunks */
+            rec_total += (cap + 15u) & ~(uint64_t)7;
+            b->pfiles.push_back(JDProgFile{cap, (uint32_t)f, rows});
+            b->pplane[f] = (int64_t)total_mcus * inf.bpm * 128;
+            b->pplane_total += b->pplane[f];
+            for (int k = 0; k < nsc; k++) {
+                JDProgScan s = fscans[k];
+                s.start += (uint32_t)b->comp_off[f]; s.end += (uint32_t)b->comp_off[f];
+                s.img = (uint32_t)f;
+                s.row_limit = rows;
+                const int ntab = (s.ss == 0 && s.ah != 0) ? 0 : s.ncs;   /* DC refinements read raw bits */
+                for (int i = 0; i < ntab; i++) {
+                    /* the batch's table list: dedupe on content */
+                    const JDProgHuff &t = ftabs[s.tab[i]];
+                    uint64_t th = 1469598103934665603ull;
+                    for (size_t q = 0; q < sizeof(t); q++) th = (th ^ ((const uint8_t *)&t)[q]) * 1099511628211ull;
+                    std::vector<uint32_t> &same = ptab_index[th];
+                    size_t q = 0;
+                    while (q < same.size() && memcmp(&b->ptabs[same[q]], &t, sizeof(t)) != 0) q++;
+                    if (q == same.size()) { same.push_back((uint32_t)b->ptabs.size()); b->ptabs.push_back(t); }
+                    s.tab[i] = same[q];
+                }
+                b->pscans.push_back(s);
+            }
+        } else {
+            rec_total += (uint64_t)JD_REC_PER_BYTE * (uint64_t)(((size_t)sizes[f] + 15) & ~(size_t)15) + (uint64_t)JD_REC_SLOT_SLACK * (d.nseg + d.nch + 1u);
+        }
 
         /* the views: the file's descriptor (its walk, blocks and records) with each view's rectangle, orientation and output.
          * The file's own descriptor keeps roi_mcu_end = 0: jdk_stitch reports its first error, jd_view_err_mcu judges it
@@ -868,6 +933,15 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
     }
     b->nseg = seg; b->nblk = blk; b->nlut = (uint32_t)lut_hash.size();
     b->rec_total = rec_total;
+    if (!b->pscans.empty()) {
+        /* one launch per wave; inside a wave the longest scans start first */
+        std::stable_sort(b->pscans.begin(), b->pscans.end(), [](const JDProgScan &x, const JDProgScan &y) {
+            return x.wave != y.wave ? x.wave < y.wave : (x.end - x.start) > (y.end - y.start);
+        });
+        for (size_t k = 0; k < b->pscans.size(); k++)
+            while (b->pwave_off.size() <= b->pscans[k].wave) b->pwave_off.push_back((uint32_t)k);
+        b->pwave_off.push_back((uint32_t)b->pscans.size());
+    }
     if ((uint64_t)b->comp_total + 32ull * seg + 4096ull >= (1ull << 32)) {
         snprintf(g_err, sizeof(g_err), "batch too large (%zu compressed bytes in %u restart segments)", b->comp_total, seg);
         delete b;
@@ -909,6 +983,8 @@ extern "C" void JPEGB200_batchDestroy(JPEGB200_BATCH *b)
     b->d_work.release(); b->d_cta_lut.release(); b->d_seg_img.release(); b->d_seg_start.release();
     b->d_seg_jmap.release(); b->d_seg_status.release(); b->d_seg_nrec.release(); b->d_seg_phase.release();
     b->d_counters.release(); b->d_blk_hdr.release(); b->d_events.release();
+    for (auto &pl : b->d_pplane) pl.release();
+    b->d_pscans.release(); b->d_ptabs.release(); b->d_pfiles.release(); b->d_pplanes.release(); b->d_perr.release();
     b->d_rs.release(); b->d_rs_coef.release(); b->d_rs_desc.release();
     b->d_tn.release(); b->d_tn_tab.release(); b->d_tn_desc.release();
     if (b->stream && b->have_ev) {   /* back to the context for the next job */
@@ -1065,10 +1141,22 @@ extern "C" int JPEGB200_batchUpload(JPEGB200_BATCH *b)
     if (b->nchunks) {
         CK(cudaMemcpyAsync(b->d_cimg_list.p, b->cimg_list.data(), b->cimg_list.size() * 4, cudaMemcpyHostToDevice, st));
     }
+    size_t prog_bytes = 0;
+    if (!b->pfiles.empty()) {
+        CK(b->d_pscans.alloc(&b->ctx->pool, b->pscans.size()));
+        CK(b->d_ptabs.alloc(&b->ctx->pool, b->ptabs.size() ? b->ptabs.size() : 1));
+        CK(b->d_pfiles.alloc(&b->ctx->pool, b->pfiles.size()));
+        CK(b->d_pplanes.alloc(&b->ctx->pool, nf));
+        CK(b->d_perr.alloc(&b->ctx->pool, nf));
+        CK(cudaMemcpyAsync(b->d_pscans.p, b->pscans.data(), b->pscans.size() * sizeof(JDProgScan), cudaMemcpyHostToDevice, st));
+        if (b->ptabs.size()) CK(cudaMemcpyAsync(b->d_ptabs.p, b->ptabs.data(), b->ptabs.size() * sizeof(JDProgHuff), cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(b->d_pfiles.p, b->pfiles.data(), b->pfiles.size() * sizeof(JDProgFile), cudaMemcpyHostToDevice, st));
+        prog_bytes = b->pscans.size() * sizeof(JDProgScan) + b->ptabs.size() * sizeof(JDProgHuff) + b->pfiles.size() * sizeof(JDProgFile);
+    }
     CK(cudaEventRecord(b->ev[1], st));
     b->uploaded = true;
     b->counters[JPEGB200_C_H2D_BYTES] = (int64_t)(b->comp_total + sizeof(JDImageDesc) * nf + 768 * (size_t)n + b->luts.size() * 2 +
-                                                  b->work.size() * 4 + b->cta_lut.size() * 4 + b->seg_img.size() * 4);
+                                                  b->work.size() * 4 + b->cta_lut.size() * 4 + b->seg_img.size() * 4 + prog_bytes);
     return 1;
 }
 
@@ -1257,6 +1345,26 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         return 0;
     }
     int launches = 0;
+    if (!b->pfiles.empty()) {
+        /* coefficient planes of the progressive files, one pooled buffer each: a file whose plane the device cannot hold
+         * gets JPEG_ERROR_MEMORY (all of its views) and the others decode */
+        b->d_pplane.resize(b->nf);
+        b->pplane_ptr.assign(b->nf, nullptr);
+        b->pwalkers = 0;
+        for (const JDProgFile &pf : b->pfiles) {
+            const int f = (int)pf.file;
+            if (b->d_pplane[f].alloc(&b->ctx->pool, (size_t)b->pplane[f] / 2) != cudaSuccess) {
+                cudaGetLastError();
+                for (int i = 0; i < n; i++) if (file_of(b, i) == f) b->parse_status[i] = JPEG_ERROR_MEMORY;
+                continue;
+            }
+            b->pplane_ptr[f] = b->d_pplane[f].p;
+            CK(cudaMemsetAsync(b->pplane_ptr[f], 0, (size_t)b->pplane[f], st));
+        }
+        for (const JDProgScan &s : b->pscans) if (b->pplane_ptr[s.img]) b->pwalkers++;
+        CK(cudaMemcpyAsync(b->d_pplanes.p, b->pplane_ptr.data(), sizeof(int16_t *) * b->nf, cudaMemcpyHostToDevice, st));
+        CK(cudaMemsetAsync(b->d_perr.p, 0xFF, sizeof(uint32_t) * b->nf, st));
+    }
     /* output placement */
     bool user_dev_out = false;
     if (b->out_device && !b->arena_owned) {
@@ -1546,11 +1654,28 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         jdk_chunk_stitch<<<gi, 128, 0, st>>>(ca);
         launches += 3;
     }
+    /* progressive files: one launch per wave of scan walkers */
+    for (size_t w = 0; w + 1 < b->pwave_off.size(); w++) {
+        const uint32_t o = b->pwave_off[w], cnt = b->pwave_off[w + 1] - o;
+        if (cnt == 0) continue;
+        jdk_prog_scan<<<(cnt + 63) / 64, 64, 0, st>>>(b->d_pscans.p + o, cnt, b->d_comp.p, b->d_ptabs.p, b->d_pplanes.p, b->d_perr.p);
+        launches++;
+    }
     CK(cudaEventRecord(b->ev[4], st));
     jdk_stitch<<<(nf + 127) / 128, 128, 0, st>>>(fdev, (uint32_t)nf, b->d_seg_jmap.p, b->d_seg_status.p, b->d_seg_phase.p, b->d_seg_nrec.p,
                                                reinterpret_cast<unsigned long long *>(b->d_counters.p + 4));
     jdk_patch<<<32, 256, 0, st>>>(fdev, b->d_events.p, b->d_counters.p, JD_EVENT_CAP, b->d_seg_phase.p, b->d_blk_hdr.p, b->d_rec.p, b->d_counters.p + 1);
     launches += 2;
+    if (!b->pfiles.empty()) {
+        /* after jdk_stitch, which gives a file without restart segments status 0: the pack writes the real one */
+        JDProgPackArgs pa;
+        pa.imgs = fdev; pa.files = b->d_pfiles.p; pa.planes = b->d_pplanes.p; pa.err_row = b->d_perr.p;
+        pa.blk_hdr = b->d_blk_hdr.p; pa.rec = b->d_rec.p;
+        pa.limit = b->sshift == 3 ? 1u : b->sshift == 2 ? 5u : 64u;
+        pa.rec_count = reinterpret_cast<unsigned long long *>(b->d_counters.p + 4);
+        jdk_prog_pack<<<(unsigned)b->pfiles.size(), 256, 0, st>>>(pa);
+        launches++;
+    }
     CK(cudaEventRecord(b->ev[5], st));
     /* IDCT + colour: one launch per run of images with the same geometry class */
     const bool half = b->sshift == 1;
@@ -1693,7 +1818,7 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
     CK(cudaEventRecord(b->ev[7], st));
     CK(cudaGetLastError());
     b->counters[JPEGB200_C_LAUNCHES] = launches;
-    b->counters[JPEGB200_C_SEGMENTS] = b->nseg_walk;
+    b->counters[JPEGB200_C_SEGMENTS] = b->nseg_walk + b->pwalkers;
     b->counters[JPEGB200_C_BLOCKS] = (int64_t)b->nblk;
     b->counters[JPEGB200_C_COMPRESSED_BYTES] = (int64_t)b->comp_total;
     int64_t ob = 0;
@@ -1969,11 +2094,13 @@ extern "C" int JPEGB200_decodeBatchViews(JPEGB200_CTX *ctx, const uint8_t *const
                 }
             }
         }
-        if ((b->resize || b->tensor) && cnt > 1 && b->rs_scratch_total + b->tn_stage_total > JD_JOB_RESIZE_SCRATCH) {
-            /* scratch of a job (resize: S + intermediate; tensor: the uint8 staging): at most JD_JOB_RESIZE_SCRATCH, or one file
-             * with all of its views */
+        if ((b->resize || b->tensor || b->pplane_total) && cnt > 1 &&
+            b->rs_scratch_total + b->tn_stage_total + b->pplane_total > JD_JOB_RESIZE_SCRATCH) {
+            /* scratch of a job (resize: S + intermediate; tensor: the uint8 staging; progressive files: the coefficient plane,
+             * counted on the file's first view): at most JD_JOB_RESIZE_SCRATCH, or one file with all of its views */
             std::vector<int64_t> sc(cv);
             for (int i = 0; i < cv; i++) sc[i] = (b->resize ? b->rs_scratch[i] : 0) + (b->tensor ? b->tn_stage[i] : 0);
+            for (int i = 0; i < cv; i++) if (i == 0 || file_of(b, i) != file_of(b, i - 1)) sc[i] += b->pplane[file_of(b, i)];
             int32_t cv3 = 0, capped3 = 0;
             const int c = jd_job_files(cnt, sizes + i0, vi, INT64_MAX, INT64_MAX, sc.data(), JD_JOB_RESIZE_SCRATCH, &cv3, &capped3);
             JPEGB200_batchDestroy(b);

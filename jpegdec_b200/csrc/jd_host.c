@@ -81,7 +81,20 @@ static int parse_dht(const uint8_t *p, int len, int avail, JDInfo *info)
 
 static int fail(JDInfo *info, int code) { info->error = code; return 0; }
 
+static int parse_header(const uint8_t *data, int size, int start, JDInfo *info, int prog_tables);
+
 int jd_parse_header(const uint8_t *data, int size, int start, JDInfo *info)
+{
+    return parse_header(data, size, start, info, 0);
+}
+
+int jd_parse_header_opt(const uint8_t *data, int size, int start, JDInfo *info, int options)
+{
+    return parse_header(data, size, start, info, (options & JPEGB200_OPT_PROGRESSIVE) != 0);
+}
+
+/* prog_tables: a progressive file's tables are checked by jd_prog_parse, not against the reference's LUT classes */
+static int parse_header(const uint8_t *data, int size, int start, JDInfo *info, int prog_tables)
 {
     const uint8_t *s = data;
     if (start == 0) {
@@ -214,7 +227,7 @@ int jd_parse_header(const uint8_t *data, int size, int start, JDInfo *info)
     }
     info->scan_offset = off;
     info->p.scan_offset = off;
-    if (!jd_check_huffman(info)) return fail(info, JPEG_UNSUPPORTED_FEATURE);
+    if (!(prog_tables && info->mode == 0xC2) && !jd_check_huffman(info)) return fail(info, JPEG_UNSUPPORTED_FEATURE);
 
     /* geometry (reference DecodeJPEG :5008-5049).  Deviation: sampling factors the reference
      * does not know end in a division by zero there (:5062); we refuse them at open. */
@@ -721,4 +734,164 @@ int jd_check_tensor_output(int index, int elt, int64_t row_bytes, int64_t rows, 
         return 0;
     }
     return 1;
+}
+
+/* ---- progressive files decoded from all their scans (JPEGB200_OPT_PROGRESSIVE) ---- */
+
+/* Canonical decoder of one DHT table (T.81 C.2, F.2.2.3).  Returns 0 for counts that overflow the code space. */
+static int prog_build_table(const uint8_t *bits, const uint8_t *vals, JDProgHuff *h)
+{
+    memset(h, 0, sizeof(*h));
+    unsigned code = 0;
+    int k = 0;
+    h->maxcode[0] = -1;
+    for (int l = 1; l <= 16; l++) {
+        const int cnt = bits[l - 1];
+        h->maxcode[l] = -1;
+        h->valoff[l] = k - (int)code;
+        for (int i = 0; i < cnt; i++, code++, k++) {
+            if (code >= (1u << l)) return 0;
+            if (l <= 8) {
+                const unsigned first = code << (8 - l), rep = 1u << (8 - l);
+                for (unsigned j = 0; j < rep; j++) h->look[first + j] = (uint16_t)((l << 8) | vals[k]);
+            }
+        }
+        if (cnt) h->maxcode[l] = (int32_t)code - 1;
+        code <<= 1;
+    }
+    memcpy(h->val, vals, (size_t)k);
+    return 1;
+}
+
+uint64_t jd_prog_rec_cap(uint64_t entropy_bytes, uint32_t nscans)
+{
+    const uint64_t c = 8u * entropy_bytes + 126u * (uint64_t)nscans + 8u;
+    return c < 0xFFFFFFFFull ? c : 0xFFFFFFFFull;
+}
+
+int jd_prog_parse(const uint8_t *data, int size, int start, const JDInfo *info, JDProgScan *scans, JDProgHuff *tabs, int *ntabs)
+{
+    struct { uint8_t bits[16], vals[256]; int defined, built; } defs[2][4];
+    int8_t lastal[3][64];   /* per component and zigzag position: Al of the last scan that sent it, -1 = none yet */
+    uint8_t comp_id[3] = {0, 0, 0}, samp[3] = {0, 0, 0};
+    int nsc = 0, nt = 0, restart = 0, have_sof = 0;
+    *ntabs = 0;
+    memset(defs, 0, sizeof(defs));
+    memset(lastal, -1, sizeof(lastal));
+    if ((uint64_t)info->mcus_x * (uint64_t)info->mcus_y * (uint64_t)info->bpm > JD_PROG_MAX_BLOCKS) return -JPEG_UNSUPPORTED_FEATURE;
+    int off = start + 2;
+    while (off + 1 < size) {
+        if (data[off] != 0xFF) { off++; continue; }
+        const unsigned m = data[off + 1];
+        if (m == 0xFF) { off++; continue; }                       /* fill byte */
+        if (m == 0xD9) break;                                      /* EOI */
+        if (m == 0x00 || m == 0x01 || (m >= 0xD0 && m <= 0xD8)) { off += 2; continue; }
+        if (off + 4 > size) break;                                 /* the file ends: scans never sent stay zero */
+        const int len = (int)be16(data + off + 2), seg = off + 4, segend = off + 2 + len;
+        if (len < 2 || segend > size) {
+            if (nsc) break;
+            return -JPEG_DECODE_ERROR;
+        }
+        if (m == 0xC2 && !have_sof) {
+            if (len < 8 + 3 * info->ncomp) return -JPEG_DECODE_ERROR;
+            for (int c = 0; c < info->ncomp; c++) { comp_id[c] = data[seg + 6 + 3 * c]; samp[c] = data[seg + 7 + 3 * c]; }
+            have_sof = 1;
+            /* the MCU layout of this library: chroma blocks are 1 x 1 per MCU */
+            if (info->ncomp == 3 && (samp[1] != 0x11 || samp[2] != 0x11)) return -JPEG_UNSUPPORTED_FEATURE;
+        } else if (m == 0xDD) {
+            if (len == 4) restart = (int)be16(data + seg);
+        } else if (m == 0xC4) {
+            for (int p = seg; p < segend;) {
+                if (p + 17 > segend) return -JPEG_DECODE_ERROR;
+                const unsigned tc = data[p] >> 4, th = data[p] & 15u;
+                int total = 0;
+                for (int i = 0; i < 16; i++) total += data[p + 1 + i];
+                if (tc > 1 || th > 3 || total > 256 || p + 17 + total > segend) return -JPEG_DECODE_ERROR;
+                memcpy(defs[tc][th].bits, data + p + 1, 16);
+                memcpy(defs[tc][th].vals, data + p + 17, (size_t)total);
+                defs[tc][th].defined = 1;
+                defs[tc][th].built = -1;
+                p += 17 + total;
+            }
+        } else if (m == 0xDA) {
+            if (!have_sof) return -JPEG_DECODE_ERROR;
+            if (nsc == JD_PROG_MAX_SCANS) return -JPEG_UNSUPPORTED_FEATURE;
+            const int ncs = len >= 3 ? data[seg] : 0;
+            if (ncs < 1 || ncs > info->ncomp || len != 6 + 2 * ncs) return -JPEG_DECODE_ERROR;
+            JDProgScan *s = &scans[nsc];
+            memset(s, 0, sizeof(*s));
+            int prev = -1, tsel[3];
+            for (int i = 0; i < ncs; i++) {
+                const unsigned cid = data[seg + 1 + 2 * i], tt = data[seg + 2 + 2 * i];
+                int c = 0;
+                while (c < info->ncomp && comp_id[c] != cid) c++;
+                if (c == info->ncomp || c <= prev) return -JPEG_DECODE_ERROR;   /* unknown, repeated or out of frame order */
+                prev = c;
+                s->comp[i] = (uint8_t)c;
+                tsel[i] = (int)tt;
+            }
+            const int p = seg + 1 + 2 * ncs;
+            const int ss = data[p], se = data[p + 1], ah = data[p + 2] >> 4, al = data[p + 2] & 15;
+            /* T.81 G.1.1.1 and the checks libjpeg makes */
+            if (se > 63 || ss > se || (ss == 0 && se != 0) || (ss > 0 && ncs != 1)) return -JPEG_DECODE_ERROR;
+            if (al > 13 || (ah != 0 && al != ah - 1)) return -JPEG_DECODE_ERROR;
+            for (int i = 0; i < ncs; i++) {
+                const int c = s->comp[i];
+                if (ss > 0 && lastal[c][0] < 0) return -JPEG_DECODE_ERROR;          /* AC before the component's first DC scan */
+                for (int k = ss; k <= se; k++)
+                    if (ah == 0 ? lastal[c][k] >= 0 : lastal[c][k] != ah) return -JPEG_DECODE_ERROR;
+            }
+            for (int i = 0; i < ncs; i++)
+                for (int k = ss; k <= se; k++) lastal[s->comp[i]][k] = (int8_t)al;
+            /* decoders: DC first scans use each component's DC table, AC scans the component's AC table; DC
+             * refinements read raw bits only */
+            if (!(ss == 0 && ah != 0)) {
+                for (int i = 0; i < ncs; i++) {
+                    const int tc = ss > 0, th = ss > 0 ? (tsel[i] & 15) : (tsel[i] >> 4);
+                    if (th > 3 || !defs[tc][th].defined) return -JPEG_DECODE_ERROR;
+                    if (defs[tc][th].built < 0) {
+                        if (nt == JD_PROG_MAX_TABS) return -JPEG_UNSUPPORTED_FEATURE;
+                        if (!prog_build_table(defs[tc][th].bits, defs[tc][th].vals, &tabs[nt])) return -JPEG_DECODE_ERROR;
+                        defs[tc][th].built = nt++;
+                    }
+                    s->tab[i] = (uint32_t)defs[tc][th].built;
+                }
+            }
+            s->ncs = (uint8_t)ncs; s->ss = (uint8_t)ss; s->se = (uint8_t)se; s->ah = (uint8_t)ah; s->al = (uint8_t)al;
+            s->restart = (uint16_t)restart;
+            s->width = (uint16_t)info->width; s->height = (uint16_t)info->height;
+            s->mcus_x = (uint16_t)info->mcus_x; s->mcus_y = (uint16_t)info->mcus_y;
+            s->row_limit = (uint32_t)info->mcus_y;
+            s->subsample = (uint8_t)info->subsample; s->ncomp = (uint8_t)info->ncomp; s->bpm = (uint8_t)info->bpm;
+            /* entropy bytes: up to the next marker that is not RSTn (FF00 is a stuffed FF) */
+            int e = segend;
+            while (e + 1 < size) {
+                if (data[e] == 0xFF) {
+                    const unsigned x = data[e + 1];
+                    if (x == 0x00 || (x >= 0xD0 && x <= 0xD7)) { e += 2; continue; }
+                    break;
+                }
+                e++;
+            }
+            if (e + 1 >= size) e = size;
+            s->start = (uint32_t)segend;
+            s->end = (uint32_t)e;
+            /* wave: after every earlier scan that shares a component and overlaps its coefficient range */
+            int w = 0;
+            for (int t = 0; t < nsc; t++) {
+                int share = 0;
+                for (int i = 0; i < ncs; i++)
+                    for (int j = 0; j < scans[t].ncs; j++) share |= scans[t].comp[j] == s->comp[i];
+                if (share && scans[t].ss <= se && ss <= scans[t].se && scans[t].wave + 1 > w) w = scans[t].wave + 1;
+            }
+            s->wave = (uint8_t)w;
+            nsc++;
+            off = e;
+            continue;
+        }
+        off = segend;
+    }
+    if (nsc == 0) return -JPEG_DECODE_ERROR;
+    *ntabs = nt;
+    return nsc;
 }

@@ -37,6 +37,9 @@ typedef struct {
 
 /* jd_host.c */
 int jd_parse_header(const uint8_t *data, int size, int start_offset, JDInfo *info);
+/* The same for a batch created with `options`: with JPEGB200_OPT_PROGRESSIVE a progressive file's Huffman tables are not
+ * held to the reference's LUT classes (its scans are decoded with jd_prog.h's own tables). */
+int jd_parse_header_opt(const uint8_t *data, int size, int start_offset, JDInfo *info, int options);
 int jd_check_huffman(const JDInfo *info);                      /* 1 ok, 0 -> JPEG_UNSUPPORTED_FEATURE */
 void jd_build_lut(const JDInfo *info, uint16_t *lut /* JD_LUT_ENTRIES_H */);
 void jd_build_quant(const JDInfo *info, int16_t *q /* [3][64] natural order, per component */);
@@ -149,6 +152,44 @@ int jd_resize_plan(int src_w, int src_h, int out_w, int out_h, int filter, int b
  * the records of its first ones.  Files under 512 MiB reach it only through the 128 spare records per restart interval.
  * (jd_device.cu; declared here so that the CPU tests can call it.) */
 uint64_t jd_rec_extent(uint64_t size, uint32_t scan_offset, uint32_t nseg, uint32_t nch);
+
+/* ---- progressive files decoded from all their scans (JPEGB200_OPT_PROGRESSIVE, jd_prog.h, DESIGN.md 4.3.1) ---- */
+#define JD_PROG_MAX_SCANS 64
+#define JD_PROG_MAX_TABS (3 * JD_PROG_MAX_SCANS)
+#define JD_PROG_MAX_BLOCKS (1u << 26)   /* plane indices (block * 64 + k) stay 32-bit */
+/* Canonical Huffman decoder of one table as a scan uses it: any valid code of 1-16 bits. */
+typedef struct {
+    uint16_t look[256];     /* next 8 bits -> code length << 8 | symbol; 0 = a longer code (or no code) */
+    int32_t maxcode[17];    /* [l]: largest code of length l, -1 = none */
+    int32_t valoff[17];     /* [l]: the symbol of code c of length l is val[c + valoff[l]] */
+    uint8_t val[256];
+} JDProgHuff;
+/* One scan of a progressive file.  Blocks of the plane are numbered like the baseline walk's block headers: MCU by MCU,
+ * luma blocks in raster order inside the MCU, then Cb, Cr. */
+typedef struct {
+    uint32_t start, end;    /* entropy bytes [start, end) up to the next marker that is not RSTn: file offsets from
+                             * jd_prog_parse, batch-buffer offsets on the device */
+    uint32_t img;           /* file index in the batch */
+    uint32_t row_limit;     /* the walk stops before this MCU row (regions of interest and views) */
+    uint16_t width, height, mcus_x, mcus_y;
+    uint16_t restart;       /* restart interval of this scan (MCUs, or blocks of a one-component scan), 0 = none */
+    uint8_t subsample, ncomp, bpm;
+    uint8_t ncs, ss, se, ah, al, wave;
+    uint8_t comp[3];        /* frame component index of each scan component */
+    uint32_t tab[3];        /* decoder of each scan component (DC or AC table): index into the table list */
+} JDProgScan;
+/* Scan list of a progressive file whose header jd_parse_header_opt accepted (start: where that parse started).  Fills
+ * scans (JD_PROG_MAX_SCANS) and tabs (JD_PROG_MAX_TABS, *ntabs used; scans[].tab index them), gives each scan its wave
+ * (a scan comes after every earlier scan of one of its components whose coefficient range overlaps its own) and returns
+ * the number of scans, or minus a JPEG_* status: JPEG_DECODE_ERROR for a file that breaks the progression rules of T.81
+ * G.1.1.1, JPEG_UNSUPPORTED_FEATURE for more than JD_PROG_MAX_SCANS scans, more than JD_PROG_MAX_BLOCKS blocks or a
+ * chroma sampling other than 1x1. */
+int jd_prog_parse(const uint8_t *data, int size, int start, const JDInfo *info, JDProgScan *scans, JDProgHuff *tabs, int *ntabs);
+/* Coefficient records a progressive image may need (the pack refuses more): every stored coefficient costs at least two
+ * bits of some scan (a code and a magnitude or sign bit) and at most two records, so 8 per entropy byte, plus the 126 that
+ * the one block where a failing scan stops may hold without paying for them (zero bits past its data), per scan; at most
+ * 2^32 - 1 (block headers hold 32-bit record indices). */
+uint64_t jd_prog_rec_cap(uint64_t entropy_bytes, uint32_t nscans);
 
 /* A caller's destination for image `index` (only named in the message): row_bytes is the tight pitch
  * (JPEGB200_batchOutputBytes), pitch <= 0 means tight.  device != 0: `out` is written by the kernels.  Returns 1, or 0 with

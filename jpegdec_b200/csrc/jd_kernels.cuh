@@ -2190,3 +2190,100 @@ __global__ void __launch_bounds__(JD_TN_THREADS) jdk_tensor(const JDTensorDesc *
         }
     }
 }
+
+/* ------------------------------------------------------------------------------------ */
+/* progressive files decoded from all their scans (JPEGB200_OPT_PROGRESSIVE, jd_prog.h)    */
+/* ------------------------------------------------------------------------------------ */
+#include "jd_prog.h"
+
+/* one progressive file of a batch, as jdk_prog_pack sees it */
+struct JDProgFile {
+    uint64_t rec_cap;   /* records its image may use above rec_base (jd_prog_rec_cap) */
+    uint32_t file;      /* file index in the batch */
+    uint32_t rows;      /* MCU rows walked and packed */
+};
+
+/* One thread per (file, scan) of one wave: the scans of a wave touch disjoint coefficients of their planes.  The file's
+ * first undecodable MCU row over all its scans is kept in err_row[file]. */
+__global__ void __launch_bounds__(64) jdk_prog_scan(const JDProgScan *__restrict__ scans, uint32_t n, const uint8_t *__restrict__ data,
+                                                    const JDProgHuff *__restrict__ tabs, int16_t *const *__restrict__ planes,
+                                                    uint32_t *__restrict__ err_row)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const JDProgScan s = scans[i];
+    int16_t *const plane = planes[s.img];
+    if (!plane) return;   /* its plane did not fit: the file is refused */
+    const uint32_t row = jd_prog_walk(s, data, tabs, plane);
+    if (row != JD_PROG_NONE) atomicMin(err_row + s.img, row);
+}
+
+struct JDProgPackArgs {
+    JDImageDesc *imgs;               /* entropy-facing (file) descriptors: status and err_mcu are written here */
+    const JDProgFile *files;         /* one CTA each */
+    int16_t *const *planes;          /* per file */
+    const uint32_t *err_row;         /* per file */
+    jd_u64 *blk_hdr;
+    uint16_t *rec;
+    uint32_t limit;                  /* zigzag positions a block stores: 1 (1/8 scale), 5 (1/4) or 64 */
+    unsigned long long *rec_count;   /* JPEGB200_C_RECORD_BYTES / 2 */
+};
+
+/* One CTA per file: 256 blocks at a time are counted, placed by a block-wide prefix sum and written as block headers and
+ * records from the image's rec_base.  An image whose records would pass its budget gets empty headers from there on and
+ * an error status instead of an overwrite.  Then the file's status: JPEG_DECODE_ERROR from the first undecodable MCU row
+ * of its scans, under the region-of-interest rule of jdk_stitch. */
+__global__ void __launch_bounds__(256) jdk_prog_pack(const JDProgPackArgs a)
+{
+    __shared__ uint8_t s_tpos[64];
+    __shared__ uint32_t s_w[8];
+    const JDProgFile pf = a.files[blockIdx.x];
+    JDImageDesc &im = a.imgs[pf.file];
+    const int16_t *const plane = a.planes[pf.file];
+    if (!plane) return;
+    if (threadIdx.x < 64) s_tpos[threadIdx.x] = c_tpos[threadIdx.x];
+    __syncthreads();
+    const uint32_t nblk = pf.rows * (uint32_t)im.mcus_x * im.bpm;
+    jd_u64 *const hdr = a.blk_hdr + im.blk_base;
+    uint16_t *const rec = a.rec + im.rec_base;
+    const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
+    uint64_t base = 0;
+    bool over = false;
+    for (uint32_t b0 = 0; b0 < nblk; b0 += 256u) {
+        const uint32_t b = b0 + threadIdx.x;
+        int16_t cf[64];
+        uint32_t cnt = 0;
+        if (b < nblk) {
+            const uint4 *src = reinterpret_cast<const uint4 *>(plane + (size_t)b * 64u);
+#pragma unroll
+            for (int j = 0; j < 8; j++) { const uint4 v = src[j]; memcpy(cf + 8 * j, &v, 16); }
+            cnt = jd_prog_pack_block(cf, a.limit, s_tpos, nullptr, 0u, nullptr);
+        }
+        uint32_t x = cnt;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, d); if (lane >= (uint32_t)d) x += y; }
+        if (lane == 31u) s_w[wid] = x;
+        __syncthreads();
+        uint32_t wbase = 0, tot = 0;
+#pragma unroll
+        for (int w2 = 0; w2 < 8; w2++) { const uint32_t t = s_w[w2]; if ((uint32_t)w2 < wid) wbase += t; tot += t; }
+        __syncthreads();
+        if (base + tot > pf.rec_cap) over = true;
+        if (b < nblk) {
+            const uint64_t off = base + wbase + x - cnt;
+            if (over) hdr[b] = jd_pack_hdr(0u, 0, 0u, 0u, 0u, 0u);
+            else jd_prog_pack_block(cf, a.limit, s_tpos, rec + off, (uint32_t)off, hdr + b);
+        }
+        if (!over) base += tot;
+    }
+    if (threadIdx.x == 0) {
+        uint32_t status = 0, err_mcu = 0;
+        const uint32_t r = a.err_row[pf.file];
+        if (r != JD_PROG_NONE) { status = JD_SEG_BADCODE; err_mcu = r * (uint32_t)im.mcus_x; }
+        else if (over) status = JD_SEG_OVERFLOW;
+        if (im.roi_mcu_end != 0u && err_mcu >= im.roi_mcu_end) { status = 0; err_mcu = 0; }
+        im.status = status;
+        im.err_mcu = err_mcu;
+        if (base) atomicAdd(a.rec_count, (unsigned long long)base);
+    }
+}
