@@ -55,6 +55,35 @@ typedef struct JPEGB200_BATCH JPEGB200_BATCH; /* one decode job: n images, one p
  * output equals B's only when B carries the same tables.  Without the bit a progressive file gives the reference's 1/8 DC
  * thumbnail of its first scan, or JPEG_UNSUPPORTED_FEATURE at other scales. */
 #define JPEGB200_OPT_PROGRESSIVE 0x100
+/* options bit of every batch entry point (JPEGB200_batchCreate* / JPEGB200_decodeBatch*, views included): image i's output
+ * is libjpeg-turbo's default decompression of the file -- what PIL.Image.open(f).convert("RGB") and
+ * torchvision.io.decode_jpeg on the CPU return -- instead of the reference's pixels:
+ *   - IDCT: jpeg_idct_islow on coefficients dequantized with the raw DQT values of each component's own table.  The
+ *     coefficients are exact: the reference's bit-window truncation is not applied (JPEGB200_C_EVENTS is 0;
+ *     JPEGB200_C_EVENT_CANDIDATES still counts the candidate reads the walk met).  Equal to x86-64 libjpeg-turbo's SIMD islow on every block whose dequantized coefficients
+ *     and first-pass outputs fit in 16 bits and whose results lie in [-256, 511] before the +128: every block an encoder
+ *     writes from 8-bit samples.  Outside it, jidctint.c's 32-bit arithmetic clamped to 0..255.
+ *   - Upsampling: libjpeg's fancy triangle filters (h2v2, h2v1, h1v2), edges replicating the component's last real
+ *     sample; plain replication for h2v1 / h2v2 components at most 2 samples wide, as libjpeg does.
+ *   - Colour: jdcolor.c's YCbCr -> RGB tables, clamped.  Colour space as libjpeg infers it: a JFIF APP0 means YCbCr;
+ *     else an Adobe APP14 decides (transform 0: RGB, no conversion); else component ids 'R','G','B' mean RGB and any
+ *     other ids YCbCr.
+ *   - Pixel types: RGB8888 stores R, G, B, 0xFF for every file (a gray file: Y, Y, Y, 0xFF = convert("RGB")), so tensors
+ *     get R, G, B without a swap; EIGHT_BIT_GRAYSCALE stores Y (= decode_jpeg(mode=GRAY)).  An RGB-space file decoded to
+ *     EIGHT_BIT_GRAYSCALE gets JPEG_UNSUPPORTED_FEATURE.
+ *   - Composes with rectangles, orientations, resize, tensors, views and JPEGB200_OPT_PROGRESSIVE (whose coefficients are
+ *     exact too), all of which work on this image instead of the reference's.
+ *   - Rectangles: the rectangle equals the same rectangle of the full decode under the bit.  Fancy upsampling reads, in
+ *     each subsampled direction, the chroma sample next to the rectangle's first and last pixel, which may lie in the
+ *     neighbouring MCU: those MCUs are transformed too, and the status reports an error iff the full decode's first
+ *     undecodable MCU lies in an MCU row at or above the last MCU row the rectangle reads (its own last row, or the one
+ *     below it).  Restart intervals below that row are not walked.
+ *   - Refused (NULL with a message): RGB565 and dithered pixel types, JPEG_SCALE_* (libjpeg's scaled IDCTs are other
+ *     algorithms), JPEG_EXIF_THUMBNAIL and JPEG_LUMA_ONLY.
+ *   - Work: jdk_lj_idct writes 8-bit planes of each image's MCU box into device scratch (MCUs x blocks x 64 bytes), then
+ *     jdk_lj_color upsamples, converts and stores; both are timed as JPEGB200_T_IDCT.  JPEGB200_decodeBatch counts the
+ *     planes in its per-job scratch bound. */
+#define JPEGB200_OPT_LIBJPEG 0x200
 
 /* stage indices for JPEGB200_batchGetTimings (milliseconds, CUDA events on the batch stream) */
 enum {

@@ -22,6 +22,7 @@ JPEG_AUTO_ROTATE, JPEG_SCALE_HALF, JPEG_SCALE_QUARTER, JPEG_SCALE_EIGHTH = 1, 2,
 JPEG_LE_PIXELS, JPEG_EXIF_THUMBNAIL, JPEG_LUMA_ONLY, JPEG_USES_DMA = 16, 32, 64, 128
 # decode progressive files from all of their scans (include/jpegdec_b200.h)
 JPEGB200_OPT_PROGRESSIVE = 0x100
+JPEGB200_OPT_LIBJPEG = 0x200   # libjpeg-turbo's default decode (= Pillow, torchvision.io.decode_jpeg): include/jpegdec_b200.h
 (RGB565_LITTLE_ENDIAN, RGB565_BIG_ENDIAN, RGB8888, EIGHT_BIT_GRAYSCALE, FOUR_BIT_DITHERED,
  TWO_BIT_DITHERED, ONE_BIT_DITHERED, INVALID_PIXEL_TYPE) = range(8)
 (JPEG_SUCCESS, JPEG_INVALID_PARAMETER, JPEG_DECODE_ERROR, JPEG_UNSUPPORTED_FEATURE,

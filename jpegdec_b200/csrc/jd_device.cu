@@ -226,8 +226,16 @@ struct JPEGB200_BATCH {
     DevBuf<JDProgFile> d_pfiles;
     DevBuf<int16_t *> d_pplanes;
     DevBuf<uint32_t> d_perr;
+    /* libjpeg's default decompression (JPEGB200_OPT_LIBJPEG, jd_ljpeg.h): per image its MCU box and planes */
+    bool lj;
+    std::vector<JDLjDesc> lj_desc;
+    std::vector<int64_t> lj_plane;       /* per image: plane bytes (256-byte aligned; 0 for a failed image) */
+    int64_t lj_plane_total;
+    uint32_t lj_max_blocks, lj_max_pixels;
+    DevBuf<uint8_t> d_lj;
+    DevBuf<JDLjDesc> d_lj_desc;
     uint32_t h_changed;
-    bool chunk_iterate;           /* restart-free scans: iterate the entry states with a host check (fallback mode) */
+    bool chunk_iterate;          /* restart-free scans: iterate the entry states with a host check (fallback mode) */
     int decode_flags;
     cudaEvent_t ev[JPEGB200_NUM_TIMINGS + 2];
     bool have_ev;
@@ -557,6 +565,16 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
                                                      const JPEGB200_TensorSpec *spec)
 {
     if (!ctx || n <= 0 || pixel_type < 0 || pixel_type >= INVALID_PIXEL_TYPE) { snprintf(g_err, sizeof(g_err), "invalid parameter"); return nullptr; }
+    if (options & JPEGB200_OPT_LIBJPEG) {
+        /* libjpeg's default decompression has no RGB565, dithered, scaled, thumbnail or luma-only counterpart */
+        const char *why = nullptr;
+        if (pixel_type != RGB8888 && pixel_type != EIGHT_BIT_GRAYSCALE) why = "pixel types other than RGB8888 and EIGHT_BIT_GRAYSCALE";
+        else if (options & (JPEG_SCALE_HALF | JPEG_SCALE_QUARTER | JPEG_SCALE_EIGHTH)) why = "JPEG_SCALE_* (libjpeg's scaled IDCTs are other algorithms)";
+        else if (options & JPEG_EXIF_THUMBNAIL) why = "JPEG_EXIF_THUMBNAIL";
+        else if (options & JPEG_LUMA_ONLY) why = "JPEG_LUMA_ONLY";
+        else if (options & 0x10000) why = "padded output";
+        if (why) { snprintf(g_err, sizeof(g_err), "JPEGB200_OPT_LIBJPEG is not supported with %s", why); return nullptr; }
+    }
     int64_t nv = n;   /* images of the batch: views */
     if (views) {
         nv = 0;
@@ -630,6 +648,10 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
         b->rs_src_w.assign(nv, 0); b->rs_src_h.assign(nv, 0); b->rs_scratch.assign(nv, 0);
     }
     b->tensor = spec != nullptr;
+    b->lj = (options & JPEGB200_OPT_LIBJPEG) != 0;
+    b->lj_plane_total = 0;
+    b->lj_max_blocks = b->lj_max_pixels = 0;
+    if (b->lj) { b->lj_desc.assign(nv, JDLjDesc{}); b->lj_plane.assign(nv, 0); }
     b->tn_stage_total = 0;
     b->tn_elt = b->tn_nc = b->tn_bpp = b->tn_planes = 0;
     if (b->tensor) {
@@ -742,7 +764,8 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
                 (inf.approx & 15) > 13) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }
         } else if (ok && inf.mode != 0xC0) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }
         if (ok && !full && !inf.tables_ok) { ok = 0; st = JPEG_DECODE_ERROR; }  /* jpeg.inl:2166 */
-        if (ok && inf.ncomp == 1 && pixel_type == RGB8888) { ok = 0; st = JPEG_INVALID_PARAMETER; }
+        if (ok && inf.ncomp == 1 && pixel_type == RGB8888 && !b->lj) { ok = 0; st = JPEG_INVALID_PARAMETER; }
+        if (ok && b->lj && pixel_type == EIGHT_BIT_GRAYSCALE && !jd_lj_is_ycc(&inf)) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }
         if (ok && (uint64_t)sizes[f] >= (512ull << 20)) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }   /* image-relative record indices are 32-bit */
         const int file_ok = ok;
         for (int i = v0; i < v0 + nvf; i++) {
@@ -762,6 +785,17 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
                                            rois ? rois + 4 * (size_t)v0 : nullptr, orients ? &ks[v0] : nullptr,
                                            out_sizes ? out_sizes + 2 * (size_t)v0 : nullptr, &b->plans[v0], &srects[4 * (size_t)v0],
                                            &vok[v0]);
+            if (walk != 0 && b->lj && b->roi) {
+                /* what libjpeg's fancy upsampling reads around each rectangle */
+                walk = 0;
+                for (int i = v0; i < v0 + nvf; i++) {
+                    if (!vok[i]) continue;
+                    const int32_t *sr = &srects[4 * (size_t)i];
+                    const int32_t r[4] = {sr[0], sr[1], orients ? sr[2] : rois[4 * (size_t)i + 2], orients ? sr[3] : rois[4 * (size_t)i + 3]};
+                    jd_lj_plan_extend(inf.width, inf.height, inf.subsample, inf.restart_interval, r, &b->plans[i]);
+                    if ((uint32_t)b->plans[i].nseg_walk > walk) walk = (uint32_t)b->plans[i].nseg_walk;
+                }
+            }
             if (walk == 0) ok = 0;   /* no valid view: the file is not walked */
         }
         const uint32_t total_mcus = ok ? (uint32_t)inf.mcus_x * inf.mcus_y : 0u;
@@ -789,6 +823,7 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
             jd_build_quant(&inf, qn);
             for (int i = v0; i < v0 + nvf; i++) {
                 int32_t *qt = &b->quant[(size_t)i * 192];
+                if (b->lj) { jd_lj_quant(&inf, qt); continue; }   /* islow dequantizes with the raw DQT values */
                 for (int cc = 0; cc < 3; cc++)
                     for (int nn = 0; nn < 64; nn++) qt[cc * 64 + (nn & 7) * 8 + (nn >> 3)] = qn[cc * 64 + nn];
             }
@@ -894,6 +929,20 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
             vd.roi_mcu_end = (uint32_t)pl.mcu_end;
             vd.orient = orients ? b->orient[i] : 0u;
         }
+        if (b->lj) {
+            /* the MCU box whose planes jdk_lj_idct writes: the rectangle's, extended by jd_lj_plan_extend */
+            JDLjDesc &L = b->lj_desc[i];
+            L.mx0 = b->roi ? (uint32_t)b->plans[i].mcu_x0 : 0u; L.my0 = b->roi ? (uint32_t)b->plans[i].mcu_y0 : 0u;
+            L.nmx = b->roi ? (uint32_t)(b->plans[i].mcu_x1 - b->plans[i].mcu_x0 + 1) : (uint32_t)inf.mcus_x;
+            L.nmy = b->roi ? (uint32_t)(b->plans[i].mcu_y1 - b->plans[i].mcu_y0 + 1) : (uint32_t)inf.mcus_y;
+            L.ycc = (uint32_t)jd_lj_is_ycc(&inf);
+            const uint64_t blocks = (uint64_t)L.nmx * L.nmy * (uint64_t)inf.bpm;
+            b->lj_plane[i] = (int64_t)((blocks * 64u + 255u) & ~(uint64_t)255);
+            b->lj_plane_total += b->lj_plane[i];
+            if (blocks > b->lj_max_blocks) b->lj_max_blocks = (uint32_t)blocks;
+            const uint64_t px = (uint64_t)vd.out_w * vd.out_h;
+            if (px > b->lj_max_pixels) b->lj_max_pixels = (uint32_t)px;
+        }
         if (b->resize) {
             /* S = what the same call without out_sizes stores; the descriptor carries the resized size from here on */
             const int bp = bytes_per_pixel_class(b->ptclass);
@@ -911,8 +960,9 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
             /* U = what the same call without spec stores (out_w x out_h); staged, then converted */
             b->tn_stage[i] = (int64_t)(((size_t)vd.out_w * vd.out_h * b->tn_bpp + 255) & ~(size_t)255);
             b->tn_stage_total += b->tn_stage[i];
-            b->tn_swap[i] = (uint8_t)(b->tn_nc == 3 &&
-                                      (jd_rgb8888_is_bgr(ctx->arith, b->sshift, inf.ncomp, inf.subsample) != 0) != (spec->bgr != 0));
+            /* a libjpeg decode stores R, G, B for every file */
+            const bool bgr = !b->lj && jd_rgb8888_is_bgr(ctx->arith, b->sshift, inf.ncomp, inf.subsample) != 0;
+            b->tn_swap[i] = (uint8_t)(b->tn_nc == 3 && bgr != (spec->bgr != 0));
         }
         size_t pitch;
         if (b->tensor) pitch = (size_t)vd.out_w * (spec->layout == JPEGB200_LAYOUT_HWC ? b->tn_nc : 1) * b->tn_elt;
@@ -987,6 +1037,7 @@ extern "C" void JPEGB200_batchDestroy(JPEGB200_BATCH *b)
     b->d_pscans.release(); b->d_ptabs.release(); b->d_pfiles.release(); b->d_pplanes.release(); b->d_perr.release();
     b->d_rs.release(); b->d_rs_coef.release(); b->d_rs_desc.release();
     b->d_tn.release(); b->d_tn_tab.release(); b->d_tn_desc.release();
+    b->d_lj.release(); b->d_lj_desc.release();
     if (b->stream && b->have_ev) {   /* back to the context for the next job */
         JDStreamSet ss;
         ss.stream = b->stream;
@@ -1664,8 +1715,11 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
     CK(cudaEventRecord(b->ev[4], st));
     jdk_stitch<<<(nf + 127) / 128, 128, 0, st>>>(fdev, (uint32_t)nf, b->d_seg_jmap.p, b->d_seg_status.p, b->d_seg_phase.p, b->d_seg_nrec.p,
                                                reinterpret_cast<unsigned long long *>(b->d_counters.p + 4));
-    jdk_patch<<<32, 256, 0, st>>>(fdev, b->d_events.p, b->d_counters.p, JD_EVENT_CAP, b->d_seg_phase.p, b->d_blk_hdr.p, b->d_rec.p, b->d_counters.p + 1);
-    launches += 2;
+    launches++;
+    if (!b->lj) {   /* a libjpeg decode reads the exact coefficients: no window truncation to apply */
+        jdk_patch<<<32, 256, 0, st>>>(fdev, b->d_events.p, b->d_counters.p, JD_EVENT_CAP, b->d_seg_phase.p, b->d_blk_hdr.p, b->d_rec.p, b->d_counters.p + 1);
+        launches++;
+    }
     if (!b->pfiles.empty()) {
         /* after jdk_stitch, which gives a file without restart segments status 0: the pack writes the real one */
         JDProgPackArgs pa;
@@ -1680,7 +1734,29 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
     /* IDCT + colour: one launch per run of images with the same geometry class */
     const bool half = b->sshift == 1;
     uint8_t *stage_out = b->dither_bits ? b->d_gray.p : b->resize ? b->d_rs.p : pipe_out;
-    for (int i0 = 0; i0 < n;) {
+    if (b->lj) {
+        /* planes of every image's MCU box, then upsampling + colour into the stores; images that failed keep nmx = 0 */
+        std::vector<JDLjDesc> ld = b->lj_desc;
+        uint64_t po = 0;
+        for (int i = 0; i < n; i++) {
+            if (b->parse_status[i] != JPEG_SUCCESS) { ld[i].nmx = ld[i].nmy = 0; continue; }
+            ld[i].plane_off = po;
+            po += (uint64_t)b->lj_plane[i];
+        }
+        CK(b->d_lj.alloc(&b->ctx->pool, po + 256));
+        CK(b->d_lj_desc.alloc(&b->ctx->pool, n));
+        CK(cudaMemcpyAsync(b->d_lj_desc.p, ld.data(), sizeof(JDLjDesc) * n, cudaMemcpyHostToDevice, st));
+        const unsigned gb = (b->lj_max_blocks + JD_LJ_THREADS - 1) / JD_LJ_THREADS, gp = (b->lj_max_pixels + JD_LJ_THREADS - 1) / JD_LJ_THREADS;
+        for (int i0 = 0; i0 < n && gb && gp; i0 += 65535) {
+            const unsigned ni = (unsigned)std::min(n - i0, 65535);
+            jdk_lj_idct<<<dim3(gb, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, b->d_lj_desc.p, b->d_blk_hdr.p, b->d_rec.p, b->d_quant.p,
+                                                                 b->d_lj.p, (uint32_t)i0);
+            if (b->ptclass == JD_PT_GRAY) jdk_lj_color<JD_PT_GRAY><<<dim3(gp, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, b->d_lj_desc.p, b->d_lj.p, stage_out, (uint32_t)i0);
+            else jdk_lj_color<JD_PT_8888><<<dim3(gp, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, b->d_lj_desc.p, b->d_lj.p, stage_out, (uint32_t)i0);
+            launches += 2;
+        }
+    }
+    for (int i0 = 0; i0 < n && !b->lj;) {
         if (b->parse_status[i0] != JPEG_SUCCESS) { i0++; continue; }
         const JDInfo &f = b->infos[file_of(b, i0)];
         int i1 = i0 + 1;
@@ -1897,7 +1973,7 @@ extern "C" int JPEGB200_batchWait(JPEGB200_BATCH *b, int32_t *status)
     int all_ok = 1;
     /* more window-truncation events than the event buffer holds: some coefficients of this job were not patched, so its
      * pixels may differ from the reference's -- report that instead of returning them as good */
-    const bool ev_overflow = b->downloaded && b->h_counters[0] > JD_EVENT_CAP;
+    const bool ev_overflow = b->downloaded && !b->lj && b->h_counters[0] > JD_EVENT_CAP;
     if (ev_overflow) snprintf(g_err, sizeof(g_err), "%u window-truncation events exceed the event buffer (%u): job rejected", b->h_counters[0], JD_EVENT_CAP);
     for (int i = 0; i < b->n; i++) {
         int st = b->parse_status[i];
@@ -2094,12 +2170,13 @@ extern "C" int JPEGB200_decodeBatchViews(JPEGB200_CTX *ctx, const uint8_t *const
                 }
             }
         }
-        if ((b->resize || b->tensor || b->pplane_total) && cnt > 1 &&
-            b->rs_scratch_total + b->tn_stage_total + b->pplane_total > JD_JOB_RESIZE_SCRATCH) {
-            /* scratch of a job (resize: S + intermediate; tensor: the uint8 staging; progressive files: the coefficient plane,
-             * counted on the file's first view): at most JD_JOB_RESIZE_SCRATCH, or one file with all of its views */
+        if ((b->resize || b->tensor || b->pplane_total || b->lj) && cnt > 1 &&
+            b->rs_scratch_total + b->tn_stage_total + b->pplane_total + b->lj_plane_total > JD_JOB_RESIZE_SCRATCH) {
+            /* scratch of a job (resize: S + intermediate; tensor: the uint8 staging; libjpeg decodes: the sample planes;
+             * progressive files: the coefficient plane, counted on the file's first view): at most JD_JOB_RESIZE_SCRATCH, or
+             * one file with all of its views */
             std::vector<int64_t> sc(cv);
-            for (int i = 0; i < cv; i++) sc[i] = (b->resize ? b->rs_scratch[i] : 0) + (b->tensor ? b->tn_stage[i] : 0);
+            for (int i = 0; i < cv; i++) sc[i] = (b->resize ? b->rs_scratch[i] : 0) + (b->tensor ? b->tn_stage[i] : 0) + (b->lj ? b->lj_plane[i] : 0);
             for (int i = 0; i < cv; i++) if (i == 0 || file_of(b, i) != file_of(b, i - 1)) sc[i] += b->pplane[file_of(b, i)];
             int32_t cv3 = 0, capped3 = 0;
             const int c = jd_job_files(cnt, sizes + i0, vi, INT64_MAX, INT64_MAX, sc.data(), JD_JOB_RESIZE_SCRATCH, &cv3, &capped3);

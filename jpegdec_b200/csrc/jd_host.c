@@ -108,6 +108,7 @@ static int parse_header(const uint8_t *data, int size, int start, JDInfo *info, 
         info->thumb_w = keep.thumb_w; info->thumb_h = keep.thumb_h;
         info->thumb_data = keep.thumb_data; info->exif = keep.exif;
     }
+    info->adobe = -1;
     if (start < 0 || start > size) return fail(info, JPEG_INVALID_FILE);
     /* the reference reads up to 2048 bytes and rejects < 256 (:1597-1602) */
     if (size - start < 256) return fail(info, JPEG_INVALID_FILE);
@@ -143,6 +144,12 @@ static int parse_header(const uint8_t *data, int size, int start, JDInfo *info, 
                         }
                     }
                 }
+                break;
+            case 0xFFE0: /* APP0: JFIF (libjpeg's colour-space inference, jd_lj_is_ycc) */
+                if (len >= 2 + 14 && off + 7 <= size && memcmp(s + off + 2, "JFIF\0", 5) == 0) info->jfif = 1;
+                break;
+            case 0xFFEE: /* APP14: Adobe, transform byte at payload offset 11 */
+                if (len >= 2 + 12 && off + 14 <= size && memcmp(s + off + 2, "Adobe", 5) == 0) info->adobe = s[off + 13];
                 break;
             case 0xFFC0: case 0xFFC2: { /* SOF (:1679-1714) */
                 if (off + 8 > size) return fail(info, JPEG_DECODE_ERROR);
@@ -542,6 +549,60 @@ int32_t jd_view_err_mcu(uint32_t file_status, uint32_t file_err_mcu, uint32_t mc
 {
     if (file_status == 0u) return -1;
     return (mcu_end == 0u || file_err_mcu < mcu_end) ? (int32_t)file_err_mcu : -1;
+}
+
+/* ---- libjpeg's default decompression (JPEGB200_OPT_LIBJPEG) ---- */
+int jd_lj_is_ycc(const JDInfo *info)
+{
+    if (info->ncomp != 3 || info->jfif) return 1;
+    if (info->adobe >= 0) return info->adobe != 0;
+    const uint8_t *id = info->p.comp_id;
+    return !(id[0] == 'R' && id[1] == 'G' && id[2] == 'B');
+}
+
+void jd_lj_quant(const JDInfo *info, int32_t *q)
+{
+    for (int c = 0; c < 3; c++) {
+        const uint16_t *raw = info->p.quant_raw[(c < info->ncomp ? info->p.comp_quant[c] : 0) & 3];
+        for (int n = 0; n < 64; n++) q[c * 64 + (n & 7) * 8 + (n >> 3)] = raw[jd_zigzag_of_natural[n]];
+    }
+}
+
+/* the chroma samples [lo, hi] that output pixels p0..p1 read along one axis (n pixels, subsampled by 2 on it; narrow: the
+ * replicating fallback), as image pixel positions 2 lo .. 2 hi */
+static void lj_reads(int p0, int p1, int n, int narrow, int *lo, int *hi)
+{
+    const int d = (n + 1) / 2;
+    int a = p0 / 2, b = p1 / 2;
+    if (!narrow) {
+        if (!(p0 & 1) && a > 0) a--;
+        if ((p1 & 1) && b + 1 < d) b++;
+    }
+    *lo = 2 * a; *hi = 2 * b;
+}
+
+void jd_lj_plan_extend(int width, int height, int subsample, int restart_interval, const int32_t *srect, JDRoiPlan *plan)
+{
+    const int hs = (subsample == 0x21 || subsample == 0x22), vs = (subsample == 0x12 || subsample == 0x22);
+    const int mw = 8 << hs, mh = 8 << vs;
+    const int mcus_x = (width + mw - 1) / mw, mcus_y = (height + mh - 1) / mh;
+    const int narrow = hs && (width + 1) / 2 <= 2;   /* jdsample.c: h2v1 / h2v2 replicate a component this narrow */
+    int lo, hi;
+    if (hs) {
+        lj_reads(srect[0], srect[0] + srect[2] - 1, width, narrow, &lo, &hi);
+        if (lo / mw < plan->mcu_x0) plan->mcu_x0 = lo / mw;
+        if (hi / mw > plan->mcu_x1) plan->mcu_x1 = hi / mw;
+    }
+    if (vs) {
+        lj_reads(srect[1], srect[1] + srect[3] - 1, height, narrow, &lo, &hi);
+        if (lo / mh < plan->mcu_y0) plan->mcu_y0 = lo / mh;
+        if (hi / mh > plan->mcu_y1) plan->mcu_y1 = hi / mh;
+        plan->mcu_end = (plan->mcu_y1 + 1) * mcus_x;
+        const int total = mcus_x * mcus_y;
+        const int mps = restart_interval > 0 ? restart_interval : total;
+        const int nseg = (total + mps - 1) / mps, walk = (plan->mcu_end - 1) / mps + 1;
+        plan->nseg_walk = walk < nseg ? walk : nseg;
+    }
 }
 
 int jd_job_files(int nf, const int32_t *sizes, const int32_t *views, int64_t max_views, int64_t max_bytes,

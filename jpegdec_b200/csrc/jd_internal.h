@@ -32,6 +32,8 @@ typedef struct {
     int tables_ok;          /* scan uses only tables 0/1 (DC and AC) */
     int error;              /* JPEG_* error code when parse fails */
     int approx;             /* first scan's successive-approximation byte (Ah << 4 | Al); progressive files */
+    int jfif;               /* a JFIF APP0 segment was seen */
+    int adobe;              /* transform byte of the last Adobe APP14 segment, -1 = none */
     JDPARSED p;
 } JDInfo;
 
@@ -190,6 +192,29 @@ int jd_prog_parse(const uint8_t *data, int size, int start, const JDInfo *info, 
  * the one block where a failing scan stops may hold without paying for them (zero bits past its data), per scan; at most
  * 2^32 - 1 (block headers hold 32-bit record indices). */
 uint64_t jd_prog_rec_cap(uint64_t entropy_bytes, uint32_t nscans);
+
+/* ---- libjpeg's default decompression (JPEGB200_OPT_LIBJPEG, jd_ljpeg.h, DESIGN.md 4.2.6) ---- */
+/* 1 when libjpeg would convert the file's 3 components from YCbCr (jdapimin.c's inference: a JFIF APP0 means YCbCr; else
+ * an Adobe APP14 decides, transform 0 = RGB; else component ids 'R', 'G', 'B' mean RGB and anything else YCbCr), 0 when
+ * they are R, G, B already.  Gray files: 1. */
+int jd_lj_is_ycc(const JDInfo *info);
+/* The raw DQT values of each component's own table, column-major per component ([c * 64 + col * 8 + row]), the layout of
+ * the batch's quant array. */
+void jd_lj_quant(const JDInfo *info, int32_t *q /* [3][64] */);
+/* Extends a view's plan (jd_roi_plan / jd_orient_plan for srect: x, y, w, h in the stored frame at full scale) to the MCUs
+ * a libjpeg decode of the rectangle reads: fancy upsampling reads, in each subsampled direction, the neighbouring chroma
+ * sample of the rectangle's first and last pixel (the one before an even first pixel, the one after an odd last pixel,
+ * clamped to the component's real samples; none in the narrow fallback), which may lie in the next MCU.  For vertically
+ * subsampled files the walk and mcu_end then reach the last MCU row read. */
+void jd_lj_plan_extend(int width, int height, int subsample, int restart_interval, const int32_t *srect, JDRoiPlan *plan);
+/* Per image of a libjpeg batch: its MCU box and where its planes live in the batch's plane scratch (jd_ljpeg.h). */
+typedef struct {
+    uint64_t plane_off;     /* byte offset of the box's planes (256-byte aligned) */
+    uint32_t mx0, my0;      /* the box's first MCU column / row */
+    uint32_t nmx, nmy;      /* its size in MCUs; 0 = nothing to decode (a failed image) */
+    uint32_t ycc;           /* jd_lj_is_ycc */
+    uint32_t pad;
+} JDLjDesc;
 
 /* A caller's destination for image `index` (only named in the message): row_bytes is the tight pitch
  * (JPEGB200_batchOutputBytes), pitch <= 0 means tight.  device != 0: `out` is written by the kernels.  Returns 1, or 0 with

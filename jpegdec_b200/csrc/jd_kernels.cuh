@@ -2287,3 +2287,79 @@ __global__ void __launch_bounds__(256) jdk_prog_pack(const JDProgPackArgs a)
         if (base) atomicAdd(a.rec_count, (unsigned long long)base);
     }
 }
+
+/* ------------------------------------------------------------------------------------ */
+/* libjpeg's default decompression (JPEGB200_OPT_LIBJPEG, jd_ljpeg.h): islow into 8-bit   */
+/* planes of each image's MCU box, then fancy upsampling + colour into the same stores as */
+/* jdk_scaled (rectangle, orientation, pitch; the resize and tensor stages read the       */
+/* result like any IDCT output).  grid.y = image (from img0), grid.x covers the launch's  */
+/* largest box / rectangle.                                                               */
+/* ------------------------------------------------------------------------------------ */
+#include "jd_ljpeg.h"
+
+#define JD_LJ_THREADS 128
+
+/* one thread per 8x8 block of the image's MCU box */
+__global__ void __launch_bounds__(JD_LJ_THREADS) jdk_lj_idct(const JDImageDesc *__restrict__ imgs, const JDLjDesc *__restrict__ ljd,
+                                                             const jd_u64 *__restrict__ blk_hdr, const uint16_t *__restrict__ rec,
+                                                             const int32_t *__restrict__ quant, uint8_t *__restrict__ planes, uint32_t img0)
+{
+    const uint32_t i = img0 + blockIdx.y;
+    const JDLjDesc L = ljd[i];
+    const uint32_t t = blockIdx.x * JD_LJ_THREADS + threadIdx.x;
+    const uint32_t bpm = imgs[i].bpm;
+    if (t >= L.nmx * L.nmy * bpm) return;
+    const JDImageDesc &im = imgs[i];
+    const uint32_t hs = (im.subsample >> 4) ? (im.subsample >> 4) : 1u, vs = (im.subsample & 15) ? (im.subsample & 15) : 1u;
+    const uint32_t m = t / bpm, b = t - m * bpm;
+    const uint32_t my = m / L.nmx, mx = m - my * L.nmx;
+    const uint32_t cmp = b < hs * vs ? 0u : b - hs * vs + 1u;
+    const jd_u64 h = blk_hdr[im.blk_base + ((size_t)(L.my0 + my) * im.mcus_x + L.mx0 + mx) * bpm + b];
+    uint32_t pitch;
+    const uint64_t off = jd_lj_block_dst(b, mx, my, L.nmx, L.nmy, hs, vs, &pitch);
+    int32_t c[64];
+    jd_lj_block(rec + im.rec_base, h, quant + (size_t)i * 192 + cmp * 64, c, planes + L.plane_off + off, pitch);
+}
+
+/* one thread per pixel of the image's rectangle in the stored frame (the whole image without one) */
+template <int PT>
+__global__ void __launch_bounds__(JD_LJ_THREADS) jdk_lj_color(const JDImageDesc *__restrict__ imgs, const JDLjDesc *__restrict__ ljd,
+                                                              const uint8_t *__restrict__ planes, uint8_t *__restrict__ out, uint32_t img0)
+{
+    const uint32_t i = img0 + blockIdx.y;
+    const JDLjDesc L = ljd[i];
+    if (L.nmx == 0u) return;
+    const JDImageDesc &im = imgs[i];
+    const bool tr = im.orient >= 5u;
+    const uint32_t sw = tr ? im.out_h : im.out_w, sh = tr ? im.out_w : im.out_h;
+    const uint32_t p = blockIdx.x * JD_LJ_THREADS + threadIdx.x;
+    if (p >= sw * sh) return;
+    const uint32_t gy = p / sw, gx = p - gy * sw;
+    const uint32_t sx = im.roi_x + gx, sy = im.roi_y + gy;
+    const uint32_t hs = (im.subsample >> 4) ? (im.subsample >> 4) : 1u, vs = (im.subsample & 15) ? (im.subsample & 15) : 1u;
+    const uint32_t yp = jd_lj_ypitch(L.nmx, hs);
+    const uint8_t *pl = planes + L.plane_off;
+    const uint32_t Y = pl[(size_t)(sy - L.my0 * vs * 8u) * yp + sx - L.mx0 * hs * 8u];
+    uint32_t v;
+    if (PT == JD_PT_GRAY) v = Y;
+    else if (im.ncomp == 1) v = Y | (Y << 8) | (Y << 16) | 0xFF000000u;
+    else {
+        const uint32_t cp = L.nmx * 8u;
+        const size_t csz = (size_t)cp * L.nmy * 8u;
+        const uint32_t dw = hs == 2u ? ((uint32_t)im.width + 1u) >> 1 : im.width, dh = vs == 2u ? ((uint32_t)im.height + 1u) >> 1 : im.height;
+        const uint8_t *pc = pl + (size_t)yp * L.nmy * vs * 8u;
+        const uint32_t cb = jd_lj_chroma(pc, cp, L.mx0 * 8u, L.my0 * 8u, sx, sy, hs, vs, dw, dh);
+        const uint32_t cr = jd_lj_chroma(pc + csz, cp, L.mx0 * 8u, L.my0 * 8u, sx, sy, hs, vs, dw, dh);
+        v = (L.ycc ? jd_lj_ycc_rgb((int32_t)Y, (int32_t)cb, (int32_t)cr) : (Y | (cb << 8) | (cr << 16))) | 0xFF000000u;
+    }
+    /* destination: mirrored in the stored frame, then transposed (jdk_scaled's addressing) */
+    uint32_t dx = gx, dy = gy;
+    if (im.orient >= 2u) {
+        const uint32_t ex = ((JD_ORIENT_MX >> im.orient) & 1u) ? sw - 1u - gx : gx;
+        const uint32_t ey = ((JD_ORIENT_MY >> im.orient) & 1u) ? sh - 1u - gy : gy;
+        dx = tr ? ey : ex; dy = tr ? ex : ey;
+    }
+    uint8_t *row = out + im.out_off + (size_t)dy * im.out_pitch;
+    if (PT == JD_PT_GRAY) row[dx] = (uint8_t)v;
+    else reinterpret_cast<uint32_t *>(row)[dx] = v;
+}
