@@ -16,8 +16,6 @@
 #include <pthread.h>
 #include "jd_internal.h"
 
-#define JPEGB200_OPT_PADDED 0x10000 /* internal option bit: write the whole MCU-aligned frame */
-
 /* One context per (device, arithmetic build), created on first use.  g_lock guards this table and the staging pool; the GPU
  * work of a decode holds only its context's lock (a context is driven by one thread at a time); the host replay of the
  * delivery rules -- which runs the user's callback -- holds no lock at all, so a callback may decode another image and

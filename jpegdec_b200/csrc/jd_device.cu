@@ -76,15 +76,20 @@ struct JDPinPool {
 
 /* a job's stream and its timing events, recycled through the context (creating them costs more than a small decode) */
 struct JDStreamSet {
-    cudaStream_t stream;
-    cudaEvent_t ev[JPEGB200_NUM_TIMINGS + 2];
+    cudaStream_t stream = nullptr;
+    cudaEvent_t ev[JPEGB200_NUM_TIMINGS + 2] = {};
+    bool complete() const { return stream && ev[JPEGB200_NUM_TIMINGS + 1]; }   /* created in this order */
+    void destroy()
+    {
+        for (auto &e : ev) if (e) cudaEventDestroy(e);
+        if (stream) cudaStreamDestroy(stream);
+    }
 };
 
 struct JPEGB200_CTX {
     std::vector<JDStreamSet> free_streams;
     int device;
     int arith;
-    char err[256];
     bool has_shared;
     uint64_t shared_hash, shared_hash2;
     uint16_t shared_lut[JD_LUT_ENTRIES];
@@ -98,18 +103,27 @@ struct JPEGB200_CTX {
     int pipe_depth;                               /* jobs in flight inside JPEGB200_decodeBatch (0 = default) */
 };
 
+static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+/* A device buffer borrowed from a pool; it goes back when the buffer dies.  Movable, not copyable: a copy would hand the
+ * same pointer to the pool twice. */
 template <typename T>
 struct DevBuf {
     T *p = nullptr;
     size_t n = 0;
     size_t bytes = 0;
     JDPool *pool = nullptr;
+    DevBuf() = default;
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    DevBuf(DevBuf &&o) noexcept : p(o.p), n(o.n), bytes(o.bytes), pool(o.pool) { o.p = nullptr; o.n = 0; o.bytes = 0; }
+    ~DevBuf() { release(); }
     cudaError_t alloc(JDPool *from, size_t count)
     {
         if (count <= n && p) return cudaSuccess;
         release();
         pool = from;
-        size_t need = ((count ? count : 1) * sizeof(T) + 255) & ~(size_t)255;
+        size_t need = align256((count ? count : 1) * sizeof(T));
         void *q = nullptr;
         cudaError_t e = pool ? pool->get(need, &q, &bytes) : cudaMalloc(&q, bytes = need);
         if (e == cudaSuccess) { p = (T *)q; n = count; }
@@ -122,52 +136,54 @@ struct DevBuf {
     }
 };
 
+/* One job.  Every member starts empty; the DevBuf members return to the context's pool when the batch is deleted
+ * (JPEGB200_batchDestroy, after the stream has drained). */
 struct JPEGB200_BATCH {
-    JPEGB200_CTX *ctx;
-    int n;                          /* images (views with JPEGB200_batchCreateViews): everything per image is per view */
+    JPEGB200_CTX *ctx = nullptr;
+    int n = 0;                      /* images (views with JPEGB200_batchCreateViews): everything per image is per view */
     /* views (JPEGB200_batchCreateViews): nf files, each walked once through its entropy-facing descriptor fdescs[f]
      * (d_fdescs); descs[i] is view i's descriptor for the IDCT and after it, carrying its file's seg / blk / rec bases.
      * Without views nf = n and descs serves both (fdescs and vfile stay empty). */
-    int nf;
-    bool views;
+    int nf = 0;
+    bool views = false;
     std::vector<int32_t> vfile;     /* per view: its file */
     std::vector<JDImageDesc> fdescs;
     DevBuf<JDImageDesc> d_fdescs;
-    int pixel_type, options, sshift, ptclass, dither_bits;
-    bool gray_out;
-    bool padded; /* write the whole MCU-aligned frame (single-image API: callbacks deliver whole MCUs) */
-    bool roi;    /* created with regions of interest or orientations (JPEGB200_batchCreateOriented) */
+    int pixel_type = 0, options = 0, sshift = 0, ptclass = 0, dither_bits = 0;
+    bool gray_out = false;
+    bool padded = false; /* write the whole MCU-aligned frame (single-image API: callbacks deliver whole MCUs) */
+    bool roi = false;    /* created with regions of interest or orientations (JPEGB200_batchCreateOriented) */
     std::vector<JDRoiPlan> plans;   /* per image, with roi */
     std::vector<int32_t> exif_tag;  /* per image: the file's EXIF Orientation tag (0 = none) */
     std::vector<uint8_t> orient;    /* per image: the transform applied, 1-8 (1 without orients) */
-    uint32_t nseg_walk;             /* restart intervals the entropy stage walks (JPEGB200_C_SEGMENTS) */
+    uint32_t nseg_walk = 0;         /* restart intervals the entropy stage walks (JPEGB200_C_SEGMENTS) */
     /* resize (JPEGB200_batchCreateResized): descs hold the resized size; the IDCT stage writes S (the unresized output,
      * rs_src_w x rs_src_h) into d_rs, the resize passes write the destination */
-    bool resize;
-    int rs_filter;
+    bool resize = false;
+    int rs_filter = 0;
     std::vector<JDResizePlan> rs_plans;
     std::vector<uint32_t> rs_src_w, rs_src_h;
     std::vector<int64_t> rs_scratch;    /* per image: S + intermediate bytes in d_rs (256-byte aligned each) */
-    int64_t rs_scratch_total;
+    int64_t rs_scratch_total = 0;
     std::vector<JDResizeDesc> rs_desc;
     DevBuf<uint8_t> d_rs;
     DevBuf<int32_t> d_rs_coef;
     DevBuf<JDResizeDesc> d_rs_desc;
     /* tensor output (JPEGB200_batchCreateTensor): descs hold the row bytes as out_pitch; the pipeline (IDCT or resize) writes
      * U (out_w x out_h, tn_bpp bytes per pixel) tightly into d_tn, jdk_tensor writes the destination */
-    bool tensor;
-    JPEGB200_TensorSpec tn_spec;
-    int tn_elt, tn_nc, tn_bpp, tn_planes;   /* tn_planes: C for CHW (the tensor is tn_planes x out_h rows), 1 for HWC */
+    bool tensor = false;
+    JPEGB200_TensorSpec tn_spec = {};
+    int tn_elt = 0, tn_nc = 0, tn_bpp = 0, tn_planes = 0;   /* tn_planes: C for CHW (the tensor is tn_planes x out_h rows), 1 for HWC */
     std::vector<uint8_t> tn_swap;           /* per image: output channel c reads byte 2 - c of a staged pixel */
     std::vector<int64_t> tn_stage;          /* per image: staging bytes (256-byte aligned) */
     std::vector<int64_t> tn_plane;          /* per image: the caller's plane stride (0 = pitch * out_h) */
-    int64_t tn_stage_total;
+    int64_t tn_stage_total = 0;
     std::vector<uint32_t> tn_table;         /* 3 x 256 elements, zero-extended to 32 bits */
     std::vector<JDTensorDesc> tn_desc;
     DevBuf<uint8_t> d_tn;
     DevBuf<uint32_t> d_tn_tab;
     DevBuf<JDTensorDesc> d_tn_desc;
-    cudaStream_t stream;
+    JDStreamSet ss;                 /* from the context on first use (batch_stream), back to it on destroy */
     std::vector<JDInfo> infos;
     std::vector<int32_t> parse_status;
     std::vector<const uint8_t *> datas;
@@ -179,25 +195,25 @@ struct JPEGB200_BATCH {
     std::vector<uint64_t> comp_off; /* offset of each file in the device blob */
     std::vector<void *> outs;
     std::vector<int64_t> pitches;
-    int index_base;                 /* index of image 0 in the caller's list (JPEGB200_decodeBatch jobs): error messages */
+    int index_base = 0;             /* index of image 0 in the caller's list (JPEGB200_decodeBatch jobs): error messages */
     std::vector<uint16_t> errinit;  /* dither: initial error line per image (reference quirk), value | 0xFF00 (tag of "the band above band 0") */
-    size_t comp_total, out_total, gray_total;
-    uint32_t nseg, nlut;
-    uint64_t nblk;
-    bool contiguous_in;
-    bool uploaded, out_device, arena_owned;
+    size_t comp_total = 0, out_total = 0, gray_total = 0;
+    uint32_t nseg = 0, nlut = 0;
+    uint64_t nblk = 0;
+    bool contiguous_in = false;
+    bool uploaded = false, out_device = false, arena_owned = false;
     DevBuf<uint8_t> d_comp, d_out, d_gray;
     DevBuf<uint16_t> d_errline;
     DevBuf<uint64_t> d_gray_off; /* [0,n): gray-stage offsets, [n,2n): packed output offsets, [2n,3n): output pitches */
     DevBuf<uint32_t> d_err_off, d_dprog;
     DevBuf<uint8_t> d_clean;       /* un-stuffed restart segments (jdk_unstuff_segs) */
     DevBuf<uint32_t> d_seg_clen;
-    uint64_t rec_total;            /* coefficient records the batch may need (JD_REC_INDEX layout) */
+    uint64_t rec_total = 0;        /* coefficient records the batch may need (JD_REC_INDEX layout) */
     DevBuf<uint4> d_dbands;        /* dither: (image, band, list position of the band above, of band - 255 or ~0) per warp */
     std::vector<uint4> dbands;
-    JDImageDesc *descs_dl;             /* descriptors read back (status, err_mcu); pinned, from ctx->pinpool */
-    size_t descs_dl_bytes;
-    bool downloaded;
+    JDImageDesc *descs_dl = nullptr;   /* descriptors read back (status, err_mcu); pinned, from ctx->pinpool */
+    size_t descs_dl_bytes = 0;
+    bool downloaded = false;
     DevBuf<JDImageDesc> d_descs;
     DevBuf<int32_t> d_quant;
     DevBuf<uint16_t> d_luts, d_rec;
@@ -207,7 +223,7 @@ struct JPEGB200_BATCH {
     std::vector<uint64_t> arena_off; /* per-image offset inside d_out */
     /* restart-free scans decoded chunk-parallel (jd_chunk.h) */
     std::vector<uint32_t> cimg_list;
-    uint32_t nchunks, max_nch;
+    uint32_t nchunks = 0, max_nch = 0;
     DevBuf<uint8_t> d_filt;
     DevBuf<uint32_t> d_cimg_list, d_flen, d_E0, d_E1, d_Ep, d_cfirst, d_cn, d_cpre, d_cjmap, d_cstatus, d_cnown;
     DevBuf<int32_t> d_cdcs, d_cpe;
@@ -217,8 +233,8 @@ struct JPEGB200_BATCH {
     std::vector<JDProgHuff> ptabs;       /* the batch's decoder tables, one per distinct content */
     std::vector<JDProgFile> pfiles;
     std::vector<int64_t> pplane;         /* per file: coefficient plane bytes (0: no such plane) */
-    int64_t pplane_total;
-    uint32_t pwalkers;                   /* walkers of files whose plane was allocated (JPEGB200_C_SEGMENTS) */
+    int64_t pplane_total = 0;
+    uint32_t pwalkers = 0;               /* walkers of files whose plane was allocated (JPEGB200_C_SEGMENTS) */
     std::vector<DevBuf<int16_t>> d_pplane;
     std::vector<int16_t *> pplane_ptr;
     DevBuf<JDProgScan> d_pscans;
@@ -227,21 +243,19 @@ struct JPEGB200_BATCH {
     DevBuf<int16_t *> d_pplanes;
     DevBuf<uint32_t> d_perr;
     /* libjpeg's default decompression (JPEGB200_OPT_LIBJPEG, jd_ljpeg.h): per image its MCU box and planes */
-    bool lj;
+    bool lj = false;
     std::vector<JDLjDesc> lj_desc;
     std::vector<int64_t> lj_plane;       /* per image: plane bytes (256-byte aligned; 0 for a failed image) */
-    int64_t lj_plane_total;
-    uint32_t lj_max_blocks, lj_max_pixels;
+    int64_t lj_plane_total = 0;
+    uint32_t lj_max_blocks = 0, lj_max_pixels = 0;
     DevBuf<uint8_t> d_lj;
     DevBuf<JDLjDesc> d_lj_desc;
-    uint32_t h_changed;
-    bool chunk_iterate;          /* restart-free scans: iterate the entry states with a host check (fallback mode) */
-    int decode_flags;
-    cudaEvent_t ev[JPEGB200_NUM_TIMINGS + 2];
-    bool have_ev;
-    float ms[JPEGB200_NUM_TIMINGS];
-    int64_t counters[JPEGB200_NUM_COUNTERS];
-    uint32_t *h_counters;              /* 8 words at the end of the descs_dl block */
+    uint32_t h_changed = 0;
+    bool chunk_iterate = false;  /* restart-free scans: iterate the entry states with a host check (fallback mode) */
+    int decode_flags = 0;
+    float ms[JPEGB200_NUM_TIMINGS] = {};
+    int64_t counters[JPEGB200_NUM_COUNTERS] = {};
+    uint32_t *h_counters = nullptr;    /* 8 words at the end of the descs_dl block */
 };
 
 static char *ctx_err() { return g_err; }
@@ -292,7 +306,6 @@ extern "C" JPEGB200_CTX *JPEGB200_create(int device, int arith_mode)
     if (!c) return nullptr;
     c->device = device;
     c->arith = arith_mode ? JPEG_ARITH_SCALAR : JPEG_ARITH_SSE2;
-    c->err[0] = 0;
     c->has_shared = false;
     c->shared_hits = 0;
     memset(c->last_counters, 0, sizeof(c->last_counters));
@@ -319,7 +332,7 @@ extern "C" void JPEGB200_destroy(JPEGB200_CTX *ctx)
     cudaDeviceSynchronize();
     ctx->pool.drain();
     ctx->pinpool.drain();
-    for (auto &ss : ctx->free_streams) { for (auto &e : ss.ev) cudaEventDestroy(e); cudaStreamDestroy(ss.stream); }
+    for (auto &ss : ctx->free_streams) ss.destroy();
     delete ctx;
 }
 
@@ -415,39 +428,6 @@ extern "C" int JPEGB200_deviceRead(JPEGB200_CTX *ctx, void *host_dst, const void
 /* ---- digests of device-resident pixels: lets a caller (bench / tests) verify a whole device-resident batch against
  * reference digests without moving the pixels to the host.  digest = sum over 8-byte words i of mix64(word ^ i * K)
  * mod 2^64 (mix64 = the splitmix64 finaliser); order independent, so it reduces in parallel. ---- */
-__device__ __forceinline__ unsigned long long jd_mix64(unsigned long long z)
-{
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    return z ^ (z >> 31);
-}
-
-__global__ void __launch_bounds__(256) jdk_digest(const uint8_t *const *ptrs, const int64_t *lens, unsigned long long *out)
-{
-    const uint32_t img = blockIdx.y;
-    const unsigned long long *w = reinterpret_cast<const unsigned long long *>(ptrs[img]);
-    const int64_t nbytes = lens[img], nfull = nbytes >> 3;
-    unsigned long long acc = 0;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nfull; i += (int64_t)gridDim.x * blockDim.x)
-        acc += jd_mix64(w[i] ^ ((unsigned long long)i * 0x9E3779B97F4A7C15ull));
-    if (blockIdx.x == 0 && threadIdx.x == 0 && (nbytes & 7)) {   /* tail bytes, zero padded */
-        unsigned long long t = 0;
-        const uint8_t *q = ptrs[img] + (nfull << 3);
-        for (int k = 0; k < (int)(nbytes & 7); k++) t |= (unsigned long long)q[k] << (8 * k);
-        acc += jd_mix64(t ^ ((unsigned long long)nfull * 0x9E3779B97F4A7C15ull));
-    }
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, d);
-    __shared__ unsigned long long s_part[8];
-    if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        unsigned long long t = 0;
-        for (int k = 0; k < 8; k++) t += s_part[k];
-        atomicAdd(out + img, t);
-    }
-}
-
 /* digests of n device byte ranges (8-byte aligned starts); synchronous */
 extern "C" int JPEGB200_digestDevice(JPEGB200_CTX *ctx, const void *const *dev_ptrs, const int64_t *lengths, int n, uint64_t *digests)
 {
@@ -559,150 +539,98 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateTensor(JPEGB200_CTX *ctx, const u
     return JPEGB200_batchCreateViews(ctx, datas, sizes, n, nullptr, pixel_type, options, rois, orients, out_sizes, filter, spec);
 }
 
-extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
-                                                     const int32_t *views, int pixel_type, int options, const int32_t *rois,
-                                                     const uint8_t *orients, const int32_t *out_sizes, int filter,
-                                                     const JPEGB200_TensorSpec *spec)
+/* ---- JPEGB200_batchCreateViews, step by step.  CreatePlan lives on its stack: the caller's per-view arguments and what
+ * one file's steps hand to the next file's. ---- */
+struct CreatePlan {
+    const uint8_t *const *datas = nullptr;
+    const int32_t *sizes = nullptr, *views = nullptr, *rois = nullptr, *out_sizes = nullptr;
+    const uint8_t *orients = nullptr;
+    const JPEGB200_TensorSpec *spec = nullptr;
+    /* where the next file's restart segments, blocks and records start; where the next view's output and gray stage start */
+    uint32_t seg = 0;
+    uint64_t blk = 0, rec_total = 0;
+    size_t out_total = 0, gray_total = 0;
+    std::vector<uint64_t> lut_hash;
+    std::vector<int> lut_owner;         /* first file that defined each LUT set: a hash match is confirmed on the DHT bytes */
+    std::vector<int32_t> srects, vok;   /* per view: its rectangle in the stored frame (jd_views_plan), and whether it is valid */
+    std::vector<uint8_t> ks;            /* per view, with orients: the transform asked for (above 8: refused by jd_views_plan) */
+    std::vector<JDProgScan> fscans;     /* jd_prog_parse's scans and tables of the current file */
+    std::vector<JDProgHuff> ftabs;
+    std::unordered_map<uint64_t, std::vector<uint32_t>> ptab_index;   /* table content hash -> its indices in b->ptabs */
+};
+
+/* what admit_file and size_file_walk find out about one file */
+struct FileAdmit {
+    int ok = 0, status = JPEG_SUCCESS;
+    bool prog = false, full = false;   /* prog: DC-only 1/8 decode of a progressive file; full: decoded from all its scans (jd_prog.h) */
+    int nsc = 0, ntb = 0;              /* full: its scans and tables in CreatePlan::fscans / ftabs */
+    uint32_t total_mcus = 0, mps = 0, nseg = 0, nch = 0;
+};
+
+/* the batch's fixed state from the (checked) arguments: feature flags, pixel class, per-view and per-file vectors sized */
+static void init_batch(JPEGB200_BATCH *b, JPEGB200_CTX *ctx, const CreatePlan &P, int n, int nv, int pixel_type, int options, int filter)
 {
-    if (!ctx || n <= 0 || pixel_type < 0 || pixel_type >= INVALID_PIXEL_TYPE) { snprintf(g_err, sizeof(g_err), "invalid parameter"); return nullptr; }
-    if (options & JPEGB200_OPT_LIBJPEG) {
-        /* libjpeg's default decompression has no RGB565, dithered, scaled, thumbnail or luma-only counterpart */
-        const char *why = nullptr;
-        if (pixel_type != RGB8888 && pixel_type != EIGHT_BIT_GRAYSCALE) why = "pixel types other than RGB8888 and EIGHT_BIT_GRAYSCALE";
-        else if (options & (JPEG_SCALE_HALF | JPEG_SCALE_QUARTER | JPEG_SCALE_EIGHTH)) why = "JPEG_SCALE_* (libjpeg's scaled IDCTs are other algorithms)";
-        else if (options & JPEG_EXIF_THUMBNAIL) why = "JPEG_EXIF_THUMBNAIL";
-        else if (options & JPEG_LUMA_ONLY) why = "JPEG_LUMA_ONLY";
-        else if (options & 0x10000) why = "padded output";
-        if (why) { snprintf(g_err, sizeof(g_err), "JPEGB200_OPT_LIBJPEG is not supported with %s", why); return nullptr; }
-    }
-    int64_t nv = n;   /* images of the batch: views */
-    if (views) {
-        nv = 0;
-        for (int f = 0; f < n; f++) {
-            if (views[f] < 1) { snprintf(g_err, sizeof(g_err), "views[%d] = %d: every file needs at least one view", f, views[f]); return nullptr; }
-            nv += views[f];
-        }
-        if (nv > INT32_MAX) { snprintf(g_err, sizeof(g_err), "%lld views: at most %d per batch", (long long)nv, INT32_MAX); return nullptr; }
-        /* like rectangles and orientations: the dither of a view is not a view of the dither; padded output is the
-         * single-image API's */
-        if (pixel_type >= FOUR_BIT_DITHERED && pixel_type <= ONE_BIT_DITHERED) {
-            snprintf(g_err, sizeof(g_err), "views are not supported with dithered pixel types");
-            return nullptr;
-        }
-        if (options & 0x10000) { snprintf(g_err, sizeof(g_err), "views are not supported with padded output"); return nullptr; }
-    }
-    if (spec) {
-        /* tensors are built from byte planes: RGB8888 (either byte order) and 8-bit gray, LUMA_ONLY folding included */
-        const int pt = ((options & JPEG_LUMA_ONLY) && pixel_type < EIGHT_BIT_GRAYSCALE) ? EIGHT_BIT_GRAYSCALE : pixel_type;
-        if (pt == RGB565_LITTLE_ENDIAN || pt == RGB565_BIG_ENDIAN) {
-            snprintf(g_err, sizeof(g_err), "tensor output is not supported with RGB565 pixel types (a packed 5/6/5 word has no byte planes)");
-            return nullptr;
-        }
-        if (pt >= FOUR_BIT_DITHERED && pt <= ONE_BIT_DITHERED) {
-            snprintf(g_err, sizeof(g_err), "tensor output is not supported with dithered pixel types");
-            return nullptr;
-        }
-        if (options & 0x10000) { snprintf(g_err, sizeof(g_err), "tensor output is not supported with padded output"); return nullptr; }
-        if (!jd_tensor_check(spec, pt == RGB8888 ? 3 : 1, g_err, (int)sizeof(g_err))) return nullptr;
-    }
-    if (out_sizes) {
-        /* resizing works on byte planes: RGB8888 (either byte order) and 8-bit gray, LUMA_ONLY folding included */
-        const int pt = ((options & JPEG_LUMA_ONLY) && pixel_type < EIGHT_BIT_GRAYSCALE) ? EIGHT_BIT_GRAYSCALE : pixel_type;
-        if (pt == RGB565_LITTLE_ENDIAN || pt == RGB565_BIG_ENDIAN) {
-            snprintf(g_err, sizeof(g_err), "resizing is not supported with RGB565 pixel types (a packed 5/6/5 word has no byte planes)");
-            return nullptr;
-        }
-        if (pt >= FOUR_BIT_DITHERED && pt <= ONE_BIT_DITHERED) {
-            snprintf(g_err, sizeof(g_err), "resizing is not supported with dithered pixel types");
-            return nullptr;
-        }
-        if (options & 0x10000) { snprintf(g_err, sizeof(g_err), "resizing is not supported with padded output"); return nullptr; }
-        if (!jd_rs_filter_ok(filter)) {
-            snprintf(g_err, sizeof(g_err), "resize filter %d is not supported (JPEGB200_RESIZE_BILINEAR 2, BICUBIC 3 or BOX 4)", filter);
-            return nullptr;
-        }
-    }
-    if (rois && pixel_type >= FOUR_BIT_DITHERED && pixel_type <= ONE_BIT_DITHERED) {
-        /* error diffusion runs across the whole image: a rectangle of the dithered image is not the dither of the rectangle */
-        snprintf(g_err, sizeof(g_err), "regions of interest are not supported with dithered pixel types");
-        return nullptr;
-    }
-    if (orients && pixel_type >= FOUR_BIT_DITHERED && pixel_type <= ONE_BIT_DITHERED) {
-        /* likewise: the dither of a rotated image is not the rotation of the dither */
-        snprintf(g_err, sizeof(g_err), "orientations are not supported with dithered pixel types");
-        return nullptr;
-    }
-    if (rois && (options & 0x10000)) { snprintf(g_err, sizeof(g_err), "regions of interest are not supported with padded output"); return nullptr; }
-    if (orients && (options & 0x10000)) { snprintf(g_err, sizeof(g_err), "orientations are not supported with padded output"); return nullptr; }
-    JPEGB200_BATCH *b = new (std::nothrow) JPEGB200_BATCH();
-    if (!b) return nullptr;
-    b->roi = rois != nullptr || orients != nullptr;
+    b->ctx = ctx;
+    b->n = nv;
+    b->nf = n;
+    b->views = P.views != nullptr;
+    b->roi = P.rois != nullptr || P.orients != nullptr;
     b->plans.assign(nv, JDRoiPlan{});   /* read with rois or orients only */
     b->exif_tag.assign(nv, 0);
     b->orient.assign(nv, 1);
-    b->resize = out_sizes != nullptr;
-    b->rs_filter = filter;
-    b->rs_scratch_total = 0;
-    if (b->resize) {
-        b->rs_plans.assign(nv, JDResizePlan{});
-        b->rs_src_w.assign(nv, 0); b->rs_src_h.assign(nv, 0); b->rs_scratch.assign(nv, 0);
-    }
-    b->tensor = spec != nullptr;
-    b->lj = (options & JPEGB200_OPT_LIBJPEG) != 0;
-    b->lj_plane_total = 0;
-    b->lj_max_blocks = b->lj_max_pixels = 0;
-    if (b->lj) { b->lj_desc.assign(nv, JDLjDesc{}); b->lj_plane.assign(nv, 0); }
-    b->tn_stage_total = 0;
-    b->tn_elt = b->tn_nc = b->tn_bpp = b->tn_planes = 0;
-    if (b->tensor) {
-        b->tn_spec = *spec;
-        b->tn_swap.assign(nv, 0); b->tn_stage.assign(nv, 0); b->tn_plane.assign(nv, 0);
-        std::vector<uint8_t> tb(3 * 256 * 4);
-        b->tn_elt = jd_tensor_table(spec, tb.data());
-        b->tn_table.assign(3 * 256, 0u);
-        for (int k = 0; k < 3 * 256; k++) memcpy(&b->tn_table[k], tb.data() + (size_t)k * b->tn_elt, (size_t)b->tn_elt);
-    }
-    b->ctx = ctx;
-    b->n = (int)nv;
-    b->nf = n;
-    b->views = views != nullptr;
-    b->index_base = 0;
-    if ((options & JPEG_LUMA_ONLY) && pixel_type < EIGHT_BIT_GRAYSCALE) pixel_type = EIGHT_BIT_GRAYSCALE; /* jpeg.inl:4991 */
+    pixel_type = jd_fold_luma_only(pixel_type, options);
     b->pixel_type = pixel_type;
-    b->padded = (options & 0x10000) != 0; /* JPEGB200_OPT_PADDED (internal, jd_api.c) */
+    b->padded = (options & JPEGB200_OPT_PADDED) != 0;
     b->options = options;
     b->sshift = (options & JPEG_SCALE_HALF) ? 1 : (options & JPEG_SCALE_QUARTER) ? 2 : (options & JPEG_SCALE_EIGHTH) ? 3 : 0;
     b->gray_out = pixel_type >= EIGHT_BIT_GRAYSCALE;
     b->ptclass = (pixel_type == RGB8888) ? JD_PT_8888 : (b->gray_out ? JD_PT_GRAY : JD_PT_565);
     b->dither_bits = (pixel_type == FOUR_BIT_DITHERED) ? 4 : (pixel_type == TWO_BIT_DITHERED) ? 2 : (pixel_type == ONE_BIT_DITHERED) ? 1 : 0;
+    b->resize = P.out_sizes != nullptr;
+    b->rs_filter = filter;
+    if (b->resize) {
+        b->rs_plans.assign(nv, JDResizePlan{});
+        b->rs_src_w.assign(nv, 0); b->rs_src_h.assign(nv, 0); b->rs_scratch.assign(nv, 0);
+    }
+    b->lj = (options & JPEGB200_OPT_LIBJPEG) != 0;
+    if (b->lj) { b->lj_desc.assign(nv, JDLjDesc{}); b->lj_plane.assign(nv, 0); }
+    b->tensor = P.spec != nullptr;
     if (b->tensor) {
+        b->tn_spec = *P.spec;
+        b->tn_swap.assign(nv, 0); b->tn_stage.assign(nv, 0); b->tn_plane.assign(nv, 0);
+        std::vector<uint8_t> tb(3 * 256 * 4);
+        b->tn_elt = jd_tensor_table(P.spec, tb.data());
+        b->tn_table.assign(3 * 256, 0u);
+        for (int k = 0; k < 3 * 256; k++) memcpy(&b->tn_table[k], tb.data() + (size_t)k * b->tn_elt, (size_t)b->tn_elt);
         b->tn_nc = b->ptclass == JD_PT_8888 ? 3 : 1;
         b->tn_bpp = bytes_per_pixel_class(b->ptclass);
-        b->tn_planes = spec->layout == JPEGB200_LAYOUT_CHW ? b->tn_nc : 1;
+        b->tn_planes = P.spec->layout == JPEGB200_LAYOUT_CHW ? b->tn_nc : 1;
     }
-    b->stream = nullptr;
-    b->descs_dl = nullptr; b->descs_dl_bytes = 0; b->downloaded = false; b->h_counters = nullptr;
-    b->nchunks = 0; b->max_nch = 0; b->chunk_iterate = false; b->decode_flags = 0;
-    b->uploaded = false; b->out_device = false; b->arena_owned = false; b->have_ev = false;
-    memset(b->ms, 0, sizeof(b->ms));
-    memset(b->counters, 0, sizeof(b->counters));
     b->infos.resize(n);
     b->parse_status.assign(nv, JPEG_SUCCESS);
-    b->datas.assign(datas, datas + n);
-    b->sizes.assign(sizes, sizes + n);
+    b->datas.assign(P.datas, P.datas + n);
+    b->sizes.assign(P.sizes, P.sizes + n);
     b->descs.resize(nv);
     if (b->views) {
         b->fdescs.resize(n);
         b->vfile.resize(nv);
-        for (int f = 0, i = 0; f < n; f++) for (int k = 0; k < views[f]; k++) b->vfile[i++] = f;
+        for (int f = 0, i = 0; f < n; f++) for (int k = 0; k < P.views[f]; k++) b->vfile[i++] = f;
     }
     b->quant.assign((size_t)nv * 192, 0);   /* per view: the IDCT kernels index it by their descriptor's index */
     b->outs.assign(nv, nullptr);
     b->pitches.assign(nv, 0);
     b->comp_off.assign(n, 0);
     b->arena_off.assign(nv, 0);
+    b->pplane.assign(n, 0);
+}
 
-    /* input layout: one span if the files already sit back to back in host memory */
+/* input layout: one span if the files already sit back to back in host memory.  Writes contiguous_in, comp_off and
+ * comp_total; 0 with a message for a batch of 3 GiB or more. */
+static int layout_input(JPEGB200_BATCH *b)
+{
+    const int n = b->nf;
+    const std::vector<const uint8_t *> &datas = b->datas;
+    const std::vector<int32_t> &sizes = b->sizes;
     bool contig = true;
     for (int i = 1; i < n && contig; i++) {
         const uint8_t *prev_end = datas[i - 1] + sizes[i - 1];
@@ -719,293 +647,315 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
     if (b->comp_total >= (3ull << 30)) {
         /* byte offsets into the batch buffer (and into the un-stuffed copy, which adds 32 bytes per segment) are 32-bit */
         snprintf(g_err, sizeof(g_err), "batch holds %zu compressed bytes; one job takes at most 3 GiB (JPEGB200_decodeBatch splits larger batches)", b->comp_total);
-        delete b;
-        return nullptr;
+        return 0;
     }
+    return 1;
+}
 
-    std::vector<uint64_t> lut_hash;
-    std::vector<int> lut_owner;      /* first image that defined each LUT set: a hash match is confirmed on the DHT bytes */
-    uint32_t seg = 0;
-    b->nseg_walk = 0;
-    uint64_t blk = 0, rec_total = 0;
-    size_t out_total = 0, gray_total = 0;
-    std::vector<int32_t> srects(4 * (size_t)nv, 0), vok((size_t)nv, 0);
-    std::vector<uint8_t> ks(orients ? (size_t)nv : 0u, 0);
-    const bool prog_scans = (options & JPEGB200_OPT_PROGRESSIVE) != 0;
-    std::vector<JDProgScan> fscans(prog_scans ? JD_PROG_MAX_SCANS : 0);
-    std::vector<JDProgHuff> ftabs(prog_scans ? JD_PROG_MAX_TABS : 0);
-    std::unordered_map<uint64_t, std::vector<uint32_t>> ptab_index;   /* table content hash -> its indices in b->ptabs */
-    b->pplane.assign(n, 0);
-    b->pplane_total = 0;
-    b->pwalkers = 0;
-    for (int f = 0, v0 = 0; f < n; v0 += views ? views[f] : 1, f++) {
-        const int nvf = views ? views[f] : 1;   /* the file's views (images) are v0 .. v0 + nvf - 1 */
-        JDInfo &inf = b->infos[f];
-        JDImageDesc &d = file_descs(b)[f];
-        memset(&d, 0, sizeof(d));
-        int ok = jd_parse_header_opt(datas[f], sizes[f], 0, &inf, options);
-        int st = ok ? JPEG_SUCCESS : inf.error;
-        if (ok && (options & JPEG_EXIF_THUMBNAIL)) {
-            if (inf.thumb_data == 0 || inf.thumb_w == 0) { ok = 0; st = JPEG_INVALID_PARAMETER; }
-            else { ok = jd_parse_header_opt(datas[f], sizes[f], inf.thumb_data, &inf, options); if (!ok) st = inf.error; }
-        }
-        bool prog = false, full = false;   /* full: a progressive file decoded from all its scans (jd_prog.h) */
-        int nsc = 0, ntb = 0;
-        if (ok && inf.mode == 0xC2 && prog_scans) {
-            nsc = jd_prog_parse(datas[f], sizes[f], (options & JPEG_EXIF_THUMBNAIL) ? inf.thumb_data : 0, &inf, fscans.data(),
-                                ftabs.data(), &ntb);
-            if (nsc <= 0) { ok = 0; st = -nsc; } else full = true;
-        } else if (ok && inf.mode == 0xC2) {
-            /* progressive: like the reference, only the DC coefficients of the first scan are decoded and a 1/8-size image
-             * is produced (jpeg.inl:4964-4966, JPEGDecodeMCU_P :1819-1884).  That needs a first scan that is the interleaved
-             * DC scan of every component (Ss = Se = 0, Ah = 0) -- what every common encoder writes -- and 1/8 scale. */
-            prog = true;
-            if (b->sshift != 3 || inf.p.ncomp_in_scan != inf.ncomp || inf.p.scan_start != 0 || inf.p.scan_end != 0 || (inf.approx >> 4) != 0 ||
-                (inf.approx & 15) > 13) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }
-        } else if (ok && inf.mode != 0xC0) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }
-        if (ok && !full && !inf.tables_ok) { ok = 0; st = JPEG_DECODE_ERROR; }  /* jpeg.inl:2166 */
-        if (ok && inf.ncomp == 1 && pixel_type == RGB8888 && !b->lj) { ok = 0; st = JPEG_INVALID_PARAMETER; }
-        if (ok && b->lj && pixel_type == EIGHT_BIT_GRAYSCALE && !jd_lj_is_ycc(&inf)) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }
-        if (ok && (uint64_t)sizes[f] >= (512ull << 20)) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }   /* image-relative record indices are 32-bit */
-        const int file_ok = ok;
-        for (int i = v0; i < v0 + nvf; i++) {
-            b->exif_tag[i] = inf.orientation;
-            if (orients) {
-                /* 0: the file's tag (none or out of range: identity); 1-8: that transform; anything else is refused below */
-                const int k = orients[i] == 0 ? ((inf.orientation >= 1 && inf.orientation <= 8) ? inf.orientation : 1) : orients[i];
-                if (k <= 8) b->orient[i] = (uint8_t)k;
-                ks[i] = (uint8_t)k;
-            }
-        }
-        /* the views' own arguments (no such transform, a rectangle outside the output, a resize target outside 1..65535) and
-         * how deep the file is walked: down to the deepest last MCU row among its valid views */
-        uint32_t walk = 0;
-        if (ok) {
-            walk = (uint32_t)jd_views_plan(inf.width, inf.height, inf.subsample, inf.restart_interval, b->sshift, nvf,
-                                           rois ? rois + 4 * (size_t)v0 : nullptr, orients ? &ks[v0] : nullptr,
-                                           out_sizes ? out_sizes + 2 * (size_t)v0 : nullptr, &b->plans[v0], &srects[4 * (size_t)v0],
-                                           &vok[v0]);
-            if (walk != 0 && b->lj && b->roi) {
-                /* what libjpeg's fancy upsampling reads around each rectangle */
-                walk = 0;
-                for (int i = v0; i < v0 + nvf; i++) {
-                    if (!vok[i]) continue;
-                    const int32_t *sr = &srects[4 * (size_t)i];
-                    const int32_t r[4] = {sr[0], sr[1], orients ? sr[2] : rois[4 * (size_t)i + 2], orients ? sr[3] : rois[4 * (size_t)i + 3]};
-                    jd_lj_plan_extend(inf.width, inf.height, inf.subsample, inf.restart_interval, r, &b->plans[i]);
-                    if ((uint32_t)b->plans[i].nseg_walk > walk) walk = (uint32_t)b->plans[i].nseg_walk;
-                }
-            }
-            if (walk == 0) ok = 0;   /* no valid view: the file is not walked */
-        }
-        const uint32_t total_mcus = ok ? (uint32_t)inf.mcus_x * inf.mcus_y : 0u;
-        const uint32_t mps = inf.restart_interval ? (uint32_t)inf.restart_interval : total_mcus;
-        const uint32_t nseg = (ok && !full) ? (total_mcus + mps - 1) / mps : 0u;   /* a full progressive file has walkers instead */
-        /* no restart markers: one long dependent stream -> chunk-parallel decode */
-        const uint32_t nch = (ok && !prog && inf.restart_interval == 0 && nseg == 1 && sizes[f] - inf.scan_offset >= 4096)
-                                 ? ((uint32_t)(sizes[f] - inf.scan_offset) + JD_CHUNK_BYTES - 1) / JD_CHUNK_BYTES + 1 : 0u;
-        if (ok && jd_rec_extent((uint64_t)sizes[f], (uint32_t)inf.scan_offset, nseg, nch) > (1ull << 32)) {
-            ok = 0; st = JPEG_UNSUPPORTED_FEATURE;   /* its record indices would wrap onto its own first records */
-        }
-        /* a failed parse first, then the view's own arguments, then the record extent */
-        for (int i = v0; i < v0 + nvf; i++) b->parse_status[i] = (file_ok && !vok[i]) ? JPEG_INVALID_PARAMETER : st;
-        if (!ok) { /* keep harmless empty descriptors */
-            d.nseg = 0; d.seg_base = seg; d.blk_base = (uint32_t)blk; d.status = (uint32_t)st;
-            for (int i = v0; i < v0 + nvf; i++) {
-                JDImageDesc &vd = b->descs[i];
-                if (b->views) vd = d;
-                vd.status = (uint32_t)b->parse_status[i];
-            }
-            continue;
-        }
-        {   /* kernels read quant column-major ([c * 8 + r]) so a lane's column is one 16-byte load; one copy per view */
-            int16_t qn[192];
-            jd_build_quant(&inf, qn);
-            for (int i = v0; i < v0 + nvf; i++) {
-                int32_t *qt = &b->quant[(size_t)i * 192];
-                if (b->lj) { jd_lj_quant(&inf, qt); continue; }   /* islow dequantizes with the raw DQT values */
-                for (int cc = 0; cc < 3; cc++)
-                    for (int nn = 0; nn < 64; nn++) qt[cc * 64 + (nn & 7) * 8 + (nn >> 3)] = qn[cc * 64 + nn];
-            }
-        }
-        /* Huffman LUT set: dedupe on the raw DHT content (a full progressive file uses its scans' own tables instead) */
-        uint32_t li = 0;
-        if (!full) {
-        const uint64_t h = jd_tables_hash(&inf);
-        for (; li < lut_hash.size(); li++) if (lut_hash[li] == h && jd_tables_equal(&inf, &b->infos[lut_owner[li]])) break;
-        const bool shared = ctx->has_shared && ctx->shared_hash == h && ctx->shared_hash2 == jd_tables_hash2(&inf);
-        if (li == lut_hash.size()) {
-            lut_hash.push_back(h); lut_owner.push_back(f);
-            b->luts.resize((size_t)(li + 1) * JD_LUT_ENTRIES);
-            if (shared) memcpy(&b->luts[(size_t)li * JD_LUT_ENTRIES], ctx->shared_lut, JD_LUT_ENTRIES * 2);
-            else jd_build_lut(&inf, &b->luts[(size_t)li * JD_LUT_ENTRIES]);
-        }
-        if (shared) ctx->shared_hits++;
-        }
-        d.scan_off = (uint32_t)(b->comp_off[f] + inf.scan_offset);
-        d.scan_end = (uint32_t)(b->comp_off[f] + sizes[f]);
-        d.width = (uint16_t)inf.width; d.height = (uint16_t)inf.height;
-        d.mcus_x = (uint16_t)inf.mcus_x; d.mcus_y = (uint16_t)inf.mcus_y;
-        d.subsample = (uint8_t)inf.subsample; d.ncomp = (uint8_t)inf.ncomp; d.bpm = (uint8_t)inf.bpm; d.tsel = (uint8_t)inf.tsel;
-        d.mcus_per_seg = mps;
-        d.nseg = nseg;
-        d.nseg_walk = full ? 0u : b->roi ? walk : d.nseg;   /* a full progressive file has no restart segments to walk */
-        d.chunk_base = 0; d.nch = 0;
-        d.prog = prog ? (1u | ((uint32_t)(inf.approx & 15) << 8)) : 0u;
-        if (nch) {
-            d.chunk_base = b->nchunks;
-            d.nch = nch;
-            b->nchunks += d.nch;
-            if (d.nch > b->max_nch) b->max_nch = d.nch;
-            b->cimg_list.push_back((uint32_t)f);
-        }
-        d.seg_base = seg;
-        d.blk_base = (uint32_t)blk;
-        d.lutset = li;
-        /* coefficient records: image-relative indices (jd_core.h JD_REC_INDEX), one slot per restart segment and per chunk */
-        d.comp_off = (uint32_t)b->comp_off[f];
-        d.rec_base = rec_total;
-        if (full) {
-            /* walkers down to the deepest MCU row a valid view needs; records sized by jd_prog_rec_cap */
-            uint32_t rows = (uint32_t)inf.mcus_y;
-            if (b->roi) {
-                rows = 0;
-                for (int i = v0; i < v0 + nvf; i++) if (vok[i] && (uint32_t)b->plans[i].mcu_y1 + 1u > rows) rows = (uint32_t)b->plans[i].mcu_y1 + 1u;
-            }
-            const uint64_t cap = jd_prog_rec_cap((uint64_t)sizes[f], (uint32_t)nsc);
-            /* whole 16-byte chunks: the entropy walk of the next image stores its records as aligned 16-byte chunks */
-            rec_total += (cap + 15u) & ~(uint64_t)7;
-            b->pfiles.push_back(JDProgFile{cap, (uint32_t)f, rows});
-            b->pplane[f] = (int64_t)total_mcus * inf.bpm * 128;
-            b->pplane_total += b->pplane[f];
-            for (int k = 0; k < nsc; k++) {
-                JDProgScan s = fscans[k];
-                s.start += (uint32_t)b->comp_off[f]; s.end += (uint32_t)b->comp_off[f];
-                s.img = (uint32_t)f;
-                s.row_limit = rows;
-                const int ntab = (s.ss == 0 && s.ah != 0) ? 0 : s.ncs;   /* DC refinements read raw bits */
-                for (int i = 0; i < ntab; i++) {
-                    /* the batch's table list: dedupe on content */
-                    const JDProgHuff &t = ftabs[s.tab[i]];
-                    uint64_t th = 1469598103934665603ull;
-                    for (size_t q = 0; q < sizeof(t); q++) th = (th ^ ((const uint8_t *)&t)[q]) * 1099511628211ull;
-                    std::vector<uint32_t> &same = ptab_index[th];
-                    size_t q = 0;
-                    while (q < same.size() && memcmp(&b->ptabs[same[q]], &t, sizeof(t)) != 0) q++;
-                    if (q == same.size()) { same.push_back((uint32_t)b->ptabs.size()); b->ptabs.push_back(t); }
-                    s.tab[i] = same[q];
-                }
-                b->pscans.push_back(s);
-            }
-        } else {
-            rec_total += (uint64_t)JD_REC_PER_BYTE * (uint64_t)(((size_t)sizes[f] + 15) & ~(size_t)15) + (uint64_t)JD_REC_SLOT_SLACK * (d.nseg + d.nch + 1u);
-        }
+/* header parse (of the thumbnail with JPEG_EXIF_THUMBNAIL), progressive mode and the per-file refusals.  Writes infos[f],
+ * and P.fscans / P.ftabs for a file decoded from all its scans. */
+static FileAdmit admit_file(JPEGB200_BATCH *b, CreatePlan &P, int f)
+{
+    FileAdmit a;
+    JDInfo &inf = b->infos[f];
+    const uint8_t *data = P.datas[f];
+    const int size = P.sizes[f], options = b->options;
+    int ok = jd_parse_header_opt(data, size, 0, &inf, options);
+    int st = ok ? JPEG_SUCCESS : inf.error;
+    if (ok && (options & JPEG_EXIF_THUMBNAIL)) {
+        if (inf.thumb_data == 0 || inf.thumb_w == 0) { ok = 0; st = JPEG_INVALID_PARAMETER; }
+        else { ok = jd_parse_header_opt(data, size, inf.thumb_data, &inf, options); if (!ok) st = inf.error; }
+    }
+    if (ok && inf.mode == 0xC2 && (options & JPEGB200_OPT_PROGRESSIVE)) {
+        a.nsc = jd_prog_parse(data, size, (options & JPEG_EXIF_THUMBNAIL) ? inf.thumb_data : 0, &inf, P.fscans.data(),
+                              P.ftabs.data(), &a.ntb);
+        if (a.nsc <= 0) { ok = 0; st = -a.nsc; } else a.full = true;
+    } else if (ok && inf.mode == 0xC2) {
+        /* progressive: like the reference, only the DC coefficients of the first scan are decoded and a 1/8-size image
+         * is produced (jpeg.inl:4964-4966, JPEGDecodeMCU_P :1819-1884).  That needs a first scan that is the interleaved
+         * DC scan of every component (Ss = Se = 0, Ah = 0) -- what every common encoder writes -- and 1/8 scale. */
+        a.prog = true;
+        if (b->sshift != 3 || inf.p.ncomp_in_scan != inf.ncomp || inf.p.scan_start != 0 || inf.p.scan_end != 0 || (inf.approx >> 4) != 0 ||
+            (inf.approx & 15) > 13) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }
+    } else if (ok && inf.mode != 0xC0) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }
+    if (ok && !a.full && !inf.tables_ok) { ok = 0; st = JPEG_DECODE_ERROR; }  /* jpeg.inl:2166 */
+    if (ok && inf.ncomp == 1 && b->pixel_type == RGB8888 && !b->lj) { ok = 0; st = JPEG_INVALID_PARAMETER; }
+    if (ok && b->lj && b->pixel_type == EIGHT_BIT_GRAYSCALE && !jd_lj_is_ycc(&inf)) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }
+    if (ok && (uint64_t)size >= (512ull << 20)) { ok = 0; st = JPEG_UNSUPPORTED_FEATURE; }   /* image-relative record indices are 32-bit */
+    a.ok = ok; a.status = st;
+    return a;
+}
 
-        /* the views: the file's descriptor (its walk, blocks and records) with each view's rectangle, orientation and output.
-         * The file's own descriptor keeps roi_mcu_end = 0: jdk_stitch reports its first error, jd_view_err_mcu judges it
-         * per view. */
-        const int s = b->sshift;
+/* the transform of each of the file's views v0 .. v0 + nvf - 1.  Writes exif_tag, orient and P.ks. */
+static void resolve_orients(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int nvf)
+{
+    const JDInfo &inf = b->infos[f];
+    for (int i = v0; i < v0 + nvf; i++) {
+        b->exif_tag[i] = inf.orientation;
+        if (P.orients) {
+            /* 0: the file's tag (none or out of range: identity); 1-8: that transform; anything else is refused by jd_views_plan */
+            const int k = P.orients[i] == 0 ? ((inf.orientation >= 1 && inf.orientation <= 8) ? inf.orientation : 1) : P.orients[i];
+            if (k <= 8) b->orient[i] = (uint8_t)k;
+            P.ks[i] = (uint8_t)k;
+        }
+    }
+}
+
+/* The views' own arguments (no such transform, a rectangle outside the output, a resize target outside 1..65535) and how
+ * deep the file is walked: down to the deepest last MCU row among its valid views.  Writes plans, P.srects and P.vok;
+ * returns the restart intervals to walk, 0 when no view is valid. */
+static uint32_t plan_views(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int nvf)
+{
+    const JDInfo &inf = b->infos[f];
+    uint32_t walk = (uint32_t)jd_views_plan(inf.width, inf.height, inf.subsample, inf.restart_interval, b->sshift, nvf,
+                                            P.rois ? P.rois + 4 * (size_t)v0 : nullptr, P.orients ? &P.ks[v0] : nullptr,
+                                            P.out_sizes ? P.out_sizes + 2 * (size_t)v0 : nullptr, &b->plans[v0], &P.srects[4 * (size_t)v0],
+                                            &P.vok[v0]);
+    if (walk != 0 && b->lj && b->roi) {
+        /* what libjpeg's fancy upsampling reads around each rectangle */
+        walk = 0;
         for (int i = v0; i < v0 + nvf; i++) {
+            if (!P.vok[i]) continue;
+            const int32_t *sr = &P.srects[4 * (size_t)i];
+            const int32_t r[4] = {sr[0], sr[1], P.orients ? sr[2] : P.rois[4 * (size_t)i + 2], P.orients ? sr[3] : P.rois[4 * (size_t)i + 3]};
+            jd_lj_plan_extend(inf.width, inf.height, inf.subsample, inf.restart_interval, r, &b->plans[i]);
+            if ((uint32_t)b->plans[i].nseg_walk > walk) walk = (uint32_t)b->plans[i].nseg_walk;
+        }
+    }
+    return walk;
+}
+
+/* restart segments and chunks of the file (none when it is not walked), and the refusal of a file whose records would not
+ * fit 32-bit image-relative indices */
+static void size_file_walk(const JPEGB200_BATCH *b, int f, FileAdmit &a)
+{
+    const JDInfo &inf = b->infos[f];
+    const int size = b->sizes[f];
+    a.total_mcus = a.ok ? (uint32_t)inf.mcus_x * inf.mcus_y : 0u;
+    a.mps = inf.restart_interval ? (uint32_t)inf.restart_interval : a.total_mcus;
+    a.nseg = (a.ok && !a.full) ? (a.total_mcus + a.mps - 1) / a.mps : 0u;   /* a full progressive file has walkers instead */
+    /* no restart markers: one long dependent stream -> chunk-parallel decode */
+    a.nch = (a.ok && !a.prog && inf.restart_interval == 0 && a.nseg == 1 && size - inf.scan_offset >= 4096)
+                ? ((uint32_t)(size - inf.scan_offset) + JD_CHUNK_BYTES - 1) / JD_CHUNK_BYTES + 1 : 0u;
+    if (a.ok && jd_rec_extent((uint64_t)size, (uint32_t)inf.scan_offset, a.nseg, a.nch) > (1ull << 32)) {
+        a.ok = 0; a.status = JPEG_UNSUPPORTED_FEATURE;   /* its record indices would wrap onto its own first records */
+    }
+}
+
+/* a file that is not walked: harmless empty descriptors for it and its views */
+static void fill_refused_descs(JPEGB200_BATCH *b, const CreatePlan &P, int f, int v0, int nvf, int status)
+{
+    JDImageDesc &d = file_descs(b)[f];
+    d.nseg = 0; d.seg_base = P.seg; d.blk_base = (uint32_t)P.blk; d.status = (uint32_t)status;
+    for (int i = v0; i < v0 + nvf; i++) {
         JDImageDesc &vd = b->descs[i];
-        if (b->views) {
-            if (b->parse_status[i] != JPEG_SUCCESS) {   /* an invalid view of a walked file: empty, like a refused image */
-                memset(&vd, 0, sizeof(vd));
-                vd.seg_base = seg; vd.blk_base = (uint32_t)blk; vd.status = (uint32_t)b->parse_status[i];
-                continue;
-            }
-            vd = d;
-        }
-        vd.out_w = (uint32_t)((inf.width + (1 << s) - 1) >> s);
-        vd.out_h = (uint32_t)((inf.height + (1 << s) - 1) >> s);
-        if (b->padded) {
-            vd.out_w = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> s);
-            vd.out_h = (uint32_t)inf.mcus_y * (uint32_t)(inf.mcu_h >> s);
-        }
-        if (b->roi) {
-            const JDRoiPlan &pl = b->plans[i];
-            vd.out_w = (uint32_t)pl.out_w; vd.out_h = (uint32_t)pl.out_h;
-            vd.roi_x = (uint16_t)srects[4 * (size_t)i]; vd.roi_y = (uint16_t)srects[4 * (size_t)i + 1];
-            vd.mcu_x0 = (uint16_t)pl.mcu_x0; vd.mcu_y0 = (uint16_t)pl.mcu_y0;
-            vd.roi_mcu_end = (uint32_t)pl.mcu_end;
-            vd.orient = orients ? b->orient[i] : 0u;
-        }
-        if (b->lj) {
-            /* the MCU box whose planes jdk_lj_idct writes: the rectangle's, extended by jd_lj_plan_extend */
-            JDLjDesc &L = b->lj_desc[i];
-            L.mx0 = b->roi ? (uint32_t)b->plans[i].mcu_x0 : 0u; L.my0 = b->roi ? (uint32_t)b->plans[i].mcu_y0 : 0u;
-            L.nmx = b->roi ? (uint32_t)(b->plans[i].mcu_x1 - b->plans[i].mcu_x0 + 1) : (uint32_t)inf.mcus_x;
-            L.nmy = b->roi ? (uint32_t)(b->plans[i].mcu_y1 - b->plans[i].mcu_y0 + 1) : (uint32_t)inf.mcus_y;
-            L.ycc = (uint32_t)jd_lj_is_ycc(&inf);
-            const uint64_t blocks = (uint64_t)L.nmx * L.nmy * (uint64_t)inf.bpm;
-            b->lj_plane[i] = (int64_t)((blocks * 64u + 255u) & ~(uint64_t)255);
-            b->lj_plane_total += b->lj_plane[i];
-            if (blocks > b->lj_max_blocks) b->lj_max_blocks = (uint32_t)blocks;
-            const uint64_t px = (uint64_t)vd.out_w * vd.out_h;
-            if (px > b->lj_max_pixels) b->lj_max_pixels = (uint32_t)px;
-        }
-        if (b->resize) {
-            /* S = what the same call without out_sizes stores; the descriptor carries the resized size from here on */
-            const int bp = bytes_per_pixel_class(b->ptclass);
-            JDResizePlan &rp = b->rs_plans[i];
-            const int32_t rw = out_sizes[2 * (size_t)i], rh = out_sizes[2 * (size_t)i + 1];
-            if (!jd_resize_plan((int)vd.out_w, (int)vd.out_h, rw, rh, filter, bp, &rp)) {
-                snprintf(g_err, sizeof(g_err), "resize plan failed for image %d", i); delete b; return nullptr;
-            }
-            b->rs_src_w[i] = vd.out_w; b->rs_src_h[i] = vd.out_h;
-            b->rs_scratch[i] = (int64_t)(((size_t)vd.out_w * vd.out_h * bp + 255) & ~(size_t)255) + ((rp.mid_bytes + 255) & ~(int64_t)255);
-            b->rs_scratch_total += b->rs_scratch[i];
-            vd.out_w = (uint32_t)rw; vd.out_h = (uint32_t)rh;
-        }
-        if (b->tensor) {
-            /* U = what the same call without spec stores (out_w x out_h); staged, then converted */
-            b->tn_stage[i] = (int64_t)(((size_t)vd.out_w * vd.out_h * b->tn_bpp + 255) & ~(size_t)255);
-            b->tn_stage_total += b->tn_stage[i];
-            /* a libjpeg decode stores R, G, B for every file */
-            const bool bgr = !b->lj && jd_rgb8888_is_bgr(ctx->arith, b->sshift, inf.ncomp, inf.subsample) != 0;
-            b->tn_swap[i] = (uint8_t)(b->tn_nc == 3 && bgr != (spec->bgr != 0));
-        }
-        size_t pitch;
-        if (b->tensor) pitch = (size_t)vd.out_w * (spec->layout == JPEGB200_LAYOUT_HWC ? b->tn_nc : 1) * b->tn_elt;
-        else if (b->dither_bits) {
-            const uint32_t pw = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> s);
-            pitch = ((size_t)pw * b->dither_bits + 7) / 8;
-            gray_total += (((size_t)pw * (size_t)inf.mcus_y * (size_t)(inf.mcu_h >> s)) + 255) & ~(size_t)255;
-        } else pitch = (size_t)vd.out_w * bytes_per_pixel_class(b->ptclass);
-        vd.out_pitch = (uint32_t)pitch;
-        b->pitches[i] = (int64_t)pitch;
-        b->arena_off[i] = out_total;
-        out_total += (pitch * vd.out_h * (b->tensor ? (size_t)b->tn_planes : 1u) + 255) & ~(size_t)255;
-        }
-        seg += d.nseg;
-        b->nseg_walk += d.nseg_walk;
-        blk += (uint64_t)total_mcus * inf.bpm;
-        if (blk >= (1ull << 32)) { snprintf(g_err, sizeof(g_err), "batch too large (block count)"); delete b; return nullptr; }
+        if (b->views) vd = d;
+        vd.status = (uint32_t)b->parse_status[i];
     }
-    b->nseg = seg; b->nblk = blk; b->nlut = (uint32_t)lut_hash.size();
-    b->rec_total = rec_total;
-    if (!b->pscans.empty()) {
-        /* one launch per wave; inside a wave the longest scans start first */
-        std::stable_sort(b->pscans.begin(), b->pscans.end(), [](const JDProgScan &x, const JDProgScan &y) {
-            return x.wave != y.wave ? x.wave < y.wave : (x.end - x.start) > (y.end - y.start);
-        });
-        for (size_t k = 0; k < b->pscans.size(); k++)
-            while (b->pwave_off.size() <= b->pscans[k].wave) b->pwave_off.push_back((uint32_t)k);
-        b->pwave_off.push_back((uint32_t)b->pscans.size());
+}
+
+/* kernels read quant column-major ([c * 8 + r]) so a lane's column is one 16-byte load; one copy per view */
+static void fill_quant(JPEGB200_BATCH *b, int f, int v0, int nvf)
+{
+    const JDInfo &inf = b->infos[f];
+    int16_t qn[192];
+    jd_build_quant(&inf, qn);
+    for (int i = v0; i < v0 + nvf; i++) {
+        int32_t *qt = &b->quant[(size_t)i * 192];
+        if (b->lj) { jd_lj_quant(&inf, qt); continue; }   /* islow dequantizes with the raw DQT values */
+        for (int cc = 0; cc < 3; cc++)
+            for (int nn = 0; nn < 64; nn++) qt[cc * 64 + (nn & 7) * 8 + (nn >> 3)] = qn[cc * 64 + nn];
     }
-    if ((uint64_t)b->comp_total + 32ull * seg + 4096ull >= (1ull << 32)) {
-        snprintf(g_err, sizeof(g_err), "batch too large (%zu compressed bytes in %u restart segments)", b->comp_total, seg);
-        delete b;
-        return nullptr;
+}
+
+/* Huffman LUT set of the file: dedupe on the raw DHT content.  Appends to luts; counts a hit of the context's shared table. */
+static uint32_t lut_set_for(JPEGB200_BATCH *b, CreatePlan &P, int f)
+{
+    JPEGB200_CTX *ctx = b->ctx;
+    const JDInfo &inf = b->infos[f];
+    uint32_t li = 0;
+    const uint64_t h = jd_tables_hash(&inf);
+    for (; li < P.lut_hash.size(); li++) if (P.lut_hash[li] == h && jd_tables_equal(&inf, &b->infos[P.lut_owner[li]])) break;
+    const bool shared = ctx->has_shared && ctx->shared_hash == h && ctx->shared_hash2 == jd_tables_hash2(&inf);
+    if (li == P.lut_hash.size()) {
+        P.lut_hash.push_back(h); P.lut_owner.push_back(f);
+        b->luts.resize((size_t)(li + 1) * JD_LUT_ENTRIES);
+        if (shared) memcpy(&b->luts[(size_t)li * JD_LUT_ENTRIES], ctx->shared_lut, JD_LUT_ENTRIES * 2);
+        else jd_build_lut(&inf, &b->luts[(size_t)li * JD_LUT_ENTRIES]);
     }
-    b->out_total = out_total; b->gray_total = gray_total;
-    /* work list: CTAs of 128 segments sharing one LUT set.  With a region of interest the restart intervals that start
-     * below its last MCU row are left out, but every interval above it stays in: the reference's bit-window phase is
-     * carried from one interval to the next (SURVEY.md fact 4, A.2), so the pixels inside the rectangle depend on the walk
-     * of every interval before them.  One entry per file: its views share the walk. */
-    b->seg_img.resize(seg ? seg : 1);
+    if (shared) ctx->shared_hits++;
+    return li;
+}
+
+/* the entropy-facing descriptor of an admitted file; a restart-free file joins the chunk list (nchunks, max_nch, cimg_list) */
+static void fill_file_desc(JPEGB200_BATCH *b, const CreatePlan &P, int f, const FileAdmit &a, uint32_t walk, uint32_t lutset)
+{
+    const JDInfo &inf = b->infos[f];
+    JDImageDesc &d = file_descs(b)[f];
+    d.scan_off = (uint32_t)(b->comp_off[f] + inf.scan_offset);
+    d.scan_end = (uint32_t)(b->comp_off[f] + b->sizes[f]);
+    d.width = (uint16_t)inf.width; d.height = (uint16_t)inf.height;
+    d.mcus_x = (uint16_t)inf.mcus_x; d.mcus_y = (uint16_t)inf.mcus_y;
+    d.subsample = (uint8_t)inf.subsample; d.ncomp = (uint8_t)inf.ncomp; d.bpm = (uint8_t)inf.bpm; d.tsel = (uint8_t)inf.tsel;
+    d.mcus_per_seg = a.mps;
+    d.nseg = a.nseg;
+    d.nseg_walk = a.full ? 0u : b->roi ? walk : d.nseg;   /* a full progressive file has no restart segments to walk */
+    d.chunk_base = 0; d.nch = 0;
+    d.prog = a.prog ? (1u | ((uint32_t)(inf.approx & 15) << 8)) : 0u;
+    if (a.nch) {
+        d.chunk_base = b->nchunks;
+        d.nch = a.nch;
+        b->nchunks += d.nch;
+        if (d.nch > b->max_nch) b->max_nch = d.nch;
+        b->cimg_list.push_back((uint32_t)f);
+    }
+    d.seg_base = P.seg;
+    d.blk_base = (uint32_t)P.blk;
+    d.lutset = lutset;
+    /* coefficient records: image-relative indices (jd_core.h JD_REC_INDEX), one slot per restart segment and per chunk */
+    d.comp_off = (uint32_t)b->comp_off[f];
+    d.rec_base = P.rec_total;
+}
+
+/* a file decoded from all its scans: its walkers (pscans) down to the deepest MCU row a valid view needs, its record cap
+ * (pfiles, P.rec_total), its coefficient plane (pplane) and its tables, de-duplicated on content (ptabs) */
+static void add_prog_file(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int nvf, const FileAdmit &a)
+{
+    const JDInfo &inf = b->infos[f];
+    uint32_t rows = (uint32_t)inf.mcus_y;
+    if (b->roi) {
+        rows = 0;
+        for (int i = v0; i < v0 + nvf; i++) if (P.vok[i] && (uint32_t)b->plans[i].mcu_y1 + 1u > rows) rows = (uint32_t)b->plans[i].mcu_y1 + 1u;
+    }
+    const uint64_t cap = jd_prog_rec_cap((uint64_t)b->sizes[f], (uint32_t)a.nsc);   /* records sized by jd_prog_rec_cap */
+    /* whole 16-byte chunks: the entropy walk of the next image stores its records as aligned 16-byte chunks */
+    P.rec_total += (cap + 15u) & ~(uint64_t)7;
+    b->pfiles.push_back(JDProgFile{cap, (uint32_t)f, rows});
+    b->pplane[f] = (int64_t)a.total_mcus * inf.bpm * 128;
+    b->pplane_total += b->pplane[f];
+    for (int k = 0; k < a.nsc; k++) {
+        JDProgScan s = P.fscans[k];
+        s.start += (uint32_t)b->comp_off[f]; s.end += (uint32_t)b->comp_off[f];
+        s.img = (uint32_t)f;
+        s.row_limit = rows;
+        const int ntab = (s.ss == 0 && s.ah != 0) ? 0 : s.ncs;   /* DC refinements read raw bits */
+        for (int i = 0; i < ntab; i++) {
+            const JDProgHuff &t = P.ftabs[s.tab[i]];
+            uint64_t th = 1469598103934665603ull;
+            for (size_t q = 0; q < sizeof(t); q++) th = (th ^ ((const uint8_t *)&t)[q]) * 1099511628211ull;
+            std::vector<uint32_t> &same = P.ptab_index[th];
+            size_t q = 0;
+            while (q < same.size() && memcmp(&b->ptabs[same[q]], &t, sizeof(t)) != 0) q++;
+            if (q == same.size()) { same.push_back((uint32_t)b->ptabs.size()); b->ptabs.push_back(t); }
+            s.tab[i] = same[q];
+        }
+        b->pscans.push_back(s);
+    }
+}
+
+/* View i of admitted file f: the file's descriptor (its walk, blocks and records) with the view's rectangle, orientation and
+ * output.  Writes descs[i], pitches[i], arena_off[i] and the view's libjpeg box, resize plan + scratch and tensor staging;
+ * advances P.out_total / P.gray_total.  The file's own descriptor keeps roi_mcu_end = 0: jdk_stitch reports its first
+ * error, jd_view_err_mcu judges it per view.  0 with a message when the resize cannot be planned. */
+static int plan_view_output(JPEGB200_BATCH *b, CreatePlan &P, int f, int i)
+{
+    const JDInfo &inf = b->infos[f];
+    const int s = b->sshift;
+    JDImageDesc &vd = b->descs[i];
+    if (b->views) {
+        if (b->parse_status[i] != JPEG_SUCCESS) {   /* an invalid view of a walked file: empty, like a refused image */
+            memset(&vd, 0, sizeof(vd));
+            vd.seg_base = P.seg; vd.blk_base = (uint32_t)P.blk; vd.status = (uint32_t)b->parse_status[i];
+            return 1;
+        }
+        vd = b->fdescs[f];
+    }
+    vd.out_w = (uint32_t)((inf.width + (1 << s) - 1) >> s);
+    vd.out_h = (uint32_t)((inf.height + (1 << s) - 1) >> s);
+    if (b->padded) {
+        vd.out_w = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> s);
+        vd.out_h = (uint32_t)inf.mcus_y * (uint32_t)(inf.mcu_h >> s);
+    }
+    if (b->roi) {
+        const JDRoiPlan &pl = b->plans[i];
+        vd.out_w = (uint32_t)pl.out_w; vd.out_h = (uint32_t)pl.out_h;
+        vd.roi_x = (uint16_t)P.srects[4 * (size_t)i]; vd.roi_y = (uint16_t)P.srects[4 * (size_t)i + 1];
+        vd.mcu_x0 = (uint16_t)pl.mcu_x0; vd.mcu_y0 = (uint16_t)pl.mcu_y0;
+        vd.roi_mcu_end = (uint32_t)pl.mcu_end;
+        vd.orient = P.orients ? b->orient[i] : 0u;
+    }
+    if (b->lj) {
+        /* the MCU box whose planes jdk_lj_idct writes: the rectangle's, extended by jd_lj_plan_extend */
+        JDLjDesc &L = b->lj_desc[i];
+        L.mx0 = b->roi ? (uint32_t)b->plans[i].mcu_x0 : 0u; L.my0 = b->roi ? (uint32_t)b->plans[i].mcu_y0 : 0u;
+        L.nmx = b->roi ? (uint32_t)(b->plans[i].mcu_x1 - b->plans[i].mcu_x0 + 1) : (uint32_t)inf.mcus_x;
+        L.nmy = b->roi ? (uint32_t)(b->plans[i].mcu_y1 - b->plans[i].mcu_y0 + 1) : (uint32_t)inf.mcus_y;
+        L.ycc = (uint32_t)jd_lj_is_ycc(&inf);
+        const uint64_t blocks = (uint64_t)L.nmx * L.nmy * (uint64_t)inf.bpm;
+        b->lj_plane[i] = (int64_t)align256(blocks * 64u);
+        b->lj_plane_total += b->lj_plane[i];
+        if (blocks > b->lj_max_blocks) b->lj_max_blocks = (uint32_t)blocks;
+        const uint64_t px = (uint64_t)vd.out_w * vd.out_h;
+        if (px > b->lj_max_pixels) b->lj_max_pixels = (uint32_t)px;
+    }
+    if (b->resize) {
+        /* S = what the same call without out_sizes stores; the descriptor carries the resized size from here on */
+        const int bp = bytes_per_pixel_class(b->ptclass);
+        JDResizePlan &rp = b->rs_plans[i];
+        const int32_t rw = P.out_sizes[2 * (size_t)i], rh = P.out_sizes[2 * (size_t)i + 1];
+        if (!jd_resize_plan((int)vd.out_w, (int)vd.out_h, rw, rh, b->rs_filter, bp, &rp)) {
+            snprintf(g_err, sizeof(g_err), "resize plan failed for image %d", i);
+            return 0;
+        }
+        b->rs_src_w[i] = vd.out_w; b->rs_src_h[i] = vd.out_h;
+        b->rs_scratch[i] = (int64_t)align256((size_t)vd.out_w * vd.out_h * bp) + (int64_t)align256((size_t)rp.mid_bytes);
+        b->rs_scratch_total += b->rs_scratch[i];
+        vd.out_w = (uint32_t)rw; vd.out_h = (uint32_t)rh;
+    }
+    if (b->tensor) {
+        /* U = what the same call without spec stores (out_w x out_h); staged, then converted */
+        b->tn_stage[i] = (int64_t)align256((size_t)vd.out_w * vd.out_h * b->tn_bpp);
+        b->tn_stage_total += b->tn_stage[i];
+        /* a libjpeg decode stores R, G, B for every file */
+        const bool bgr = !b->lj && jd_rgb8888_is_bgr(b->ctx->arith, b->sshift, inf.ncomp, inf.subsample) != 0;
+        b->tn_swap[i] = (uint8_t)(b->tn_nc == 3 && bgr != (b->tn_spec.bgr != 0));
+    }
+    size_t pitch;
+    if (b->tensor) pitch = (size_t)vd.out_w * (b->tn_spec.layout == JPEGB200_LAYOUT_HWC ? b->tn_nc : 1) * b->tn_elt;
+    else if (b->dither_bits) {
+        const uint32_t pw = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> s);
+        pitch = ((size_t)pw * b->dither_bits + 7) / 8;
+        P.gray_total += align256((size_t)pw * (size_t)inf.mcus_y * (size_t)(inf.mcu_h >> s));
+    } else pitch = (size_t)vd.out_w * bytes_per_pixel_class(b->ptclass);
+    vd.out_pitch = (uint32_t)pitch;
+    b->pitches[i] = (int64_t)pitch;
+    b->arena_off[i] = P.out_total;
+    P.out_total += align256(pitch * vd.out_h * (b->tensor ? (size_t)b->tn_planes : 1u));
+    return 1;
+}
+
+/* one launch per wave of scan walkers; inside a wave the longest scans start first.  Sorts pscans, writes pwave_off. */
+static void sort_prog_waves(JPEGB200_BATCH *b)
+{
+    if (b->pscans.empty()) return;
+    std::stable_sort(b->pscans.begin(), b->pscans.end(), [](const JDProgScan &x, const JDProgScan &y) {
+        return x.wave != y.wave ? x.wave < y.wave : (x.end - x.start) > (y.end - y.start);
+    });
+    for (size_t k = 0; k < b->pscans.size(); k++)
+        while (b->pwave_off.size() <= b->pscans[k].wave) b->pwave_off.push_back((uint32_t)k);
+    b->pwave_off.push_back((uint32_t)b->pscans.size());
+}
+
+/* Work list (work, cta_lut, seg_img): CTAs of 128 segments sharing one LUT set.  With a region of interest the restart
+ * intervals that start below its last MCU row are left out, but every interval above it stays in: the reference's
+ * bit-window phase is carried from one interval to the next (SURVEY.md fact 4, A.2), so the pixels inside the rectangle
+ * depend on the walk of every interval before them.  One entry per file: its views share the walk. */
+static void build_work_list(JPEGB200_BATCH *b)
+{
+    b->seg_img.resize(b->nseg ? b->nseg : 1);
     const std::vector<JDImageDesc> &fd = file_descs(b);
     for (uint32_t li = 0; li < (b->nlut ? b->nlut : 1); li++) {
-        for (int i = 0; i < n; i++) {
+        for (int i = 0; i < b->nf; i++) {
             const JDImageDesc &d = fd[i];
             if (d.nseg == 0 || d.lutset != li) continue;   /* nseg = 0: a file that is not walked */
             for (uint32_t s2 = 0; s2 < d.nseg; s2++) {
@@ -1016,6 +966,70 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
         while (b->work.size() % JD_ENTROPY_THREADS) b->work.push_back(JD_NONE);
         while (b->cta_lut.size() < b->work.size() / JD_ENTROPY_THREADS) b->cta_lut.push_back(li);
     }
+}
+
+/* every file in turn: admission, its views' plans, its descriptor and tables, its views' outputs.  0 with a message when
+ * the batch as a whole is refused. */
+static int plan_files(JPEGB200_BATCH *b, CreatePlan &P)
+{
+    for (int f = 0, v0 = 0; f < b->nf; v0 += P.views ? P.views[f] : 1, f++) {
+        const int nvf = P.views ? P.views[f] : 1;   /* the file's views (images) are v0 .. v0 + nvf - 1 */
+        const JDInfo &inf = b->infos[f];
+        memset(&file_descs(b)[f], 0, sizeof(JDImageDesc));
+        FileAdmit a = admit_file(b, P, f);
+        const int file_ok = a.ok;
+        resolve_orients(b, P, f, v0, nvf);
+        uint32_t walk = 0;
+        if (a.ok) {
+            walk = plan_views(b, P, f, v0, nvf);
+            if (walk == 0) a.ok = 0;   /* no valid view: the file is not walked */
+        }
+        size_file_walk(b, f, a);
+        /* a failed parse first, then the view's own arguments, then the record extent */
+        for (int i = v0; i < v0 + nvf; i++) b->parse_status[i] = (file_ok && !P.vok[i]) ? JPEG_INVALID_PARAMETER : a.status;
+        if (!a.ok) { fill_refused_descs(b, P, f, v0, nvf, a.status); continue; }
+        fill_quant(b, f, v0, nvf);
+        const uint32_t lutset = a.full ? 0u : lut_set_for(b, P, f);   /* a full progressive file uses its scans' own tables */
+        fill_file_desc(b, P, f, a, walk, lutset);
+        if (a.full) add_prog_file(b, P, f, v0, nvf, a);
+        else P.rec_total += (uint64_t)JD_REC_PER_BYTE * (uint64_t)(((size_t)b->sizes[f] + 15) & ~(size_t)15) + (uint64_t)JD_REC_SLOT_SLACK * (a.nseg + a.nch + 1u);
+        for (int i = v0; i < v0 + nvf; i++) if (!plan_view_output(b, P, f, i)) return 0;
+        P.seg += a.nseg;
+        b->nseg_walk += file_descs(b)[f].nseg_walk;
+        P.blk += (uint64_t)a.total_mcus * inf.bpm;
+        if (P.blk >= (1ull << 32)) { snprintf(g_err, sizeof(g_err), "batch too large (block count)"); return 0; }
+    }
+    b->nseg = P.seg; b->nblk = P.blk; b->nlut = (uint32_t)P.lut_hash.size();
+    b->rec_total = P.rec_total;
+    b->out_total = P.out_total; b->gray_total = P.gray_total;
+    if ((uint64_t)b->comp_total + 32ull * P.seg + 4096ull >= (1ull << 32)) {
+        snprintf(g_err, sizeof(g_err), "batch too large (%zu compressed bytes in %u restart segments)", b->comp_total, P.seg);
+        return 0;
+    }
+    return 1;
+}
+
+extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                                     const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                                     const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                                     const JPEGB200_TensorSpec *spec)
+{
+    if (!ctx) { snprintf(g_err, sizeof(g_err), "invalid parameter"); return nullptr; }
+    int64_t nv = 0;   /* images of the batch: views */
+    if (!jd_check_batch_features(pixel_type, options, n, views, rois != nullptr, orients != nullptr, out_sizes != nullptr, filter, spec,
+                                 &nv, g_err, (int)sizeof(g_err)))
+        return nullptr;
+    JPEGB200_BATCH *b = new (std::nothrow) JPEGB200_BATCH();
+    if (!b) return nullptr;
+    CreatePlan P;
+    P.datas = datas; P.sizes = sizes; P.views = views; P.rois = rois; P.orients = orients; P.out_sizes = out_sizes; P.spec = spec;
+    P.srects.assign(4 * (size_t)nv, 0); P.vok.assign((size_t)nv, 0);
+    P.ks.assign(orients ? (size_t)nv : 0u, 0);
+    if (options & JPEGB200_OPT_PROGRESSIVE) { P.fscans.resize(JD_PROG_MAX_SCANS); P.ftabs.resize(JD_PROG_MAX_TABS); }
+    init_batch(b, ctx, P, n, (int)nv, pixel_type, options, filter);
+    if (!layout_input(b) || !plan_files(b, P)) { delete b; return nullptr; }
+    sort_prog_waves(b);
+    build_work_list(b);
     return b;
 }
 
@@ -1023,32 +1037,11 @@ extern "C" void JPEGB200_batchDestroy(JPEGB200_BATCH *b)
 {
     if (!b) return;
     cudaSetDevice(b->ctx->device);
-    if (b->stream) cudaStreamSynchronize(b->stream);
-    b->d_comp.release(); b->d_out.release(); b->d_gray.release(); b->d_errline.release();
-    b->d_gray_off.release(); b->d_err_off.release(); b->d_dprog.release(); b->d_dbands.release();
-    b->d_clean.release(); b->d_seg_clen.release();
-    b->d_filt.release(); b->d_cimg_list.release(); b->d_flen.release(); b->d_E0.release(); b->d_E1.release(); b->d_Ep.release(); b->d_cfirst.release();
-    b->d_cn.release(); b->d_cpre.release(); b->d_cjmap.release(); b->d_cstatus.release(); b->d_cnown.release(); b->d_cdcs.release(); b->d_cpe.release();
-    b->d_descs.release(); b->d_fdescs.release(); b->d_quant.release(); b->d_luts.release(); b->d_rec.release();
-    b->d_work.release(); b->d_cta_lut.release(); b->d_seg_img.release(); b->d_seg_start.release();
-    b->d_seg_jmap.release(); b->d_seg_status.release(); b->d_seg_nrec.release(); b->d_seg_phase.release();
-    b->d_counters.release(); b->d_blk_hdr.release(); b->d_events.release();
-    for (auto &pl : b->d_pplane) pl.release();
-    b->d_pscans.release(); b->d_ptabs.release(); b->d_pfiles.release(); b->d_pplanes.release(); b->d_perr.release();
-    b->d_rs.release(); b->d_rs_coef.release(); b->d_rs_desc.release();
-    b->d_tn.release(); b->d_tn_tab.release(); b->d_tn_desc.release();
-    b->d_lj.release(); b->d_lj_desc.release();
-    if (b->stream && b->have_ev) {   /* back to the context for the next job */
-        JDStreamSet ss;
-        ss.stream = b->stream;
-        for (int i = 0; i < JPEGB200_NUM_TIMINGS + 2; i++) ss.ev[i] = b->ev[i];
-        b->ctx->free_streams.push_back(ss);
-    } else {
-        if (b->have_ev) for (auto &e : b->ev) cudaEventDestroy(e);
-        if (b->stream) cudaStreamDestroy(b->stream);
-    }
+    if (b->ss.stream) cudaStreamSynchronize(b->ss.stream);
+    if (b->ss.complete()) b->ctx->free_streams.push_back(b->ss);   /* back to the context for the next job */
+    else b->ss.destroy();
     if (b->descs_dl) b->ctx->pinpool.put(b->descs_dl, b->descs_dl_bytes);
-    delete b;
+    delete b;   /* after the synchronise: its device buffers go back to the pool for the next job to reuse */
 }
 
 extern "C" int JPEGB200_batchCount(JPEGB200_BATCH *b) { return b ? b->n : 0; }
@@ -1101,22 +1094,16 @@ extern "C" int JPEGB200_batchSetOutput(JPEGB200_BATCH *b, int i, void *out, int6
 static int batch_stream(JPEGB200_BATCH *b)
 {
     CK(cudaSetDevice(b->ctx->device));
-    if (!b->stream && !b->have_ev && !b->ctx->free_streams.empty()) {
-        const JDStreamSet ss = b->ctx->free_streams.back();
+    if (!b->ss.stream && !b->ctx->free_streams.empty()) {
+        b->ss = b->ctx->free_streams.back();
         b->ctx->free_streams.pop_back();
-        b->stream = ss.stream;
-        for (int i = 0; i < JPEGB200_NUM_TIMINGS + 2; i++) b->ev[i] = ss.ev[i];
-        b->have_ev = true;
     }
-    if (!b->stream) CK(cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking));
-    if (!b->have_ev) {
-        for (auto &e : b->ev) CK(cudaEventCreate(&e));
-        b->have_ev = true;
-    }
+    if (!b->ss.stream) CK(cudaStreamCreateWithFlags(&b->ss.stream, cudaStreamNonBlocking));
+    for (auto &e : b->ss.ev) if (!e) CK(cudaEventCreate(&e));
     return 1;
 }
 
-extern "C" void *JPEGB200_batchStream(JPEGB200_BATCH *b) { if (!b || !batch_stream(b)) return nullptr; return (void *)b->stream; }
+extern "C" void *JPEGB200_batchStream(JPEGB200_BATCH *b) { if (!b || !batch_stream(b)) return nullptr; return (void *)b->ss.stream; }
 
 extern "C" int JPEGB200_batchAllocDeviceOutput(JPEGB200_BATCH *b)
 {
@@ -1140,7 +1127,7 @@ extern "C" int JPEGB200_batchReadOutput(JPEGB200_BATCH *b, int i, void *host_dst
 {
     if (!b || i < 0 || i >= b->n || !b->d_out.p || !host_dst) return 0;
     CK(cudaSetDevice(b->ctx->device));
-    if (b->stream) CK(cudaStreamSynchronize(b->stream));
+    if (b->ss.stream) CK(cudaStreamSynchronize(b->ss.stream));
     CK(cudaMemcpy(host_dst, b->d_out.p + b->arena_off[i], (size_t)JPEGB200_batchOutputBytes(b, i, nullptr), cudaMemcpyDeviceToHost));
     return 1;
 }
@@ -1172,8 +1159,8 @@ extern "C" int JPEGB200_batchUpload(JPEGB200_BATCH *b)
     CK(b->d_blk_hdr.alloc(&b->ctx->pool, b->nblk ? b->nblk : 1));
     CK(b->d_rec.alloc(&b->ctx->pool, b->rec_total + 1024));
     CK(b->d_events.alloc(&b->ctx->pool, JD_EVENT_CAP));
-    cudaStream_t st = b->stream;
-    CK(cudaEventRecord(b->ev[0], st));
+    cudaStream_t st = b->ss.stream;
+    CK(cudaEventRecord(b->ss.ev[0], st));
     /* zero the tail padding so word loads past the last file read zeros */
     CK(cudaMemsetAsync(b->d_comp.p + b->comp_total, 0, 256, st));
     if (b->contiguous_in) {
@@ -1204,7 +1191,7 @@ extern "C" int JPEGB200_batchUpload(JPEGB200_BATCH *b)
         CK(cudaMemcpyAsync(b->d_pfiles.p, b->pfiles.data(), b->pfiles.size() * sizeof(JDProgFile), cudaMemcpyHostToDevice, st));
         prog_bytes = b->pscans.size() * sizeof(JDProgScan) + b->ptabs.size() * sizeof(JDProgHuff) + b->pfiles.size() * sizeof(JDProgFile);
     }
-    CK(cudaEventRecord(b->ev[1], st));
+    CK(cudaEventRecord(b->ss.ev[1], st));
     b->uploaded = true;
     b->counters[JPEGB200_C_H2D_BYTES] = (int64_t)(b->comp_total + sizeof(JDImageDesc) * nf + 768 * (size_t)n + b->luts.size() * 2 +
                                                   b->work.size() * 4 + b->cta_lut.size() * 4 + b->seg_img.size() * 4 + prog_bytes);
@@ -1241,8 +1228,22 @@ static void launch_idct_pt(const JDIdctArgs &a, dim3 grid, int arith, bool half,
     }
 }
 
-static int g_use_tb = -1; /* thread-per-block IDCT kernel (default) unless JPEGDEC_B200_IDCT=lanes */
-static int g_tb_mpb = 0;  /* development switch JPEGDEC_B200_TB_MPB=16|20: force the strip width */
+/* Which IDCT kernels a context's decodes take.  JPEGDEC_B200_IDCT (A/B and test switch): unset = the default choice
+ * (launch_idct); "lanes" = the 8-lanes-per-block kernels everywhere; "tb" = those, and jdk_idct_tb for 4:2:0 colour at full
+ * size, also for the SSE2-build arithmetic; "packed" = the packed kernel for 4:2:0 colour at full size too.
+ * JPEGDEC_B200_TB_MPB=16|20 (development switch): force jdk_idct_tb's strip width. */
+enum JDIdctKernels { JD_IDCT_DEFAULT, JD_IDCT_LANES, JD_IDCT_TB, JD_IDCT_PACKED };
+struct JDIdctChoice { JDIdctKernels kernels; int tb_mpb; };
+static const JDIdctChoice &idct_choice()
+{
+    static const JDIdctChoice choice = [] {
+        const char *e = getenv("JPEGDEC_B200_IDCT"), *m = getenv("JPEGDEC_B200_TB_MPB");
+        const JDIdctKernels k = !e ? JD_IDCT_DEFAULT : strcmp(e, "lanes") == 0 ? JD_IDCT_LANES : strcmp(e, "tb") == 0 ? JD_IDCT_TB
+                                : strcmp(e, "packed") == 0 ? JD_IDCT_PACKED : JD_IDCT_DEFAULT;
+        return JDIdctChoice{k, m ? atoi(m) : 0};
+    }();
+    return choice;
+}
 
 template <int HS, int VS, int NC, int MPB, int PT>
 static void launch_idct_tb(const JDIdctArgs &a, uint32_t mcus_x, uint32_t mcus_y, uint32_t nimg, int arith, cudaStream_t st)
@@ -1336,16 +1337,13 @@ template <int HS, int VS, int MPB3, int MPB1>
 static int launch_idct_geo(const JDIdctArgs &a, uint32_t mcus_x, uint32_t mcus_y, uint32_t nimg, int ncomp, int ptclass,
                            int arith, bool half, cudaStream_t st)
 {
-    if (g_use_tb < 0) {
-        const char *e = getenv("JPEGDEC_B200_IDCT"); g_use_tb = (e && strcmp(e, "lanes") == 0) ? 0 : 1;
-        const char *m = getenv("JPEGDEC_B200_TB_MPB"); g_tb_mpb = m ? atoi(m) : 0;
-    }
-    if (g_use_tb && !half && HS == 2 && VS == 2 && ncomp == 3 && ptclass != JD_PT_GRAY) {
+    const JDIdctChoice &choice = idct_choice();
+    if (choice.kernels != JD_IDCT_LANES && !half && HS == 2 && VS == 2 && ncomp == 3 && ptclass != JD_PT_GRAY) {
         /* 4:2:0 colour, full size: the throughput configuration */
         /* strips of 20 MCUs (320 px) unless that wastes more MCU slots than strips of 16 (1920 and 3840 px divide evenly by 320;
          * measured faster there than strips of 16) */
         const uint32_t pad16 = (mcus_x + 15) / 16 * 16 - mcus_x, pad20 = (mcus_x + 19) / 20 * 20 - mcus_x;
-        const bool wide = g_tb_mpb == 20 || (g_tb_mpb == 0 && pad20 <= pad16);
+        const bool wide = choice.tb_mpb == 20 || (choice.tb_mpb == 0 && pad20 <= pad16);
         if (wide) {
             if (ptclass == JD_PT_565) launch_idct_tb<2, 2, 3, 20, JD_PT_565>(a, mcus_x, mcus_y, nimg, arith, st);
             else launch_idct_tb<2, 2, 3, 20, JD_PT_8888>(a, mcus_x, mcus_y, nimg, arith, st);
@@ -1370,60 +1368,76 @@ static int launch_idct_geo(const JDIdctArgs &a, uint32_t mcus_x, uint32_t mcus_y
     return 1;
 }
 
-#ifndef JD_DITHER_MINB
-#define JD_DITHER_MINB 9
-#endif
-#ifndef JD_DITHER_SKEW
-#define JD_DITHER_SKEW 2   /* pixels by which a row trails the row above: 3 = the error from above is folded into the NEXT pixel's
-                             forward error (one step of slack for the shuffle); 2 = it is added to the current pixel */
-#endif
-template <int BITS>
-__global__ void jdk_dither(const JDImageDesc *imgs, uint32_t nimg, const uint8_t *gray, const uint64_t *gray_off,
-                           uint16_t *errlines, const uint32_t *err_off, uint8_t *out, uint32_t sshift,
-                           const uint4 *bands, uint32_t nbands, uint32_t *progress);
-
-extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
+/* One IDCT + colour launch for a run of nimg images of one sampling.  The SSE2-build arithmetic takes the packed
+ * thread-per-block kernel for every sampling / pixel type / half scale except 4:2:0 colour at full size, which keeps
+ * jdk_idct_tb (measured faster there -- there is no packed 16-bit subtract instruction, __vsub2 costs three, which eats what
+ * the packed adds save).  0 when there is no kernel for the combination. */
+static int launch_idct(const JDIdctArgs &ia, int subsample, int ncomp, int ptclass, int arith, bool half, uint32_t mcus_x,
+                       uint32_t mcus_y, uint32_t nimg, cudaStream_t st)
 {
-    if (!b) return 0;
-    if (!b->uploaded) { snprintf(g_err, sizeof(g_err), "batchDecode before batchUpload"); return 0; }
-    if (!batch_stream(b)) return 0;
-    cudaStream_t st = b->stream;
-    const int n = b->n;
-    b->out_device = (flags & JPEGB200_OUT_DEVICE) != 0;
-    b->decode_flags = flags;
-    if (b->tensor && !b->out_device) {
-        snprintf(g_err, sizeof(g_err), "tensor output is written to device memory only: decode with JPEGB200_OUT_DEVICE");
-        return 0;
+    const JDIdctKernels k = idct_choice().kernels;
+    const bool tb_case = subsample == 0x22 && ncomp == 3 && ptclass != JD_PT_GRAY && !half;
+    const bool packed = arith == JPEG_ARITH_SSE2 && k != JD_IDCT_LANES && k != JD_IDCT_TB && (!tb_case || k == JD_IDCT_PACKED);
+#define JD_IDCT_SAMPLING(HS_, VS_, MPB3_, MPB1_)                                                                 \
+    return packed ? launch_idct_packed<HS_, VS_>(ia, mcus_x, mcus_y, nimg, ncomp, ptclass, half, st)             \
+                  : launch_idct_geo<HS_, VS_, MPB3_, MPB1_>(ia, mcus_x, mcus_y, nimg, ncomp, ptclass, arith, half, st)
+    switch (subsample) {
+        case 0x00: case 0x11: JD_IDCT_SAMPLING(1, 1, 16, 32);
+        case 0x21: JD_IDCT_SAMPLING(2, 1, 8, 16);
+        case 0x12: JD_IDCT_SAMPLING(1, 2, 8, 16);
+        case 0x22: JD_IDCT_SAMPLING(2, 2, 8, 8);
     }
+#undef JD_IDCT_SAMPLING
+    return 0;
+}
+
+/* ---- JPEGB200_batchDecode, step by step.  What several steps share lives on its stack. ---- */
+struct DecodeState {
+    std::vector<JDImageDesc> descs_stage;   /* the descriptors the kernels read: b->descs keeps the tight pitch (JPEGB200_batchOutputBytes, the arena) */
+    bool user_dev_out = false;              /* the pixels go to the caller's device pointers, not to the arena */
+    uint8_t *out_base = nullptr;            /* the destination: the arena, or the lowest of the caller's pointers */
+    uint8_t *pipe_out = nullptr;            /* where the pixel pipeline (IDCT, resize) writes: out_base, or the tensor staging */
+    uint8_t *stage_out = nullptr;           /* where the IDCT stage writes: pipe_out, or the gray stage / the resize source */
+    uint32_t tn_ctas = 0, rs_ctas[4] = {0u, 0u, 0u, 0u};
     int launches = 0;
-    if (!b->pfiles.empty()) {
-        /* coefficient planes of the progressive files, one pooled buffer each: a file whose plane the device cannot hold
-         * gets JPEG_ERROR_MEMORY (all of its views) and the others decode */
-        b->d_pplane.resize(b->nf);
-        b->pplane_ptr.assign(b->nf, nullptr);
-        b->pwalkers = 0;
-        for (const JDProgFile &pf : b->pfiles) {
-            const int f = (int)pf.file;
-            if (b->d_pplane[f].alloc(&b->ctx->pool, (size_t)b->pplane[f] / 2) != cudaSuccess) {
-                cudaGetLastError();
-                for (int i = 0; i < n; i++) if (file_of(b, i) == f) b->parse_status[i] = JPEG_ERROR_MEMORY;
-                continue;
-            }
-            b->pplane_ptr[f] = b->d_pplane[f].p;
-            CK(cudaMemsetAsync(b->pplane_ptr[f], 0, (size_t)b->pplane[f], st));
+};
+
+/* coefficient planes of the progressive files, one pooled buffer each: a file whose plane the device cannot hold gets
+ * JPEG_ERROR_MEMORY (all of its views) and the others decode.  Writes d_pplane, pplane_ptr, pwalkers, parse_status. */
+static int alloc_prog_planes(JPEGB200_BATCH *b)
+{
+    if (b->pfiles.empty()) return 1;
+    cudaStream_t st = b->ss.stream;
+    b->d_pplane.resize(b->nf);
+    b->pplane_ptr.assign(b->nf, nullptr);
+    b->pwalkers = 0;
+    for (const JDProgFile &pf : b->pfiles) {
+        const int f = (int)pf.file;
+        if (b->d_pplane[f].alloc(&b->ctx->pool, (size_t)b->pplane[f] / 2) != cudaSuccess) {
+            cudaGetLastError();
+            for (int i = 0; i < b->n; i++) if (file_of(b, i) == f) b->parse_status[i] = JPEG_ERROR_MEMORY;
+            continue;
         }
-        for (const JDProgScan &s : b->pscans) if (b->pplane_ptr[s.img]) b->pwalkers++;
-        CK(cudaMemcpyAsync(b->d_pplanes.p, b->pplane_ptr.data(), sizeof(int16_t *) * b->nf, cudaMemcpyHostToDevice, st));
-        CK(cudaMemsetAsync(b->d_perr.p, 0xFF, sizeof(uint32_t) * b->nf, st));
+        b->pplane_ptr[f] = b->d_pplane[f].p;
+        CK(cudaMemsetAsync(b->pplane_ptr[f], 0, (size_t)b->pplane[f], st));
     }
-    /* output placement */
-    bool user_dev_out = false;
+    for (const JDProgScan &s : b->pscans) if (b->pplane_ptr[s.img]) b->pwalkers++;
+    CK(cudaMemcpyAsync(b->d_pplanes.p, b->pplane_ptr.data(), sizeof(int16_t *) * b->nf, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(b->d_perr.p, 0xFF, sizeof(uint32_t) * b->nf, st));
+    return 1;
+}
+
+/* output placement: the caller's device pointers (checked before anything is enqueued) or the arena.  Writes
+ * D.user_dev_out, D.out_base and D.descs_stage with each image's out_off / out_pitch. */
+static int place_outputs(JPEGB200_BATCH *b, DecodeState &D)
+{
+    const int n = b->n;
     if (b->out_device && !b->arena_owned) {
-        user_dev_out = true;
-        for (int i = 0; i < n; i++) if (!b->outs[i] && b->parse_status[i] == JPEG_SUCCESS) user_dev_out = false;
+        D.user_dev_out = true;
+        for (int i = 0; i < n; i++) if (!b->outs[i] && b->parse_status[i] == JPEG_SUCCESS) D.user_dev_out = false;
         bool any_ptr = false;
         for (int i = 0; i < n; i++) if (b->outs[i]) any_ptr = true;
-        if (!user_dev_out && any_ptr) { snprintf(g_err, sizeof(g_err), "device output pointers given for some images only"); return 0; }
+        if (!D.user_dev_out && any_ptr) { snprintf(g_err, sizeof(g_err), "device output pointers given for some images only"); return 0; }
         /* the kernels store through these pointers: refuse misaligned ones before anything is enqueued */
         for (int i = 0; i < n; i++)
             if (b->outs[i] && !b->tensor && !jd_check_output(b->index_base + i, b->pixel_type, (int64_t)b->descs[i].out_pitch, b->outs[i], b->pitches[i], 1,
@@ -1442,283 +1456,308 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
             }
         }
     }
-    /* the descriptors the kernels read: b->descs keeps the tight pitch (JPEGB200_batchOutputBytes, the arena) */
-    std::vector<JDImageDesc> descs_stage = b->descs;
-    uint8_t *out_base = nullptr;
-    if (user_dev_out) {
+    D.descs_stage = b->descs;
+    if (D.user_dev_out) {
         /* user device pointers: offsets relative to the lowest pointer */
         uintptr_t lo = ~(uintptr_t)0;
         for (int i = 0; i < n; i++) if (b->outs[i] && (uintptr_t)b->outs[i] < lo) lo = (uintptr_t)b->outs[i];
-        out_base = (uint8_t *)lo;
+        D.out_base = (uint8_t *)lo;
         for (int i = 0; i < n; i++) {
-            descs_stage[i].out_off = b->outs[i] ? (uint64_t)((uintptr_t)b->outs[i] - lo) : 0;
-            descs_stage[i].out_pitch = (uint32_t)b->pitches[i];
+            D.descs_stage[i].out_off = b->outs[i] ? (uint64_t)((uintptr_t)b->outs[i] - lo) : 0;
+            D.descs_stage[i].out_pitch = (uint32_t)b->pitches[i];
         }
     } else {
         if (!b->d_out.p) { CK(b->d_out.alloc(&b->ctx->pool, b->out_total + 256)); b->arena_owned = true; }
-        out_base = b->d_out.p;
-        for (int i = 0; i < n; i++) descs_stage[i].out_off = b->arena_off[i];
+        D.out_base = b->d_out.p;
+        for (int i = 0; i < n; i++) D.descs_stage[i].out_off = b->arena_off[i];
     }
-    /* tensor: the pipeline below writes U tightly into d_tn (pipe_out) where it would have written the destination;
-     * jdk_tensor then writes the destination */
-    uint8_t *pipe_out = out_base;
-    uint32_t tn_ctas = 0;
-    if (b->tensor) {
-        b->tn_desc.assign(n, JDTensorDesc{});
-        constexpr uint32_t px_per_thread[5] = {0u, 16u, 8u, 0u, 4u};
-        const uint32_t PX = px_per_thread[b->tn_elt];
-        uint64_t so = 0, ctas = 0;
-        for (int i = 0; i < n; i++) {
-            JDTensorDesc &t = b->tn_desc[i];
-            t.blk = (uint32_t)ctas;
-            if (b->parse_status[i] != JPEG_SUCCESS) continue;
-            const JDImageDesc &d = b->descs[i];
-            t.w = d.out_w; t.h = d.out_h; t.swap = b->tn_swap[i];
-            t.src_off = so;
-            so += (uint64_t)b->tn_stage[i];
-            t.dst_off = descs_stage[i].out_off;
-            t.pitch = user_dev_out ? (uint64_t)b->pitches[i] : (uint64_t)d.out_pitch;
-            t.plane = (user_dev_out && b->tn_plane[i]) ? (uint64_t)b->tn_plane[i] : t.pitch * d.out_h;
-            ctas += ((uint64_t)(d.out_w + PX - 1) / PX * d.out_h + JD_TN_THREADS - 1) / JD_TN_THREADS;
-            descs_stage[i].out_off = t.src_off;
-            descs_stage[i].out_pitch = d.out_w * (uint32_t)b->tn_bpp;
-        }
-        if (ctas >= (1ull << 31)) { snprintf(g_err, sizeof(g_err), "tensor output: too many elements in one job"); return 0; }
-        tn_ctas = (uint32_t)ctas;
-        CK(b->d_tn.alloc(&b->ctx->pool, so + 256));
-        CK(b->d_tn_tab.alloc(&b->ctx->pool, 3 * 256));
-        CK(b->d_tn_desc.alloc(&b->ctx->pool, n));
-        CK(cudaMemcpyAsync(b->d_tn_tab.p, b->tn_table.data(), 3 * 256 * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(b->d_tn_desc.p, b->tn_desc.data(), sizeof(JDTensorDesc) * n, cudaMemcpyHostToDevice, st));
-        pipe_out = b->d_tn.p;
-    }
-    /* resize: the IDCT stage writes S tightly into d_rs; jdk_resize_v writes where the IDCT would have */
-    uint32_t rs_ctas[4] = {0u, 0u, 0u, 0u};
-    if (b->resize) {
-        const int bp = bytes_per_pixel_class(b->ptclass);
-        b->rs_desc.assign(n, JDResizeDesc{});
-        uint64_t so = 0, co = 0, ctas[4] = {0, 0, 0, 0};
-        for (int i = 0; i < n; i++) {
-            JDResizeDesc &r = b->rs_desc[i];
-            r.blk_c = (uint32_t)ctas[0]; r.blk_h = (uint32_t)ctas[1]; r.blk_v = (uint32_t)ctas[2]; r.blk_h2 = (uint32_t)ctas[3];
-            if (b->parse_status[i] != JPEG_SUCCESS) continue;
-            const JDResizePlan &rp = b->rs_plans[i];
-            r.src_w = b->rs_src_w[i]; r.src_h = b->rs_src_h[i]; r.dst_w = b->descs[i].out_w; r.dst_h = b->descs[i].out_h;
-            r.dst_off = descs_stage[i].out_off; r.dst_pitch = descs_stage[i].out_pitch;
-            r.ksize_h = (uint32_t)rp.ksize_h; r.ksize_v = (uint32_t)rp.ksize_v;
-            r.ybox0 = (uint32_t)rp.ybox0; r.rows = (uint32_t)rp.rows;
-            r.flags = (rp.need_h ? 1u : 0u) | (rp.need_v ? 2u : 0u) | (rp.vfirst ? 4u : 0u);
-            r.src_off = so;
-            so += ((uint64_t)r.src_w * r.src_h * bp + 255) & ~(uint64_t)255;
-            r.mid_off = so;
-            so += ((uint64_t)rp.mid_bytes + 255) & ~(uint64_t)255;
-            r.coef_h = co;
-            co += rp.need_h ? (uint64_t)r.dst_w * (r.ksize_h + 2) : 0;
-            r.coef_v = co;
-            co += rp.need_v ? (uint64_t)r.dst_h * (r.ksize_v + 2) : 0;
-            const uint64_t q = ((rp.vfirst ? r.src_w : r.dst_w) + 16 / bp - 1) / (16 / bp);
-            ctas[0] += ((rp.need_h ? r.dst_w : 0u) + (rp.need_v ? r.dst_h : 0u) + JD_RS_THREADS - 1) / JD_RS_THREADS;
-            if (rp.need_h && !rp.vfirst)   /* jdk_resize_h<4, 0>: one thread per pixel; <1, 0>: column chunks x row blocks */
-                ctas[1] += bp == 4 ? ((uint64_t)r.rows * r.dst_w + JD_RS_THREADS - 1) / JD_RS_THREADS
-                                   : (uint64_t)((r.dst_w + JD_RS_HCOLS - 1) / JD_RS_HCOLS) * ((r.rows + JD_RS_HROWS - 1) / JD_RS_HROWS);
-            ctas[2] += (q * r.dst_h + JD_RS_THREADS - 1) / JD_RS_THREADS;
-            ctas[3] += rp.vfirst ? ((uint64_t)r.dst_h * r.dst_w + JD_RS_THREADS - 1) / JD_RS_THREADS : 0;
-            descs_stage[i].out_off = r.src_off;
-            descs_stage[i].out_pitch = r.src_w * (uint32_t)bp;
-            descs_stage[i].out_w = r.src_w; descs_stage[i].out_h = r.src_h;
-        }
-        if (ctas[1] >= (1ull << 31) || ctas[2] >= (1ull << 31) || ctas[3] >= (1ull << 31)) {
-            snprintf(g_err, sizeof(g_err), "resize: too many output pixels in one job");
-            return 0;
-        }
-        for (int c = 0; c < 4; c++) rs_ctas[c] = (uint32_t)ctas[c];
-        CK(b->d_rs.alloc(&b->ctx->pool, so + 256));
-        CK(b->d_rs_coef.alloc(&b->ctx->pool, co + 64));
-        CK(b->d_rs_desc.alloc(&b->ctx->pool, n));
-        CK(cudaMemcpyAsync(b->d_rs_desc.p, b->rs_desc.data(), sizeof(JDResizeDesc) * n, cudaMemcpyHostToDevice, st));
-    }
-    /* dither: the IDCT stage writes an MCU-aligned 8-bit image first */
-    std::vector<uint64_t> gray_off;
-    std::vector<uint32_t> err_off;
-    if (b->dither_bits) {
-        CK(b->d_gray.alloc(&b->ctx->pool, b->gray_total + 256));
-        size_t go = 0, eo = 0;
-        gray_off.resize(3 * (size_t)n); err_off.resize(n);
-        b->errinit.clear();
-        for (int i = 0; i < n; i++) {
-            const JDInfo &inf = b->infos[i];
-            gray_off[i] = go; err_off[i] = (uint32_t)eo;
-            gray_off[(size_t)n + i] = descs_stage[i].out_off;         /* where jdk_dither writes the packed rows ... */
-            gray_off[2 * (size_t)n + i] = descs_stage[i].out_pitch;   /* ... and their pitch: the caller's, or tight in the arena */
-            if (b->parse_status[i] != JPEG_SUCCESS) continue;
-            const uint32_t pw = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> b->sshift);
-            const uint32_t ph = (uint32_t)inf.mcus_y * (uint32_t)(inf.mcu_h >> b->sshift);
-            descs_stage[i].out_off = go;
-            descs_stage[i].out_pitch = pw;
-            go += (((size_t)pw * ph) + 255) & ~(size_t)255;
-            /* initial error line = the reference's DHT scratch bytes (they share usPixels, jpeg.inl:843 / :4881) */
-            const size_t el = ((size_t)pw + 16 + 15) & ~(size_t)15;
-            b->errinit.resize(eo + el, (uint16_t)0xFF00u);
-            /* device line S[x] = errors[x + 2] */
-            const size_t cp = (el + 2 < JD_HUFFVALS_BYTES) ? el : JD_HUFFVALS_BYTES - 2;
-            for (size_t q = 0; q < cp; q++) b->errinit[eo + q] = (uint16_t)(0xFF00u | inf.p.huffvals[q + 2]);
-            eo += el;
-        }
-        CK(b->d_errline.alloc(&b->ctx->pool, eo + 16));
-        CK(cudaMemcpyAsync(b->d_errline.p, b->errinit.data(), eo * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
-        CK(b->d_gray_off.alloc(&b->ctx->pool, 3 * (size_t)n)); CK(b->d_err_off.alloc(&b->ctx->pool, n));
-        /* pageable sources: the runtime stages them before returning, so the vectors may go out of scope */
-        CK(cudaMemcpyAsync(b->d_gray_off.p, gray_off.data(), (size_t)n * 24, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(b->d_err_off.p, err_off.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-        /* one warp per band of 32 rows, band-major (band k of every image, then band k + 1): a band's producer is always
-         * launched before it, and the warps resident at any time are bands that can actually run (a band may start ~113
-         * steps after the one above it, so only ~W/113 bands of an image are ever active together) */
-        b->dbands.clear();
-        {
-            /* .w: the list position of band k - 255 of the same image, which band k >= 256 waits for (jdk_dither), else ~0 */
-            uint32_t maxb = 0;
-            std::vector<uint32_t> nb(n, 0), prevpos(n, 0), first(n, 0);
-            for (int i = 0; i < n; i++) if (b->parse_status[i] == JPEG_SUCCESS) { nb[i] = (b->descs[i].out_h + 31) / 32; if (nb[i] > maxb) maxb = nb[i]; }
-            std::vector<uint32_t> where;                       /* list position of band k of image i at first[i] + k */
-            for (int i = 0; i < n; i++) { first[i] = (uint32_t)where.size(); where.resize(where.size() + nb[i]); }
-            for (uint32_t k = 0; k < maxb; k++)
-                for (int i = 0; i < n; i++) {
-                    if (k >= nb[i]) continue;
-                    const uint32_t pos = (uint32_t)b->dbands.size();
-                    where[first[i] + k] = pos;
-                    b->dbands.push_back(make_uint4((uint32_t)i, k, prevpos[i], k >= 256 ? where[first[i] + k - 255] : ~0u));
-                    prevpos[i] = pos;
-                }
-        }
-        CK(b->d_dbands.alloc(&b->ctx->pool, b->dbands.size() ? b->dbands.size() : 1)); CK(b->d_dprog.alloc(&b->ctx->pool, b->dbands.size() + 1));
-        if (!b->dbands.empty()) CK(cudaMemcpyAsync(b->d_dbands.p, b->dbands.data(), b->dbands.size() * sizeof(uint4), cudaMemcpyHostToDevice, st));
-        CK(cudaMemsetAsync(b->d_dprog.p, 0, (b->dbands.size() + 1) * 4, st));
-    }
-    CK(cudaMemcpyAsync(b->d_descs.p, descs_stage.data(), sizeof(JDImageDesc) * n, cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(b->d_counters.p, 0, 32, st));
-    if (b->nchunks) CK(cudaMemsetAsync(b->d_blk_hdr.p, 0, (size_t)b->nblk * 8, st)); /* blocks a truncated restart-free scan never reaches stay empty */
+    D.pipe_out = D.out_base;
+    return 1;
+}
 
-    /* prescan, entropy walk, stitch and patch: one entropy-facing descriptor per file (its views share them) */
-    JDImageDesc *const fdev = file_descs_dev(b);
-    const int nf = b->nf;
-    CK(cudaEventRecord(b->ev[2], st));
-    jdk_prescan<<<nf, 256, 0, st>>>(b->d_comp.p, fdev, b->d_seg_start.p);
-    launches++;
-    CK(cudaEventRecord(b->ev[3], st));
-    if (!b->work.empty()) {
-        JDEntropyArgs ea;
-        ea.data = b->d_comp.p; ea.imgs = fdev; ea.luts = b->d_luts.p; ea.work = b->d_work.p; ea.cta_lut = b->d_cta_lut.p;
-        ea.seg_img = b->d_seg_img.p; ea.seg_start = b->d_seg_start.p; ea.blk_hdr = b->d_blk_hdr.p; ea.rec = b->d_rec.p;
-        ea.seg_jmap = b->d_seg_jmap.p; ea.seg_status = b->d_seg_status.p; ea.seg_nrec = b->d_seg_nrec.p;
-        ea.events = b->d_events.p; ea.event_count = b->d_counters.p; ea.event_cap = JD_EVENT_CAP;
-        ea.nwork = (uint32_t)b->work.size(); ea.dc_output = (b->sshift == 3) ? 1u : (b->sshift == 2) ? 2u : 0u;
-        /* default ("raw"): the entropy kernel un-stuffs in its bit reader, 64-thread CTAs.  JPEGDEC_B200_ENTROPY=clean:
-         * jdk_unstuff_segs first, so that the reader is a plain word stream (128-thread CTAs).  On the H100 the raw walk is
-         * the faster one (DESIGN.md 4.1). */
-        static int use_clean = -1;
-        if (use_clean < 0) { const char *e = getenv("JPEGDEC_B200_ENTROPY"); use_clean = (e && strcmp(e, "clean") == 0) ? 1 : 0; }
-        const unsigned egrid = (unsigned)(b->work.size() / JD_ENTROPY_THREADS);
-#ifdef JD_ENTROPY_PROBE
-        /* development build: time the un-stuffing (clean pipeline) and the walk apart; the walk's warps print their own lines */
-        cudaEvent_t pev[3];
-        for (auto &e : pev) CK(cudaEventCreate(&e));
-        CK(cudaEventRecord(pev[0], st));
-#endif
-        if (use_clean) {
-            CK(b->d_clean.alloc(&b->ctx->pool, b->comp_total + 32 * (size_t)b->nseg + 4096));
-            CK(b->d_seg_clen.alloc(&b->ctx->pool, b->nseg ? b->nseg : 1));
-            jdk_unstuff_segs<<<(b->nseg * 32u + JD_UNSTUFF_WARPS * 32u - 1u) / (JD_UNSTUFF_WARPS * 32u), JD_UNSTUFF_WARPS * 32, 0, st>>>(
-                b->d_comp.p, fdev, b->d_seg_img.p, b->d_seg_start.p, b->nseg, b->d_clean.p, b->d_seg_clen.p);
-            ea.clean = b->d_clean.p; ea.seg_clen = b->d_seg_clen.p;
-        } else {
-            ea.clean = nullptr; ea.seg_clen = nullptr;
-        }
-#ifdef JD_ENTROPY_PROBE
-        CK(cudaEventRecord(pev[1], st));
-#endif
-        const unsigned ecta = use_clean ? jd_entropy_cta_threads(true) : jd_entropy_cta_threads(false);
-        const unsigned egrid_walk = egrid * (JD_ENTROPY_THREADS / ecta);
-        if (use_clean) jdk_entropy<true><<<egrid_walk, ecta, 0, st>>>(ea);
-        else jdk_entropy<false><<<egrid_walk, ecta, 0, st>>>(ea);
-        launches += use_clean ? 2 : 1;
-#ifdef JD_ENTROPY_PROBE
-        CK(cudaEventRecord(pev[2], st));
-        CK(cudaStreamSynchronize(st));
-        float ms_u = 0.f, ms_w = 0.f;
-        CK(cudaEventElapsedTime(&ms_u, pev[0], pev[1]));
-        CK(cudaEventElapsedTime(&ms_w, pev[1], pev[2]));
-        printf("JDP_LAUNCH nwork %u ctas %u unstuff_ms %.4f walk_ms %.4f\n", (unsigned)b->work.size(), egrid_walk, ms_u, ms_w);
-        fflush(stdout);
-        for (auto &e : pev) CK(cudaEventDestroy(e));
-#endif
+/* tensor: the pipeline writes U tightly into d_tn (D.pipe_out) where it would have written the destination; jdk_tensor then
+ * writes the destination.  Uploads tn_desc and the element table; rewrites D.descs_stage for the stage before it. */
+static int stage_tensor(JPEGB200_BATCH *b, DecodeState &D)
+{
+    const int n = b->n;
+    cudaStream_t st = b->ss.stream;
+    b->tn_desc.assign(n, JDTensorDesc{});
+    constexpr uint32_t px_per_thread[5] = {0u, 16u, 8u, 0u, 4u};
+    const uint32_t PX = px_per_thread[b->tn_elt];
+    uint64_t so = 0, ctas = 0;
+    for (int i = 0; i < n; i++) {
+        JDTensorDesc &t = b->tn_desc[i];
+        t.blk = (uint32_t)ctas;
+        if (b->parse_status[i] != JPEG_SUCCESS) continue;
+        const JDImageDesc &d = b->descs[i];
+        t.w = d.out_w; t.h = d.out_h; t.swap = b->tn_swap[i];
+        t.src_off = so;
+        so += (uint64_t)b->tn_stage[i];
+        t.dst_off = D.descs_stage[i].out_off;
+        t.pitch = D.user_dev_out ? (uint64_t)b->pitches[i] : (uint64_t)d.out_pitch;
+        t.plane = (D.user_dev_out && b->tn_plane[i]) ? (uint64_t)b->tn_plane[i] : t.pitch * d.out_h;
+        ctas += ((uint64_t)(d.out_w + PX - 1) / PX * d.out_h + JD_TN_THREADS - 1) / JD_TN_THREADS;
+        D.descs_stage[i].out_off = t.src_off;
+        D.descs_stage[i].out_pitch = d.out_w * (uint32_t)b->tn_bpp;
     }
-    if (b->nchunks) {
-        /* restart-free scans: un-stuff, iterate the chunk entry states to their fix point, then emit */
-        JDChunkArgs ca;
-        ca.comp = b->d_comp.p; ca.filt = b->d_filt.p; ca.imgs = fdev; ca.luts = b->d_luts.p;
-        ca.cimg_list = b->d_cimg_list.p; ca.ncimg = (uint32_t)b->cimg_list.size(); ca.flen = b->d_flen.p;
-        ca.nchunks = b->nchunks;
-        ca.cn = b->d_cn.p; ca.cpre = b->d_cpre.p; ca.cjmap = b->d_cjmap.p; ca.cstatus = b->d_cstatus.p; ca.cnown = b->d_cnown.p;
-        ca.cdcs = b->d_cdcs.p; ca.cpe = b->d_cpe.p; ca.changed = b->d_counters.p + 2;
-        ca.blk_hdr = b->d_blk_hdr.p; ca.rec = b->d_rec.p;
-        ca.events = b->d_events.p; ca.event_count = b->d_counters.p; ca.event_cap = JD_EVENT_CAP;
-        ca.seg_phase = b->d_seg_phase.p; ca.seg_jmap = b->d_seg_jmap.p; ca.seg_status = b->d_seg_status.p; ca.nseg_total = b->nseg;
-        const unsigned gi = ((unsigned)b->cimg_list.size() * 32 + 127) / 128;
-        ca.max_nch = b->max_nch; ca.Ep = b->d_Ep.p; ca.cfirst = b->d_cfirst.p;
-        const dim3 gchunks((b->max_nch + 127) / 128, (unsigned)b->cimg_list.size());
-        /* guess: every chunk starts a block at its first bit (exit state of every left neighbour = (0, 0, 0)); no chunk parsed yet */
-        CK(cudaMemsetAsync(b->d_E0.p, 0, (size_t)(b->nchunks + 1) * 4, st));
-        CK(cudaMemsetAsync(b->d_Ep.p, 0xFE, (size_t)b->nchunks * 4, st));
-        {
-            const dim3 gu(((b->max_nch * JD_CHUNK_BYTES + JD_UNSTUFF_PIECE - 1) / JD_UNSTUFF_PIECE + 3) / 4, (unsigned)b->cimg_list.size());
-            jdk_unstuff<false><<<gu, 128, 0, st>>>(ca);
-            jdk_unstuff<true><<<gu, 128, 0, st>>>(ca);
-        }
-        launches += 2;
-        uint32_t *Xin = b->d_E0.p, *Xout = b->d_E1.p;
-        int passes = 0;
-        /* The entry states reach their fix point in 2-4 passes on real streams (a chunk re-synchronises well inside its 512
-         * bytes), and from the third pass on only the chunks whose entry state moved are parsed again.  Normal mode:
-         * JD_CHUNK_PASSES passes back to back, the last one verifying (it raises a flag if an exit state still moved) -- no
-         * host round trip, so jobs of JPEGB200_decodeBatch stay in flight; batchWait re-runs the job in the iterating mode
-         * below if the flag came back set. */
-        static int fixed_passes = -1;   /* JPEGDEC_B200_CHUNK_PASSES=n: test hook (n = 1 forces the fallback) */
-        if (fixed_passes < 0) { const char *e = getenv("JPEGDEC_B200_CHUNK_PASSES"); fixed_passes = (e && atoi(e) > 0) ? atoi(e) : JD_CHUNK_PASSES; }
-        const int fixed = b->chunk_iterate ? 0 : fixed_passes;
-        for (;;) {
-            const int burst = fixed ? fixed : 3;
-            for (int k = 0; k < burst; k++) {
-                if (k == burst - 1) CK(cudaMemsetAsync(b->d_counters.p + 2, 0, 4, st));
-                ca.X_in = Xin; ca.X_out = Xout;
-                jdk_chunk_parse<<<gchunks, 128, 0, st>>>(ca);
-                launches++; passes++;
-                uint32_t *tmp = Xin; Xin = Xout; Xout = tmp;
+    if (ctas >= (1ull << 31)) { snprintf(g_err, sizeof(g_err), "tensor output: too many elements in one job"); return 0; }
+    D.tn_ctas = (uint32_t)ctas;
+    CK(b->d_tn.alloc(&b->ctx->pool, so + 256));
+    CK(b->d_tn_tab.alloc(&b->ctx->pool, 3 * 256));
+    CK(b->d_tn_desc.alloc(&b->ctx->pool, n));
+    CK(cudaMemcpyAsync(b->d_tn_tab.p, b->tn_table.data(), 3 * 256 * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(b->d_tn_desc.p, b->tn_desc.data(), sizeof(JDTensorDesc) * n, cudaMemcpyHostToDevice, st));
+    D.pipe_out = b->d_tn.p;
+    return 1;
+}
+
+/* resize: the IDCT stage writes S tightly into d_rs; jdk_resize_v writes where the IDCT would have.  Uploads rs_desc with the
+ * CTA prefix sums of the four passes (D.rs_ctas); rewrites D.descs_stage for the IDCT stage. */
+static int stage_resize(JPEGB200_BATCH *b, DecodeState &D)
+{
+    const int n = b->n;
+    const int bp = bytes_per_pixel_class(b->ptclass);
+    b->rs_desc.assign(n, JDResizeDesc{});
+    uint64_t so = 0, co = 0, ctas[4] = {0, 0, 0, 0};
+    for (int i = 0; i < n; i++) {
+        JDResizeDesc &r = b->rs_desc[i];
+        r.blk_c = (uint32_t)ctas[0]; r.blk_h = (uint32_t)ctas[1]; r.blk_v = (uint32_t)ctas[2]; r.blk_h2 = (uint32_t)ctas[3];
+        if (b->parse_status[i] != JPEG_SUCCESS) continue;
+        const JDResizePlan &rp = b->rs_plans[i];
+        r.src_w = b->rs_src_w[i]; r.src_h = b->rs_src_h[i]; r.dst_w = b->descs[i].out_w; r.dst_h = b->descs[i].out_h;
+        r.dst_off = D.descs_stage[i].out_off; r.dst_pitch = D.descs_stage[i].out_pitch;
+        r.ksize_h = (uint32_t)rp.ksize_h; r.ksize_v = (uint32_t)rp.ksize_v;
+        r.ybox0 = (uint32_t)rp.ybox0; r.rows = (uint32_t)rp.rows;
+        r.flags = (rp.need_h ? 1u : 0u) | (rp.need_v ? 2u : 0u) | (rp.vfirst ? 4u : 0u);
+        r.src_off = so;
+        so += align256((size_t)r.src_w * r.src_h * bp);
+        r.mid_off = so;
+        so += align256((size_t)rp.mid_bytes);
+        r.coef_h = co;
+        co += rp.need_h ? (uint64_t)r.dst_w * (r.ksize_h + 2) : 0;
+        r.coef_v = co;
+        co += rp.need_v ? (uint64_t)r.dst_h * (r.ksize_v + 2) : 0;
+        const uint64_t q = ((rp.vfirst ? r.src_w : r.dst_w) + 16 / bp - 1) / (16 / bp);
+        ctas[0] += ((rp.need_h ? r.dst_w : 0u) + (rp.need_v ? r.dst_h : 0u) + JD_RS_THREADS - 1) / JD_RS_THREADS;
+        if (rp.need_h && !rp.vfirst)   /* jdk_resize_h<4, 0>: one thread per pixel; <1, 0>: column chunks x row blocks */
+            ctas[1] += bp == 4 ? ((uint64_t)r.rows * r.dst_w + JD_RS_THREADS - 1) / JD_RS_THREADS
+                               : (uint64_t)((r.dst_w + JD_RS_HCOLS - 1) / JD_RS_HCOLS) * ((r.rows + JD_RS_HROWS - 1) / JD_RS_HROWS);
+        ctas[2] += (q * r.dst_h + JD_RS_THREADS - 1) / JD_RS_THREADS;
+        ctas[3] += rp.vfirst ? ((uint64_t)r.dst_h * r.dst_w + JD_RS_THREADS - 1) / JD_RS_THREADS : 0;
+        D.descs_stage[i].out_off = r.src_off;
+        D.descs_stage[i].out_pitch = r.src_w * (uint32_t)bp;
+        D.descs_stage[i].out_w = r.src_w; D.descs_stage[i].out_h = r.src_h;
+    }
+    if (ctas[1] >= (1ull << 31) || ctas[2] >= (1ull << 31) || ctas[3] >= (1ull << 31)) {
+        snprintf(g_err, sizeof(g_err), "resize: too many output pixels in one job");
+        return 0;
+    }
+    for (int c = 0; c < 4; c++) D.rs_ctas[c] = (uint32_t)ctas[c];
+    CK(b->d_rs.alloc(&b->ctx->pool, so + 256));
+    CK(b->d_rs_coef.alloc(&b->ctx->pool, co + 64));
+    CK(b->d_rs_desc.alloc(&b->ctx->pool, n));
+    CK(cudaMemcpyAsync(b->d_rs_desc.p, b->rs_desc.data(), sizeof(JDResizeDesc) * n, cudaMemcpyHostToDevice, b->ss.stream));
+    return 1;
+}
+
+/* dither: the IDCT stage writes an MCU-aligned 8-bit image into d_gray first.  Uploads the gray / output offsets and
+ * pitches, the initial error lines and the band list (dbands); rewrites D.descs_stage for the IDCT stage. */
+static int stage_dither(JPEGB200_BATCH *b, DecodeState &D)
+{
+    const int n = b->n;
+    cudaStream_t st = b->ss.stream;
+    std::vector<uint64_t> gray_off(3 * (size_t)n);
+    std::vector<uint32_t> err_off(n);
+    CK(b->d_gray.alloc(&b->ctx->pool, b->gray_total + 256));
+    size_t go = 0, eo = 0;
+    b->errinit.clear();
+    for (int i = 0; i < n; i++) {
+        const JDInfo &inf = b->infos[i];
+        gray_off[i] = go; err_off[i] = (uint32_t)eo;
+        gray_off[(size_t)n + i] = D.descs_stage[i].out_off;         /* where jdk_dither writes the packed rows ... */
+        gray_off[2 * (size_t)n + i] = D.descs_stage[i].out_pitch;   /* ... and their pitch: the caller's, or tight in the arena */
+        if (b->parse_status[i] != JPEG_SUCCESS) continue;
+        const uint32_t pw = (uint32_t)inf.mcus_x * (uint32_t)(inf.mcu_w >> b->sshift);
+        const uint32_t ph = (uint32_t)inf.mcus_y * (uint32_t)(inf.mcu_h >> b->sshift);
+        D.descs_stage[i].out_off = go;
+        D.descs_stage[i].out_pitch = pw;
+        go += align256((size_t)pw * ph);
+        /* initial error line = the reference's DHT scratch bytes (they share usPixels, jpeg.inl:843 / :4881) */
+        const size_t el = ((size_t)pw + 16 + 15) & ~(size_t)15;
+        b->errinit.resize(eo + el, (uint16_t)0xFF00u);
+        /* device line S[x] = errors[x + 2] */
+        const size_t cp = (el + 2 < JD_HUFFVALS_BYTES) ? el : JD_HUFFVALS_BYTES - 2;
+        for (size_t q = 0; q < cp; q++) b->errinit[eo + q] = (uint16_t)(0xFF00u | inf.p.huffvals[q + 2]);
+        eo += el;
+    }
+    CK(b->d_errline.alloc(&b->ctx->pool, eo + 16));
+    CK(cudaMemcpyAsync(b->d_errline.p, b->errinit.data(), eo * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
+    CK(b->d_gray_off.alloc(&b->ctx->pool, 3 * (size_t)n)); CK(b->d_err_off.alloc(&b->ctx->pool, n));
+    /* pageable sources: the runtime stages them before returning, so the vectors may go out of scope */
+    CK(cudaMemcpyAsync(b->d_gray_off.p, gray_off.data(), (size_t)n * 24, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(b->d_err_off.p, err_off.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    /* one warp per band of 32 rows, band-major (band k of every image, then band k + 1): a band's producer is always
+     * launched before it, and the warps resident at any time are bands that can actually run (a band may start ~113
+     * steps after the one above it, so only ~W/113 bands of an image are ever active together) */
+    b->dbands.clear();
+    {
+        /* .w: the list position of band k - 255 of the same image, which band k >= 256 waits for (jdk_dither), else ~0 */
+        uint32_t maxb = 0;
+        std::vector<uint32_t> nb(n, 0), prevpos(n, 0), first(n, 0);
+        for (int i = 0; i < n; i++) if (b->parse_status[i] == JPEG_SUCCESS) { nb[i] = (b->descs[i].out_h + 31) / 32; if (nb[i] > maxb) maxb = nb[i]; }
+        std::vector<uint32_t> where;                       /* list position of band k of image i at first[i] + k */
+        for (int i = 0; i < n; i++) { first[i] = (uint32_t)where.size(); where.resize(where.size() + nb[i]); }
+        for (uint32_t k = 0; k < maxb; k++)
+            for (int i = 0; i < n; i++) {
+                if (k >= nb[i]) continue;
+                const uint32_t pos = (uint32_t)b->dbands.size();
+                where[first[i] + k] = pos;
+                b->dbands.push_back(make_uint4((uint32_t)i, k, prevpos[i], k >= 256 ? where[first[i] + k - 255] : ~0u));
+                prevpos[i] = pos;
             }
-            if (fixed) break;
-            CK(cudaMemcpyAsync(&b->h_changed, b->d_counters.p + 2, 4, cudaMemcpyDeviceToHost, st));
-            CK(cudaStreamSynchronize(st));
-            if (!b->h_changed || passes > (int)b->nchunks + 8) break;
-        }
-        ca.X_in = Xin; ca.X_out = Xout;
-        jdk_chunk_prefix<<<gi, 128, 0, st>>>(ca);
-        jdk_chunk_emit<<<gchunks, 128, 0, st>>>(ca);
-        jdk_chunk_stitch<<<gi, 128, 0, st>>>(ca);
-        launches += 3;
     }
-    /* progressive files: one launch per wave of scan walkers */
+    CK(b->d_dbands.alloc(&b->ctx->pool, b->dbands.size() ? b->dbands.size() : 1)); CK(b->d_dprog.alloc(&b->ctx->pool, b->dbands.size() + 1));
+    if (!b->dbands.empty()) CK(cudaMemcpyAsync(b->d_dbands.p, b->dbands.data(), b->dbands.size() * sizeof(uint4), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(b->d_dprog.p, 0, (b->dbands.size() + 1) * 4, st));
+    return 1;
+}
+
+/* the entropy walk of the work list: every restart interval of the files that have restart markers */
+static int run_entropy(JPEGB200_BATCH *b, DecodeState &D)
+{
+    if (b->work.empty()) return 1;
+    cudaStream_t st = b->ss.stream;
+    JDImageDesc *const fdev = file_descs_dev(b);
+    JDEntropyArgs ea;
+    ea.data = b->d_comp.p; ea.imgs = fdev; ea.luts = b->d_luts.p; ea.work = b->d_work.p; ea.cta_lut = b->d_cta_lut.p;
+    ea.seg_img = b->d_seg_img.p; ea.seg_start = b->d_seg_start.p; ea.blk_hdr = b->d_blk_hdr.p; ea.rec = b->d_rec.p;
+    ea.seg_jmap = b->d_seg_jmap.p; ea.seg_status = b->d_seg_status.p; ea.seg_nrec = b->d_seg_nrec.p;
+    ea.events = b->d_events.p; ea.event_count = b->d_counters.p; ea.event_cap = JD_EVENT_CAP;
+    ea.nwork = (uint32_t)b->work.size(); ea.dc_output = (b->sshift == 3) ? 1u : (b->sshift == 2) ? 2u : 0u;
+    /* default ("raw"): the entropy kernel un-stuffs in its bit reader, 64-thread CTAs.  JPEGDEC_B200_ENTROPY=clean:
+     * jdk_unstuff_segs first, so that the reader is a plain word stream (128-thread CTAs).  On the H100 the raw walk is
+     * the faster one (DESIGN.md 4.1). */
+    static int use_clean = -1;
+    if (use_clean < 0) { const char *e = getenv("JPEGDEC_B200_ENTROPY"); use_clean = (e && strcmp(e, "clean") == 0) ? 1 : 0; }
+    const unsigned egrid = (unsigned)(b->work.size() / JD_ENTROPY_THREADS);
+#ifdef JD_ENTROPY_PROBE
+    /* development build: time the un-stuffing (clean pipeline) and the walk apart; the walk's warps print their own lines */
+    cudaEvent_t pev[3];
+    for (auto &e : pev) CK(cudaEventCreate(&e));
+    CK(cudaEventRecord(pev[0], st));
+#endif
+    if (use_clean) {
+        CK(b->d_clean.alloc(&b->ctx->pool, b->comp_total + 32 * (size_t)b->nseg + 4096));
+        CK(b->d_seg_clen.alloc(&b->ctx->pool, b->nseg ? b->nseg : 1));
+        jdk_unstuff_segs<<<(b->nseg * 32u + JD_UNSTUFF_WARPS * 32u - 1u) / (JD_UNSTUFF_WARPS * 32u), JD_UNSTUFF_WARPS * 32, 0, st>>>(
+            b->d_comp.p, fdev, b->d_seg_img.p, b->d_seg_start.p, b->nseg, b->d_clean.p, b->d_seg_clen.p);
+        ea.clean = b->d_clean.p; ea.seg_clen = b->d_seg_clen.p;
+    } else {
+        ea.clean = nullptr; ea.seg_clen = nullptr;
+    }
+#ifdef JD_ENTROPY_PROBE
+    CK(cudaEventRecord(pev[1], st));
+#endif
+    const unsigned ecta = use_clean ? jd_entropy_cta_threads(true) : jd_entropy_cta_threads(false);
+    const unsigned egrid_walk = egrid * (JD_ENTROPY_THREADS / ecta);
+    if (use_clean) jdk_entropy<true><<<egrid_walk, ecta, 0, st>>>(ea);
+    else jdk_entropy<false><<<egrid_walk, ecta, 0, st>>>(ea);
+    D.launches += use_clean ? 2 : 1;
+#ifdef JD_ENTROPY_PROBE
+    CK(cudaEventRecord(pev[2], st));
+    CK(cudaStreamSynchronize(st));
+    float ms_u = 0.f, ms_w = 0.f;
+    CK(cudaEventElapsedTime(&ms_u, pev[0], pev[1]));
+    CK(cudaEventElapsedTime(&ms_w, pev[1], pev[2]));
+    printf("JDP_LAUNCH nwork %u ctas %u unstuff_ms %.4f walk_ms %.4f\n", (unsigned)b->work.size(), egrid_walk, ms_u, ms_w);
+    fflush(stdout);
+    for (auto &e : pev) CK(cudaEventDestroy(e));
+#endif
+    return 1;
+}
+
+/* restart-free scans: un-stuff, iterate the chunk entry states to their fix point, then emit */
+static int run_chunks(JPEGB200_BATCH *b, DecodeState &D)
+{
+    if (!b->nchunks) return 1;
+    cudaStream_t st = b->ss.stream;
+    JDChunkArgs ca;
+    ca.comp = b->d_comp.p; ca.filt = b->d_filt.p; ca.imgs = file_descs_dev(b); ca.luts = b->d_luts.p;
+    ca.cimg_list = b->d_cimg_list.p; ca.ncimg = (uint32_t)b->cimg_list.size(); ca.flen = b->d_flen.p;
+    ca.nchunks = b->nchunks;
+    ca.cn = b->d_cn.p; ca.cpre = b->d_cpre.p; ca.cjmap = b->d_cjmap.p; ca.cstatus = b->d_cstatus.p; ca.cnown = b->d_cnown.p;
+    ca.cdcs = b->d_cdcs.p; ca.cpe = b->d_cpe.p; ca.changed = b->d_counters.p + 2;
+    ca.blk_hdr = b->d_blk_hdr.p; ca.rec = b->d_rec.p;
+    ca.events = b->d_events.p; ca.event_count = b->d_counters.p; ca.event_cap = JD_EVENT_CAP;
+    ca.seg_phase = b->d_seg_phase.p; ca.seg_jmap = b->d_seg_jmap.p; ca.seg_status = b->d_seg_status.p; ca.nseg_total = b->nseg;
+    const unsigned gi = ((unsigned)b->cimg_list.size() * 32 + 127) / 128;
+    ca.max_nch = b->max_nch; ca.Ep = b->d_Ep.p; ca.cfirst = b->d_cfirst.p;
+    const dim3 gchunks((b->max_nch + 127) / 128, (unsigned)b->cimg_list.size());
+    /* guess: every chunk starts a block at its first bit (exit state of every left neighbour = (0, 0, 0)); no chunk parsed yet */
+    CK(cudaMemsetAsync(b->d_E0.p, 0, (size_t)(b->nchunks + 1) * 4, st));
+    CK(cudaMemsetAsync(b->d_Ep.p, 0xFE, (size_t)b->nchunks * 4, st));
+    {
+        const dim3 gu(((b->max_nch * JD_CHUNK_BYTES + JD_UNSTUFF_PIECE - 1) / JD_UNSTUFF_PIECE + 3) / 4, (unsigned)b->cimg_list.size());
+        jdk_unstuff<false><<<gu, 128, 0, st>>>(ca);
+        jdk_unstuff<true><<<gu, 128, 0, st>>>(ca);
+    }
+    D.launches += 2;
+    uint32_t *Xin = b->d_E0.p, *Xout = b->d_E1.p;
+    int passes = 0;
+    /* The entry states reach their fix point in 2-4 passes on real streams (a chunk re-synchronises well inside its 512
+     * bytes), and from the third pass on only the chunks whose entry state moved are parsed again.  Normal mode:
+     * JD_CHUNK_PASSES passes back to back, the last one verifying (it raises a flag if an exit state still moved) -- no
+     * host round trip, so jobs of JPEGB200_decodeBatch stay in flight; batchWait re-runs the job in the iterating mode
+     * below if the flag came back set. */
+    static int fixed_passes = -1;   /* JPEGDEC_B200_CHUNK_PASSES=n: test hook (n = 1 forces the fallback) */
+    if (fixed_passes < 0) { const char *e = getenv("JPEGDEC_B200_CHUNK_PASSES"); fixed_passes = (e && atoi(e) > 0) ? atoi(e) : JD_CHUNK_PASSES; }
+    const int fixed = b->chunk_iterate ? 0 : fixed_passes;
+    for (;;) {
+        const int burst = fixed ? fixed : 3;
+        for (int k = 0; k < burst; k++) {
+            if (k == burst - 1) CK(cudaMemsetAsync(b->d_counters.p + 2, 0, 4, st));
+            ca.X_in = Xin; ca.X_out = Xout;
+            jdk_chunk_parse<<<gchunks, 128, 0, st>>>(ca);
+            D.launches++; passes++;
+            uint32_t *tmp = Xin; Xin = Xout; Xout = tmp;
+        }
+        if (fixed) break;
+        CK(cudaMemcpyAsync(&b->h_changed, b->d_counters.p + 2, 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        if (!b->h_changed || passes > (int)b->nchunks + 8) break;
+    }
+    ca.X_in = Xin; ca.X_out = Xout;
+    jdk_chunk_prefix<<<gi, 128, 0, st>>>(ca);
+    jdk_chunk_emit<<<gchunks, 128, 0, st>>>(ca);
+    jdk_chunk_stitch<<<gi, 128, 0, st>>>(ca);
+    D.launches += 3;
+    return 1;
+}
+
+/* progressive files: one launch per wave of scan walkers */
+static void run_prog_waves(JPEGB200_BATCH *b, DecodeState &D)
+{
     for (size_t w = 0; w + 1 < b->pwave_off.size(); w++) {
         const uint32_t o = b->pwave_off[w], cnt = b->pwave_off[w + 1] - o;
         if (cnt == 0) continue;
-        jdk_prog_scan<<<(cnt + 63) / 64, 64, 0, st>>>(b->d_pscans.p + o, cnt, b->d_comp.p, b->d_ptabs.p, b->d_pplanes.p, b->d_perr.p);
-        launches++;
+        jdk_prog_scan<<<(cnt + 63) / 64, 64, 0, b->ss.stream>>>(b->d_pscans.p + o, cnt, b->d_comp.p, b->d_ptabs.p, b->d_pplanes.p, b->d_perr.p);
+        D.launches++;
     }
-    CK(cudaEventRecord(b->ev[4], st));
+}
+
+/* per file: the first error of its segments (stitch), the window-truncation events (patch), and the records of the
+ * progressive files from their coefficient planes (pack) */
+static void run_stitch_patch_pack(JPEGB200_BATCH *b, DecodeState &D)
+{
+    cudaStream_t st = b->ss.stream;
+    JDImageDesc *const fdev = file_descs_dev(b);
+    const int nf = b->nf;
     jdk_stitch<<<(nf + 127) / 128, 128, 0, st>>>(fdev, (uint32_t)nf, b->d_seg_jmap.p, b->d_seg_status.p, b->d_seg_phase.p, b->d_seg_nrec.p,
                                                reinterpret_cast<unsigned long long *>(b->d_counters.p + 4));
-    launches++;
+    D.launches++;
     if (!b->lj) {   /* a libjpeg decode reads the exact coefficients: no window truncation to apply */
         jdk_patch<<<32, 256, 0, st>>>(fdev, b->d_events.p, b->d_counters.p, JD_EVENT_CAP, b->d_seg_phase.p, b->d_blk_hdr.p, b->d_rec.p, b->d_counters.p + 1);
-        launches++;
+        D.launches++;
     }
     if (!b->pfiles.empty()) {
         /* after jdk_stitch, which gives a file without restart segments status 0: the pack writes the real one */
@@ -1728,35 +1767,75 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         pa.limit = b->sshift == 3 ? 1u : b->sshift == 2 ? 5u : 64u;
         pa.rec_count = reinterpret_cast<unsigned long long *>(b->d_counters.p + 4);
         jdk_prog_pack<<<(unsigned)b->pfiles.size(), 256, 0, st>>>(pa);
-        launches++;
+        D.launches++;
     }
-    CK(cudaEventRecord(b->ev[5], st));
-    /* IDCT + colour: one launch per run of images with the same geometry class */
-    const bool half = b->sshift == 1;
-    uint8_t *stage_out = b->dither_bits ? b->d_gray.p : b->resize ? b->d_rs.p : pipe_out;
-    if (b->lj) {
-        /* planes of every image's MCU box, then upsampling + colour into the stores; images that failed keep nmx = 0 */
-        std::vector<JDLjDesc> ld = b->lj_desc;
-        uint64_t po = 0;
-        for (int i = 0; i < n; i++) {
-            if (b->parse_status[i] != JPEG_SUCCESS) { ld[i].nmx = ld[i].nmy = 0; continue; }
-            ld[i].plane_off = po;
-            po += (uint64_t)b->lj_plane[i];
-        }
-        CK(b->d_lj.alloc(&b->ctx->pool, po + 256));
-        CK(b->d_lj_desc.alloc(&b->ctx->pool, n));
-        CK(cudaMemcpyAsync(b->d_lj_desc.p, ld.data(), sizeof(JDLjDesc) * n, cudaMemcpyHostToDevice, st));
-        const unsigned gb = (b->lj_max_blocks + JD_LJ_THREADS - 1) / JD_LJ_THREADS, gp = (b->lj_max_pixels + JD_LJ_THREADS - 1) / JD_LJ_THREADS;
-        for (int i0 = 0; i0 < n && gb && gp; i0 += 65535) {
-            const unsigned ni = (unsigned)std::min(n - i0, 65535);
-            jdk_lj_idct<<<dim3(gb, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, b->d_lj_desc.p, b->d_blk_hdr.p, b->d_rec.p, b->d_quant.p,
-                                                                 b->d_lj.p, (uint32_t)i0);
-            if (b->ptclass == JD_PT_GRAY) jdk_lj_color<JD_PT_GRAY><<<dim3(gp, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, b->d_lj_desc.p, b->d_lj.p, stage_out, (uint32_t)i0);
-            else jdk_lj_color<JD_PT_8888><<<dim3(gp, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, b->d_lj_desc.p, b->d_lj.p, stage_out, (uint32_t)i0);
-            launches += 2;
-        }
+}
+
+/* libjpeg decode: planes of every image's MCU box, then upsampling + colour into the stores; images that failed keep nmx = 0 */
+static int run_lj(JPEGB200_BATCH *b, DecodeState &D)
+{
+    const int n = b->n;
+    cudaStream_t st = b->ss.stream;
+    std::vector<JDLjDesc> ld = b->lj_desc;
+    uint64_t po = 0;
+    for (int i = 0; i < n; i++) {
+        if (b->parse_status[i] != JPEG_SUCCESS) { ld[i].nmx = ld[i].nmy = 0; continue; }
+        ld[i].plane_off = po;
+        po += (uint64_t)b->lj_plane[i];
     }
-    for (int i0 = 0; i0 < n && !b->lj;) {
+    CK(b->d_lj.alloc(&b->ctx->pool, po + 256));
+    CK(b->d_lj_desc.alloc(&b->ctx->pool, n));
+    CK(cudaMemcpyAsync(b->d_lj_desc.p, ld.data(), sizeof(JDLjDesc) * n, cudaMemcpyHostToDevice, st));
+    const unsigned gb = (b->lj_max_blocks + JD_LJ_THREADS - 1) / JD_LJ_THREADS, gp = (b->lj_max_pixels + JD_LJ_THREADS - 1) / JD_LJ_THREADS;
+    for (int i0 = 0; i0 < n && gb && gp; i0 += 65535) {
+        const unsigned ni = (unsigned)std::min(n - i0, 65535);
+        jdk_lj_idct<<<dim3(gb, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, b->d_lj_desc.p, b->d_blk_hdr.p, b->d_rec.p, b->d_quant.p,
+                                                             b->d_lj.p, (uint32_t)i0);
+        if (b->ptclass == JD_PT_GRAY) jdk_lj_color<JD_PT_GRAY><<<dim3(gp, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, b->d_lj_desc.p, b->d_lj.p, D.stage_out, (uint32_t)i0);
+        else jdk_lj_color<JD_PT_8888><<<dim3(gp, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, b->d_lj_desc.p, b->d_lj.p, D.stage_out, (uint32_t)i0);
+        D.launches += 2;
+    }
+    return 1;
+}
+
+/* the IDCT + colour (or scaled) launch of images i0 .. i0 + nimg - 1, which share a geometry class, for one orientation
+ * class; the grid covers max_mx x max_my MCUs per image */
+static int launch_idct_run(JPEGB200_BATCH *b, const DecodeState &D, int i0, uint32_t nimg, uint32_t max_mx, uint32_t max_my, uint32_t orc)
+{
+    cudaStream_t st = b->ss.stream;
+    const JDInfo &f = b->infos[file_of(b, i0)];
+    if (b->sshift >= 2) {
+        JDScaledArgs sa;
+        sa.imgs = b->d_descs.p; sa.blk_hdr = b->d_blk_hdr.p; sa.rec = b->d_rec.p; sa.quant = b->d_quant.p;
+        sa.out = D.stage_out; sa.img0 = (uint32_t)i0; sa.pixel_type = (uint32_t)b->pixel_type; sa.eighth = (b->sshift == 3);
+        sa.padded = (b->dither_bits || b->padded) ? 1u : 0u;
+        dim3 grid((max_mx * max_my + 127) / 128, nimg);
+        if (orc == JD_ORC_FLIP) jdk_scaled<true, JD_ORC_FLIP><<<grid, 128, 0, st>>>(sa);
+        else if (orc == JD_ORC_TRANSPOSE) jdk_scaled<true, JD_ORC_TRANSPOSE><<<grid, 128, 0, st>>>(sa);
+        else if (b->roi) jdk_scaled<true><<<grid, 128, 0, st>>>(sa);
+        else jdk_scaled<false><<<grid, 128, 0, st>>>(sa);
+        return 1;
+    }
+    JDIdctArgs ia;
+    ia.imgs = b->d_descs.p; ia.blk_hdr = b->d_blk_hdr.p; ia.rec = b->d_rec.p; ia.quant = b->d_quant.p;
+    ia.out = D.stage_out; ia.img0 = (uint32_t)i0;
+    ia.big_endian = (f.ncomp == 1) ? (b->pixel_type != RGB565_LITTLE_ENDIAN) : (b->pixel_type == RGB565_BIG_ENDIAN);
+    ia.padded = (b->dither_bits || b->padded) ? 1u : 0u;
+    ia.mcus_x = (uint32_t)f.mcus_x; ia.mcus_y = (uint32_t)f.mcus_y; ia.width = (uint32_t)f.width; ia.height = (uint32_t)f.height;
+    ia.bpm = (uint32_t)f.bpm;
+    ia.roi = b->roi ? 1u + orc : 0u;
+    if (!launch_idct(ia, f.subsample, f.ncomp, b->ptclass, b->ctx->arith, b->sshift == 1, max_mx, max_my, nimg, st)) {
+        snprintf(g_err, sizeof(g_err), "no kernel for subsample 0x%02x / pixel type %d", f.subsample, b->pixel_type);
+        return 0;
+    }
+    return 1;
+}
+
+/* IDCT + colour: one launch per run of images with the same geometry class (and per orientation class of the run) */
+static int run_idct(JPEGB200_BATCH *b, DecodeState &D)
+{
+    const int n = b->n;
+    for (int i0 = 0; i0 < n;) {
         if (b->parse_status[i0] != JPEG_SUCCESS) { i0++; continue; }
         const JDInfo &f = b->infos[file_of(b, i0)];
         int i1 = i0 + 1;
@@ -1768,7 +1847,6 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
             if ((uint32_t)g.mcus_y > max_my) max_my = g.mcus_y;
             i1++;
         }
-        const uint32_t nimg = (uint32_t)(i1 - i0);
         if (b->roi) {
             /* the grid covers the largest box of MCUs a rectangle of the group touches, from each image's first MCU column / row */
             max_mx = max_my = 0;
@@ -1792,125 +1870,140 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
         else if (!any_tr) classes[nclass++] = JD_ORC_NONE;
         if (any_tr) classes[nclass++] = JD_ORC_TRANSPOSE;
         for (int ci = 0; ci < nclass; ci++) {
-        const uint32_t orc = classes[ci];
-        if (b->sshift >= 2) {
-            JDScaledArgs sa;
-            sa.imgs = b->d_descs.p; sa.blk_hdr = b->d_blk_hdr.p; sa.rec = b->d_rec.p; sa.quant = b->d_quant.p;
-            sa.out = stage_out; sa.img0 = (uint32_t)i0; sa.pixel_type = (uint32_t)b->pixel_type; sa.eighth = (b->sshift == 3);
-            sa.padded = (b->dither_bits || b->padded) ? 1u : 0u;
-            dim3 grid((max_mx * max_my + 127) / 128, nimg);
-            if (orc == JD_ORC_FLIP) jdk_scaled<true, JD_ORC_FLIP><<<grid, 128, 0, st>>>(sa);
-            else if (orc == JD_ORC_TRANSPOSE) jdk_scaled<true, JD_ORC_TRANSPOSE><<<grid, 128, 0, st>>>(sa);
-            else if (b->roi) jdk_scaled<true><<<grid, 128, 0, st>>>(sa);
-            else jdk_scaled<false><<<grid, 128, 0, st>>>(sa);
-        } else {
-            JDIdctArgs ia;
-            ia.imgs = b->d_descs.p; ia.blk_hdr = b->d_blk_hdr.p; ia.rec = b->d_rec.p; ia.quant = b->d_quant.p;
-            ia.out = stage_out; ia.img0 = (uint32_t)i0;
-            ia.big_endian = (f.ncomp == 1) ? (b->pixel_type != RGB565_LITTLE_ENDIAN) : (b->pixel_type == RGB565_BIG_ENDIAN);
-            ia.padded = (b->dither_bits || b->padded) ? 1u : 0u;
-            ia.mcus_x = (uint32_t)f.mcus_x; ia.mcus_y = (uint32_t)f.mcus_y; ia.width = (uint32_t)f.width; ia.height = (uint32_t)f.height;
-            ia.bpm = (uint32_t)f.bpm;
-            ia.roi = b->roi ? 1u + orc : 0u;
-            int ok = 0;
-            const int ar = b->ctx->arith;
-            static int use_packed = -1;   /* JPEGDEC_B200_IDCT=lanes|tb: the round-1 kernels also for the SSE2-build arithmetic (A/B) */
-            if (use_packed < 0) { const char *e = getenv("JPEGDEC_B200_IDCT"); use_packed = (e && (strcmp(e, "lanes") == 0 || strcmp(e, "tb") == 0)) ? 0 : 1; }
-            /* 4:2:0 colour at full size keeps jdk_idct_tb (measured faster there -- there is no packed 16-bit subtract
-             * instruction, __vsub2 costs three, which eats what the packed adds save); every other
-             * sampling / pixel type / half scale takes the packed thread-per-block kernel instead of the 8-lanes-per-block one */
-            const bool tb_case = f.subsample == 0x22 && f.ncomp == 3 && b->ptclass != JD_PT_GRAY && !half;
-            static int force_packed = -1;
-            if (force_packed < 0) { const char *e = getenv("JPEGDEC_B200_IDCT"); force_packed = (e && strcmp(e, "packed") == 0) ? 1 : 0; }
-            if (ar == JPEG_ARITH_SSE2 && use_packed && (!tb_case || force_packed)) {
-                switch (f.subsample) {
-                    case 0x00: case 0x11: ok = launch_idct_packed<1, 1>(ia, max_mx, max_my, nimg, f.ncomp, b->ptclass, half, st); break;
-                    case 0x21: ok = launch_idct_packed<2, 1>(ia, max_mx, max_my, nimg, f.ncomp, b->ptclass, half, st); break;
-                    case 0x12: ok = launch_idct_packed<1, 2>(ia, max_mx, max_my, nimg, f.ncomp, b->ptclass, half, st); break;
-                    case 0x22: ok = launch_idct_packed<2, 2>(ia, max_mx, max_my, nimg, f.ncomp, b->ptclass, half, st); break;
-                }
-            } else
-            switch (f.subsample) {
-                case 0x00: case 0x11: ok = launch_idct_geo<1, 1, 16, 32>(ia, max_mx, max_my, nimg, f.ncomp, b->ptclass, ar, half, st); break;
-                case 0x21: ok = launch_idct_geo<2, 1, 8, 16>(ia, max_mx, max_my, nimg, f.ncomp, b->ptclass, ar, half, st); break;
-                case 0x12: ok = launch_idct_geo<1, 2, 8, 16>(ia, max_mx, max_my, nimg, f.ncomp, b->ptclass, ar, half, st); break;
-                case 0x22: ok = launch_idct_geo<2, 2, 8, 8>(ia, max_mx, max_my, nimg, f.ncomp, b->ptclass, ar, half, st); break;
-            }
-            if (!ok) { snprintf(g_err, sizeof(g_err), "no kernel for subsample 0x%02x / pixel type %d", f.subsample, b->pixel_type); return 0; }
-        }
-        launches++;
+            if (!launch_idct_run(b, D, i0, (uint32_t)(i1 - i0), max_mx, max_my, classes[ci])) return 0;
+            D.launches++;
         }
         i0 = i1;
     }
-    CK(cudaEventRecord(b->ev[6], st));
-    if (b->dither_bits) {
-        if (!b->dbands.empty()) {
-            const unsigned dgrid = ((unsigned)b->dbands.size() * 32 + 127) / 128;
-#define JD_DITHER_ARGS b->d_descs.p, (uint32_t)n, b->d_gray.p, b->d_gray_off.p, b->d_errline.p, b->d_err_off.p, out_base, (uint32_t)b->sshift, \
+    return 1;
+}
+
+static void run_dither(JPEGB200_BATCH *b, DecodeState &D)
+{
+    if (b->dbands.empty()) return;
+    cudaStream_t st = b->ss.stream;
+    const unsigned dgrid = ((unsigned)b->dbands.size() * 32 + 127) / 128;
+#define JD_DITHER_ARGS b->d_descs.p, (uint32_t)b->n, b->d_gray.p, b->d_gray_off.p, b->d_errline.p, b->d_err_off.p, D.out_base, (uint32_t)b->sshift, \
                        b->d_dbands.p, (uint32_t)b->dbands.size(), b->d_dprog.p
-            if (b->dither_bits == 1) jdk_dither<1><<<dgrid, 128, 0, st>>>(JD_DITHER_ARGS);
-            else if (b->dither_bits == 2) jdk_dither<2><<<dgrid, 128, 0, st>>>(JD_DITHER_ARGS);
-            else jdk_dither<4><<<dgrid, 128, 0, st>>>(JD_DITHER_ARGS);
+    if (b->dither_bits == 1) jdk_dither<1><<<dgrid, 128, 0, st>>>(JD_DITHER_ARGS);
+    else if (b->dither_bits == 2) jdk_dither<2><<<dgrid, 128, 0, st>>>(JD_DITHER_ARGS);
+    else jdk_dither<4><<<dgrid, 128, 0, st>>>(JD_DITHER_ARGS);
 #undef JD_DITHER_ARGS
-            launches++;
-        }
+    D.launches++;
+}
+
+/* timed in the dither slot (the pixel pass after the IDCT): the two never occur together */
+static void run_resize(JPEGB200_BATCH *b, DecodeState &D)
+{
+    cudaStream_t st = b->ss.stream;
+    const uint32_t n = (uint32_t)b->n;
+    const bool gray = b->ptclass == JD_PT_GRAY;
+    const uint32_t *rs_ctas = D.rs_ctas;
+    if (rs_ctas[0]) { jdk_resize_coeffs<<<rs_ctas[0], JD_RS_THREADS, 0, st>>>(b->d_rs_desc.p, n, b->d_rs_coef.p, b->rs_filter); D.launches++; }
+#define JD_RS_ARGS b->d_rs_desc.p, n, b->d_rs.p, b->d_rs_coef.p, D.pipe_out
+    if (rs_ctas[1]) {
+        if (gray) jdk_resize_h<1, 0><<<rs_ctas[1], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
+        else jdk_resize_h<4, 0><<<rs_ctas[1], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
+        D.launches++;
     }
-    if (b->resize) {
-        /* timed in the dither slot (the pixel pass after the IDCT): the two never occur together */
-        const bool gray = b->ptclass == JD_PT_GRAY;
-        if (rs_ctas[0]) { jdk_resize_coeffs<<<rs_ctas[0], JD_RS_THREADS, 0, st>>>(b->d_rs_desc.p, (uint32_t)n, b->d_rs_coef.p, b->rs_filter); launches++; }
-#define JD_RS_ARGS b->d_rs_desc.p, (uint32_t)n, b->d_rs.p, b->d_rs_coef.p, pipe_out
-        if (rs_ctas[1]) {
-            if (gray) jdk_resize_h<1, 0><<<rs_ctas[1], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
-            else jdk_resize_h<4, 0><<<rs_ctas[1], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
-            launches++;
-        }
-        if (rs_ctas[2]) {
-            if (gray) jdk_resize_v<1><<<rs_ctas[2], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
-            else jdk_resize_v<4><<<rs_ctas[2], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
-            launches++;
-        }
-        if (rs_ctas[3]) {   /* images whose vertical pass ran first (JDResizePlan.vfirst) */
-            if (gray) jdk_resize_h<1, 1><<<rs_ctas[3], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
-            else jdk_resize_h<4, 1><<<rs_ctas[3], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
-            launches++;
-        }
+    if (rs_ctas[2]) {
+        if (gray) jdk_resize_v<1><<<rs_ctas[2], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
+        else jdk_resize_v<4><<<rs_ctas[2], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
+        D.launches++;
+    }
+    if (rs_ctas[3]) {   /* images whose vertical pass ran first (JDResizePlan.vfirst) */
+        if (gray) jdk_resize_h<1, 1><<<rs_ctas[3], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
+        else jdk_resize_h<4, 1><<<rs_ctas[3], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
+        D.launches++;
+    }
 #undef JD_RS_ARGS
-    }
-    if (b->tensor && tn_ctas) {
-        /* timed in the dither slot too, after the resize */
-        const bool hwc = b->tn_spec.layout == JPEGB200_LAYOUT_HWC;
+}
+
+/* timed in the dither slot too, after the resize */
+static void run_tensor(JPEGB200_BATCH *b, DecodeState &D)
+{
+    if (!D.tn_ctas) return;
+    cudaStream_t st = b->ss.stream;
+    const uint32_t n = (uint32_t)b->n, tn_ctas = D.tn_ctas;
+    const bool hwc = b->tn_spec.layout == JPEGB200_LAYOUT_HWC;
 #define JD_TN_LAUNCH(ELT_, NC_)                                                                                           \
-        if (hwc) jdk_tensor<ELT_, 1, NC_><<<tn_ctas, JD_TN_THREADS, 0, st>>>(b->d_tn_desc.p, (uint32_t)n, b->d_tn.p, b->d_tn_tab.p, out_base); \
-        else jdk_tensor<ELT_, 0, NC_><<<tn_ctas, JD_TN_THREADS, 0, st>>>(b->d_tn_desc.p, (uint32_t)n, b->d_tn.p, b->d_tn_tab.p, out_base);
-        if (b->tn_nc == 3) {
-            if (b->tn_elt == 4) { JD_TN_LAUNCH(4, 3) } else if (b->tn_elt == 2) { JD_TN_LAUNCH(2, 3) } else { JD_TN_LAUNCH(1, 3) }
-        } else {
-            if (b->tn_elt == 4) { JD_TN_LAUNCH(4, 1) } else if (b->tn_elt == 2) { JD_TN_LAUNCH(2, 1) } else { JD_TN_LAUNCH(1, 1) }
-        }
-#undef JD_TN_LAUNCH
-        launches++;
+    if (hwc) jdk_tensor<ELT_, 1, NC_><<<tn_ctas, JD_TN_THREADS, 0, st>>>(b->d_tn_desc.p, n, b->d_tn.p, b->d_tn_tab.p, D.out_base); \
+    else jdk_tensor<ELT_, 0, NC_><<<tn_ctas, JD_TN_THREADS, 0, st>>>(b->d_tn_desc.p, n, b->d_tn.p, b->d_tn_tab.p, D.out_base);
+    if (b->tn_nc == 3) {
+        if (b->tn_elt == 4) { JD_TN_LAUNCH(4, 3) } else if (b->tn_elt == 2) { JD_TN_LAUNCH(2, 3) } else { JD_TN_LAUNCH(1, 3) }
+    } else {
+        if (b->tn_elt == 4) { JD_TN_LAUNCH(4, 1) } else if (b->tn_elt == 2) { JD_TN_LAUNCH(2, 1) } else { JD_TN_LAUNCH(1, 1) }
     }
-    CK(cudaEventRecord(b->ev[7], st));
-    CK(cudaGetLastError());
-    b->counters[JPEGB200_C_LAUNCHES] = launches;
+#undef JD_TN_LAUNCH
+    D.launches++;
+}
+
+static void set_decode_counters(JPEGB200_BATCH *b, const DecodeState &D)
+{
+    b->counters[JPEGB200_C_LAUNCHES] = D.launches;
     b->counters[JPEGB200_C_SEGMENTS] = b->nseg_walk + b->pwalkers;
     b->counters[JPEGB200_C_BLOCKS] = (int64_t)b->nblk;
     b->counters[JPEGB200_C_COMPRESSED_BYTES] = (int64_t)b->comp_total;
     int64_t ob = 0;
-    for (int i = 0; i < n; i++)
+    for (int i = 0; i < b->n; i++)
         if (b->parse_status[i] == JPEG_SUCCESS)
             ob += b->tensor ? JPEGB200_batchOutputBytes(b, i, nullptr) : (int64_t)b->pitches[i] * b->descs[i].out_h;
     b->counters[JPEGB200_C_OUTPUT_BYTES] = ob;
+}
+
+/* The host pipeline of one job, in stream order.  The events ev[2] .. ev[7] bound the published stage timings
+ * (JPEGB200_batchWait): prescan, entropy, stitch, IDCT, and the pixel pass after it (dither, resize, tensor). */
+extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
+{
+    if (!b) return 0;
+    if (!b->uploaded) { snprintf(g_err, sizeof(g_err), "batchDecode before batchUpload"); return 0; }
+    if (!batch_stream(b)) return 0;
+    cudaStream_t st = b->ss.stream;
+    const cudaEvent_t *ev = b->ss.ev;
+    b->out_device = (flags & JPEGB200_OUT_DEVICE) != 0;
+    b->decode_flags = flags;
+    if (b->tensor && !b->out_device) {
+        snprintf(g_err, sizeof(g_err), "tensor output is written to device memory only: decode with JPEGB200_OUT_DEVICE");
+        return 0;
+    }
+    DecodeState D;
+    if (!alloc_prog_planes(b) || !place_outputs(b, D)) return 0;
+    /* each stage that writes through scratch redirects the stage before it: tensor <- resize <- IDCT, dither <- IDCT */
+    if (b->tensor && !stage_tensor(b, D)) return 0;
+    if (b->resize && !stage_resize(b, D)) return 0;
+    if (b->dither_bits && !stage_dither(b, D)) return 0;
+    CK(cudaMemcpyAsync(b->d_descs.p, D.descs_stage.data(), sizeof(JDImageDesc) * b->n, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(b->d_counters.p, 0, 32, st));
+    if (b->nchunks) CK(cudaMemsetAsync(b->d_blk_hdr.p, 0, (size_t)b->nblk * 8, st)); /* blocks a truncated restart-free scan never reaches stay empty */
+
+    /* prescan, entropy walk, stitch and patch: one entropy-facing descriptor per file (its views share them) */
+    CK(cudaEventRecord(ev[2], st));
+    jdk_prescan<<<b->nf, 256, 0, st>>>(b->d_comp.p, file_descs_dev(b), b->d_seg_start.p);
+    D.launches++;
+    CK(cudaEventRecord(ev[3], st));
+    if (!run_entropy(b, D) || !run_chunks(b, D)) return 0;
+    run_prog_waves(b, D);
+    CK(cudaEventRecord(ev[4], st));
+    run_stitch_patch_pack(b, D);
+    CK(cudaEventRecord(ev[5], st));
+    D.stage_out = b->dither_bits ? b->d_gray.p : b->resize ? b->d_rs.p : D.pipe_out;
+    if (b->lj ? !run_lj(b, D) : !run_idct(b, D)) return 0;
+    CK(cudaEventRecord(ev[6], st));
+    if (b->dither_bits) run_dither(b, D);
+    if (b->resize) run_resize(b, D);
+    if (b->tensor) run_tensor(b, D);
+    CK(cudaEventRecord(ev[7], st));
+    CK(cudaGetLastError());
+    set_decode_counters(b, D);
     return 1;
 }
 
 extern "C" int JPEGB200_batchDownload(JPEGB200_BATCH *b)
 {
-    if (!b || !b->stream) return 0;
-    cudaStream_t st = b->stream;
+    if (!b || !b->ss.stream) return 0;
+    cudaStream_t st = b->ss.stream;
     CK(cudaSetDevice(b->ctx->device));
-    CK(cudaEventRecord(b->ev[8], st));
+    CK(cudaEventRecord(b->ss.ev[8], st));
     int64_t bytes = 0;
     if (!b->out_device) {
         const int n = b->n;
@@ -1949,16 +2042,16 @@ extern "C" int JPEGB200_batchDownload(JPEGB200_BATCH *b)
     CK(cudaMemcpyAsync(b->h_counters, b->d_counters.p, 32, cudaMemcpyDeviceToHost, st));
     b->downloaded = true;
     bytes += (int64_t)sizeof(JDImageDesc) * b->nf + 32;
-    CK(cudaEventRecord(b->ev[9], st));
+    CK(cudaEventRecord(b->ss.ev[9], st));
     b->counters[JPEGB200_C_D2H_BYTES] = bytes;
     return 1;
 }
 
 extern "C" int JPEGB200_batchWait(JPEGB200_BATCH *b, int32_t *status)
 {
-    if (!b || !b->stream) return 0;
+    if (!b || !b->ss.stream) return 0;
     CK(cudaSetDevice(b->ctx->device));
-    CK(cudaStreamSynchronize(b->stream));
+    CK(cudaStreamSynchronize(b->ss.stream));
     CK(cudaGetLastError());
     if (b->nchunks && b->downloaded && !b->chunk_iterate && b->h_counters[2] != 0u) {
         /* a restart-free scan whose chunk entry states had not settled after the fixed passes: decode the job again,
@@ -1967,7 +2060,7 @@ extern "C" int JPEGB200_batchWait(JPEGB200_BATCH *b, int32_t *status)
         const int again = JPEGB200_batchDecode(b, b->decode_flags) && JPEGB200_batchDownload(b);
         b->chunk_iterate = false;
         if (!again) return 0;
-        CK(cudaStreamSynchronize(b->stream));
+        CK(cudaStreamSynchronize(b->ss.stream));
         CK(cudaGetLastError());
     }
     int all_ok = 1;
@@ -1989,7 +2082,7 @@ extern "C" int JPEGB200_batchWait(JPEGB200_BATCH *b, int32_t *status)
         b->counters[JPEGB200_C_RECORD_BYTES] = 2 * (int64_t)(((uint64_t)b->h_counters[5] << 32) | b->h_counters[4]);
     }
     float t;
-    auto el = [&](int a, int c) { t = 0; cudaEventElapsedTime(&t, b->ev[a], b->ev[c]); return t; };
+    auto el = [&](int a, int c) { t = 0; cudaEventElapsedTime(&t, b->ss.ev[a], b->ss.ev[c]); return t; };
     b->ms[JPEGB200_T_H2D] = el(0, 1);
     b->ms[JPEGB200_T_PRESCAN] = el(2, 3);
     b->ms[JPEGB200_T_ENTROPY] = el(3, 4);
@@ -2095,15 +2188,8 @@ extern "C" int JPEGB200_decodeBatchViews(JPEGB200_CTX *ctx, const uint8_t *const
                                          const int64_t *plane_strides, int flags, int32_t *status)
 {
     if (!ctx || n <= 0) return 0;
-    int64_t nv = n;   /* images (views) of the call */
-    if (views) {
-        nv = 0;
-        for (int f = 0; f < n; f++) {
-            if (views[f] < 1) { snprintf(g_err, sizeof(g_err), "views[%d] = %d: every file needs at least one view", f, views[f]); return 0; }
-            nv += views[f];
-        }
-        if (nv > INT32_MAX) { snprintf(g_err, sizeof(g_err), "%lld views: at most %d per call", (long long)nv, INT32_MAX); return 0; }
-    }
+    const int64_t nv = jd_count_views(n, views, "call", g_err, (int)sizeof(g_err));   /* images (views) of the call */
+    if (nv < 0) return 0;
     const bool dev_out = (flags & JPEGB200_OUT_DEVICE) != 0;
     if (spec && !dev_out) {
         snprintf(g_err, sizeof(g_err), "tensor output is written to device memory only: call with JPEGB200_OUT_DEVICE");
@@ -2223,250 +2309,4 @@ extern "C" int JPEGB200_lastCallCounters(JPEGB200_CTX *ctx, int64_t *counters)
     if (!ctx || !counters) return 0;
     memcpy(counters, ctx->last_counters, sizeof(ctx->last_counters));
     return 1;
-}
-
-/* ------------------------------------------------------------------------------------ */
-/* Floyd-Steinberg dither (reference JPEGDither src/jpeg.inl:4871-4940).                    */
-/*                                                                                          */
-/* One warp per band of 32 rows, a wavefront inside the warp and a second one across the warps  */
-/* of an image.  Inside: lane l works on row (band*32 + l) and trails lane l-1 by two pixels:    */
-/* the error row l-1 sends down to a pixel (e2 of its left neighbour + e3 + e4 of its right     */
-/* neighbour, summed in uint8 like the reference's error line) is complete one step before the  */
-/* pixel is due and travels to the next lane with one shuffle per step.  Across: the last       */
-/* lane's outgoing errors go through an error line in global memory to the next band -- the     */
-/* same line the reference keeps in usPixels: it persists across MCU rows, only entries 0..2    */
-/* are cleared per MCU row (:4881), and before the first row it holds the DHT scratch bytes     */
-/* (the host uploads them, see batchDecode).  Band b+1 runs concurrently about 80 steps behind  */
-/* band b.  Every entry of the line is 16 bits: the error and the number (mod 256) of the band  */
-/* that wrote it; band b+1 reads 16 entries at a time and asks again until all of them carry    */
-/* band b's number, so value and "ready" arrive in one store and the bands need no counters or  */
-/* fences between them.  Each entry is read by band b+1 before band b+1 overwrites it (64 steps */
-/* later), so one line per image serves all bands, as in the reference -- provided no entry can  */
-/* carry band b's number mod 256 without band b having written it.  Every band is claimed at     */
-/* once, so in an image of more than 256 bands band b+1 may start while the entries still hold    */
-/* band b-256's tag (or, for band 256, the initial line's "band -1"): a band b >= 256 therefore  */
-/* first waits until band b-255 has finished (one flag per band in `progress`, written once with */
-/* a release store at the band's end).  Every entry's last writer is then one of bands           */
-/* b-255 .. b-1, whose numbers mod 256 are distinct.  An image is a chain of                     */
-/* ~(bands x 80 + width) dependent steps whatever the batch size; with fewer than ~500 images    */
-/* that chain, not throughput, sets the kernel's time (DESIGN.md section 4).                     */
-/* ------------------------------------------------------------------------------------ */
-/* 16 bytes starting at byte offset `mo` (0..15) of the 32-byte pair (a, b) */
-__device__ __forceinline__ uint4 jd_window16(const uint4 a, const uint4 b, uint32_t mo)
-{
-    uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-    const uint32_t ws = mo >> 2, bs = (mo & 3u) * 8u;
-    uint32_t v[5];
-#pragma unroll
-    for (int i = 0; i < 5; i++) {
-        /* v[i] = w[ws + i] without dynamic register indexing */
-        uint32_t x = w[i];
-        if (ws == 1) x = w[i + 1]; else if (ws == 2) x = w[i + 2]; else if (ws == 3) x = (i + 3 < 8) ? w[i + 3] : 0u;
-        v[i] = x;
-    }
-    return make_uint4(__funnelshift_r(v[0], v[1], bs), __funnelshift_r(v[1], v[2], bs), __funnelshift_r(v[2], v[3], bs),
-                      __funnelshift_r(v[3], v[4], bs));
-}
-
-template <int BITS /* output bits per pixel: 1, 2, 4 */>
-__global__ void __launch_bounds__(128, JD_DITHER_MINB)
-jdk_dither(const JDImageDesc *imgs, uint32_t nimg, const uint8_t *gray, const uint64_t *gray_off,
-           uint16_t *errlines, const uint32_t *err_off, uint8_t *out, uint32_t sshift,
-           const uint4 *bands, uint32_t nbands, uint32_t *progress)
-{
-    constexpr uint32_t bits = BITS;
-    /* Bands are handed out through a ticket counter (progress[nbands]; progress[k] is set once band k of the list has
-     * finished, which only bands 256 and later of an image wait for) in the order in which warps START, not by warp index:
-     * the list is band-major (band k of every image before band k + 1), so the band a warp waits on was always claimed by a
-     * warp that is already running -- forward progress does not depend on the order in which the hardware schedules CTAs. */
-    const uint32_t lane = threadIdx.x & 31u;
-    uint32_t wg = 0;
-    if (lane == 0) wg = atomicAdd(progress + nbands, 1u);
-    wg = __shfl_sync(0xffffffffu, wg, 0);
-    if (wg >= nbands) return;
-    const uint4 bd = bands[wg];
-    const uint32_t i = bd.x, bi = bd.y;
-    const JDImageDesc &im = imgs[i];
-    const uint32_t hs = (im.subsample >> 4) ? (im.subsample >> 4) : 1, vs = (im.subsample & 15) ? (im.subsample & 15) : 1;
-    const uint32_t mcu_h = (vs * 8) >> sshift;
-    const int W = (int)((uint32_t)im.mcus_x * ((hs * 8) >> sshift)); /* padded width = pitch of the gray stage (multiple of 8) */
-    const uint32_t rows = im.out_h;
-    const uint8_t *src = gray + gray_off[i];
-    /* S[x] = error flowing from the row above into pixel x+1 (the reference's errors[x + 2]) in the low byte, and in the high
-     * byte the number (mod 256) of the band that wrote it: the band below polls the entries themselves until they carry the
-     * tag of the band above it.  Value and tag travel in one 16-bit store, so no fence and no progress counter is needed (a
-     * release store per 16-32 steps sat on the critical path of an image). */
-    uint16_t *S = errlines + err_off[i];
-    const uint32_t tag_mine = (bi & 0xFFu) << 8, tag_above = ((bi - 1u) & 0xFFu) * 0x01000100u;
-    uint8_t *o = out + gray_off[nimg + i];
-    const size_t opitch = (size_t)gray_off[2 * nimg + i];       /* the caller's pitch, or the tight packed width in the arena */
-    const int mask = (bits == 4) ? 0xF0 : (bits == 2 ? 0xC0 : 0x80);
-    const uint32_t xmask = (bits == 4) ? 1u : (bits == 2 ? 3u : 7u);
-    const bool vec = ((W & 15) == 0);
-    /* Lane l works on pixel x = t - JD_DITHER_SKEW * l at step t.  To keep every global load at a warp-uniform step (a load into a
-     * register that other lanes are still consuming would serialise the whole warp on the scoreboard), each lane reads
-     * its row through a pointer skewed by that many bytes: at step t every lane needs byte t of its skewed row, so all lanes
-     * cross 16-byte boundaries together.  The skewed 16 bytes are cut out of two aligned chunks (jd_window16). */
-    const int skew = JD_DITHER_SKEW * (int)lane;
-    const uint32_t mo = (uint32_t)((16 - (skew & 15)) & 15);   /* byte offset of the window inside the aligned pair */
-    const int jsh = (skew + 15) >> 4;                           /* aligned chunk index of window m = m - jsh */
-    const int nchunks = W >> 4;
-    /* 16 line entries starting at entry 16 * m (two 16-byte loads that bypass L1 and are never hoisted) */
-    auto line_load = [&](int m, uint4 &lo, uint4 &hi) {
-        const uint16_t *q = S + 16 * m;
-        asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(lo.x), "=r"(lo.y), "=r"(lo.z), "=r"(lo.w) : "l"(q) : "memory");
-        asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(hi.x), "=r"(hi.y), "=r"(hi.z), "=r"(hi.w) : "l"(q + 8) : "memory");
-    };
-    auto line_ok = [&](const uint4 &lo, const uint4 &hi) {
-        const uint32_t bad = ((lo.x ^ tag_above) | (lo.y ^ tag_above) | (lo.z ^ tag_above) | (lo.w ^ tag_above) |
-                              (hi.x ^ tag_above) | (hi.y ^ tag_above) | (hi.z ^ tag_above) | (hi.w ^ tag_above)) & 0xFF00FF00u;
-        return bad == 0u;
-    };
-    /* lane 0: make (lo, hi) the entries of window m as the band above left them */
-    auto line_settle = [&](int m, uint4 &lo, uint4 &hi) {
-        uint32_t ns = 128;
-        while (!line_ok(lo, hi)) { __nanosleep(ns); if (ns < 1024u) ns *= 2u; line_load(m, lo, hi); }
-    };
-    {
-        const uint32_t band = bi * 32u;
-        const uint32_t y = band + lane;
-        const bool live = y < rows;
-        const bool mcu_first = (y % mcu_h) == 0;        /* errors[0..2] are cleared at each JPEGDither call */
-        const uint8_t *p = src + (size_t)(live ? y : 0) * W;
-        uint8_t *d = o + (size_t)(live ? y : 0) * opitch;
-        int fwd = 0;                 /* lFErr: e1 of the previous pixel + error arriving from above */
-        int e2_prev = 0;             /* e2(x-1) */
-        int down_m1 = 0;             /* partial outgoing error for pixel x-1: e2(x-2) + e3(x-1) */
-        uint32_t acc = 0;
-        uint32_t from_above = 0;     /* D[x+1] of the row above, delivered by the previous step's shuffle */
-        const uint4 zero4 = make_uint4(0, 0, 0, 0);
-        /* aligned chunks A0 = chunk(m - jsh), A1 = chunk(m - jsh + 1), A2 = prefetch of chunk(m - jsh + 2) */
-        uint4 A0 = zero4, A1 = zero4, win = zero4;
-        uint4 ewin = zero4;                    /* lane 0: the 16 error values of this window (the entries' low bytes) */
-        auto line_values = [](const uint4 &lo, const uint4 &hi) {
-            return make_uint4(__byte_perm(lo.x, lo.y, 0x6420), __byte_perm(lo.z, lo.w, 0x6420), __byte_perm(hi.x, hi.y, 0x6420), __byte_perm(hi.z, hi.w, 0x6420));
-        };
-        auto chunk = [&](int j) -> uint4 {
-            return (live && j >= 0 && j < nchunks) ? *reinterpret_cast<const uint4 *>(p + 16 * j) : zero4;
-        };
-        /* what the next window switch will load is requested one window ahead with prefetches (no registers held across the
-         * 16 unrolled steps): the pixel chunk into L1, the line entries -- written by another SM -- into L2 */
-        auto prefetch_next = [&](int m) {
-            const int j = m - jsh + 1;
-            if (live && j >= 0 && j < nchunks) asm volatile("prefetch.global.L1 [%0];" ::"l"(p + 16 * j));
-            if (lane == 0 && m < nchunks) asm volatile("prefetch.global.L2 [%0];" ::"l"(S + 16 * m));
-        };
-        if (lane == 0 && bd.w != ~0u) {
-            /* band >= 256: wait until band bi - 255 (list position bd.w) has finished before the first read of the line.  It
-             * is ~255 x 80 steps ahead, so this rarely spins. */
-            uint32_t v, ns = 128;
-            for (;;) {
-                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(progress + bd.w) : "memory");
-                if (v) break;
-                __nanosleep(ns); if (ns < 1024u) ns *= 2u;
-            }
-        }
-        if (vec) {
-            A0 = chunk(-jsh); A1 = chunk(1 - jsh);
-            if (lane == 0) {
-                uint4 lo, hi;
-                line_load(0, lo, hi);
-                line_settle(0, lo, hi);
-                ewin = line_values(lo, hi);
-            }
-            win = jd_window16(A0, A1, mo);
-            prefetch_next(1);
-        }
-        const bool parks = live && (lane == 31 || y + 1 == rows);
-        const int nsteps = W + JD_DITHER_SKEW * 31 + 2;
-        uint32_t line_prev = 0;     /* lane 0, skew 2: the line entry of the previous step (= error into the current pixel) */
-        for (int tb = 0; tb < nsteps; tb += 16) {
-#pragma unroll
-        for (int k = 0; k < 16; k++) {                    /* unrolled: byte k of the 16-byte windows is a constant extract */
-            const int t = tb + k;
-            const int x = t - skew;
-            const bool inrow = live && x >= 0 && x < W;
-            uint32_t pix, inc = from_above;
-            if (vec) {
-                /* warp-uniform: byte t of every lane's skewed row, and (lane 0) entry t of the error line */
-                const uint32_t ww = (k < 4) ? win.x : (k < 8) ? win.y : (k < 12) ? win.z : win.w;
-                const uint32_t ee = (k < 4) ? ewin.x : (k < 8) ? ewin.y : (k < 12) ? ewin.z : ewin.w;
-                pix = (ww >> (8 * (k & 3))) & 0xFFu;
-                if (lane == 0) {
-                    const uint32_t line_now = (ee >> (8 * (k & 3))) & 0xFFu;   /* S[t] = error into pixel t + 1 */
-                    inc = (JD_DITHER_SKEW == 3) ? line_now : line_prev;
-                    line_prev = line_now;
-                }
-            } else {
-                pix = inrow ? p[x] : 0u;
-                if (lane == 0 && inrow && (JD_DITHER_SKEW == 3 || x >= 1)) {
-                    /* unusual widths: entry by entry */
-                    uint32_t v, ns = 128;
-                    for (;;) {
-                        asm volatile("ld.volatile.global.u16 %0, [%1];" : "=r"(v) : "l"(S + (JD_DITHER_SKEW == 3 ? x : x - 1)) : "memory");
-                        if (((v ^ tag_above) & 0xFF00u) == 0u) break;
-                        __nanosleep(ns); if (ns < 1024u) ns *= 2u;
-                    }
-                    inc = v & 0xFFu;
-                }
-            }
-            uint32_t dcomplete = 0;   /* outgoing error for pixel x-1, complete after this step */
-            if (inrow) {
-                int c = (int)pix + fwd;
-                if (JD_DITHER_SKEW == 2) {
-                    /* error arriving at THIS pixel from the row above: none at pixel 0, and pixel 1's slot (errors[2]) is cleared at
-                     * the first row of every MCU row */
-                    uint32_t upc = inc & 0xFFu;
-                    if (x == 0 || (mcu_first && x == 1)) upc = 0;
-                    c += (int)upc;
-                }
-                if (c > 255) c = 255;
-                acc = ((acc << bits) | ((uint32_t)c >> (8 - bits))) & 0xFFu;
-                if (((uint32_t)x & xmask) == xmask) { *d++ = (uint8_t)acc; acc = 0; }
-                const int v = c - (c & mask);
-                const int h = v >> 1;
-                const int e1 = (7 * h) >> 3, e2 = h - e1, e3 = (5 * h) >> 3, e4 = h - e3;
-                /* error arriving at pixel x+1 from the row above; pixel 1's slot (errors[2]) is cleared at the first row of
-                 * every MCU row, and nothing ever reaches pixel 0 from above (lFErr starts at 0) */
-                uint32_t up = inc & 0xFFu;
-                if (mcu_first && x == 0) up = 0;
-                fwd = (JD_DITHER_SKEW == 3) ? e1 + (int)up : e1;
-                dcomplete = (uint32_t)(down_m1 + e4) & 0xFFu;   /* D[x-1] = e2(x-2) + e3(x-1) + e4(x) */
-                down_m1 = e2_prev + e3;                          /* becomes D[x] once e4(x+1) arrives */
-                e2_prev = e2;
-            } else if (live && x == W) {
-                dcomplete = (uint32_t)down_m1 & 0xFFu;           /* D[W-1] = e2(W-2) + e3(W-1) (no right neighbour) */
-            }
-            /* the last row of the band parks what it sends down: D[x-1] feeds pixel x-1 of the next band's first row = S[x-2].
-             * One entry more than anybody consumes (x = W + 1 -> S[W-1], value 0): the band below waits for the tags of whole
-             * windows. */
-            if (parks && x >= 2 && x <= W + 1) {
-                const uint16_t ev = (uint16_t)(dcomplete | tag_mine);
-                asm volatile("st.relaxed.gpu.global.u16 [%0], %1;" ::"l"(S + (x - 2)), "h"(ev) : "memory");
-            }
-            /* next step lane l+1 handles pixel x-2 and needs D[x-1] of this row */
-            from_above = __shfl_up_sync(0xffffffffu, dcomplete, 1);
-        }
-            /* ---- every 16 steps: next windows ---- */
-            if (vec) {
-                const int m = (tb >> 4) + 1;               /* next window index */
-                A0 = A1; A1 = chunk(m - jsh + 1);
-                win = jd_window16(A0, A1, mo);
-                if (lane == 0 && m < nchunks) {
-                    /* usually the band above wrote these entries long before (it runs >= 95 + 16 steps ahead), else ask again until
-                     * they carry its tag */
-                    /* read now, not a window ahead: a band that follows the one above in lock step would mostly have read
-                     * entries that were not written yet (measured slower) */
-                    uint4 lo, hi;
-                    line_load(m, lo, hi);
-                    line_settle(m, lo, hi);
-                    ewin = line_values(lo, hi);
-                }
-                prefetch_next(m + 1);
-            }
-        }
-        /* this band is finished: the lane that parked the line (lane 31 in every band but an image's last) publishes it, after
-         * its own stores to the line */
-        if (parks) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(progress + wg), "r"(1u) : "memory");
-    }
 }

@@ -679,6 +679,79 @@ int jd_check_output(int index, int pixel_type, int64_t row_bytes, const void *ou
     return 1;
 }
 
+int64_t jd_count_views(int nfiles, const int32_t *views, const char *per, char *msg, int msg_len)
+{
+    if (!views) return nfiles;
+    int64_t nv = 0;
+    for (int f = 0; f < nfiles; f++) {
+        if (views[f] < 1) {
+            snprintf(msg, (size_t)msg_len, "views[%d] = %d: every file needs at least one view", f, views[f]);
+            return -1;
+        }
+        nv += views[f];
+    }
+    if (nv > INT32_MAX) {
+        snprintf(msg, (size_t)msg_len, "%lld views: at most %d per %s", (long long)nv, INT32_MAX, per);
+        return -1;
+    }
+    return nv;
+}
+
+/* What a batch feature can refuse, and the rules in the order in which they are reported.  Views, rectangles and
+ * orientations: the dither of a view (rectangle, rotation) is not the view of the dither -- error diffusion runs across the
+ * whole image.  Tensors and resizing work on byte planes: RGB8888 (either byte order) and 8-bit gray.  Padded output is the
+ * single-image API's. */
+enum { JD_F_VIEWS, JD_F_TENSOR, JD_F_RESIZE, JD_F_ROI, JD_F_ORIENT, JD_F_COUNT };
+enum { JD_R_RGB565, JD_R_DITHER, JD_R_PADDED, JD_R_SPEC /* jd_tensor_check */, JD_R_FILTER /* jd_rs_filter_ok */ };
+static const char *const jd_feature_name[JD_F_COUNT] = {"views are", "tensor output is", "resizing is", "regions of interest are",
+                                                        "orientations are"};
+static const char *const jd_refused_name[3] = {"RGB565 pixel types (a packed 5/6/5 word has no byte planes)", "dithered pixel types",
+                                               "padded output"};
+static const struct { uint8_t feature, refuses; } jd_feature_rules[] = {
+    {JD_F_VIEWS, JD_R_DITHER},   {JD_F_VIEWS, JD_R_PADDED},
+    {JD_F_TENSOR, JD_R_RGB565},  {JD_F_TENSOR, JD_R_DITHER},  {JD_F_TENSOR, JD_R_PADDED}, {JD_F_TENSOR, JD_R_SPEC},
+    {JD_F_RESIZE, JD_R_RGB565},  {JD_F_RESIZE, JD_R_DITHER},  {JD_F_RESIZE, JD_R_PADDED}, {JD_F_RESIZE, JD_R_FILTER},
+    {JD_F_ROI, JD_R_DITHER},     {JD_F_ORIENT, JD_R_DITHER},  {JD_F_ROI, JD_R_PADDED},    {JD_F_ORIENT, JD_R_PADDED},
+};
+
+int jd_check_batch_features(int pixel_type, int options, int nfiles, const int32_t *views, int has_rois, int has_orients,
+                            int has_out_sizes, int filter, const JPEGB200_TensorSpec *spec, int64_t *nviews, char *msg,
+                            int msg_len)
+{
+    if (nfiles <= 0 || pixel_type < 0 || pixel_type >= INVALID_PIXEL_TYPE) { snprintf(msg, (size_t)msg_len, "invalid parameter"); return 0; }
+    if (options & JPEGB200_OPT_LIBJPEG) {
+        /* libjpeg's default decompression has no RGB565, dithered, scaled, thumbnail or luma-only counterpart */
+        const char *why = NULL;
+        if (pixel_type != RGB8888 && pixel_type != EIGHT_BIT_GRAYSCALE) why = "pixel types other than RGB8888 and EIGHT_BIT_GRAYSCALE";
+        else if (options & (JPEG_SCALE_HALF | JPEG_SCALE_QUARTER | JPEG_SCALE_EIGHTH)) why = "JPEG_SCALE_* (libjpeg's scaled IDCTs are other algorithms)";
+        else if (options & JPEG_EXIF_THUMBNAIL) why = "JPEG_EXIF_THUMBNAIL";
+        else if (options & JPEG_LUMA_ONLY) why = "JPEG_LUMA_ONLY";
+        else if (options & JPEGB200_OPT_PADDED) why = "padded output";
+        if (why) { snprintf(msg, (size_t)msg_len, "JPEGB200_OPT_LIBJPEG is not supported with %s", why); return 0; }
+    }
+    const int64_t nv = jd_count_views(nfiles, views, "batch", msg, msg_len);
+    if (nv < 0) return 0;
+    const int has[JD_F_COUNT] = {views != NULL, spec != NULL, has_out_sizes, has_rois, has_orients};
+    const int pt = jd_fold_luma_only(pixel_type, options);
+    for (size_t k = 0; k < sizeof(jd_feature_rules) / sizeof(jd_feature_rules[0]); k++) {
+        const int r = jd_feature_rules[k].refuses;
+        if (!has[jd_feature_rules[k].feature]) continue;
+        if (r == JD_R_SPEC) { if (!jd_tensor_check(spec, pt == RGB8888 ? 3 : 1, msg, msg_len)) return 0; continue; }
+        if (r == JD_R_FILTER) {
+            if (jd_rs_filter_ok(filter)) continue;
+            snprintf(msg, (size_t)msg_len, "resize filter %d is not supported (JPEGB200_RESIZE_BILINEAR 2, BICUBIC 3 or BOX 4)", filter);
+            return 0;
+        }
+        if (r == JD_R_RGB565 ? (pt == RGB565_LITTLE_ENDIAN || pt == RGB565_BIG_ENDIAN)
+                             : r == JD_R_DITHER ? (pt >= FOUR_BIT_DITHERED && pt <= ONE_BIT_DITHERED) : (options & JPEGB200_OPT_PADDED) != 0) {
+            snprintf(msg, (size_t)msg_len, "%s not supported with %s", jd_feature_name[jd_feature_rules[k].feature], jd_refused_name[r]);
+            return 0;
+        }
+    }
+    *nviews = nv;
+    return 1;
+}
+
 /* ---- tensor output (JPEGB200_batchCreateTensor) ---- */
 int jd_rgb8888_is_bgr(int arith, int sshift, int ncomp, int subsample)
 {

@@ -222,6 +222,25 @@ typedef struct {
 int jd_check_output(int index, int pixel_type, int64_t row_bytes, const void *out, int64_t pitch, int device,
                     char *msg, int msg_len);
 
+#define JPEGB200_OPT_PADDED 0x10000 /* internal option bit (the single-image API, jd_api.c): write the whole MCU-aligned frame */
+
+/* JPEG_LUMA_ONLY turns the colour pixel types into 8-bit gray (jpeg.inl:4991) */
+static inline int jd_fold_luma_only(int pixel_type, int options)
+{
+    return ((options & JPEG_LUMA_ONLY) && pixel_type < EIGHT_BIT_GRAYSCALE) ? EIGHT_BIT_GRAYSCALE : pixel_type;
+}
+/* The images of a batch or call of nfiles files: the sum of views[f] (each at least 1, at most INT32_MAX in all; `per` names
+ * "batch" or "call" in that message), nfiles without views.  -1 with a message. */
+int64_t jd_count_views(int nfiles, const int32_t *views, const char *per, char *msg, int msg_len);
+/* Which combinations of pixel type, options and features (views, a tensor spec, out_sizes with `filter`, rois, orients) a
+ * batch accepts: JPEGB200_batchCreateViews' argument rules.  Returns 1 and the batch's image count in *nviews, or 0 with the
+ * message of the first rule broken: an invalid parameter, JPEGB200_OPT_LIBJPEG's own rules, the view counts, then
+ * per feature what it is not supported with (views, tensor and its spec, resize and its filter, rois / orients with
+ * dithered types, rois / orients with padded output). */
+int jd_check_batch_features(int pixel_type, int options, int nfiles, const int32_t *views, int has_rois, int has_orients,
+                            int has_out_sizes, int filter, const JPEGB200_TensorSpec *spec, int64_t *nviews, char *msg,
+                            int msg_len);
+
 /* Tensor output (JPEGB200_batchCreateTensor).  The byte order of an RGB8888 output: 1 = B,G,R,A, 0 = R,G,B,A.  The
  * SSE2-build arithmetic stores B,G,R,A at full scale for 3-component 4:2:0 and 4:4:4 files (its SIMD colour paths);
  * every other case takes the scalar colour code, which stores R,G,B,A.  Depends on the image, so it is asked per image. */

@@ -2363,3 +2363,290 @@ __global__ void __launch_bounds__(JD_LJ_THREADS) jdk_lj_color(const JDImageDesc 
     if (PT == JD_PT_GRAY) row[dx] = (uint8_t)v;
     else reinterpret_cast<uint32_t *>(row)[dx] = v;
 }
+
+/* digest of device byte ranges (JPEGB200_digestDevice, jd_device.cu) */
+__device__ __forceinline__ unsigned long long jd_mix64(unsigned long long z)
+{
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+__global__ void __launch_bounds__(256) jdk_digest(const uint8_t *const *ptrs, const int64_t *lens, unsigned long long *out)
+{
+    const uint32_t img = blockIdx.y;
+    const unsigned long long *w = reinterpret_cast<const unsigned long long *>(ptrs[img]);
+    const int64_t nbytes = lens[img], nfull = nbytes >> 3;
+    unsigned long long acc = 0;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nfull; i += (int64_t)gridDim.x * blockDim.x)
+        acc += jd_mix64(w[i] ^ ((unsigned long long)i * 0x9E3779B97F4A7C15ull));
+    if (blockIdx.x == 0 && threadIdx.x == 0 && (nbytes & 7)) {   /* tail bytes, zero padded */
+        unsigned long long t = 0;
+        const uint8_t *q = ptrs[img] + (nfull << 3);
+        for (int k = 0; k < (int)(nbytes & 7); k++) t |= (unsigned long long)q[k] << (8 * k);
+        acc += jd_mix64(t ^ ((unsigned long long)nfull * 0x9E3779B97F4A7C15ull));
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, d);
+    __shared__ unsigned long long s_part[8];
+    if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned long long t = 0;
+        for (int k = 0; k < 8; k++) t += s_part[k];
+        atomicAdd(out + img, t);
+    }
+}
+
+#ifndef JD_DITHER_MINB
+#define JD_DITHER_MINB 9
+#endif
+#ifndef JD_DITHER_SKEW
+#define JD_DITHER_SKEW 2   /* pixels by which a row trails the row above: 3 = the error from above is folded into the NEXT pixel's
+                             forward error (one step of slack for the shuffle); 2 = it is added to the current pixel */
+#endif
+/* ------------------------------------------------------------------------------------ */
+/* Floyd-Steinberg dither (reference JPEGDither src/jpeg.inl:4871-4940).                    */
+/*                                                                                          */
+/* One warp per band of 32 rows, a wavefront inside the warp and a second one across the warps  */
+/* of an image.  Inside: lane l works on row (band*32 + l) and trails lane l-1 by two pixels:    */
+/* the error row l-1 sends down to a pixel (e2 of its left neighbour + e3 + e4 of its right     */
+/* neighbour, summed in uint8 like the reference's error line) is complete one step before the  */
+/* pixel is due and travels to the next lane with one shuffle per step.  Across: the last       */
+/* lane's outgoing errors go through an error line in global memory to the next band -- the     */
+/* same line the reference keeps in usPixels: it persists across MCU rows, only entries 0..2    */
+/* are cleared per MCU row (:4881), and before the first row it holds the DHT scratch bytes     */
+/* (the host uploads them, see stage_dither). Band b+1 runs concurrently about 80 steps behind  */
+/* band b.  Every entry of the line is 16 bits: the error and the number (mod 256) of the band  */
+/* that wrote it; band b+1 reads 16 entries at a time and asks again until all of them carry    */
+/* band b's number, so value and "ready" arrive in one store and the bands need no counters or  */
+/* fences between them.  Each entry is read by band b+1 before band b+1 overwrites it (64 steps */
+/* later), so one line per image serves all bands, as in the reference -- provided no entry can  */
+/* carry band b's number mod 256 without band b having written it.  Every band is claimed at     */
+/* once, so in an image of more than 256 bands band b+1 may start while the entries still hold    */
+/* band b-256's tag (or, for band 256, the initial line's "band -1"): a band b >= 256 therefore  */
+/* first waits until band b-255 has finished (one flag per band in `progress`, written once with */
+/* a release store at the band's end).  Every entry's last writer is then one of bands           */
+/* b-255 .. b-1, whose numbers mod 256 are distinct.  An image is a chain of                     */
+/* ~(bands x 80 + width) dependent steps whatever the batch size; with fewer than ~500 images    */
+/* that chain, not throughput, sets the kernel's time (DESIGN.md section 4).                     */
+/* ------------------------------------------------------------------------------------ */
+/* 16 bytes starting at byte offset `mo` (0..15) of the 32-byte pair (a, b) */
+__device__ __forceinline__ uint4 jd_window16(const uint4 a, const uint4 b, uint32_t mo)
+{
+    uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    const uint32_t ws = mo >> 2, bs = (mo & 3u) * 8u;
+    uint32_t v[5];
+#pragma unroll
+    for (int i = 0; i < 5; i++) {
+        /* v[i] = w[ws + i] without dynamic register indexing */
+        uint32_t x = w[i];
+        if (ws == 1) x = w[i + 1]; else if (ws == 2) x = w[i + 2]; else if (ws == 3) x = (i + 3 < 8) ? w[i + 3] : 0u;
+        v[i] = x;
+    }
+    return make_uint4(__funnelshift_r(v[0], v[1], bs), __funnelshift_r(v[1], v[2], bs), __funnelshift_r(v[2], v[3], bs),
+                      __funnelshift_r(v[3], v[4], bs));
+}
+
+template <int BITS /* output bits per pixel: 1, 2, 4 */>
+__global__ void __launch_bounds__(128, JD_DITHER_MINB)
+jdk_dither(const JDImageDesc *imgs, uint32_t nimg, const uint8_t *gray, const uint64_t *gray_off,
+           uint16_t *errlines, const uint32_t *err_off, uint8_t *out, uint32_t sshift,
+           const uint4 *bands, uint32_t nbands, uint32_t *progress)
+{
+    constexpr uint32_t bits = BITS;
+    /* Bands are handed out through a ticket counter (progress[nbands]; progress[k] is set once band k of the list has
+     * finished, which only bands 256 and later of an image wait for) in the order in which warps START, not by warp index:
+     * the list is band-major (band k of every image before band k + 1), so the band a warp waits on was always claimed by a
+     * warp that is already running -- forward progress does not depend on the order in which the hardware schedules CTAs. */
+    const uint32_t lane = threadIdx.x & 31u;
+    uint32_t wg = 0;
+    if (lane == 0) wg = atomicAdd(progress + nbands, 1u);
+    wg = __shfl_sync(0xffffffffu, wg, 0);
+    if (wg >= nbands) return;
+    const uint4 bd = bands[wg];
+    const uint32_t i = bd.x, bi = bd.y;
+    const JDImageDesc &im = imgs[i];
+    const uint32_t hs = (im.subsample >> 4) ? (im.subsample >> 4) : 1, vs = (im.subsample & 15) ? (im.subsample & 15) : 1;
+    const uint32_t mcu_h = (vs * 8) >> sshift;
+    const int W = (int)((uint32_t)im.mcus_x * ((hs * 8) >> sshift)); /* padded width = pitch of the gray stage (multiple of 8) */
+    const uint32_t rows = im.out_h;
+    const uint8_t *src = gray + gray_off[i];
+    /* S[x] = error flowing from the row above into pixel x+1 (the reference's errors[x + 2]) in the low byte, and in the high
+     * byte the number (mod 256) of the band that wrote it: the band below polls the entries themselves until they carry the
+     * tag of the band above it.  Value and tag travel in one 16-bit store, so no fence and no progress counter is needed (a
+     * release store per 16-32 steps sat on the critical path of an image). */
+    uint16_t *S = errlines + err_off[i];
+    const uint32_t tag_mine = (bi & 0xFFu) << 8, tag_above = ((bi - 1u) & 0xFFu) * 0x01000100u;
+    uint8_t *o = out + gray_off[nimg + i];
+    const size_t opitch = (size_t)gray_off[2 * nimg + i];       /* the caller's pitch, or the tight packed width in the arena */
+    const int mask = (bits == 4) ? 0xF0 : (bits == 2 ? 0xC0 : 0x80);
+    const uint32_t xmask = (bits == 4) ? 1u : (bits == 2 ? 3u : 7u);
+    const bool vec = ((W & 15) == 0);
+    /* Lane l works on pixel x = t - JD_DITHER_SKEW * l at step t.  To keep every global load at a warp-uniform step (a load into a
+     * register that other lanes are still consuming would serialise the whole warp on the scoreboard), each lane reads
+     * its row through a pointer skewed by that many bytes: at step t every lane needs byte t of its skewed row, so all lanes
+     * cross 16-byte boundaries together.  The skewed 16 bytes are cut out of two aligned chunks (jd_window16). */
+    const int skew = JD_DITHER_SKEW * (int)lane;
+    const uint32_t mo = (uint32_t)((16 - (skew & 15)) & 15);   /* byte offset of the window inside the aligned pair */
+    const int jsh = (skew + 15) >> 4;                           /* aligned chunk index of window m = m - jsh */
+    const int nchunks = W >> 4;
+    /* 16 line entries starting at entry 16 * m (two 16-byte loads that bypass L1 and are never hoisted) */
+    auto line_load = [&](int m, uint4 &lo, uint4 &hi) {
+        const uint16_t *q = S + 16 * m;
+        asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(lo.x), "=r"(lo.y), "=r"(lo.z), "=r"(lo.w) : "l"(q) : "memory");
+        asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(hi.x), "=r"(hi.y), "=r"(hi.z), "=r"(hi.w) : "l"(q + 8) : "memory");
+    };
+    auto line_ok = [&](const uint4 &lo, const uint4 &hi) {
+        const uint32_t bad = ((lo.x ^ tag_above) | (lo.y ^ tag_above) | (lo.z ^ tag_above) | (lo.w ^ tag_above) |
+                              (hi.x ^ tag_above) | (hi.y ^ tag_above) | (hi.z ^ tag_above) | (hi.w ^ tag_above)) & 0xFF00FF00u;
+        return bad == 0u;
+    };
+    /* lane 0: make (lo, hi) the entries of window m as the band above left them */
+    auto line_settle = [&](int m, uint4 &lo, uint4 &hi) {
+        uint32_t ns = 128;
+        while (!line_ok(lo, hi)) { __nanosleep(ns); if (ns < 1024u) ns *= 2u; line_load(m, lo, hi); }
+    };
+    {
+        const uint32_t band = bi * 32u;
+        const uint32_t y = band + lane;
+        const bool live = y < rows;
+        const bool mcu_first = (y % mcu_h) == 0;        /* errors[0..2] are cleared at each JPEGDither call */
+        const uint8_t *p = src + (size_t)(live ? y : 0) * W;
+        uint8_t *d = o + (size_t)(live ? y : 0) * opitch;
+        int fwd = 0;                 /* lFErr: e1 of the previous pixel + error arriving from above */
+        int e2_prev = 0;             /* e2(x-1) */
+        int down_m1 = 0;             /* partial outgoing error for pixel x-1: e2(x-2) + e3(x-1) */
+        uint32_t acc = 0;
+        uint32_t from_above = 0;     /* D[x+1] of the row above, delivered by the previous step's shuffle */
+        const uint4 zero4 = make_uint4(0, 0, 0, 0);
+        /* aligned chunks A0 = chunk(m - jsh), A1 = chunk(m - jsh + 1), A2 = prefetch of chunk(m - jsh + 2) */
+        uint4 A0 = zero4, A1 = zero4, win = zero4;
+        uint4 ewin = zero4;                    /* lane 0: the 16 error values of this window (the entries' low bytes) */
+        auto line_values = [](const uint4 &lo, const uint4 &hi) {
+            return make_uint4(__byte_perm(lo.x, lo.y, 0x6420), __byte_perm(lo.z, lo.w, 0x6420), __byte_perm(hi.x, hi.y, 0x6420), __byte_perm(hi.z, hi.w, 0x6420));
+        };
+        auto chunk = [&](int j) -> uint4 {
+            return (live && j >= 0 && j < nchunks) ? *reinterpret_cast<const uint4 *>(p + 16 * j) : zero4;
+        };
+        /* what the next window switch will load is requested one window ahead with prefetches (no registers held across the
+         * 16 unrolled steps): the pixel chunk into L1, the line entries -- written by another SM -- into L2 */
+        auto prefetch_next = [&](int m) {
+            const int j = m - jsh + 1;
+            if (live && j >= 0 && j < nchunks) asm volatile("prefetch.global.L1 [%0];" ::"l"(p + 16 * j));
+            if (lane == 0 && m < nchunks) asm volatile("prefetch.global.L2 [%0];" ::"l"(S + 16 * m));
+        };
+        if (lane == 0 && bd.w != ~0u) {
+            /* band >= 256: wait until band bi - 255 (list position bd.w) has finished before the first read of the line.  It
+             * is ~255 x 80 steps ahead, so this rarely spins. */
+            uint32_t v, ns = 128;
+            for (;;) {
+                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(progress + bd.w) : "memory");
+                if (v) break;
+                __nanosleep(ns); if (ns < 1024u) ns *= 2u;
+            }
+        }
+        if (vec) {
+            A0 = chunk(-jsh); A1 = chunk(1 - jsh);
+            if (lane == 0) {
+                uint4 lo, hi;
+                line_load(0, lo, hi);
+                line_settle(0, lo, hi);
+                ewin = line_values(lo, hi);
+            }
+            win = jd_window16(A0, A1, mo);
+            prefetch_next(1);
+        }
+        const bool parks = live && (lane == 31 || y + 1 == rows);
+        const int nsteps = W + JD_DITHER_SKEW * 31 + 2;
+        uint32_t line_prev = 0;     /* lane 0, skew 2: the line entry of the previous step (= error into the current pixel) */
+        for (int tb = 0; tb < nsteps; tb += 16) {
+#pragma unroll
+        for (int k = 0; k < 16; k++) {                    /* unrolled: byte k of the 16-byte windows is a constant extract */
+            const int t = tb + k;
+            const int x = t - skew;
+            const bool inrow = live && x >= 0 && x < W;
+            uint32_t pix, inc = from_above;
+            if (vec) {
+                /* warp-uniform: byte t of every lane's skewed row, and (lane 0) entry t of the error line */
+                const uint32_t ww = (k < 4) ? win.x : (k < 8) ? win.y : (k < 12) ? win.z : win.w;
+                const uint32_t ee = (k < 4) ? ewin.x : (k < 8) ? ewin.y : (k < 12) ? ewin.z : ewin.w;
+                pix = (ww >> (8 * (k & 3))) & 0xFFu;
+                if (lane == 0) {
+                    const uint32_t line_now = (ee >> (8 * (k & 3))) & 0xFFu;   /* S[t] = error into pixel t + 1 */
+                    inc = (JD_DITHER_SKEW == 3) ? line_now : line_prev;
+                    line_prev = line_now;
+                }
+            } else {
+                pix = inrow ? p[x] : 0u;
+                if (lane == 0 && inrow && (JD_DITHER_SKEW == 3 || x >= 1)) {
+                    /* unusual widths: entry by entry */
+                    uint32_t v, ns = 128;
+                    for (;;) {
+                        asm volatile("ld.volatile.global.u16 %0, [%1];" : "=r"(v) : "l"(S + (JD_DITHER_SKEW == 3 ? x : x - 1)) : "memory");
+                        if (((v ^ tag_above) & 0xFF00u) == 0u) break;
+                        __nanosleep(ns); if (ns < 1024u) ns *= 2u;
+                    }
+                    inc = v & 0xFFu;
+                }
+            }
+            uint32_t dcomplete = 0;   /* outgoing error for pixel x-1, complete after this step */
+            if (inrow) {
+                int c = (int)pix + fwd;
+                if (JD_DITHER_SKEW == 2) {
+                    /* error arriving at THIS pixel from the row above: none at pixel 0, and pixel 1's slot (errors[2]) is cleared at
+                     * the first row of every MCU row */
+                    uint32_t upc = inc & 0xFFu;
+                    if (x == 0 || (mcu_first && x == 1)) upc = 0;
+                    c += (int)upc;
+                }
+                if (c > 255) c = 255;
+                acc = ((acc << bits) | ((uint32_t)c >> (8 - bits))) & 0xFFu;
+                if (((uint32_t)x & xmask) == xmask) { *d++ = (uint8_t)acc; acc = 0; }
+                const int v = c - (c & mask);
+                const int h = v >> 1;
+                const int e1 = (7 * h) >> 3, e2 = h - e1, e3 = (5 * h) >> 3, e4 = h - e3;
+                /* error arriving at pixel x+1 from the row above; pixel 1's slot (errors[2]) is cleared at the first row of
+                 * every MCU row, and nothing ever reaches pixel 0 from above (lFErr starts at 0) */
+                uint32_t up = inc & 0xFFu;
+                if (mcu_first && x == 0) up = 0;
+                fwd = (JD_DITHER_SKEW == 3) ? e1 + (int)up : e1;
+                dcomplete = (uint32_t)(down_m1 + e4) & 0xFFu;   /* D[x-1] = e2(x-2) + e3(x-1) + e4(x) */
+                down_m1 = e2_prev + e3;                          /* becomes D[x] once e4(x+1) arrives */
+                e2_prev = e2;
+            } else if (live && x == W) {
+                dcomplete = (uint32_t)down_m1 & 0xFFu;           /* D[W-1] = e2(W-2) + e3(W-1) (no right neighbour) */
+            }
+            /* the last row of the band parks what it sends down: D[x-1] feeds pixel x-1 of the next band's first row = S[x-2].
+             * One entry more than anybody consumes (x = W + 1 -> S[W-1], value 0): the band below waits for the tags of whole
+             * windows. */
+            if (parks && x >= 2 && x <= W + 1) {
+                const uint16_t ev = (uint16_t)(dcomplete | tag_mine);
+                asm volatile("st.relaxed.gpu.global.u16 [%0], %1;" ::"l"(S + (x - 2)), "h"(ev) : "memory");
+            }
+            /* next step lane l+1 handles pixel x-2 and needs D[x-1] of this row */
+            from_above = __shfl_up_sync(0xffffffffu, dcomplete, 1);
+        }
+            /* ---- every 16 steps: next windows ---- */
+            if (vec) {
+                const int m = (tb >> 4) + 1;               /* next window index */
+                A0 = A1; A1 = chunk(m - jsh + 1);
+                win = jd_window16(A0, A1, mo);
+                if (lane == 0 && m < nchunks) {
+                    /* usually the band above wrote these entries long before (it runs >= 95 + 16 steps ahead), else ask again until
+                     * they carry its tag */
+                    /* read now, not a window ahead: a band that follows the one above in lock step would mostly have read
+                     * entries that were not written yet (measured slower) */
+                    uint4 lo, hi;
+                    line_load(m, lo, hi);
+                    line_settle(m, lo, hi);
+                    ewin = line_values(lo, hi);
+                }
+                prefetch_next(m + 1);
+            }
+        }
+        /* this band is finished: the lane that parked the line (lane 31 in every band but an image's last) publishes it, after
+         * its own stores to the line */
+        if (parks) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(progress + wg), "r"(1u) : "memory");
+    }
+}
