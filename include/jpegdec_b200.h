@@ -295,6 +295,26 @@ JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const uint8_t *cons
                                           const int32_t *views, int pixel_type, int options, const int32_t *rois,
                                           const uint8_t *orients, const int32_t *out_sizes, int filter,
                                           const JPEGB200_TensorSpec *spec);
+/* Reduced-size decodes per view, bit-exact with Pillow's Image.draft() (libjpeg-turbo's scale_num / scale_denom = 1 / s):
+ * the arguments of JPEGB200_batchCreateViews plus draft, one denominator s per VIEW (1, 2, 4 or 8).  draft = NULL is
+ * JPEGB200_batchCreateViews, which forwards here.
+ *   - View v with s = draft[v]: its unrotated, uncropped image is libjpeg-turbo's decode at 1 / s, ceil(W / s) x
+ *     ceil(H / s) pixels, made with libjpeg's reduced IDCTs (jidctred.c 4x4 / 2x2 / 1x1, and islow where a chroma component
+ *     keeps 8x8) and its upsampling at that scale (fancy, none, or replication at 1/8).  rois are in that frame after
+ *     orientation; orientation, resize and tensor output then apply unchanged, and batchImageInfo / batchOutputBytes
+ *     report the scaled sizes.  s = 1 is byte for byte the JPEGB200_OPT_LIBJPEG output.  Views of one file may use
+ *     different scales; the file is still walked once, at full scale.
+ *   - Status, batchErrMcu and the walked intervals follow the rules of JPEGB200_batchCreateViews, with each view's MCU box
+ *     computed in its scaled frame.
+ *   - Needs JPEGB200_OPT_LIBJPEG: a non-NULL draft without it returns NULL with a message.  A value other than 1, 2, 4 or
+ *     8 gives that view alone JPEG_INVALID_PARAMETER.  JPEG_SCALE_* stays refused with JPEGB200_OPT_LIBJPEG. */
+JPEGB200_BATCH *JPEGB200_batchCreateDraft(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                          const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                          const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                          const JPEGB200_TensorSpec *spec, const uint8_t *draft);
+/* Pillow's choice of s for draft(mode, (req_w, req_h)) on a W x H file: k = min(W / req_w, H / req_h) (integer division),
+ * then the largest of 8, 4, 2, 1 that is at most k, else 1.  A request of 0 (where Pillow would divide by zero) gives 1. */
+int JPEGB200_draftScale(int width, int height, int req_w, int req_h);
 void JPEGB200_batchDestroy(JPEGB200_BATCH *b);
 int JPEGB200_batchCount(JPEGB200_BATCH *b);
 /* per-image facts after batchCreate: status is JPEG_SUCCESS or the open() error the reference would give */
@@ -379,6 +399,13 @@ int JPEGB200_decodeBatchViews(JPEGB200_CTX *ctx, const uint8_t *const *datas, co
                               const int32_t *views, int pixel_type, int options, const int32_t *rois,
                               const uint8_t *orients, const int32_t *out_sizes, int filter,
                               const JPEGB200_TensorSpec *spec, void *const *outs, const int64_t *pitches,
+                              const int64_t *plane_strides, int flags, int32_t *status);
+/* The same with a draft scale per view (semantics of JPEGB200_batchCreateDraft; NULL = JPEGB200_decodeBatchViews, which
+ * forwards here).  The 1 GiB of scratch per job counts each view's sample planes at its own scale. */
+int JPEGB200_decodeBatchDraft(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                              const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                              const uint8_t *orients, const int32_t *out_sizes, int filter,
+                              const JPEGB200_TensorSpec *spec, const uint8_t *draft, void *const *outs, const int64_t *pitches,
                               const int64_t *plane_strides, int flags, int32_t *status);
 /* JPEGB200_NUM_COUNTERS counters summed over the jobs of the last JPEGB200_decodeBatch on this context */
 int JPEGB200_lastCallCounters(JPEGB200_CTX *ctx, int64_t *counters);

@@ -123,6 +123,13 @@ def lib():
     L.JPEGB200_decodeBatchViews.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, i32p, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
                                             i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(vp), C.POINTER(C.c_int64),
                                             C.POINTER(C.c_int64), C.c_int, i32p]
+    L.JPEGB200_batchCreateDraft.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, i32p, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
+                                            i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(C.c_uint8)]
+    L.JPEGB200_batchCreateDraft.restype = vp
+    L.JPEGB200_decodeBatchDraft.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, i32p, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
+                                            i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(C.c_uint8), C.POINTER(vp),
+                                            C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int, i32p]
+    L.JPEGB200_draftScale.argtypes = [C.c_int] * 4
     L.JPEGB200_batchSetOutputTensor.argtypes = [vp, C.c_int, vp, C.c_int64, C.c_int64]
     L.JPEGB200_decodeBatchTensor.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
                                              i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(vp), C.POINTER(C.c_int64),
@@ -351,6 +358,24 @@ def _roi_array(rois, n):
     return (C.c_int32 * (4 * n))(*flat)
 
 
+def _draft_array(draft, n):
+    """per-view draft denominators -> uint8[n] (values are checked by the library: 1, 2, 4 or 8); None = full size"""
+    if draft is None:
+        return None
+    d = [int(v) for v in draft]
+    if len(d) != n:
+        raise ValueError("draft: one scale denominator per image (view)")
+    if any(v < 0 or v > 255 for v in d):
+        raise ValueError("draft: denominators are 1, 2, 4 or 8")
+    return (C.c_uint8 * n)(*d)
+
+
+def draft_scale(width, height, req_w, req_h):
+    """Pillow's JpegImageFile.draft choice of the scale denominator s (1, 2, 4 or 8) for a (req_w, req_h) request on a
+    width x height file (JPEGB200_draftScale); a request of 0 gives 1 where Pillow would divide by zero."""
+    return lib().JPEGB200_draftScale(int(width), int(height), int(req_w), int(req_h))
+
+
 def _orient_array(orients, n):
     """n EXIF transforms (0 = from the file, 1-8) -> uint8[n] for the C ABI (None stays None = no orientation)"""
     if orients is None:
@@ -381,10 +406,11 @@ class Batch:
     with `filter` (RESIZE_BILINEAR / _BICUBIC / _BOX) of the upright crop (JPEGB200_batchCreateResized), or None.
     views: one view count per file (JPEGB200_batchCreateViews: file i's views come next to each other and share one
     entropy walk), or None for one per file; rois / orients / out_sizes and every per-image call are then per view, and
-    self.n is the number of views."""
+    self.n is the number of views.  draft: one scale denominator (1, 2, 4, 8) per image or view, each decoded as Pillow's
+    draft() at that scale (JPEGB200_batchCreateDraft; needs JPEGB200_OPT_LIBJPEG), or None."""
 
     def __init__(self, ctx, ptrs, sizes, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
-                 filter=RESIZE_BILINEAR, spec=None, views=None):
+                 filter=RESIZE_BILINEAR, spec=None, views=None, draft=None):
         nf = len(ptrs)
         self._views, n = _views_array(views, nf)
         self.n = n
@@ -394,7 +420,13 @@ class Batch:
         self._orients = _orient_array(orients, n)
         self._out_sizes = _size_array(out_sizes, n)
         self.ctx = ctx
-        if spec is None and views is None:
+        self._draft = _draft_array(draft, n)
+        if draft is not None:
+            self._spec = spec
+            self.h = lib().JPEGB200_batchCreateDraft(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
+                                                     self._rois, self._orients, self._out_sizes, int(filter),
+                                                     C.byref(spec) if spec is not None else None, self._draft)
+        elif spec is None and views is None:
             self.h = lib().JPEGB200_batchCreateResized(ctx.h, self._ptrs, self._sizes, n, pixel_type, options, self._rois,
                                                        self._orients, self._out_sizes, int(filter))
         else:   # views and / or a TensorSpec (device outputs only): JPEGB200_batchCreateViews
@@ -478,12 +510,13 @@ class Batch:
 
 
 def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flags=0, rois=None, orients=None,
-                 out_sizes=None, filter=RESIZE_BILINEAR, views=None):
+                 out_sizes=None, filter=RESIZE_BILINEAR, views=None, draft=None):
     """JPEGB200_decodeBatch(ROI / Oriented / Resized / Views): one call for n files (host pointers) -> n outputs (host
     pointers, or device pointers with JPEGB200_OUT_DEVICE); rois: one (x, y, w, h) per image or None; orients: one EXIF
     transform per image (0 = from the file) or None; out_sizes: one (W, H) per image (resized with `filter`) or None.
     views: one view count per file, or None; outs, pitches and the per-image lists are then per view.  Returns (rc,
-    per-image status list, counters summed over the internal jobs)."""
+    per-image status list, counters summed over the internal jobs).  draft: one scale denominator per image (view), or
+    None (JPEGB200_decodeBatchDraft)."""
     nf = len(ptrs)
     va, n = _views_array(views, nf)
     pa = (C.c_void_p * nf)(*ptrs)
@@ -493,7 +526,11 @@ def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flag
     oa = (C.c_void_p * n)(*outs)
     pi = (C.c_int64 * n)(*pitches) if pitches is not None else None
     st = (C.c_int32 * n)()
-    if views is None:
+    if draft is not None:
+        rc = lib().JPEGB200_decodeBatchDraft(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
+                                             _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None,
+                                             _draft_array(draft, n), oa, pi, None, flags, st)
+    elif views is None:
         rc = lib().JPEGB200_decodeBatchResized(ctx.h, pa, sa, n, pixel_type, options, _roi_array(rois, n),
                                                _orient_array(orients, n), _size_array(out_sizes, n), int(filter), oa, pi, flags,
                                                st)
@@ -507,15 +544,16 @@ def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flag
 
 
 def decode_batch_to_host(ctx, jpegs, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
-                         filter=RESIZE_BILINEAR, views=None):
+                         filter=RESIZE_BILINEAR, views=None, draft=None):
     """Convenience: list of bytes -> list of numpy arrays [out_h, pitch_bytes] (uint8).
     One public-API call per batch with HOST buffers on both sides.  rois: one (x, y, w, h) per image (the arrays are then
     h rows of w pixels), or None.  orients: one EXIF transform per image (0 = from the file), or None.  out_sizes: one
     (W, H) per image (the arrays are then H rows of W pixels, resized with `filter`), or None.  views: one view count
-    per file, or None; the lists (and rois / orients / out_sizes) are then per view."""
+    per file, or None; the lists (and rois / orients / out_sizes) are then per view.  draft: one scale denominator per
+    image (view), or None."""
     bufs = [np.frombuffer(j, dtype=np.uint8) for j in jpegs]
     b = Batch(ctx, [x.ctypes.data for x in bufs], [len(x) for x in bufs], pixel_type, options, rois, orients, out_sizes,
-              filter, views=views)
+              filter, views=views, draft=draft)
     try:
         outs = []
         for i in range(b.n):
@@ -563,7 +601,7 @@ def tensor_spec(dtype, layout="CHW", scale="div255", mean=(0.0, 0.0, 0.0), std=(
 
 def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, orients=None, out_sizes=None,
                         filter=RESIZE_BILINEAR, dtype=None, layout="CHW", scale="div255", mean=(0.0, 0.0, 0.0),
-                        std=(1.0, 1.0, 1.0), bgr=False, out=None, views=None):
+                        std=(1.0, 1.0, 1.0), bgr=False, out=None, views=None, draft=None):
     """JPEGB200_decodeBatchTensor: list of bytes -> the model's input tensor on the context's GPU, and the status list.
 
     Image i becomes a C x H x W (layout "CHW") or H x W x C ("HWC") tensor of `dtype` (torch.float32 by default, float16,
@@ -574,7 +612,9 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     out: a CUDA tensor of that shape and dtype on the context's device (any row / plane strides the library accepts), or
     a list of per-image tensors; else the result is allocated with torch.empty.
     views: one view count per file (JPEGB200_decodeBatchViews: the views of a file share one entropy walk), or None; the
-    images are then the views: rois / orients / out_sizes / out and the result ([V, C, H, W], or a list) are per view."""
+    images are then the views: rois / orients / out_sizes / out and the result ([V, C, H, W], or a list) are per view.
+    draft: one scale denominator (1, 2, 4, 8) per image (view), Pillow's draft() at that scale (JPEGB200_decodeBatchDraft),
+    or None."""
     import torch
     dtype = torch.float32 if dtype is None else dtype
     spec = tensor_spec(dtype, layout, scale, mean, std, bgr)
@@ -588,7 +628,7 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     elif rois is not None:
         hw = [(int(r[3]), int(r[2])) for r in rois]
     else:   # sizes from a header-only batch (no GPU work); an image refused there has size 0 x 0
-        b = Batch(ctx, ptrs, sizes, pixel_type, options, rois, orients, out_sizes, filter, spec=spec, views=views)
+        b = Batch(ctx, ptrs, sizes, pixel_type, options, rois, orients, out_sizes, filter, spec=spec, views=views, draft=draft)
         try:
             hw = [(b.info(i)["out_h"], b.info(i)["out_w"]) for i in range(n)]
         finally:
@@ -629,10 +669,10 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     st = (C.c_int32 * n)()
     with torch.cuda.device(dev):
         torch.cuda.current_stream(dev).synchronize()   # the library's streams do not order against torch's
-        rc = lib().JPEGB200_decodeBatchViews(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
+        rc = lib().JPEGB200_decodeBatchDraft(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
                                              _orient_array(orients, n), _size_array(out_sizes, n), int(filter),
-                                             C.byref(spec), (C.c_void_p * n)(*ptr_l), (C.c_int64 * n)(*pitch_l),
-                                             (C.c_int64 * n)(*plane_l), JPEGB200_OUT_DEVICE, st)
+                                             C.byref(spec), _draft_array(draft, n), (C.c_void_p * n)(*ptr_l),
+                                             (C.c_int64 * n)(*pitch_l), (C.c_int64 * n)(*plane_l), JPEGB200_OUT_DEVICE, st)
     if rc == 0:
         raise RuntimeError("decodeBatchViews failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
     return out, list(st)

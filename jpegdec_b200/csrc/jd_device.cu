@@ -248,6 +248,7 @@ struct JPEGB200_BATCH {
     std::vector<int64_t> lj_plane;       /* per image: plane bytes (256-byte aligned; 0 for a failed image) */
     int64_t lj_plane_total = 0;
     uint32_t lj_max_blocks = 0, lj_max_pixels = 0;
+    uint32_t lj_s_blocks[4] = {}, lj_s_pixels[4] = {};   /* the same per draft shift 1-3 (JPEGB200_batchCreateDraft) */
     DevBuf<uint8_t> d_lj;
     DevBuf<JDLjDesc> d_lj_desc;
     uint32_t h_changed = 0;
@@ -546,6 +547,7 @@ struct CreatePlan {
     const int32_t *sizes = nullptr, *views = nullptr, *rois = nullptr, *out_sizes = nullptr;
     const uint8_t *orients = nullptr;
     const JPEGB200_TensorSpec *spec = nullptr;
+    const uint8_t *draft = nullptr;     /* per view: draft scale denominator (JPEGB200_batchCreateDraft), NULL = 1 */
     /* where the next file's restart segments, blocks and records start; where the next view's output and gray stage start */
     uint32_t seg = 0;
     uint64_t blk = 0, rec_total = 0;
@@ -707,10 +709,26 @@ static void resolve_orients(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int
 static uint32_t plan_views(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int nvf)
 {
     const JDInfo &inf = b->infos[f];
-    uint32_t walk = (uint32_t)jd_views_plan(inf.width, inf.height, inf.subsample, inf.restart_interval, b->sshift, nvf,
-                                            P.rois ? P.rois + 4 * (size_t)v0 : nullptr, P.orients ? &P.ks[v0] : nullptr,
-                                            P.out_sizes ? P.out_sizes + 2 * (size_t)v0 : nullptr, &b->plans[v0], &P.srects[4 * (size_t)v0],
-                                            &P.vok[v0]);
+    uint32_t walk = 0;
+    if (!P.draft) {
+        walk = (uint32_t)jd_views_plan(inf.width, inf.height, inf.subsample, inf.restart_interval, b->sshift, nvf,
+                                       P.rois ? P.rois + 4 * (size_t)v0 : nullptr, P.orients ? &P.ks[v0] : nullptr,
+                                       P.out_sizes ? P.out_sizes + 2 * (size_t)v0 : nullptr, &b->plans[v0], &P.srects[4 * (size_t)v0],
+                                       &P.vok[v0]);
+    } else {
+        /* each view at its own scale (a libjpeg batch walks at full scale: b->sshift is 0); an unknown denominator
+         * invalidates that view alone */
+        for (int i = v0; i < v0 + nvf; i++) {
+            const int sh = jd_draft_shift(P.draft[i]);
+            const uint32_t w = (uint32_t)jd_views_plan(inf.width, inf.height, inf.subsample, inf.restart_interval, sh < 0 ? 0 : sh, 1,
+                                                       P.rois ? P.rois + 4 * (size_t)i : nullptr, P.orients ? &P.ks[i] : nullptr,
+                                                       P.out_sizes ? P.out_sizes + 2 * (size_t)i : nullptr, &b->plans[i],
+                                                       &P.srects[4 * (size_t)i], &P.vok[i]);
+            if (sh < 0) { P.vok[i] = 0; continue; }
+            b->lj_desc[i].shift = (uint32_t)sh;
+            if (w > walk) walk = w;
+        }
+    }
     if (walk != 0 && b->lj && b->roi) {
         /* what libjpeg's fancy upsampling reads around each rectangle */
         walk = 0;
@@ -718,7 +736,7 @@ static uint32_t plan_views(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int 
             if (!P.vok[i]) continue;
             const int32_t *sr = &P.srects[4 * (size_t)i];
             const int32_t r[4] = {sr[0], sr[1], P.orients ? sr[2] : P.rois[4 * (size_t)i + 2], P.orients ? sr[3] : P.rois[4 * (size_t)i + 3]};
-            jd_lj_plan_extend(inf.width, inf.height, inf.subsample, inf.restart_interval, r, &b->plans[i]);
+            jd_lj_plan_extend_s(inf.width, inf.height, inf.subsample, inf.restart_interval, (int)b->lj_desc[i].shift, r, &b->plans[i]);
             if ((uint32_t)b->plans[i].nseg_walk > walk) walk = (uint32_t)b->plans[i].nseg_walk;
         }
     }
@@ -860,7 +878,7 @@ static void add_prog_file(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int n
 static int plan_view_output(JPEGB200_BATCH *b, CreatePlan &P, int f, int i)
 {
     const JDInfo &inf = b->infos[f];
-    const int s = b->sshift;
+    const int s = b->lj ? (int)b->lj_desc[i].shift : b->sshift;   /* a libjpeg batch scales per view (draft) */
     JDImageDesc &vd = b->descs[i];
     if (b->views) {
         if (b->parse_status[i] != JPEG_SUCCESS) {   /* an invalid view of a walked file: empty, like a refused image */
@@ -892,11 +910,21 @@ static int plan_view_output(JPEGB200_BATCH *b, CreatePlan &P, int f, int i)
         L.nmy = b->roi ? (uint32_t)(b->plans[i].mcu_y1 - b->plans[i].mcu_y0 + 1) : (uint32_t)inf.mcus_y;
         L.ycc = (uint32_t)jd_lj_is_ycc(&inf);
         const uint64_t blocks = (uint64_t)L.nmx * L.nmy * (uint64_t)inf.bpm;
-        b->lj_plane[i] = (int64_t)align256(blocks * 64u);
-        b->lj_plane_total += b->lj_plane[i];
-        if (blocks > b->lj_max_blocks) b->lj_max_blocks = (uint32_t)blocks;
         const uint64_t px = (uint64_t)vd.out_w * vd.out_h;
-        if (px > b->lj_max_pixels) b->lj_max_pixels = (uint32_t)px;
+        if (L.shift == 0) {
+            b->lj_plane[i] = (int64_t)align256(blocks * 64u);
+            if (blocks > b->lj_max_blocks) b->lj_max_blocks = (uint32_t)blocks;
+            if (px > b->lj_max_pixels) b->lj_max_pixels = (uint32_t)px;
+        } else {
+            /* size_c x size_c samples per block of each component (jd_ljpeg.h) */
+            const uint32_t hs = (inf.subsample >> 4) ? (uint32_t)(inf.subsample >> 4) : 1u, vs = (inf.subsample & 15) ? (uint32_t)(inf.subsample & 15) : 1u;
+            const uint64_t ys = 8u >> L.shift, cs = jd_lj_csize(L.shift, hs, vs);
+            const uint64_t per_mcu = hs * vs * ys * ys + (uint64_t)(inf.ncomp - 1) * cs * cs;
+            b->lj_plane[i] = (int64_t)align256((uint64_t)L.nmx * L.nmy * per_mcu);
+            if (blocks > b->lj_s_blocks[L.shift]) b->lj_s_blocks[L.shift] = (uint32_t)blocks;
+            if (px > b->lj_s_pixels[L.shift]) b->lj_s_pixels[L.shift] = (uint32_t)px;
+        }
+        b->lj_plane_total += b->lj_plane[i];
     }
     if (b->resize) {
         /* S = what the same call without out_sizes stores; the descriptor carries the resized size from here on */
@@ -1014,15 +1042,25 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateViews(JPEGB200_CTX *ctx, const ui
                                                      const uint8_t *orients, const int32_t *out_sizes, int filter,
                                                      const JPEGB200_TensorSpec *spec)
 {
+    return JPEGB200_batchCreateDraft(ctx, datas, sizes, n, views, pixel_type, options, rois, orients, out_sizes, filter, spec, nullptr);
+}
+
+extern "C" JPEGB200_BATCH *JPEGB200_batchCreateDraft(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                                     const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                                     const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                                     const JPEGB200_TensorSpec *spec, const uint8_t *draft)
+{
     if (!ctx) { snprintf(g_err, sizeof(g_err), "invalid parameter"); return nullptr; }
     int64_t nv = 0;   /* images of the batch: views */
     if (!jd_check_batch_features(pixel_type, options, n, views, rois != nullptr, orients != nullptr, out_sizes != nullptr, filter, spec,
-                                 &nv, g_err, (int)sizeof(g_err)))
+                                 &nv, g_err, (int)sizeof(g_err)) ||
+        !jd_check_draft(options, draft, g_err, (int)sizeof(g_err)))
         return nullptr;
     JPEGB200_BATCH *b = new (std::nothrow) JPEGB200_BATCH();
     if (!b) return nullptr;
     CreatePlan P;
     P.datas = datas; P.sizes = sizes; P.views = views; P.rois = rois; P.orients = orients; P.out_sizes = out_sizes; P.spec = spec;
+    P.draft = draft;
     P.srects.assign(4 * (size_t)nv, 0); P.vok.assign((size_t)nv, 0);
     P.ks.assign(orients ? (size_t)nv : 0u, 0);
     if (options & JPEGB200_OPT_PROGRESSIVE) { P.fscans.resize(JD_PROG_MAX_SCANS); P.ftabs.resize(JD_PROG_MAX_TABS); }
@@ -1771,6 +1809,27 @@ static void run_stitch_patch_pack(JPEGB200_BATCH *b, DecodeState &D)
     }
 }
 
+/* draft views (JPEGB200_batchCreateDraft): one IDCT and one colour launch per scale present; ljd holds the scaled set of
+ * descriptors (full-scale views have nmx = 0) */
+static int run_lj_scaled(JPEGB200_BATCH *b, DecodeState &D, const JDLjDesc *ljd)
+{
+    const int n = b->n;
+    cudaStream_t st = b->ss.stream;
+    for (uint32_t sh = 1; sh <= 3; sh++) {
+        const unsigned gb = (b->lj_s_blocks[sh] + JD_LJ_THREADS - 1) / JD_LJ_THREADS, gp = (b->lj_s_pixels[sh] + JD_LJ_THREADS - 1) / JD_LJ_THREADS;
+        for (int i0 = 0; i0 < n && gb && gp; i0 += 65535) {
+            const unsigned ni = (unsigned)std::min(n - i0, 65535);
+            if (sh == 1) jdk_lj_idct_s<1><<<dim3(gb, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, ljd, b->d_blk_hdr.p, b->d_rec.p, b->d_quant.p, b->d_lj.p, (uint32_t)i0);
+            else if (sh == 2) jdk_lj_idct_s<2><<<dim3(gb, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, ljd, b->d_blk_hdr.p, b->d_rec.p, b->d_quant.p, b->d_lj.p, (uint32_t)i0);
+            else jdk_lj_idct_s<3><<<dim3(gb, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, ljd, b->d_blk_hdr.p, b->d_rec.p, b->d_quant.p, b->d_lj.p, (uint32_t)i0);
+            if (b->ptclass == JD_PT_GRAY) jdk_lj_color_s<JD_PT_GRAY><<<dim3(gp, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, ljd, b->d_lj.p, D.stage_out, (uint32_t)i0, sh);
+            else jdk_lj_color_s<JD_PT_8888><<<dim3(gp, ni), JD_LJ_THREADS, 0, st>>>(b->d_descs.p, ljd, b->d_lj.p, D.stage_out, (uint32_t)i0, sh);
+            D.launches += 2;
+        }
+    }
+    return 1;
+}
+
 /* libjpeg decode: planes of every image's MCU box, then upsampling + colour into the stores; images that failed keep nmx = 0 */
 static int run_lj(JPEGB200_BATCH *b, DecodeState &D)
 {
@@ -1783,9 +1842,21 @@ static int run_lj(JPEGB200_BATCH *b, DecodeState &D)
         ld[i].plane_off = po;
         po += (uint64_t)b->lj_plane[i];
     }
+    /* descriptors [0, n) for the full-scale kernels, [n, 2n) for the scaled ones: each set leaves the other's views empty */
+    bool scaled = false;
+    for (int i = 0; i < n; i++) scaled = scaled || ld[i].shift != 0;
+    const int nd = scaled ? 2 * n : n;
+    if (scaled) {
+        ld.resize((size_t)nd);
+        for (int i = 0; i < n; i++) {
+            ld[n + i] = ld[i];
+            if (ld[i].shift != 0) ld[i].nmx = ld[i].nmy = 0; else ld[n + i].nmx = ld[n + i].nmy = 0;
+        }
+    }
     CK(b->d_lj.alloc(&b->ctx->pool, po + 256));
-    CK(b->d_lj_desc.alloc(&b->ctx->pool, n));
-    CK(cudaMemcpyAsync(b->d_lj_desc.p, ld.data(), sizeof(JDLjDesc) * n, cudaMemcpyHostToDevice, st));
+    CK(b->d_lj_desc.alloc(&b->ctx->pool, nd));
+    CK(cudaMemcpyAsync(b->d_lj_desc.p, ld.data(), sizeof(JDLjDesc) * nd, cudaMemcpyHostToDevice, st));
+    if (scaled && !run_lj_scaled(b, D, b->d_lj_desc.p + n)) return 0;
     const unsigned gb = (b->lj_max_blocks + JD_LJ_THREADS - 1) / JD_LJ_THREADS, gp = (b->lj_max_pixels + JD_LJ_THREADS - 1) / JD_LJ_THREADS;
     for (int i0 = 0; i0 < n && gb && gp; i0 += 65535) {
         const unsigned ni = (unsigned)std::min(n - i0, 65535);
@@ -2187,6 +2258,16 @@ extern "C" int JPEGB200_decodeBatchViews(JPEGB200_CTX *ctx, const uint8_t *const
                                          const JPEGB200_TensorSpec *spec, void *const *outs, const int64_t *pitches,
                                          const int64_t *plane_strides, int flags, int32_t *status)
 {
+    return JPEGB200_decodeBatchDraft(ctx, datas, sizes, n, views, pixel_type, options, rois, orients, out_sizes, filter, spec, nullptr,
+                                     outs, pitches, plane_strides, flags, status);
+}
+
+extern "C" int JPEGB200_decodeBatchDraft(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                         const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                         const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                         const JPEGB200_TensorSpec *spec, const uint8_t *draft, void *const *outs,
+                                         const int64_t *pitches, const int64_t *plane_strides, int flags, int32_t *status)
+{
     if (!ctx || n <= 0) return 0;
     const int64_t nv = jd_count_views(n, views, "call", g_err, (int)sizeof(g_err));   /* images (views) of the call */
     if (nv < 0) return 0;
@@ -2233,8 +2314,9 @@ extern "C" int JPEGB200_decodeBatchViews(JPEGB200_CTX *ctx, const uint8_t *const
         const int32_t *vi = views ? views + i0 : nullptr;
         int cnt = jd_job_files(n - i0, sizes + i0, vi, maxcnt, limit, nullptr, 0, &cv, &capped);
         auto create = [&](int c) {
-            return JPEGB200_batchCreateViews(ctx, datas + i0, sizes + i0, c, vi, pixel_type, options, rois ? rois + 4 * (size_t)v0 : nullptr,
-                                             orients ? orients + v0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)v0 : nullptr, filter, spec);
+            return JPEGB200_batchCreateDraft(ctx, datas + i0, sizes + i0, c, vi, pixel_type, options, rois ? rois + 4 * (size_t)v0 : nullptr,
+                                             orients ? orients + v0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)v0 : nullptr, filter, spec,
+                                             draft ? draft + v0 : nullptr);
         };
         JPEGB200_BATCH *b = create(cnt);
         if (!b) { rc = 0; break; }

@@ -583,18 +583,31 @@ static void lj_reads(int p0, int p1, int n, int narrow, int *lo, int *hi)
 
 void jd_lj_plan_extend(int width, int height, int subsample, int restart_interval, const int32_t *srect, JDRoiPlan *plan)
 {
-    const int hs = (subsample == 0x21 || subsample == 0x22), vs = (subsample == 0x12 || subsample == 0x22);
-    const int mw = 8 << hs, mh = 8 << vs;
-    const int mcus_x = (width + mw - 1) / mw, mcus_y = (height + mh - 1) / mh;
-    const int narrow = hs && (width + 1) / 2 <= 2;   /* jdsample.c: h2v1 / h2v2 replicate a component this narrow */
+    jd_lj_plan_extend_s(width, height, subsample, restart_interval, 0, srect, plan);
+}
+
+void jd_lj_plan_extend_s(int width, int height, int subsample, int restart_interval, int shift, const int32_t *srect,
+                         JDRoiPlan *plan)
+{
+    const int h2 = (subsample == 0x21 || subsample == 0x22), v2 = (subsample == 0x12 || subsample == 0x22);
+    const int mcus_x = (width + (8 << h2) - 1) / (8 << h2), mcus_y = (height + (8 << v2) - 1) / (8 << v2);
+    const int mw = (8 << h2) >> shift, mh = (8 << v2) >> shift;   /* the MCU in scaled pixels */
+    /* jd_ljpeg.h's geometry: chroma IDCT size cs, upsampled by 2 along an axis where (1 << h2) * (8 >> shift) > cs, with the
+     * fancy filter while 8 >> shift > 1; dw: the component's real samples across at this scale */
+    int cs = 8 >> shift;
+    while (cs < 8 && (((1 << h2) * (8 >> shift)) % (2 * cs)) == 0 && (((1 << v2) * (8 >> shift)) % (2 * cs)) == 0) cs *= 2;
+    const int fancy = shift < 3;
+    const int hs = fancy && ((1 << h2) * (8 >> shift)) > cs, vs = fancy && ((1 << v2) * (8 >> shift)) > cs;
+    const int dw = (int)(((int64_t)width * cs + (8 << h2) - 1) / (8 << h2)), dh = (int)(((int64_t)height * cs + (8 << v2) - 1) / (8 << v2));
+    const int narrow = hs && dw <= 2;   /* jdsample.c: h2v1 / h2v2 replicate a component this narrow */
     int lo, hi;
     if (hs) {
-        lj_reads(srect[0], srect[0] + srect[2] - 1, width, narrow, &lo, &hi);
+        lj_reads(srect[0], srect[0] + srect[2] - 1, 2 * dw, narrow, &lo, &hi);
         if (lo / mw < plan->mcu_x0) plan->mcu_x0 = lo / mw;
         if (hi / mw > plan->mcu_x1) plan->mcu_x1 = hi / mw;
     }
     if (vs) {
-        lj_reads(srect[1], srect[1] + srect[3] - 1, height, narrow, &lo, &hi);
+        lj_reads(srect[1], srect[1] + srect[3] - 1, 2 * dh, narrow, &lo, &hi);
         if (lo / mh < plan->mcu_y0) plan->mcu_y0 = lo / mh;
         if (hi / mh > plan->mcu_y1) plan->mcu_y1 = hi / mh;
         plan->mcu_end = (plan->mcu_y1 + 1) * mcus_x;
@@ -603,6 +616,24 @@ void jd_lj_plan_extend(int width, int height, int subsample, int restart_interva
         const int nseg = (total + mps - 1) / mps, walk = (plan->mcu_end - 1) / mps + 1;
         plan->nseg_walk = walk < nseg ? walk : nseg;
     }
+}
+
+int jd_check_draft(int options, const uint8_t *draft, char *msg, int msg_len)
+{
+    if (draft && !(options & JPEGB200_OPT_LIBJPEG)) {
+        snprintf(msg, (size_t)msg_len, "draft scales need JPEGB200_OPT_LIBJPEG (they are libjpeg-turbo's reduced-size decodes)");
+        return 0;
+    }
+    return 1;
+}
+
+/* Pillow's JpegImageFile.draft: k = min(W // req_w, H // req_h), then the largest of 8, 4, 2, 1 that is at most k (1 when
+ * k is 0).  Pillow divides by a request of 0; here it gives 1. */
+int JPEGB200_draftScale(int width, int height, int req_w, int req_h)
+{
+    if (req_w <= 0 || req_h <= 0 || width <= 0 || height <= 0) return 1;
+    const int kw = width / req_w, kh = height / req_h, k = kw < kh ? kw : kh;
+    return k >= 8 ? 8 : k >= 4 ? 4 : k >= 2 ? 2 : 1;
 }
 
 int jd_job_files(int nf, const int32_t *sizes, const int32_t *views, int64_t max_views, int64_t max_bytes,

@@ -207,13 +207,24 @@ void jd_lj_quant(const JDInfo *info, int32_t *q /* [3][64] */);
  * clamped to the component's real samples; none in the narrow fallback), which may lie in the next MCU.  For vertically
  * subsampled files the walk and mcu_end then reach the last MCU row read. */
 void jd_lj_plan_extend(int width, int height, int subsample, int restart_interval, const int32_t *srect, JDRoiPlan *plan);
+/* The same for a view decoded at 1 / 2^shift (JPEGB200_batchCreateDraft): srect in the stored frame of the scaled image, plan
+ * jd_roi_plan's at that shift.  Upsampling reads a neighbouring chroma sample only along an axis that is still upsampled at
+ * this scale with the fancy filter (jd_ljpeg.h); shift 0 is jd_lj_plan_extend. */
+void jd_lj_plan_extend_s(int width, int height, int subsample, int restart_interval, int shift, const int32_t *srect,
+                         JDRoiPlan *plan);
+/* Per-view scale denominators of JPEGB200_batchCreateDraft: 1 with draft == NULL or with JPEGB200_OPT_LIBJPEG; 0 with a
+ * message for a draft without JPEGB200_OPT_LIBJPEG.  A value other than 1, 2, 4 or 8 is not refused here: that view alone
+ * gets JPEG_INVALID_PARAMETER (jd_draft_shift). */
+int jd_check_draft(int options, const uint8_t *draft, char *msg, int msg_len);
+/* log2 of a draft denominator (1, 2, 4, 8 -> 0..3), -1 for any other value */
+static inline int jd_draft_shift(uint8_t s) { return s == 1 ? 0 : s == 2 ? 1 : s == 4 ? 2 : s == 8 ? 3 : -1; }
 /* Per image of a libjpeg batch: its MCU box and where its planes live in the batch's plane scratch (jd_ljpeg.h). */
 typedef struct {
     uint64_t plane_off;     /* byte offset of the box's planes (256-byte aligned) */
     uint32_t mx0, my0;      /* the box's first MCU column / row */
     uint32_t nmx, nmy;      /* its size in MCUs; 0 = nothing to decode (a failed image) */
     uint32_t ycc;           /* jd_lj_is_ycc */
-    uint32_t pad;
+    uint32_t shift;         /* the view's scale 1 / 2^shift (JPEGB200_batchCreateDraft); 0 = full scale */
 } JDLjDesc;
 
 /* A caller's destination for image `index` (only named in the message): row_bytes is the tight pitch

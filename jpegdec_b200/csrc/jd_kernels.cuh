@@ -2364,6 +2364,83 @@ __global__ void __launch_bounds__(JD_LJ_THREADS) jdk_lj_color(const JDImageDesc 
     else reinterpret_cast<uint32_t *>(row)[dx] = v;
 }
 
+/* Draft views (JPEGB200_batchCreateDraft) at 1 / 2^SH: one thread per block of the image's MCU box, writing size_c x size_c
+ * samples (jd_ljpeg.h: luma 8 >> SH, chroma jd_lj_csize).  Only views of this scale have a box in ljd. */
+template <int SH>
+__global__ void __launch_bounds__(JD_LJ_THREADS) jdk_lj_idct_s(const JDImageDesc *__restrict__ imgs, const JDLjDesc *__restrict__ ljd,
+                                                               const jd_u64 *__restrict__ blk_hdr, const uint16_t *__restrict__ rec,
+                                                               const int32_t *__restrict__ quant, uint8_t *__restrict__ planes, uint32_t img0)
+{
+    const uint32_t i = img0 + blockIdx.y;
+    const JDLjDesc L = ljd[i];
+    if (L.shift != (uint32_t)SH) return;
+    const uint32_t t = blockIdx.x * JD_LJ_THREADS + threadIdx.x;
+    const uint32_t bpm = imgs[i].bpm;
+    if (t >= L.nmx * L.nmy * bpm) return;
+    const JDImageDesc &im = imgs[i];
+    const uint32_t hs = (im.subsample >> 4) ? (im.subsample >> 4) : 1u, vs = (im.subsample & 15) ? (im.subsample & 15) : 1u;
+    const uint32_t m = t / bpm, b = t - m * bpm;
+    const uint32_t my = m / L.nmx, mx = m - my * L.nmx;
+    const uint32_t cmp = b < hs * vs ? 0u : b - hs * vs + 1u;
+    const uint32_t ys = 8u >> SH, cs = jd_lj_csize(SH, hs, vs), sz = cmp ? cs : ys;
+    const jd_u64 h = blk_hdr[im.blk_base + ((size_t)(L.my0 + my) * im.mcus_x + L.mx0 + mx) * bpm + b];
+    uint32_t pitch;
+    uint8_t *dst = planes + L.plane_off + jd_lj_block_dst_s(b, mx, my, L.nmx, L.nmy, hs, vs, ys, cs, &pitch);
+    const int32_t *q = quant + (size_t)i * 192 + cmp * 64;
+    if (sz == 1u) *dst = jd_lj_block1(h, q);
+    else if (sz == 2u) jd_lj_block_red<2>(rec + im.rec_base, h, q, dst, pitch);
+    else if (sz == 4u) jd_lj_block_red<4>(rec + im.rec_base, h, q, dst, pitch);
+    else if (SH == 1) {   /* a 4:2:0 chroma block at 1/2 keeps the 8x8 islow (no 8x8 size below 1/2) */
+        int32_t c[64];
+        jd_lj_block(rec + im.rec_base, h, q, c, dst, pitch);
+    }
+}
+
+/* one thread per pixel of a draft view's rectangle in the stored scaled frame: jdk_lj_color with the plane geometry and
+ * upsampling mode of scale 1 / 2^sh (jd_lj_chroma_s) */
+template <int PT>
+__global__ void __launch_bounds__(JD_LJ_THREADS) jdk_lj_color_s(const JDImageDesc *__restrict__ imgs, const JDLjDesc *__restrict__ ljd,
+                                                                const uint8_t *__restrict__ planes, uint8_t *__restrict__ out, uint32_t img0,
+                                                                uint32_t sh)
+{
+    const uint32_t i = img0 + blockIdx.y;
+    const JDLjDesc L = ljd[i];
+    if (L.nmx == 0u || L.shift != sh) return;
+    const JDImageDesc &im = imgs[i];
+    const bool tr = im.orient >= 5u;
+    const uint32_t sw = tr ? im.out_h : im.out_w, sth = tr ? im.out_w : im.out_h;
+    const uint32_t p = blockIdx.x * JD_LJ_THREADS + threadIdx.x;
+    if (p >= sw * sth) return;
+    const uint32_t gy = p / sw, gx = p - gy * sw;
+    const uint32_t sx = im.roi_x + gx, sy = im.roi_y + gy;
+    const uint32_t hs = (im.subsample >> 4) ? (im.subsample >> 4) : 1u, vs = (im.subsample & 15) ? (im.subsample & 15) : 1u;
+    const uint32_t ys = 8u >> sh, yp = L.nmx * hs * ys;
+    const uint8_t *pl = planes + L.plane_off;
+    const uint32_t Y = pl[(size_t)(sy - L.my0 * vs * ys) * yp + sx - L.mx0 * hs * ys];
+    uint32_t v;
+    if (PT == JD_PT_GRAY) v = Y;
+    else if (im.ncomp == 1) v = Y | (Y << 8) | (Y << 16) | 0xFF000000u;
+    else {
+        const uint32_t cs = jd_lj_csize(sh, hs, vs), cp = L.nmx * cs;
+        const size_t csz = (size_t)cp * L.nmy * cs;
+        const uint32_t dw = ((uint32_t)im.width * cs + hs * 8u - 1u) / (hs * 8u), dh = ((uint32_t)im.height * cs + vs * 8u - 1u) / (vs * 8u);
+        const uint32_t hr = hs * ys / cs, vr = vs * ys / cs, fancy = ys > 1u;
+        const uint8_t *pc = pl + (size_t)yp * L.nmy * vs * ys;
+        const uint32_t cb = jd_lj_chroma_s(pc, cp, L.mx0 * cs, L.my0 * cs, sx, sy, hr, vr, fancy, dw, dh);
+        const uint32_t cr = jd_lj_chroma_s(pc + csz, cp, L.mx0 * cs, L.my0 * cs, sx, sy, hr, vr, fancy, dw, dh);
+        v = (L.ycc ? jd_lj_ycc_rgb((int32_t)Y, (int32_t)cb, (int32_t)cr) : (Y | (cb << 8) | (cr << 16))) | 0xFF000000u;
+    }
+    uint32_t dx = gx, dy = gy;
+    if (im.orient >= 2u) {
+        const uint32_t ex = ((JD_ORIENT_MX >> im.orient) & 1u) ? sw - 1u - gx : gx;
+        const uint32_t ey = ((JD_ORIENT_MY >> im.orient) & 1u) ? sth - 1u - gy : gy;
+        dx = tr ? ey : ex; dy = tr ? ex : ey;
+    }
+    uint8_t *row = out + im.out_off + (size_t)dy * im.out_pitch;
+    if (PT == JD_PT_GRAY) row[dx] = (uint8_t)v;
+    else reinterpret_cast<uint32_t *>(row)[dx] = v;
+}
+
 /* digest of device byte ranges (JPEGB200_digestDevice, jd_device.cu) */
 __device__ __forceinline__ unsigned long long jd_mix64(unsigned long long z)
 {

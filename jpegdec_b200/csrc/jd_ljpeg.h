@@ -150,4 +150,159 @@ JD_HD uint32_t jd_lj_ycc_rgb(int32_t y, int32_t cb, int32_t cr)
     return jd_lj_clamp(r) | (jd_lj_clamp(g) << 8) | (jd_lj_clamp(b) << 16);
 }
 
+/* ---- scaled decodes (JPEGB200_batchCreateDraft: Pillow's draft(), libjpeg-turbo at scale 1/s, s = 2^shift) ----
+ *
+ * Geometry (jdmaster.c, jdsample.c).  The base IDCT size is m = 8 >> shift.  Luma keeps m; a chroma component (1 x 1 in a
+ * file of hs x vs luma) starts at m and doubles while it is below 8 and hs * m, vs * m are both multiples of twice its
+ * size.  Its upsampling ratio is then hs * m / size across and vs * m / size down (1 or 2); a ratio of 2 uses the fancy
+ * filter when m > 1 and replicates at m = 1, and the narrow rule of the full-scale decode applies to the scaled component
+ * width ceil(W * size / (hs * 8)).
+ *
+ * The reduced IDCTs (jidctred.c: jpeg_idct_4x4, _2x2, _1x1) use 13-bit constants and 2 extra bits between the passes, on
+ * coefficients dequantized with the raw DQT values.  4x4 never reads coefficient row or column 4; 2x2 reads rows and
+ * columns 0, 1, 3, 5 and 7 only; 1x1 reads the DC alone.  Their first pass is an integer-linear function of the
+ * dequantized coefficients up to its descale, so it is computed here as sums over the block's records, kept in registers
+ * (no 64-word array); the sums wrap in 32 bits like jidctint.c's restatement above.  The domain note of the 8x8 islow
+ * applies unchanged (tests/test_draft_host.py pins these against Pillow on random blocks and on every fixture). */
+#define JD_LJ_R0211 1730
+#define JD_LJ_R0509 4176
+#define JD_LJ_R0601 4926
+#define JD_LJ_R0720 5906
+#define JD_LJ_R0850 6967
+#define JD_LJ_R1061 8697
+#define JD_LJ_R1272 10426
+#define JD_LJ_R1451 11893
+#define JD_LJ_R2172 17799
+#define JD_LJ_R3624 29692
+
+/* IDCT size of a 1 x 1 chroma component of an hs x vs file at 1 / 2^shift (luma: 8 >> shift) */
+JD_HD uint32_t jd_lj_csize(uint32_t shift, uint32_t hs, uint32_t vs)
+{
+    const uint32_t m = 8u >> shift;
+    uint32_t s = m;
+    while (s < 8u && (hs * m) % (2u * s) == 0u && (vs * m) % (2u * s) == 0u) s *= 2u;
+    return s;
+}
+
+/* the multiplier of input r (0..7) in output j of a 1-D pass: jpeg_idct_4x4 (n = 4: outputs tmp10 + tmp2, tmp12 + tmp0,
+ * tmp12 - tmp0, tmp10 - tmp2) and jpeg_idct_2x2 (n = 2: tmp10 + tmp0, tmp10 - tmp0) */
+JD_HD int32_t jd_lj_kred(uint32_t n, uint32_t j, uint32_t r)
+{
+    if (n == 2u) {
+        const int32_t sg = j == 0u ? 1 : -1;
+        switch (r) {
+        case 0: return 1 << 15;
+        case 1: return sg * JD_LJ_R3624;
+        case 3: return -sg * JD_LJ_R1272;
+        case 5: return sg * JD_LJ_R0850;
+        case 7: return -sg * JD_LJ_R0720;
+        default: return 0;
+        }
+    }
+    const bool outer = j == 0u || j == 3u;              /* tmp10 +- tmp2 */
+    const int32_t sg = (j == 0u || j == 1u) ? 1 : -1;   /* + or - the odd part */
+    switch (r) {
+    case 0: return 1 << 14;
+    case 2: return outer ? JD_LJ_F1847 : -JD_LJ_F1847;
+    case 6: return outer ? -JD_LJ_F0765 : JD_LJ_F0765;
+    case 1: return sg * (outer ? JD_LJ_F2562 : JD_LJ_R1061);
+    case 3: return sg * (outer ? JD_LJ_F0899 : -JD_LJ_R2172);
+    case 5: return sg * (outer ? -JD_LJ_R0601 : JD_LJ_R1451);
+    case 7: return sg * (outer ? -JD_LJ_R0509 : -JD_LJ_R0211);
+    default: return 0;
+    }
+}
+
+JD_HD int32_t jd_lj_mul(int32_t a, int32_t k) { return (int32_t)((uint32_t)a * (uint32_t)k); }
+
+/* One block at N x N (N = 4 or 2): the coefficients of block header h (records from irec) dequantized with q, the N x N
+ * samples written to dst (row pitch `pitch` bytes). */
+template <int N>
+JD_HD void jd_lj_block_red(const uint16_t *irec, jd_u64 h, const int32_t *q, uint8_t *dst, uint32_t pitch)
+{
+    int32_t p[N][8];   /* first-pass sums: output row j of column col */
+    const int32_t dc = JD_HDR_DC(h) * q[0];
+#pragma unroll
+    for (int j = 0; j < N; j++) {
+        p[j][0] = jd_lj_mul(dc, jd_lj_kred(N, j, 0));
+#pragma unroll
+        for (int c = 1; c < 8; c++) p[j][c] = 0;
+    }
+    const uint32_t ri = JD_HDR_REC(h), n = JD_HDR_NCOEF(h);
+    const bool big = JD_HDR_BIG(h) != 0;
+    for (uint32_t i = 0; i < n; i++) {
+        uint32_t t;
+        int32_t v;
+        if (big) { t = irec[ri + 2 * i] & 63u; v = (int32_t)(int16_t)irec[ri + 2 * i + 1]; }
+        else { const uint32_t r = irec[ri + i]; t = r >> 10; v = (int32_t)(r << 22) >> 22; }
+        const uint32_t row = t & 7u, col = t >> 3;
+        if (jd_lj_kred(N, 0, row) == 0 || jd_lj_kred(N, 0, col) == 0) continue;   /* a row / column this size never reads */
+        v *= q[t];
+        int32_t a[N];
+#pragma unroll
+        for (int j = 0; j < N; j++) a[j] = jd_lj_mul(v, jd_lj_kred(N, j, row));
+        switch (col) {   /* constant indices only: the sums stay in registers */
+#define JD_LJ_ACC(cc) case cc: { _Pragma("unroll") for (int j = 0; j < N; j++) p[j][cc] += a[j]; } break;
+        JD_LJ_ACC(0) JD_LJ_ACC(1) JD_LJ_ACC(2) JD_LJ_ACC(3) JD_LJ_ACC(5) JD_LJ_ACC(6) JD_LJ_ACC(7)
+#undef JD_LJ_ACC
+        default: break;
+        }
+    }
+    /* descale of pass 1 (13 - 2 + log2(8 / N) bits), then pass 2 over each row (13 + 2 + 3 + log2(8 / N) bits) */
+    const int sh1 = N == 4 ? 12 : 13, sh2 = N == 4 ? 19 : 20;
+#pragma unroll
+    for (int j = 0; j < N; j++) {
+        int32_t w[8];
+#pragma unroll
+        for (int c = 0; c < 8; c++) w[c] = (int32_t)((uint32_t)p[j][c] + (1u << (sh1 - 1))) >> sh1;
+        uint32_t packed = 0;
+#pragma unroll
+        for (int k = 0; k < N; k++) {
+            int32_t s = 0;
+#pragma unroll
+            for (int c = 0; c < 8; c++) s = (int32_t)((uint32_t)s + (uint32_t)jd_lj_mul(w[c], jd_lj_kred(N, k, c)));
+            packed |= jd_lj_clamp(((int32_t)((uint32_t)s + (1u << (sh2 - 1))) >> sh2) + 128) << (8 * k);
+        }
+        uint8_t *d = dst + (size_t)j * pitch;
+#ifdef __CUDA_ARCH__
+        if (N == 4) *reinterpret_cast<uint32_t *>(d) = packed;
+        else *reinterpret_cast<uint16_t *>(d) = (uint16_t)packed;
+#else
+        for (int k = 0; k < N; k++) d[k] = (uint8_t)(packed >> (8 * k));
+#endif
+    }
+}
+
+/* jpeg_idct_1x1: the DC alone */
+JD_HD uint8_t jd_lj_block1(jd_u64 h, const int32_t *q)
+{
+    const int32_t dc = JD_HDR_DC(h) * q[0];
+    return (uint8_t)jd_lj_clamp(((dc + 4) >> 3) + 128);
+}
+
+/* Planes of one image's MCU box at a reduced scale: luma blocks of ys x ys samples, chroma blocks of cs x cs; component 0
+ * is (nmx * hs * ys) x (nmy * vs * ys) samples, each chroma component (nmx * cs) x (nmy * cs).  At ys = cs = 8 this is
+ * jd_lj_block_dst's layout.  Block b of MCU (mx, my) of the box goes to: */
+JD_HD uint64_t jd_lj_block_dst_s(uint32_t b, uint32_t mx, uint32_t my, uint32_t nmx, uint32_t nmy, uint32_t hs, uint32_t vs,
+                                 uint32_t ys, uint32_t cs, uint32_t *pitch)
+{
+    const uint32_t nl = hs * vs, yp = nmx * hs * ys;
+    if (b < nl) {
+        *pitch = yp;
+        return (uint64_t)((my * vs + b / hs) * ys) * yp + (mx * hs + b % hs) * ys;
+    }
+    const uint32_t cp = nmx * cs;
+    *pitch = cp;
+    return (uint64_t)yp * nmy * vs * ys + (b - nl) * ((uint64_t)cp * nmy * cs) + (uint64_t)(my * cs) * cp + mx * cs;
+}
+
+/* Chroma sample of scaled pixel (x, y): ratios hr, vr (1 or 2) from the plane to the pixels, fancy = m > 1; dw x dh = the
+ * component's real samples at this scale */
+JD_HD uint32_t jd_lj_chroma_s(const uint8_t *p, uint32_t cp, uint32_t cx0, uint32_t cy0, uint32_t x, uint32_t y,
+                              uint32_t hr, uint32_t vr, uint32_t fancy, uint32_t dw, uint32_t dh)
+{
+    if (!fancy) return jd_lj_chroma(p, cp, cx0, cy0, x / hr, y / vr, 1u, 1u, dw, dh);   /* h2v1 / int_upsample replicate */
+    return jd_lj_chroma(p, cp, cx0, cy0, x, y, hr, vr, dw, dh);
+}
+
 #endif
