@@ -315,6 +315,42 @@ JPEGB200_BATCH *JPEGB200_batchCreateDraft(JPEGB200_CTX *ctx, const uint8_t *cons
 /* Pillow's choice of s for draft(mode, (req_w, req_h)) on a W x H file: k = min(W / req_w, H / req_h) (integer division),
  * then the largest of 8, 4, 2, 1 that is at most k, else 1.  A request of 0 (where Pillow would divide by zero) gives 1. */
 int JPEGB200_draftScale(int width, int height, int req_w, int req_h);
+/* Resize with a source box and a reducing gap, bit-exact with Pillow's Image.resize((W, H), filter, box=, reducing_gap=)
+ * (what Image.thumbnail() runs after its draft): the arguments of JPEGB200_batchCreateDraft plus, per VIEW,
+ * boxes[4 v .. 4 v + 3] = x0, y0, x1, y1 (doubles, fractional allowed) and reducing_gaps[v] (0 = Pillow's None).
+ *   - S_v is what JPEGB200_batchCreateDraft stores for view v without out_sizes (crop, then orientation, at its draft
+ *     scale).  View v's output is Pillow's resize of every byte plane of S_v to out_sizes[v] with that box and gap:
+ *     with a gap, the reduce (Image.reduce) by int(box extent / out / gap) or 1 per axis of the box widened by the
+ *     filter's support, the box carried into the reduced frame; Pillow's vertical-pass-first rule for sources more than
+ *     100 times taller than wide; the C resize's passes for any box that does not start at 0 and end at the output size.
+ *   - boxes = NULL means (0, 0, S_w, S_h) and reducing_gaps = NULL no reduce; with both NULL this is
+ *     JPEGB200_batchCreateDraft, which forwards here.  Status, batchErrMcu, the walked intervals and the destination rules
+ *     are those of the same call without boxes and gaps.
+ *   - Filters are those of the resize (BILINEAR, BICUBIC, BOX).  Boxes or gaps without out_sizes return NULL with a message.
+ *     A view whose box or gap Pillow refuses (a box value that is not finite, a negative offset, past S_v or with a negative
+ *     extent, checked on the box as float; gap < 1), whose reduce would be empty or reduce boxes of 2^23 pixels or more,
+ *     gets JPEG_INVALID_PARAMETER alone.  A box past S_v is refused even where Pillow's reduce would carry it inside the
+ *     reduced image.
+ *   - The reduce and the boxed coefficient tables are timed in the JPEGB200_T_DITHER slot with the resize; the reduced
+ *     image counts in the one-call path's scratch bound. */
+JPEGB200_BATCH *JPEGB200_batchCreateBox(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                        const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                        const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                        const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
+                                        const double *reducing_gaps);
+/* Pillow's Image.thumbnail((req_w, req_h), BICUBIC, reducing_gap) decision for a W x H JPEG (reducing_gap 0 = None):
+ * preserve_aspect_ratio (floor or ceil of the exact side, whichever keeps W / H closer, floor on a tie, at least 1), the
+ * draft scale of the request int(req * gap) (JPEGB200_draftScale; 1 without a gap) and the box (0, 0, W / s, H / s).
+ * Writes *draft, *out_w x *out_h and box[4] such that JPEGB200_batchCreateBox with draft, out_sizes, boxes and reducing_gaps
+ * (the same gap) decodes the file's thumbnail.  Returns JPEGB200_THUMB_RESIZE; JPEGB200_THUMB_DRAFT when the draft decode is
+ * already the final size (Pillow stores it without a resize; box is then the whole drafted image); JPEGB200_THUMB_NONE when
+ * the request covers the file (Pillow leaves it alone: draft 1, the file's size, the whole image); 0 for a size or request
+ * below 1, a gap below 1 that is not 0, or a NULL output. */
+#define JPEGB200_THUMB_RESIZE 1
+#define JPEGB200_THUMB_DRAFT  2
+#define JPEGB200_THUMB_NONE   3
+int JPEGB200_thumbnailPlan(int width, int height, int req_w, int req_h, double reducing_gap, int *draft, int *out_w, int *out_h,
+                           double *box);
 void JPEGB200_batchDestroy(JPEGB200_BATCH *b);
 int JPEGB200_batchCount(JPEGB200_BATCH *b);
 /* per-image facts after batchCreate: status is JPEG_SUCCESS or the open() error the reference would give */
@@ -407,6 +443,13 @@ int JPEGB200_decodeBatchDraft(JPEGB200_CTX *ctx, const uint8_t *const *datas, co
                               const uint8_t *orients, const int32_t *out_sizes, int filter,
                               const JPEGB200_TensorSpec *spec, const uint8_t *draft, void *const *outs, const int64_t *pitches,
                               const int64_t *plane_strides, int flags, int32_t *status);
+/* The same with a box and a reducing gap per view (semantics of JPEGB200_batchCreateBox; both NULL =
+ * JPEGB200_decodeBatchDraft, which forwards here).  The reduced images count in the 1 GiB of scratch per job. */
+int JPEGB200_decodeBatchBox(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n, const int32_t *views,
+                            int pixel_type, int options, const int32_t *rois, const uint8_t *orients, const int32_t *out_sizes,
+                            int filter, const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
+                            const double *reducing_gaps, void *const *outs, const int64_t *pitches, const int64_t *plane_strides,
+                            int flags, int32_t *status);
 /* JPEGB200_NUM_COUNTERS counters summed over the jobs of the last JPEGB200_decodeBatch on this context */
 int JPEGB200_lastCallCounters(JPEGB200_CTX *ctx, int64_t *counters);
 /* CUDA-event stage times (JPEGB200_NUM_TIMINGS, ms) summed over those jobs, and how many jobs there were.  Jobs overlap

@@ -130,6 +130,14 @@ def lib():
                                             i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(C.c_uint8), C.POINTER(vp),
                                             C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int, i32p]
     L.JPEGB200_draftScale.argtypes = [C.c_int] * 4
+    dp = C.POINTER(C.c_double)
+    L.JPEGB200_batchCreateBox.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, i32p, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
+                                          i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(C.c_uint8), dp, dp]
+    L.JPEGB200_batchCreateBox.restype = vp
+    L.JPEGB200_decodeBatchBox.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, i32p, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
+                                          i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(C.c_uint8), dp, dp, C.POINTER(vp),
+                                          C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int, i32p]
+    L.JPEGB200_thumbnailPlan.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, ip, ip, ip, dp]
     L.JPEGB200_batchSetOutputTensor.argtypes = [vp, C.c_int, vp, C.c_int64, C.c_int64]
     L.JPEGB200_decodeBatchTensor.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
                                              i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(vp), C.POINTER(C.c_int64),
@@ -376,6 +384,43 @@ def draft_scale(width, height, req_w, req_h):
     return lib().JPEGB200_draftScale(int(width), int(height), int(req_w), int(req_h))
 
 
+def _box_array(box, n):
+    """one (x0, y0, x1, y1) for every image, or one per image -> double[4n] (None stays None = the whole image)"""
+    if box is None:
+        return None
+    box = list(box)
+    if len(box) == 4 and all(isinstance(v, (int, float, np.integer, np.floating)) for v in box):
+        box = [box] * n
+    flat = [float(v) for b in box for v in b]
+    if len(box) != n or len(flat) != 4 * n:
+        raise ValueError("box: one (x0, y0, x1, y1), or one per image (view)")
+    return (C.c_double * (4 * n))(*flat)
+
+
+def _gap_array(reducing_gap, n):
+    """one reducing gap for every image, or one per image (None = Pillow's None) -> double[n] (0 = None); None stays None"""
+    if reducing_gap is None:
+        return None
+    g = list(reducing_gap) if isinstance(reducing_gap, (list, tuple)) else [reducing_gap] * n
+    if len(g) != n:
+        raise ValueError("reducing_gap: one value, or one per image (view)")
+    return (C.c_double * n)(*[0.0 if v is None else float(v) for v in g])
+
+
+def thumbnail_plan(width, height, size, reducing_gap=2.0):
+    """Pillow's Image.thumbnail(size, BICUBIC, reducing_gap) decision for a width x height JPEG (JPEGB200_thumbnailPlan):
+    (draft, (w, h), box) such that draft=, out_sizes=, box= and the same reducing_gap= (with RESIZE_BICUBIC and
+    JPEGB200_OPT_LIBJPEG) decode the file's thumbnail.  Where Pillow stores the drafted image without a resize, or leaves
+    a file no larger than the request alone, box is the whole drafted image and (w, h) its size."""
+    d, w, h = C.c_int(), C.c_int(), C.c_int()
+    box = (C.c_double * 4)()
+    if not lib().JPEGB200_thumbnailPlan(int(width), int(height), int(size[0]), int(size[1]),
+                                        0.0 if reducing_gap is None else float(reducing_gap), C.byref(d), C.byref(w),
+                                        C.byref(h), box):
+        raise ValueError("thumbnail_plan: sizes and request must be at least 1 and reducing_gap None or at least 1.0")
+    return d.value, (w.value, h.value), tuple(box)
+
+
 def _orient_array(orients, n):
     """n EXIF transforms (0 = from the file, 1-8) -> uint8[n] for the C ABI (None stays None = no orientation)"""
     if orients is None:
@@ -407,10 +452,13 @@ class Batch:
     views: one view count per file (JPEGB200_batchCreateViews: file i's views come next to each other and share one
     entropy walk), or None for one per file; rois / orients / out_sizes and every per-image call are then per view, and
     self.n is the number of views.  draft: one scale denominator (1, 2, 4, 8) per image or view, each decoded as Pillow's
-    draft() at that scale (JPEGB200_batchCreateDraft; needs JPEGB200_OPT_LIBJPEG), or None."""
+    draft() at that scale (JPEGB200_batchCreateDraft; needs JPEGB200_OPT_LIBJPEG), or None.  box: one (x0, y0, x1, y1) of
+    doubles for every image or one per image, and reducing_gap: one value or one per image (None = Pillow's None): the
+    resize is then Pillow's resize(out_size, filter, box=box, reducing_gap=gap) of the unresized output
+    (JPEGB200_batchCreateBox; needs out_sizes)."""
 
     def __init__(self, ctx, ptrs, sizes, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
-                 filter=RESIZE_BILINEAR, spec=None, views=None, draft=None):
+                 filter=RESIZE_BILINEAR, spec=None, views=None, draft=None, box=None, reducing_gap=None):
         nf = len(ptrs)
         self._views, n = _views_array(views, nf)
         self.n = n
@@ -421,7 +469,14 @@ class Batch:
         self._out_sizes = _size_array(out_sizes, n)
         self.ctx = ctx
         self._draft = _draft_array(draft, n)
-        if draft is not None:
+        self._box, self._gap = _box_array(box, n), _gap_array(reducing_gap, n)
+        if box is not None or reducing_gap is not None:
+            self._spec = spec
+            self.h = lib().JPEGB200_batchCreateBox(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
+                                                   self._rois, self._orients, self._out_sizes, int(filter),
+                                                   C.byref(spec) if spec is not None else None, self._draft, self._box,
+                                                   self._gap)
+        elif draft is not None:
             self._spec = spec
             self.h = lib().JPEGB200_batchCreateDraft(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
                                                      self._rois, self._orients, self._out_sizes, int(filter),
@@ -510,13 +565,13 @@ class Batch:
 
 
 def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flags=0, rois=None, orients=None,
-                 out_sizes=None, filter=RESIZE_BILINEAR, views=None, draft=None):
+                 out_sizes=None, filter=RESIZE_BILINEAR, views=None, draft=None, box=None, reducing_gap=None):
     """JPEGB200_decodeBatch(ROI / Oriented / Resized / Views): one call for n files (host pointers) -> n outputs (host
     pointers, or device pointers with JPEGB200_OUT_DEVICE); rois: one (x, y, w, h) per image or None; orients: one EXIF
     transform per image (0 = from the file) or None; out_sizes: one (W, H) per image (resized with `filter`) or None.
     views: one view count per file, or None; outs, pitches and the per-image lists are then per view.  Returns (rc,
     per-image status list, counters summed over the internal jobs).  draft: one scale denominator per image (view), or
-    None (JPEGB200_decodeBatchDraft)."""
+    None (JPEGB200_decodeBatchDraft).  box / reducing_gap: as in Batch (JPEGB200_decodeBatchBox)."""
     nf = len(ptrs)
     va, n = _views_array(views, nf)
     pa = (C.c_void_p * nf)(*ptrs)
@@ -526,7 +581,12 @@ def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flag
     oa = (C.c_void_p * n)(*outs)
     pi = (C.c_int64 * n)(*pitches) if pitches is not None else None
     st = (C.c_int32 * n)()
-    if draft is not None:
+    if box is not None or reducing_gap is not None:
+        rc = lib().JPEGB200_decodeBatchBox(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
+                                           _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None,
+                                           _draft_array(draft, n), _box_array(box, n), _gap_array(reducing_gap, n), oa, pi,
+                                           None, flags, st)
+    elif draft is not None:
         rc = lib().JPEGB200_decodeBatchDraft(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
                                              _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None,
                                              _draft_array(draft, n), oa, pi, None, flags, st)
@@ -544,16 +604,16 @@ def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flag
 
 
 def decode_batch_to_host(ctx, jpegs, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
-                         filter=RESIZE_BILINEAR, views=None, draft=None):
+                         filter=RESIZE_BILINEAR, views=None, draft=None, box=None, reducing_gap=None):
     """Convenience: list of bytes -> list of numpy arrays [out_h, pitch_bytes] (uint8).
     One public-API call per batch with HOST buffers on both sides.  rois: one (x, y, w, h) per image (the arrays are then
     h rows of w pixels), or None.  orients: one EXIF transform per image (0 = from the file), or None.  out_sizes: one
     (W, H) per image (the arrays are then H rows of W pixels, resized with `filter`), or None.  views: one view count
     per file, or None; the lists (and rois / orients / out_sizes) are then per view.  draft: one scale denominator per
-    image (view), or None."""
+    image (view), or None.  box / reducing_gap: as in Batch."""
     bufs = [np.frombuffer(j, dtype=np.uint8) for j in jpegs]
     b = Batch(ctx, [x.ctypes.data for x in bufs], [len(x) for x in bufs], pixel_type, options, rois, orients, out_sizes,
-              filter, views=views, draft=draft)
+              filter, views=views, draft=draft, box=box, reducing_gap=reducing_gap)
     try:
         outs = []
         for i in range(b.n):
@@ -601,7 +661,7 @@ def tensor_spec(dtype, layout="CHW", scale="div255", mean=(0.0, 0.0, 0.0), std=(
 
 def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, orients=None, out_sizes=None,
                         filter=RESIZE_BILINEAR, dtype=None, layout="CHW", scale="div255", mean=(0.0, 0.0, 0.0),
-                        std=(1.0, 1.0, 1.0), bgr=False, out=None, views=None, draft=None):
+                        std=(1.0, 1.0, 1.0), bgr=False, out=None, views=None, draft=None, box=None, reducing_gap=None):
     """JPEGB200_decodeBatchTensor: list of bytes -> the model's input tensor on the context's GPU, and the status list.
 
     Image i becomes a C x H x W (layout "CHW") or H x W x C ("HWC") tensor of `dtype` (torch.float32 by default, float16,
@@ -614,7 +674,7 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     views: one view count per file (JPEGB200_decodeBatchViews: the views of a file share one entropy walk), or None; the
     images are then the views: rois / orients / out_sizes / out and the result ([V, C, H, W], or a list) are per view.
     draft: one scale denominator (1, 2, 4, 8) per image (view), Pillow's draft() at that scale (JPEGB200_decodeBatchDraft),
-    or None."""
+    or None.  box / reducing_gap: as in Batch (JPEGB200_decodeBatchBox)."""
     import torch
     dtype = torch.float32 if dtype is None else dtype
     spec = tensor_spec(dtype, layout, scale, mean, std, bgr)
@@ -669,10 +729,11 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     st = (C.c_int32 * n)()
     with torch.cuda.device(dev):
         torch.cuda.current_stream(dev).synchronize()   # the library's streams do not order against torch's
-        rc = lib().JPEGB200_decodeBatchDraft(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
-                                             _orient_array(orients, n), _size_array(out_sizes, n), int(filter),
-                                             C.byref(spec), _draft_array(draft, n), (C.c_void_p * n)(*ptr_l),
-                                             (C.c_int64 * n)(*pitch_l), (C.c_int64 * n)(*plane_l), JPEGB200_OUT_DEVICE, st)
+        rc = lib().JPEGB200_decodeBatchBox(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
+                                           _orient_array(orients, n), _size_array(out_sizes, n), int(filter),
+                                           C.byref(spec), _draft_array(draft, n), _box_array(box, n),
+                                           _gap_array(reducing_gap, n), (C.c_void_p * n)(*ptr_l), (C.c_int64 * n)(*pitch_l),
+                                           (C.c_int64 * n)(*plane_l), JPEGB200_OUT_DEVICE, st)
     if rc == 0:
         raise RuntimeError("decodeBatchViews failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
     return out, list(st)

@@ -169,6 +169,12 @@ struct JPEGB200_BATCH {
     DevBuf<uint8_t> d_rs;
     DevBuf<int32_t> d_rs_coef;
     DevBuf<JDResizeDesc> d_rs_desc;
+    /* box resize (JPEGB200_batchCreateBox with boxes or gaps): every view resizes through its box plan; a reduce writes the
+     * resize source after S in d_rs */
+    bool box = false;
+    std::vector<JDBoxPlan> bx_plans;
+    std::vector<JDBoxDesc> bx_desc;
+    DevBuf<JDBoxDesc> d_bx_desc;
     /* tensor output (JPEGB200_batchCreateTensor): descs hold the row bytes as out_pitch; the pipeline (IDCT or resize) writes
      * U (out_w x out_h, tn_bpp bytes per pixel) tightly into d_tn, jdk_tensor writes the destination */
     bool tensor = false;
@@ -548,6 +554,7 @@ struct CreatePlan {
     const uint8_t *orients = nullptr;
     const JPEGB200_TensorSpec *spec = nullptr;
     const uint8_t *draft = nullptr;     /* per view: draft scale denominator (JPEGB200_batchCreateDraft), NULL = 1 */
+    const double *boxes = nullptr, *gaps = nullptr;   /* per view: resize box and reducing gap (JPEGB200_batchCreateBox) */
     /* where the next file's restart segments, blocks and records start; where the next view's output and gray stage start */
     uint32_t seg = 0;
     uint64_t blk = 0, rec_total = 0;
@@ -594,6 +601,8 @@ static void init_batch(JPEGB200_BATCH *b, JPEGB200_CTX *ctx, const CreatePlan &P
         b->rs_plans.assign(nv, JDResizePlan{});
         b->rs_src_w.assign(nv, 0); b->rs_src_h.assign(nv, 0); b->rs_scratch.assign(nv, 0);
     }
+    b->box = P.boxes != nullptr || P.gaps != nullptr;
+    if (b->box) b->bx_plans.assign(nv, JDBoxPlan{});
     b->lj = (options & JPEGB200_OPT_LIBJPEG) != 0;
     if (b->lj) { b->lj_desc.assign(nv, JDLjDesc{}); b->lj_plane.assign(nv, 0); }
     b->tensor = P.spec != nullptr;
@@ -738,6 +747,31 @@ static uint32_t plan_views(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int 
             const int32_t r[4] = {sr[0], sr[1], P.orients ? sr[2] : P.rois[4 * (size_t)i + 2], P.orients ? sr[3] : P.rois[4 * (size_t)i + 3]};
             jd_lj_plan_extend_s(inf.width, inf.height, inf.subsample, inf.restart_interval, (int)b->lj_desc[i].shift, r, &b->plans[i]);
             if ((uint32_t)b->plans[i].nseg_walk > walk) walk = (uint32_t)b->plans[i].nseg_walk;
+        }
+    }
+    if (walk != 0 && b->box) {
+        /* each valid view's box and gap on S, its output before the resize; a refused view leaves the walk to the others */
+        bool dropped = false;
+        for (int i = v0; i < v0 + nvf; i++) {
+            if (!P.vok[i]) continue;
+            const int s = b->lj ? (int)b->lj_desc[i].shift : b->sshift;
+            const int sw = b->roi ? b->plans[i].out_w : (inf.width + (1 << s) - 1) >> s;
+            const int sh = b->roi ? b->plans[i].out_h : (inf.height + (1 << s) - 1) >> s;
+            const double whole[4] = {0.0, 0.0, (double)sw, (double)sh};
+            if (!jd_box_plan(sw, sh, P.out_sizes[2 * (size_t)i], P.out_sizes[2 * (size_t)i + 1], b->rs_filter,
+                             P.boxes ? P.boxes + 4 * (size_t)i : whole, P.gaps ? P.gaps[i] : 0.0, bytes_per_pixel_class(b->ptclass),
+                             &b->bx_plans[i])) {
+                P.vok[i] = 0;
+                dropped = true;
+            }
+        }
+        if (dropped) {   /* without a rectangle every view walks the whole file */
+            uint32_t kept = 0;
+            for (int i = v0; i < v0 + nvf; i++) {
+                const uint32_t w = b->roi ? (uint32_t)b->plans[i].nseg_walk : walk;
+                if (P.vok[i] && w > kept) kept = w;
+            }
+            walk = kept;
         }
     }
     return walk;
@@ -931,12 +965,15 @@ static int plan_view_output(JPEGB200_BATCH *b, CreatePlan &P, int f, int i)
         const int bp = bytes_per_pixel_class(b->ptclass);
         JDResizePlan &rp = b->rs_plans[i];
         const int32_t rw = P.out_sizes[2 * (size_t)i], rh = P.out_sizes[2 * (size_t)i + 1];
-        if (!jd_resize_plan((int)vd.out_w, (int)vd.out_h, rw, rh, b->rs_filter, bp, &rp)) {
+        if (b->box) rp = b->bx_plans[i].rp;   /* planned with the box by plan_views */
+        else if (!jd_resize_plan((int)vd.out_w, (int)vd.out_h, rw, rh, b->rs_filter, bp, &rp)) {
             snprintf(g_err, sizeof(g_err), "resize plan failed for image %d", i);
             return 0;
         }
         b->rs_src_w[i] = vd.out_w; b->rs_src_h[i] = vd.out_h;
         b->rs_scratch[i] = (int64_t)align256((size_t)vd.out_w * vd.out_h * bp) + (int64_t)align256((size_t)rp.mid_bytes);
+        if (b->box && (b->bx_plans[i].fx > 1 || b->bx_plans[i].fy > 1))   /* the reduced image */
+            b->rs_scratch[i] += (int64_t)align256((size_t)b->bx_plans[i].rw * b->bx_plans[i].rh * bp);
         b->rs_scratch_total += b->rs_scratch[i];
         vd.out_w = (uint32_t)rw; vd.out_h = (uint32_t)rh;
     }
@@ -1050,17 +1087,27 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateDraft(JPEGB200_CTX *ctx, const ui
                                                      const uint8_t *orients, const int32_t *out_sizes, int filter,
                                                      const JPEGB200_TensorSpec *spec, const uint8_t *draft)
 {
+    return JPEGB200_batchCreateBox(ctx, datas, sizes, n, views, pixel_type, options, rois, orients, out_sizes, filter, spec, draft,
+                                   nullptr, nullptr);
+}
+
+extern "C" JPEGB200_BATCH *JPEGB200_batchCreateBox(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                                   const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                                   const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                                   const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
+                                                   const double *reducing_gaps)
+{
     if (!ctx) { snprintf(g_err, sizeof(g_err), "invalid parameter"); return nullptr; }
     int64_t nv = 0;   /* images of the batch: views */
     if (!jd_check_batch_features(pixel_type, options, n, views, rois != nullptr, orients != nullptr, out_sizes != nullptr, filter, spec,
                                  &nv, g_err, (int)sizeof(g_err)) ||
-        !jd_check_draft(options, draft, g_err, (int)sizeof(g_err)))
+        !jd_check_draft(options, draft, g_err, (int)sizeof(g_err)) || !jd_check_box(out_sizes, boxes, reducing_gaps, g_err, (int)sizeof(g_err)))
         return nullptr;
     JPEGB200_BATCH *b = new (std::nothrow) JPEGB200_BATCH();
     if (!b) return nullptr;
     CreatePlan P;
     P.datas = datas; P.sizes = sizes; P.views = views; P.rois = rois; P.orients = orients; P.out_sizes = out_sizes; P.spec = spec;
-    P.draft = draft;
+    P.draft = draft; P.boxes = boxes; P.gaps = reducing_gaps;
     P.srects.assign(4 * (size_t)nv, 0); P.vok.assign((size_t)nv, 0);
     P.ks.assign(orients ? (size_t)nv : 0u, 0);
     if (options & JPEGB200_OPT_PROGRESSIVE) { P.fscans.resize(JD_PROG_MAX_SCANS); P.ftabs.resize(JD_PROG_MAX_TABS); }
@@ -1437,6 +1484,7 @@ struct DecodeState {
     uint8_t *pipe_out = nullptr;            /* where the pixel pipeline (IDCT, resize) writes: out_base, or the tensor staging */
     uint8_t *stage_out = nullptr;           /* where the IDCT stage writes: pipe_out, or the gray stage / the resize source */
     uint32_t tn_ctas = 0, rs_ctas[4] = {0u, 0u, 0u, 0u};
+    uint32_t bx_ctas[2] = {0u, 0u};         /* box batches: jdk_resize_coeffs_box, jdk_reduce */
     int launches = 0;
 };
 
@@ -1556,19 +1604,38 @@ static int stage_resize(JPEGB200_BATCH *b, DecodeState &D)
     const int n = b->n;
     const int bp = bytes_per_pixel_class(b->ptclass);
     b->rs_desc.assign(n, JDResizeDesc{});
-    uint64_t so = 0, co = 0, ctas[4] = {0, 0, 0, 0};
+    if (b->box) b->bx_desc.assign(n, JDBoxDesc{});
+    uint64_t so = 0, co = 0, ctas[4] = {0, 0, 0, 0}, bx_ctas[2] = {0, 0};
     for (int i = 0; i < n; i++) {
         JDResizeDesc &r = b->rs_desc[i];
         r.blk_c = (uint32_t)ctas[0]; r.blk_h = (uint32_t)ctas[1]; r.blk_v = (uint32_t)ctas[2]; r.blk_h2 = (uint32_t)ctas[3];
+        if (b->box) { b->bx_desc[i].blk_c = (uint32_t)bx_ctas[0]; b->bx_desc[i].blk_r = (uint32_t)bx_ctas[1]; }
         if (b->parse_status[i] != JPEG_SUCCESS) continue;
         const JDResizePlan &rp = b->rs_plans[i];
-        r.src_w = b->rs_src_w[i]; r.src_h = b->rs_src_h[i]; r.dst_w = b->descs[i].out_w; r.dst_h = b->descs[i].out_h;
+        const uint32_t sw = b->rs_src_w[i], sh = b->rs_src_h[i];   /* S, where the IDCT stage writes */
+        r.src_w = sw; r.src_h = sh; r.dst_w = b->descs[i].out_w; r.dst_h = b->descs[i].out_h;
         r.dst_off = D.descs_stage[i].out_off; r.dst_pitch = D.descs_stage[i].out_pitch;
         r.ksize_h = (uint32_t)rp.ksize_h; r.ksize_v = (uint32_t)rp.ksize_v;
         r.ybox0 = (uint32_t)rp.ybox0; r.rows = (uint32_t)rp.rows;
         r.flags = (rp.need_h ? 1u : 0u) | (rp.need_v ? 2u : 0u) | (rp.vfirst ? 4u : 0u);
         r.src_off = so;
-        so += align256((size_t)r.src_w * r.src_h * bp);
+        so += align256((size_t)sw * sh * bp);
+        if (b->box) {
+            /* the resize reads the reduced image (written after S), or S itself */
+            const JDBoxPlan &p = b->bx_plans[i];
+            JDBoxDesc &x = b->bx_desc[i];
+            x.s_off = r.src_off; x.s_w = sw;
+            for (int k = 0; k < 4; k++) x.box[k] = p.box[k];
+            x.rx0 = (uint32_t)p.rx0; x.ry0 = (uint32_t)p.ry0; x.rbw = (uint32_t)(p.rx1 - p.rx0); x.rbh = (uint32_t)(p.ry1 - p.ry0);
+            x.fx = (uint32_t)p.fx; x.fy = (uint32_t)p.fy;
+            r.src_w = (uint32_t)p.rw; r.src_h = (uint32_t)p.rh;
+            if (p.fx > 1 || p.fy > 1) {
+                r.src_off = so;
+                so += align256((size_t)r.src_w * r.src_h * bp);
+                bx_ctas[1] += ((uint64_t)r.src_w * r.src_h + JD_RS_THREADS - 1) / JD_RS_THREADS;
+            }
+            bx_ctas[0] += ((rp.need_h ? r.dst_w : 0u) + (rp.need_v ? r.dst_h : 0u) + JD_RS_THREADS - 1) / JD_RS_THREADS;
+        }
         r.mid_off = so;
         so += align256((size_t)rp.mid_bytes);
         r.coef_h = co;
@@ -1576,25 +1643,30 @@ static int stage_resize(JPEGB200_BATCH *b, DecodeState &D)
         r.coef_v = co;
         co += rp.need_v ? (uint64_t)r.dst_h * (r.ksize_v + 2) : 0;
         const uint64_t q = ((rp.vfirst ? r.src_w : r.dst_w) + 16 / bp - 1) / (16 / bp);
-        ctas[0] += ((rp.need_h ? r.dst_w : 0u) + (rp.need_v ? r.dst_h : 0u) + JD_RS_THREADS - 1) / JD_RS_THREADS;
+        if (!b->box) ctas[0] += ((rp.need_h ? r.dst_w : 0u) + (rp.need_v ? r.dst_h : 0u) + JD_RS_THREADS - 1) / JD_RS_THREADS;
         if (rp.need_h && !rp.vfirst)   /* jdk_resize_h<4, 0>: one thread per pixel; <1, 0>: column chunks x row blocks */
             ctas[1] += bp == 4 ? ((uint64_t)r.rows * r.dst_w + JD_RS_THREADS - 1) / JD_RS_THREADS
                                : (uint64_t)((r.dst_w + JD_RS_HCOLS - 1) / JD_RS_HCOLS) * ((r.rows + JD_RS_HROWS - 1) / JD_RS_HROWS);
         ctas[2] += (q * r.dst_h + JD_RS_THREADS - 1) / JD_RS_THREADS;
         ctas[3] += rp.vfirst ? ((uint64_t)r.dst_h * r.dst_w + JD_RS_THREADS - 1) / JD_RS_THREADS : 0;
-        D.descs_stage[i].out_off = r.src_off;
-        D.descs_stage[i].out_pitch = r.src_w * (uint32_t)bp;
-        D.descs_stage[i].out_w = r.src_w; D.descs_stage[i].out_h = r.src_h;
+        D.descs_stage[i].out_off = b->box ? b->bx_desc[i].s_off : r.src_off;
+        D.descs_stage[i].out_pitch = sw * (uint32_t)bp;
+        D.descs_stage[i].out_w = sw; D.descs_stage[i].out_h = sh;
     }
-    if (ctas[1] >= (1ull << 31) || ctas[2] >= (1ull << 31) || ctas[3] >= (1ull << 31)) {
+    if (ctas[1] >= (1ull << 31) || ctas[2] >= (1ull << 31) || ctas[3] >= (1ull << 31) || bx_ctas[1] >= (1ull << 31)) {
         snprintf(g_err, sizeof(g_err), "resize: too many output pixels in one job");
         return 0;
     }
     for (int c = 0; c < 4; c++) D.rs_ctas[c] = (uint32_t)ctas[c];
+    D.bx_ctas[0] = (uint32_t)bx_ctas[0]; D.bx_ctas[1] = (uint32_t)bx_ctas[1];
     CK(b->d_rs.alloc(&b->ctx->pool, so + 256));
     CK(b->d_rs_coef.alloc(&b->ctx->pool, co + 64));
     CK(b->d_rs_desc.alloc(&b->ctx->pool, n));
     CK(cudaMemcpyAsync(b->d_rs_desc.p, b->rs_desc.data(), sizeof(JDResizeDesc) * n, cudaMemcpyHostToDevice, b->ss.stream));
+    if (b->box) {
+        CK(b->d_bx_desc.alloc(&b->ctx->pool, n));
+        CK(cudaMemcpyAsync(b->d_bx_desc.p, b->bx_desc.data(), sizeof(JDBoxDesc) * n, cudaMemcpyHostToDevice, b->ss.stream));
+    }
     return 1;
 }
 
@@ -1971,6 +2043,15 @@ static void run_resize(JPEGB200_BATCH *b, DecodeState &D)
     const bool gray = b->ptclass == JD_PT_GRAY;
     const uint32_t *rs_ctas = D.rs_ctas;
     if (rs_ctas[0]) { jdk_resize_coeffs<<<rs_ctas[0], JD_RS_THREADS, 0, st>>>(b->d_rs_desc.p, n, b->d_rs_coef.p, b->rs_filter); D.launches++; }
+    if (D.bx_ctas[1]) {   /* box batches: the reduce of S into the resize source, then the boxed tables */
+        if (gray) jdk_reduce<1><<<D.bx_ctas[1], JD_RS_THREADS, 0, st>>>(b->d_rs_desc.p, b->d_bx_desc.p, n, b->d_rs.p);
+        else jdk_reduce<4><<<D.bx_ctas[1], JD_RS_THREADS, 0, st>>>(b->d_rs_desc.p, b->d_bx_desc.p, n, b->d_rs.p);
+        D.launches++;
+    }
+    if (D.bx_ctas[0]) {
+        jdk_resize_coeffs_box<<<D.bx_ctas[0], JD_RS_THREADS, 0, st>>>(b->d_rs_desc.p, b->d_bx_desc.p, n, b->d_rs_coef.p, b->rs_filter);
+        D.launches++;
+    }
 #define JD_RS_ARGS b->d_rs_desc.p, n, b->d_rs.p, b->d_rs_coef.p, D.pipe_out
     if (rs_ctas[1]) {
         if (gray) jdk_resize_h<1, 0><<<rs_ctas[1], JD_RS_THREADS, 0, st>>>(JD_RS_ARGS);
@@ -2268,6 +2349,17 @@ extern "C" int JPEGB200_decodeBatchDraft(JPEGB200_CTX *ctx, const uint8_t *const
                                          const JPEGB200_TensorSpec *spec, const uint8_t *draft, void *const *outs,
                                          const int64_t *pitches, const int64_t *plane_strides, int flags, int32_t *status)
 {
+    return JPEGB200_decodeBatchBox(ctx, datas, sizes, n, views, pixel_type, options, rois, orients, out_sizes, filter, spec, draft,
+                                   nullptr, nullptr, outs, pitches, plane_strides, flags, status);
+}
+
+extern "C" int JPEGB200_decodeBatchBox(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                       const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                       const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                       const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
+                                       const double *reducing_gaps, void *const *outs, const int64_t *pitches,
+                                       const int64_t *plane_strides, int flags, int32_t *status)
+{
     if (!ctx || n <= 0) return 0;
     const int64_t nv = jd_count_views(n, views, "call", g_err, (int)sizeof(g_err));   /* images (views) of the call */
     if (nv < 0) return 0;
@@ -2314,9 +2406,10 @@ extern "C" int JPEGB200_decodeBatchDraft(JPEGB200_CTX *ctx, const uint8_t *const
         const int32_t *vi = views ? views + i0 : nullptr;
         int cnt = jd_job_files(n - i0, sizes + i0, vi, maxcnt, limit, nullptr, 0, &cv, &capped);
         auto create = [&](int c) {
-            return JPEGB200_batchCreateDraft(ctx, datas + i0, sizes + i0, c, vi, pixel_type, options, rois ? rois + 4 * (size_t)v0 : nullptr,
-                                             orients ? orients + v0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)v0 : nullptr, filter, spec,
-                                             draft ? draft + v0 : nullptr);
+            return JPEGB200_batchCreateBox(ctx, datas + i0, sizes + i0, c, vi, pixel_type, options, rois ? rois + 4 * (size_t)v0 : nullptr,
+                                           orients ? orients + v0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)v0 : nullptr, filter, spec,
+                                           draft ? draft + v0 : nullptr, boxes ? boxes + 4 * (size_t)v0 : nullptr,
+                                           reducing_gaps ? reducing_gaps + v0 : nullptr);
         };
         JPEGB200_BATCH *b = create(cnt);
         if (!b) { rc = 0; break; }
@@ -2340,7 +2433,7 @@ extern "C" int JPEGB200_decodeBatchDraft(JPEGB200_CTX *ctx, const uint8_t *const
         }
         if ((b->resize || b->tensor || b->pplane_total || b->lj) && cnt > 1 &&
             b->rs_scratch_total + b->tn_stage_total + b->pplane_total + b->lj_plane_total > JD_JOB_RESIZE_SCRATCH) {
-            /* scratch of a job (resize: S + intermediate; tensor: the uint8 staging; libjpeg decodes: the sample planes;
+            /* scratch of a job (resize: S + the reduced image of a box batch + intermediate; tensor: the uint8 staging; libjpeg decodes: the sample planes;
              * progressive files: the coefficient plane, counted on the file's first view): at most JD_JOB_RESIZE_SCRATCH, or
              * one file with all of its views */
             std::vector<int64_t> sc(cv);

@@ -13,6 +13,7 @@
 #include <math.h>
 #include "jd_internal.h"
 #include "jd_resize.h"
+#include "jd_reduce.h"
 
 #define HUFF_TABLEN 273 /* reference src/JPEGDEC.h:58: stride of one DHT table in the scratch area */
 
@@ -677,6 +678,102 @@ int jd_resize_plan(int src_w, int src_h, int out_w, int out_h, int filter, int b
     plan->coef_words = (plan->need_h ? (int64_t)out_w * (plan->ksize_h + 2) : 0) +
                        (plan->need_v ? (int64_t)out_h * (plan->ksize_v + 2) : 0);
     return 1;
+}
+
+/* Box plan (JDBoxPlan): Image.resize's Python steps in double (jd_internal.h), then the C resize's pass choice and row box
+ * for the float box, like jd_resize_plan */
+int jd_box_plan(int sw, int sh, int out_w, int out_h, int filter, const double *box, double gap, int bytes_per_pixel, JDBoxPlan *p)
+{
+    if (!jd_rs_filter_ok(filter) || sw < 1 || sh < 1 || sw > 65535 || sh > 65535 || out_w < 1 || out_h < 1 || out_w > 65535 ||
+        out_h > 65535 || !isfinite(gap) || (gap != 0.0 && gap < 1.0)) return 0;
+    for (int k = 0; k < 4; k++)   /* anything outside [0, 2^17] is past the image (and stays inside int and float) */
+        if (!isfinite(box[k]) || box[k] < 0.0 || box[k] > 131072.0) return 0;
+    const float f0 = (float)box[0], f1 = (float)box[1], f2 = (float)box[2], f3 = (float)box[3];
+    if (f0 < 0.0f || f1 < 0.0f || f2 > (float)sw || f3 > (float)sh || f2 < f0 || f3 < f1) return 0;
+    double b[4] = {box[0], box[1], box[2], box[3]};
+    p->fx = p->fy = 1;
+    p->rx0 = p->ry0 = 0; p->rx1 = sw; p->ry1 = sh;
+    if (gap != 0.0) {
+        int fx = (int)((box[2] - box[0]) / out_w / gap), fy = (int)((box[3] - box[1]) / out_h / gap);
+        if (fx == 0) fx = 1;
+        if (fy == 0) fy = 1;
+        if (fx > 1 || fy > 1) {
+            /* _get_safe_box: the box widened by (support - 0.5) x scale, int() at the low end, ceil at the high end */
+            const double fs = jd_rs_support(filter) - 0.5;
+            const double sx = fs * ((box[2] - box[0]) / out_w), sy = fs * ((box[3] - box[1]) / out_h);
+            const int x0 = (int)(box[0] - sx), y0 = (int)(box[1] - sy);
+            const double x1 = ceil(box[2] + sx), y1 = ceil(box[3] + sy);
+            p->rx0 = x0 > 0 ? x0 : 0; p->ry0 = y0 > 0 ? y0 : 0;
+            p->rx1 = x1 < sw ? (int)x1 : sw; p->ry1 = y1 < sh ? (int)y1 : sh;
+            if (p->rx1 <= p->rx0 || p->ry1 <= p->ry0 || (int64_t)fx * fy >= (1 << 23)) return 0;
+            p->fx = fx; p->fy = fy;
+            b[0] = (box[0] - p->rx0) / fx; b[1] = (box[1] - p->ry0) / fy;
+            b[2] = (box[2] - p->rx0) / fx; b[3] = (box[3] - p->ry0) / fy;
+        }
+    }
+    p->rw = (p->rx1 - p->rx0 + p->fx - 1) / p->fx;
+    p->rh = (p->ry1 - p->ry0 + p->fy - 1) / p->fy;
+    for (int k = 0; k < 4; k++) p->box[k] = (float)b[k];
+    const float *fb = p->box;
+    JDResizePlan *rp = &p->rp;
+    rp->need_h = out_w != p->rw || fb[0] != 0.0f || fb[2] != (float)out_w;
+    rp->need_v = out_h != p->rh || fb[1] != 0.0f || fb[3] != (float)out_h;
+    rp->ksize_h = jd_rs_ksize_box(fb[0], fb[2], out_w, filter);
+    rp->ksize_v = jd_rs_ksize_box(fb[1], fb[3], out_h, filter);
+    int32_t y0, n0, y1, n1;
+    jd_rs_bounds_box(p->rh, fb[1], fb[3], out_h, filter, 0, &y0, &n0);
+    jd_rs_bounds_box(p->rh, fb[1], fb[3], out_h, filter, out_h - 1, &y1, &n1);
+    rp->ybox0 = rp->need_v ? y0 : 0;
+    rp->rows = rp->need_v ? y1 + n1 - y0 : p->rh;
+    rp->vfirst = rp->need_h && rp->need_v && out_h < p->rh && (int64_t)p->rh > 100 * (int64_t)p->rw;
+    if (rp->vfirst) rp->mid_bytes = (int64_t)out_h * p->rw * bytes_per_pixel;
+    else rp->mid_bytes = rp->need_h ? (int64_t)rp->rows * out_w * bytes_per_pixel : 0;
+    rp->coef_words = (rp->need_h ? (int64_t)out_w * (rp->ksize_h + 2) : 0) + (rp->need_v ? (int64_t)out_h * (rp->ksize_v + 2) : 0);
+    return 1;
+}
+
+int jd_check_box(const int32_t *out_sizes, const double *boxes, const double *gaps, char *msg, int msg_len)
+{
+    if ((boxes || gaps) && !out_sizes) {
+        snprintf(msg, (size_t)msg_len, "boxes and reducing gaps need out_sizes (they describe a resize)");
+        return 0;
+    }
+    return 1;
+}
+
+/* Pillow's Image.thumbnail(size, BICUBIC, reducing_gap) decision for a W x H JPEG (include/jpegdec_b200.h) */
+int JPEGB200_thumbnailPlan(int width, int height, int req_w, int req_h, double reducing_gap, int *draft, int *out_w, int *out_h,
+                           double *box)
+{
+    if (width < 1 || height < 1 || req_w < 1 || req_h < 1 || !isfinite(reducing_gap) || (reducing_gap != 0.0 && reducing_gap < 1.0) ||
+        !draft || !out_w || !out_h || !box) return 0;
+    *draft = 1; *out_w = width; *out_h = height;
+    box[0] = box[1] = 0.0; box[2] = width; box[3] = height;
+    if (req_w >= width && req_h >= height) return JPEGB200_THUMB_NONE;
+    /* preserve_aspect_ratio: floor or ceil of the exact side, whichever keeps the aspect closer (floor on a tie), at least 1 */
+    const double aspect = (double)width / height;
+    int x = req_w, y = req_h;
+    if ((double)x / y >= aspect) {
+        const double num = y * aspect, fl = floor(num), ce = ceil(num);
+        const double r = fabs(aspect - ce / y) < fabs(aspect - fl / y) ? ce : fl;
+        x = r < 1.0 ? 1 : (int)r;
+    } else {
+        const double num = x / aspect, fl = floor(num), ce = ceil(num);
+        const double kf = fl == 0.0 ? 0.0 : fabs(aspect - x / fl), kc = ce == 0.0 ? 0.0 : fabs(aspect - x / ce);
+        const double r = kc < kf ? ce : fl;
+        y = r < 1.0 ? 1 : (int)r;
+    }
+    *out_w = x; *out_h = y;
+    int s = 1;
+    if (reducing_gap != 0.0) {   /* draft(None, (int(req_w * gap), int(req_h * gap))) */
+        const double qw = req_w * reducing_gap, qh = req_h * reducing_gap;
+        s = JPEGB200_draftScale(width, height, qw >= 2147483647.0 ? 2147483647 : (int)qw, qh >= 2147483647.0 ? 2147483647 : (int)qh);
+        box[2] = (double)width / s; box[3] = (double)height / s;
+    }
+    *draft = s;
+    const int dw = (width + s - 1) / s, dh = (height + s - 1) / s;
+    if (dw == x && dh == y) { box[2] = dw; box[3] = dh; return JPEGB200_THUMB_DRAFT; }
+    return JPEGB200_THUMB_RESIZE;
 }
 
 /* A caller's output for one image.  Host and device: a pitch below the row bytes would make rows overlap (and the last

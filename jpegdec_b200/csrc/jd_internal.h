@@ -147,6 +147,27 @@ typedef struct {
 /* Returns 0 for a filter other than JPEGB200_RESIZE_* or a size outside 1..65535. */
 int jd_resize_plan(int src_w, int src_h, int out_w, int out_h, int filter, int bytes_per_pixel, JDResizePlan *plan);
 
+/* Box resize of one view (JPEGB200_batchCreateBox): Pillow's resize(out, filter, box, reducing_gap) of S (sw x sh) as its
+ * Python code decides it, in double: factor = int(box extent / out / gap) or 1 per axis; with a factor above 1 the region
+ * _get_safe_box(out, filter, box) of S is reduced (jd_reduce.h) and the box carried into the reduced frame; then the C
+ * resize of the resize source (the reduced image, or S) with that box as float, vertical pass first for a source more
+ * than 100 times taller than wide that shrinks vertically (two calls in Pillow, the same passes here). */
+typedef struct {
+    int32_t fx, fy;             /* reduce factors; 1 x 1 = no reduce */
+    int32_t rx0, ry0, rx1, ry1; /* the reduced region of S (the safe box), S itself without a reduce */
+    int32_t rw, rh;             /* the resize source: ceil(region / factor) */
+    float box[4];               /* x0, y0, x1, y1 of the resize in the source's frame, as Pillow's C resize receives it */
+    JDResizePlan rp;            /* the passes from the source to out_w x out_h: need_h / need_v are true for any box that
+                                 * does not start at 0 and end at the output size (Pillow's C test) */
+} JDBoxPlan;
+/* box: x0, y0, x1, y1 in S; gap: reducing_gap, 0 = None.  Returns 0 for what Pillow refuses with a ValueError (a box
+ * value that is not finite, a float box with a negative offset, past sw / sh or with a negative extent, gap < 1), for a
+ * reduce to an empty image or of boxes of 2^23 pixels or more, and for jd_resize_plan's refusals.  The box is checked in
+ * S's frame: one past the edge is refused even where Pillow's reduce would carry it inside the reduced image. */
+int jd_box_plan(int sw, int sh, int out_w, int out_h, int filter, const double *box, double gap, int bytes_per_pixel, JDBoxPlan *plan);
+/* Batch-level rule of JPEGB200_batchCreateBox: boxes or reducing_gaps need out_sizes.  0 with a message otherwise. */
+int jd_check_box(const int32_t *out_sizes, const double *boxes, const double *gaps, char *msg, int msg_len);
+
 /* Coefficient records an image's entropy walks can address above its record base: the largest JD_REC_INDEX + JD_REC_CAP
  * (jd_core.h) over its restart segments (slots 0 .. nseg - 1, each ending at or before the file's end) and the chunks of a
  * restart-free scan (slots nseg .. nseg + nch - 1, 512 bytes each from scan_offset), computed in 64 bits.  Those indices

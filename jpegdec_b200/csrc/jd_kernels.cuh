@@ -2079,6 +2079,81 @@ __global__ void __launch_bounds__(JD_RS_THREADS) jdk_resize_v(const JDResizeDesc
 }
 
 /* ------------------------------------------------------------------------------------ */
+/* Box resize (JPEGB200_batchCreateBox, jd_reduce.h): the IDCT stage has written S tightly  */
+/* at s_off; jdk_reduce writes the reduced image where the JDResizeDesc's source lies, and  */
+/* jdk_resize_coeffs_box the tables for the box.  jdk_resize_h / _v then run unchanged: the */
+/* tables carry absolute first taps.  A view without a reduce resizes S itself.             */
+/* ------------------------------------------------------------------------------------ */
+#include "jd_reduce.h"
+
+struct JDBoxDesc {
+    uint64_t s_off;            /* S (s_w wide, tight) in the scratch */
+    float box[4];              /* x0, y0, x1, y1 of the resize in its source's frame (JDResizeDesc src_w x src_h) */
+    uint32_t s_w;
+    uint32_t rx0, ry0, rbw, rbh;  /* the reduced region of S */
+    uint32_t fx, fy;           /* reduce factors (1 x 1: no reduce, no CTAs in jdk_reduce) */
+    uint32_t blk_c, blk_r;     /* first CTA of this view in jdk_resize_coeffs_box and jdk_reduce */
+};
+
+template <int F>
+__device__ __forceinline__ uint32_t jd_bx_find(const JDBoxDesc *bd, uint32_t n, uint32_t b)
+{
+    uint32_t lo = 0, hi = n - 1;   /* as jd_rs_find */
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if ((F == 0 ? bd[mid].blk_c : bd[mid].blk_r) <= b) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+/* jdk_resize_coeffs for boxed views: one thread per output column and per output row */
+__global__ void __launch_bounds__(JD_RS_THREADS) jdk_resize_coeffs_box(const JDResizeDesc *rd, const JDBoxDesc *bd, uint32_t n,
+                                                                       int32_t *coef, int filter)
+{
+    const uint32_t v = jd_bx_find<0>(bd, n, blockIdx.x);
+    const JDResizeDesc &r = rd[v];
+    const JDBoxDesc &x = bd[v];
+    const uint32_t item = (blockIdx.x - x.blk_c) * JD_RS_THREADS + threadIdx.x;
+    const uint32_t nh = (r.flags & 1u) ? r.dst_w : 0u, nv = (r.flags & 2u) ? r.dst_h : 0u;
+    int32_t xmin;
+    if (item < nh) {
+        int32_t *tab = coef + r.coef_h;
+        const int taps = jd_rs_coeffs_box((int)r.src_w, x.box[0], x.box[2], (int)r.dst_w, filter, (int)item, &xmin,
+                                          tab + 2 * (uint64_t)r.dst_w + item, r.dst_w);
+        tab[2 * item] = xmin;
+        tab[2 * item + 1] = taps;
+    } else if (item < nh + nv) {
+        const uint32_t yy = item - nh;
+        int32_t *tab = coef + r.coef_v + (uint64_t)yy * (r.ksize_v + 2);
+        const int taps = jd_rs_coeffs_box((int)r.src_h, x.box[1], x.box[3], (int)r.dst_h, filter, (int)yy, &xmin, tab + 2, 1);
+        tab[0] = xmin;
+        tab[1] = taps;
+    }
+}
+
+/* Reduce: one thread per reduced pixel (an RGB8888 word or a gray byte), summing its fx x fy box of S (fewer at the
+ * region's right and bottom edges) and writing the resize source.  Neighbouring threads read neighbouring boxes, so a
+ * warp's loads of one box row cover 32 fx contiguous pixels. */
+template <int BPP>
+__global__ void __launch_bounds__(JD_RS_THREADS) jdk_reduce(const JDResizeDesc *rd, const JDBoxDesc *bd, uint32_t n, uint8_t *scratch)
+{
+    const uint32_t v = jd_bx_find<1>(bd, n, blockIdx.x);
+    const JDResizeDesc &r = rd[v];
+    const JDBoxDesc &x = bd[v];
+    const uint64_t item = (uint64_t)(blockIdx.x - x.blk_r) * JD_RS_THREADS + threadIdx.x;
+    if (item >= (uint64_t)r.src_w * r.src_h) return;
+    const uint32_t oy = (uint32_t)(item / r.src_w), ox = (uint32_t)(item % r.src_w);
+    const uint32_t sx = ox * x.fx, sy = oy * x.fy;
+    const int nx = (int)(x.rbw - sx < x.fx ? x.rbw - sx : x.fx), ny = (int)(x.rbh - sy < x.fy ? x.rbh - sy : x.fy);
+    const uint64_t at = (uint64_t)(x.ry0 + sy) * x.s_w + x.rx0 + sx;
+    if (BPP == 4)
+        reinterpret_cast<uint32_t *>(scratch + r.src_off)[item] =
+            jd_rd_pixel4(reinterpret_cast<const uint32_t *>(scratch + x.s_off) + at, x.s_w, nx, ny);
+    else
+        scratch[r.src_off + item] = (uint8_t)jd_rd_pixel1(scratch + x.s_off + at, x.s_w, nx, ny);
+}
+
+/* ------------------------------------------------------------------------------------ */
 /* Tensor output (JPEGB200_batchCreateTensor): the pipeline has written each image's uint8  */
 /* output U tightly into the staging buffer; jdk_tensor looks every byte up in the C x 256  */
 /* table the host computed (jd_tensor_table) and stores the elements in CHW or HWC order.   */
