@@ -351,6 +351,49 @@ JPEGB200_BATCH *JPEGB200_batchCreateBox(JPEGB200_CTX *ctx, const uint8_t *const 
 #define JPEGB200_THUMB_NONE   3
 int JPEGB200_thumbnailPlan(int width, int height, int req_w, int req_h, double reducing_gap, int *draft, int *out_w, int *out_h,
                            double *box);
+/* Per-view colour operations, bit-exact with torchvision's ColorJitter (adjust_brightness / _contrast / _saturation / _hue),
+ * RandomGrayscale and RandomSolarize on a PIL image (Pillow 12's arithmetic): the arguments of JPEGB200_batchCreateBox plus
+ * color_ops, V x JPEGB200_COLOR_MAX_OPS entries, row v holding view v's operations in order and ending at the first op 0.
+ *   - F_v is what JPEGB200_batchCreateBox stores for view v (crop, orientation, draft, box, reduce, resize), as uint8 pixels.
+ *     View v's operations run on F_v in the order given, before the tensor conversion, on true R, G, B (the byte order of
+ *     an RGB8888 view, R, G, B, A or B, G, R, A, is that of the same call; the alpha byte is left as it is):
+ *       BRIGHTNESS f  ImageEnhance.Brightness: c = blend(0, c, f)
+ *       CONTRAST f    ImageEnhance.Contrast: c = blend(m, c, f), m = int(sum of L over the current image / (W H) + 0.5)
+ *       SATURATION f  ImageEnhance.Color: c = blend(L, c, f)
+ *       HUE h         adjust_hue: Pillow's convert("HSV"), H += uint8(int32(h * 255)) mod 256, convert("RGB").  The HSV round
+ *                     trip itself changes pixels, so h = 0 is not the identity (it is torchvision's adjust_hue(img, 0)).
+ *       GRAYSCALE     to_grayscale(img, 3): R = G = B = L (arg ignored)
+ *       SOLARIZE t    ImageOps.solarize(img, t): c < t ? c : 255 - c, t compared as a double
+ *     with L = (19595 R + 38470 G + 7471 B + 0x8000) >> 16 (convert("L")) and blend(a, b, f) = Image.blend: t = (float)a +
+ *     (float)f * (float)(b - a) in float32; (uint8)t for 0 <= f <= 1, else clamped to 0 .. 255 and truncated.
+ *   - 8-bit gray output (EIGHT_BIT_GRAYSCALE, JPEG_LUMA_ONLY) is a Pillow "L" image: brightness, contrast (m over the bytes)
+ *     and solarize apply; saturation, hue and grayscale leave it unchanged, as in Pillow and torchvision.
+ *   - color_ops = NULL is JPEGB200_batchCreateBox, which forwards here.  A view whose row is empty stores F_v.  Factor 1
+ *     and a solarize threshold above 255 store F_v too.  Status, batchErrMcu, the walked intervals, sizes, output bytes and
+ *     the destination rules are those of the same call without operations; only the image's own bytes are rewritten.
+ *   - Returns NULL with a message for RGB565, dithered pixel types and padded output when any view has an operation.  A view
+ *     with an unknown op, an argument that is not finite or HUE outside [-0.5, 0.5] gets JPEG_INVALID_PARAMETER alone.
+ *     Negative factors are accepted: Pillow extrapolates.
+ *   - Device work: the operations run in place on each view's uint8 result (the destination, the arena or the tensor
+ *     staging).  A view's list is cut at each CONTRAST; each piece is one jdk_color launch over all views, and a piece
+ *     before a contrast also sums L per view (exact, in 64 bits).  1 + the most CONTRAST operations of any view launches,
+ *     none when no view has an operation; timed in the JPEGB200_T_DITHER slot and counted in JPEGB200_C_LAUNCHES. */
+#define JPEGB200_COLOR_BRIGHTNESS 1
+#define JPEGB200_COLOR_CONTRAST   2
+#define JPEGB200_COLOR_SATURATION 3
+#define JPEGB200_COLOR_HUE        4
+#define JPEGB200_COLOR_GRAYSCALE  5
+#define JPEGB200_COLOR_SOLARIZE   6
+#define JPEGB200_COLOR_MAX_OPS    8
+typedef struct {
+    int32_t op;                        /* JPEGB200_COLOR_*, 0 = end of the view's list */
+    double arg;                        /* factor, hue shift (-0.5 .. 0.5) or solarize threshold */
+} JPEGB200_ColorOp;
+JPEGB200_BATCH *JPEGB200_batchCreateColor(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                          const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                          const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                          const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
+                                          const double *reducing_gaps, const JPEGB200_ColorOp *color_ops);
 void JPEGB200_batchDestroy(JPEGB200_BATCH *b);
 int JPEGB200_batchCount(JPEGB200_BATCH *b);
 /* per-image facts after batchCreate: status is JPEG_SUCCESS or the open() error the reference would give */
@@ -450,6 +493,15 @@ int JPEGB200_decodeBatchBox(JPEGB200_CTX *ctx, const uint8_t *const *datas, cons
                             int filter, const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
                             const double *reducing_gaps, void *const *outs, const int64_t *pitches, const int64_t *plane_strides,
                             int flags, int32_t *status);
+/* The same with colour operations per view (color_ops: V x JPEGB200_COLOR_MAX_OPS, semantics of JPEGB200_batchCreateColor;
+ * NULL = JPEGB200_decodeBatchBox, which forwards here).  The jobs are those of the call without operations: the
+ * operations need no scratch beyond 8 bytes per view and contrast. */
+int JPEGB200_decodeBatchColor(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                              const int32_t *views, int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
+                              const int32_t *out_sizes, int filter, const JPEGB200_TensorSpec *spec, const uint8_t *draft,
+                              const double *boxes, const double *reducing_gaps, const JPEGB200_ColorOp *color_ops,
+                              void *const *outs, const int64_t *pitches, const int64_t *plane_strides, int flags,
+                              int32_t *status);
 /* JPEGB200_NUM_COUNTERS counters summed over the jobs of the last JPEGB200_decodeBatch on this context */
 int JPEGB200_lastCallCounters(JPEGB200_CTX *ctx, int64_t *counters);
 /* CUDA-event stage times (JPEGB200_NUM_TIMINGS, ms) summed over those jobs, and how many jobs there were.  Jobs overlap

@@ -36,6 +36,9 @@ RESIZE_BILINEAR, RESIZE_BICUBIC, RESIZE_BOX = 2, 3, 4
 DT_U8, DT_F32, DT_F16, DT_BF16 = 0, 1, 2, 3
 LAYOUT_CHW, LAYOUT_HWC = 0, 1
 SCALE_NONE, SCALE_DIV255, SCALE_MUL255 = 0, 1, 2
+# colour operations (JPEGB200_ColorOp): torchvision's ColorJitter / RandomGrayscale / RandomSolarize on PIL images
+COLOR_BRIGHTNESS, COLOR_CONTRAST, COLOR_SATURATION, COLOR_HUE, COLOR_GRAYSCALE, COLOR_SOLARIZE = 1, 2, 3, 4, 5, 6
+COLOR_MAX_OPS = 8
 TIMING_NAMES = ["h2d", "prescan", "entropy", "stitch", "idct", "dither", "d2h", "total"]
 COUNTER_NAMES = ["launches", "segments", "blocks", "events", "compressed_bytes", "output_bytes",
                  "record_bytes", "h2d_bytes", "d2h_bytes", "event_candidates"]
@@ -46,6 +49,11 @@ class TensorSpec(C.Structure):
     """JPEGB200_TensorSpec (include/jpegdec_b200.h)"""
     _fields_ = [("dtype", C.c_int32), ("layout", C.c_int32), ("scale", C.c_int32), ("bgr", C.c_int32),
                 ("mean", C.c_float * 3), ("std", C.c_float * 3)]
+
+
+class ColorOp(C.Structure):
+    """JPEGB200_ColorOp (include/jpegdec_b200.h)"""
+    _fields_ = [("op", C.c_int32), ("arg", C.c_double)]
 
 
 class JPEGDRAW(C.Structure):
@@ -137,6 +145,13 @@ def lib():
     L.JPEGB200_decodeBatchBox.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, i32p, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
                                           i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(C.c_uint8), dp, dp, C.POINTER(vp),
                                           C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int, i32p]
+    cop = C.POINTER(ColorOp)
+    L.JPEGB200_batchCreateColor.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, i32p, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
+                                            i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(C.c_uint8), dp, dp, cop]
+    L.JPEGB200_batchCreateColor.restype = vp
+    L.JPEGB200_decodeBatchColor.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, i32p, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
+                                            i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(C.c_uint8), dp, dp, cop,
+                                            C.POINTER(vp), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int, i32p]
     L.JPEGB200_thumbnailPlan.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, ip, ip, ip, dp]
     L.JPEGB200_batchSetOutputTensor.argtypes = [vp, C.c_int, vp, C.c_int64, C.c_int64]
     L.JPEGB200_decodeBatchTensor.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
@@ -421,6 +436,45 @@ def thumbnail_plan(width, height, size, reducing_gap=2.0):
     return d.value, (w.value, h.value), tuple(box)
 
 
+def _color_array(color, n):
+    """one sequence of operations for every image, or one list of them per image -> ColorOp[n * COLOR_MAX_OPS] (None stays
+    None).  An operation is a tuple (op, arg), or the bare constant for an op without an argument (COLOR_GRAYSCALE)."""
+    if color is None:
+        return None
+    color = list(color)
+    def row(ops):
+        out = []
+        for o in ops:
+            o = (o, 0.0) if isinstance(o, (int, np.integer)) else tuple(o)
+            out.append((int(o[0]), float(o[1])))
+        if len(out) > COLOR_MAX_OPS:
+            raise ValueError("color: at most %d operations per image (view)" % COLOR_MAX_OPS)
+        return out
+    def is_op(o):
+        return isinstance(o, (int, np.integer)) or (isinstance(o, tuple) and len(o) == 2 and isinstance(o[0], (int, np.integer)))
+    rows = [row(color)] * n if all(is_op(o) for o in color) else [row(r) for r in color]
+    if len(rows) != n:
+        raise ValueError("color: one sequence of (op, arg) for every image, or one per image (view)")
+    a = (ColorOp * (n * COLOR_MAX_OPS))()
+    for v, r in enumerate(rows):
+        for k, (op, arg) in enumerate(r):
+            a[v * COLOR_MAX_OPS + k].op = op
+            a[v * COLOR_MAX_OPS + k].arg = arg
+    return a
+
+
+def color_jitter_ops(params):
+    """The (op, arg) sequence of torchvision's ColorJitter for the draw `params` = ColorJitter.get_params(...) =
+    (fn_idx, brightness, contrast, saturation, hue), entries that are None skipped, in fn_idx's order."""
+    fn_idx, b, c, s, h = params
+    ops = []
+    for fn in [int(i) for i in fn_idx]:
+        v = (b, c, s, h)[fn]
+        if v is not None:
+            ops.append(((COLOR_BRIGHTNESS, COLOR_CONTRAST, COLOR_SATURATION, COLOR_HUE)[fn], float(v)))
+    return ops
+
+
 def _orient_array(orients, n):
     """n EXIF transforms (0 = from the file, 1-8) -> uint8[n] for the C ABI (None stays None = no orientation)"""
     if orients is None:
@@ -455,10 +509,11 @@ class Batch:
     draft() at that scale (JPEGB200_batchCreateDraft; needs JPEGB200_OPT_LIBJPEG), or None.  box: one (x0, y0, x1, y1) of
     doubles for every image or one per image, and reducing_gap: one value or one per image (None = Pillow's None): the
     resize is then Pillow's resize(out_size, filter, box=box, reducing_gap=gap) of the unresized output
-    (JPEGB200_batchCreateBox; needs out_sizes)."""
+    (JPEGB200_batchCreateBox; needs out_sizes).  color: one sequence of (op, arg) (COLOR_*) for every image or one per
+    image, run on each final uint8 image as torchvision's PIL transforms do (JPEGB200_batchCreateColor), or None."""
 
     def __init__(self, ctx, ptrs, sizes, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
-                 filter=RESIZE_BILINEAR, spec=None, views=None, draft=None, box=None, reducing_gap=None):
+                 filter=RESIZE_BILINEAR, spec=None, views=None, draft=None, box=None, reducing_gap=None, color=None):
         nf = len(ptrs)
         self._views, n = _views_array(views, nf)
         self.n = n
@@ -470,7 +525,14 @@ class Batch:
         self.ctx = ctx
         self._draft = _draft_array(draft, n)
         self._box, self._gap = _box_array(box, n), _gap_array(reducing_gap, n)
-        if box is not None or reducing_gap is not None:
+        self._color = _color_array(color, n)
+        if color is not None:
+            self._spec = spec
+            self.h = lib().JPEGB200_batchCreateColor(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
+                                                     self._rois, self._orients, self._out_sizes, int(filter),
+                                                     C.byref(spec) if spec is not None else None, self._draft, self._box,
+                                                     self._gap, self._color)
+        elif box is not None or reducing_gap is not None:
             self._spec = spec
             self.h = lib().JPEGB200_batchCreateBox(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
                                                    self._rois, self._orients, self._out_sizes, int(filter),
@@ -565,13 +627,14 @@ class Batch:
 
 
 def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flags=0, rois=None, orients=None,
-                 out_sizes=None, filter=RESIZE_BILINEAR, views=None, draft=None, box=None, reducing_gap=None):
+                 out_sizes=None, filter=RESIZE_BILINEAR, views=None, draft=None, box=None, reducing_gap=None, color=None):
     """JPEGB200_decodeBatch(ROI / Oriented / Resized / Views): one call for n files (host pointers) -> n outputs (host
     pointers, or device pointers with JPEGB200_OUT_DEVICE); rois: one (x, y, w, h) per image or None; orients: one EXIF
     transform per image (0 = from the file) or None; out_sizes: one (W, H) per image (resized with `filter`) or None.
     views: one view count per file, or None; outs, pitches and the per-image lists are then per view.  Returns (rc,
     per-image status list, counters summed over the internal jobs).  draft: one scale denominator per image (view), or
-    None (JPEGB200_decodeBatchDraft).  box / reducing_gap: as in Batch (JPEGB200_decodeBatchBox)."""
+    None (JPEGB200_decodeBatchDraft).  box / reducing_gap: as in Batch (JPEGB200_decodeBatchBox).  color: as in Batch
+    (JPEGB200_decodeBatchColor)."""
     nf = len(ptrs)
     va, n = _views_array(views, nf)
     pa = (C.c_void_p * nf)(*ptrs)
@@ -581,7 +644,12 @@ def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flag
     oa = (C.c_void_p * n)(*outs)
     pi = (C.c_int64 * n)(*pitches) if pitches is not None else None
     st = (C.c_int32 * n)()
-    if box is not None or reducing_gap is not None:
+    if color is not None:
+        rc = lib().JPEGB200_decodeBatchColor(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
+                                             _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None,
+                                             _draft_array(draft, n), _box_array(box, n), _gap_array(reducing_gap, n),
+                                             _color_array(color, n), oa, pi, None, flags, st)
+    elif box is not None or reducing_gap is not None:
         rc = lib().JPEGB200_decodeBatchBox(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
                                            _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None,
                                            _draft_array(draft, n), _box_array(box, n), _gap_array(reducing_gap, n), oa, pi,
@@ -604,16 +672,16 @@ def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flag
 
 
 def decode_batch_to_host(ctx, jpegs, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
-                         filter=RESIZE_BILINEAR, views=None, draft=None, box=None, reducing_gap=None):
+                         filter=RESIZE_BILINEAR, views=None, draft=None, box=None, reducing_gap=None, color=None):
     """Convenience: list of bytes -> list of numpy arrays [out_h, pitch_bytes] (uint8).
     One public-API call per batch with HOST buffers on both sides.  rois: one (x, y, w, h) per image (the arrays are then
     h rows of w pixels), or None.  orients: one EXIF transform per image (0 = from the file), or None.  out_sizes: one
     (W, H) per image (the arrays are then H rows of W pixels, resized with `filter`), or None.  views: one view count
     per file, or None; the lists (and rois / orients / out_sizes) are then per view.  draft: one scale denominator per
-    image (view), or None.  box / reducing_gap: as in Batch."""
+    image (view), or None.  box / reducing_gap / color: as in Batch."""
     bufs = [np.frombuffer(j, dtype=np.uint8) for j in jpegs]
     b = Batch(ctx, [x.ctypes.data for x in bufs], [len(x) for x in bufs], pixel_type, options, rois, orients, out_sizes,
-              filter, views=views, draft=draft, box=box, reducing_gap=reducing_gap)
+              filter, views=views, draft=draft, box=box, reducing_gap=reducing_gap, color=color)
     try:
         outs = []
         for i in range(b.n):
@@ -661,7 +729,8 @@ def tensor_spec(dtype, layout="CHW", scale="div255", mean=(0.0, 0.0, 0.0), std=(
 
 def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, orients=None, out_sizes=None,
                         filter=RESIZE_BILINEAR, dtype=None, layout="CHW", scale="div255", mean=(0.0, 0.0, 0.0),
-                        std=(1.0, 1.0, 1.0), bgr=False, out=None, views=None, draft=None, box=None, reducing_gap=None):
+                        std=(1.0, 1.0, 1.0), bgr=False, out=None, views=None, draft=None, box=None, reducing_gap=None,
+                        color=None):
     """JPEGB200_decodeBatchTensor: list of bytes -> the model's input tensor on the context's GPU, and the status list.
 
     Image i becomes a C x H x W (layout "CHW") or H x W x C ("HWC") tensor of `dtype` (torch.float32 by default, float16,
@@ -674,7 +743,8 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     views: one view count per file (JPEGB200_decodeBatchViews: the views of a file share one entropy walk), or None; the
     images are then the views: rois / orients / out_sizes / out and the result ([V, C, H, W], or a list) are per view.
     draft: one scale denominator (1, 2, 4, 8) per image (view), Pillow's draft() at that scale (JPEGB200_decodeBatchDraft),
-    or None.  box / reducing_gap: as in Batch (JPEGB200_decodeBatchBox)."""
+    or None.  box / reducing_gap: as in Batch (JPEGB200_decodeBatchBox).  color: as in Batch, before the conversion
+    (JPEGB200_decodeBatchColor)."""
     import torch
     dtype = torch.float32 if dtype is None else dtype
     spec = tensor_spec(dtype, layout, scale, mean, std, bgr)
@@ -729,11 +799,11 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     st = (C.c_int32 * n)()
     with torch.cuda.device(dev):
         torch.cuda.current_stream(dev).synchronize()   # the library's streams do not order against torch's
-        rc = lib().JPEGB200_decodeBatchBox(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
-                                           _orient_array(orients, n), _size_array(out_sizes, n), int(filter),
-                                           C.byref(spec), _draft_array(draft, n), _box_array(box, n),
-                                           _gap_array(reducing_gap, n), (C.c_void_p * n)(*ptr_l), (C.c_int64 * n)(*pitch_l),
-                                           (C.c_int64 * n)(*plane_l), JPEGB200_OUT_DEVICE, st)
+        rc = lib().JPEGB200_decodeBatchColor(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
+                                             _orient_array(orients, n), _size_array(out_sizes, n), int(filter),
+                                             C.byref(spec), _draft_array(draft, n), _box_array(box, n),
+                                             _gap_array(reducing_gap, n), _color_array(color, n), (C.c_void_p * n)(*ptr_l),
+                                             (C.c_int64 * n)(*pitch_l), (C.c_int64 * n)(*plane_l), JPEGB200_OUT_DEVICE, st)
     if rc == 0:
         raise RuntimeError("decodeBatchViews failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
     return out, list(st)

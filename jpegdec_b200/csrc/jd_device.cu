@@ -175,6 +175,16 @@ struct JPEGB200_BATCH {
     std::vector<JDBoxPlan> bx_plans;
     std::vector<JDBoxDesc> bx_desc;
     DevBuf<JDBoxDesc> d_bx_desc;
+    /* colour operations (JPEGB200_batchCreateColor): per view its plan and byte order; jdk_color rewrites the view's final
+     * uint8 image in place, before jdk_tensor */
+    bool color = false;
+    std::vector<JDColorPlan> co_plans;
+    std::vector<uint8_t> co_bgr;
+    std::vector<JDColorDesc> co_desc;
+    std::vector<uint32_t> co_blk;           /* per launch, per view: its first CTA */
+    DevBuf<JDColorDesc> d_co_desc;
+    DevBuf<uint32_t> d_co_blk;
+    DevBuf<unsigned long long> d_co_sum;    /* per view, per contrast: the sum of L before it */
     /* tensor output (JPEGB200_batchCreateTensor): descs hold the row bytes as out_pitch; the pipeline (IDCT or resize) writes
      * U (out_w x out_h, tn_bpp bytes per pixel) tightly into d_tn, jdk_tensor writes the destination */
     bool tensor = false;
@@ -555,6 +565,7 @@ struct CreatePlan {
     const JPEGB200_TensorSpec *spec = nullptr;
     const uint8_t *draft = nullptr;     /* per view: draft scale denominator (JPEGB200_batchCreateDraft), NULL = 1 */
     const double *boxes = nullptr, *gaps = nullptr;   /* per view: resize box and reducing gap (JPEGB200_batchCreateBox) */
+    const JPEGB200_ColorOp *color = nullptr;          /* per view: JPEGB200_COLOR_MAX_OPS operations (JPEGB200_batchCreateColor) */
     /* where the next file's restart segments, blocks and records start; where the next view's output and gray stage start */
     uint32_t seg = 0;
     uint64_t blk = 0, rec_total = 0;
@@ -603,6 +614,8 @@ static void init_batch(JPEGB200_BATCH *b, JPEGB200_CTX *ctx, const CreatePlan &P
     }
     b->box = P.boxes != nullptr || P.gaps != nullptr;
     if (b->box) b->bx_plans.assign(nv, JDBoxPlan{});
+    b->color = P.color != nullptr;
+    if (b->color) { b->co_plans.assign(nv, JDColorPlan{}); b->co_bgr.assign(nv, 0); }
     b->lj = (options & JPEGB200_OPT_LIBJPEG) != 0;
     if (b->lj) { b->lj_desc.assign(nv, JDLjDesc{}); b->lj_plane.assign(nv, 0); }
     b->tensor = P.spec != nullptr;
@@ -712,6 +725,18 @@ static void resolve_orients(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int
     }
 }
 
+/* the walk of a file after some of its views were refused late (box, colour operations): without a rectangle every view
+ * walks the whole file, with rectangles the deepest valid view sets it */
+static uint32_t kept_walk(const JPEGB200_BATCH *b, const CreatePlan &P, int v0, int nvf, uint32_t walk)
+{
+    uint32_t kept = 0;
+    for (int i = v0; i < v0 + nvf; i++) {
+        const uint32_t w = b->roi ? (uint32_t)b->plans[i].nseg_walk : walk;
+        if (P.vok[i] && w > kept) kept = w;
+    }
+    return kept;
+}
+
 /* The views' own arguments (no such transform, a rectangle outside the output, a resize target outside 1..65535) and how
  * deep the file is walked: down to the deepest last MCU row among its valid views.  Writes plans, P.srects and P.vok;
  * returns the restart intervals to walk, 0 when no view is valid. */
@@ -765,14 +790,19 @@ static uint32_t plan_views(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int 
                 dropped = true;
             }
         }
-        if (dropped) {   /* without a rectangle every view walks the whole file */
-            uint32_t kept = 0;
-            for (int i = v0; i < v0 + nvf; i++) {
-                const uint32_t w = b->roi ? (uint32_t)b->plans[i].nseg_walk : walk;
-                if (P.vok[i] && w > kept) kept = w;
+        if (dropped) walk = kept_walk(b, P, v0, nvf, walk);
+    }
+    if (walk != 0 && b->color) {
+        /* each valid view's operations; one Pillow or torchvision refuses leaves the walk to the others */
+        bool dropped = false;
+        for (int i = v0; i < v0 + nvf; i++) {
+            if (!P.vok[i]) continue;
+            if (!jd_color_plan(P.color + JPEGB200_COLOR_MAX_OPS * (size_t)i, b->ptclass == JD_PT_GRAY, &b->co_plans[i])) {
+                P.vok[i] = 0;
+                dropped = true;
             }
-            walk = kept;
         }
+        if (dropped) walk = kept_walk(b, P, v0, nvf, walk);
     }
     return walk;
 }
@@ -985,6 +1015,8 @@ static int plan_view_output(JPEGB200_BATCH *b, CreatePlan &P, int f, int i)
         const bool bgr = !b->lj && jd_rgb8888_is_bgr(b->ctx->arith, b->sshift, inf.ncomp, inf.subsample) != 0;
         b->tn_swap[i] = (uint8_t)(b->tn_nc == 3 && bgr != (b->tn_spec.bgr != 0));
     }
+    if (b->color)   /* the colour operations read true R, G, B: a libjpeg decode stores R, G, B for every file */
+        b->co_bgr[i] = (uint8_t)(b->ptclass == JD_PT_8888 && !b->lj && jd_rgb8888_is_bgr(b->ctx->arith, b->sshift, inf.ncomp, inf.subsample));
     size_t pitch;
     if (b->tensor) pitch = (size_t)vd.out_w * (b->tn_spec.layout == JPEGB200_LAYOUT_HWC ? b->tn_nc : 1) * b->tn_elt;
     else if (b->dither_bits) {
@@ -1097,17 +1129,28 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateBox(JPEGB200_CTX *ctx, const uint
                                                    const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
                                                    const double *reducing_gaps)
 {
+    return JPEGB200_batchCreateColor(ctx, datas, sizes, n, views, pixel_type, options, rois, orients, out_sizes, filter, spec, draft,
+                                     boxes, reducing_gaps, nullptr);
+}
+
+extern "C" JPEGB200_BATCH *JPEGB200_batchCreateColor(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                                     const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                                     const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                                     const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
+                                                     const double *reducing_gaps, const JPEGB200_ColorOp *color_ops)
+{
     if (!ctx) { snprintf(g_err, sizeof(g_err), "invalid parameter"); return nullptr; }
     int64_t nv = 0;   /* images of the batch: views */
     if (!jd_check_batch_features(pixel_type, options, n, views, rois != nullptr, orients != nullptr, out_sizes != nullptr, filter, spec,
                                  &nv, g_err, (int)sizeof(g_err)) ||
-        !jd_check_draft(options, draft, g_err, (int)sizeof(g_err)) || !jd_check_box(out_sizes, boxes, reducing_gaps, g_err, (int)sizeof(g_err)))
+        !jd_check_draft(options, draft, g_err, (int)sizeof(g_err)) || !jd_check_box(out_sizes, boxes, reducing_gaps, g_err, (int)sizeof(g_err)) ||
+        !jd_check_color(pixel_type, options, nv, color_ops, g_err, (int)sizeof(g_err)))
         return nullptr;
     JPEGB200_BATCH *b = new (std::nothrow) JPEGB200_BATCH();
     if (!b) return nullptr;
     CreatePlan P;
     P.datas = datas; P.sizes = sizes; P.views = views; P.rois = rois; P.orients = orients; P.out_sizes = out_sizes; P.spec = spec;
-    P.draft = draft; P.boxes = boxes; P.gaps = reducing_gaps;
+    P.draft = draft; P.boxes = boxes; P.gaps = reducing_gaps; P.color = color_ops;
     P.srects.assign(4 * (size_t)nv, 0); P.vok.assign((size_t)nv, 0);
     P.ks.assign(orients ? (size_t)nv : 0u, 0);
     if (options & JPEGB200_OPT_PROGRESSIVE) { P.fscans.resize(JD_PROG_MAX_SCANS); P.ftabs.resize(JD_PROG_MAX_TABS); }
@@ -1485,6 +1528,8 @@ struct DecodeState {
     uint8_t *stage_out = nullptr;           /* where the IDCT stage writes: pipe_out, or the gray stage / the resize source */
     uint32_t tn_ctas = 0, rs_ctas[4] = {0u, 0u, 0u, 0u};
     uint32_t bx_ctas[2] = {0u, 0u};         /* box batches: jdk_resize_coeffs_box, jdk_reduce */
+    std::vector<uint32_t> co_ctas;          /* colour operations: CTAs of each jdk_color launch */
+    uint32_t co_nsum = 0;                   /* sum slots per view: the most contrasts of any view */
     int launches = 0;
 };
 
@@ -1594,6 +1639,47 @@ static int stage_tensor(JPEGB200_BATCH *b, DecodeState &D)
     CK(cudaMemcpyAsync(b->d_tn_tab.p, b->tn_table.data(), 3 * 256 * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(b->d_tn_desc.p, b->tn_desc.data(), sizeof(JDTensorDesc) * n, cudaMemcpyHostToDevice, st));
     D.pipe_out = b->d_tn.p;
+    return 1;
+}
+
+/* colour operations: where each view's final uint8 image lies before the resize and dither stages redirect the stages
+ * before them (D.pipe_out + out_off, out_pitch).  Uploads co_desc, the per-launch CTA starts and zeroed contrast sums. */
+static int stage_color(JPEGB200_BATCH *b, DecodeState &D)
+{
+    const int n = b->n;
+    cudaStream_t st = b->ss.stream;
+    uint32_t nl = 0;
+    for (int i = 0; i < n; i++)
+        if (b->parse_status[i] == JPEG_SUCCESS && b->co_plans[i].nops && b->co_plans[i].ncontrast + 1 > nl) nl = b->co_plans[i].ncontrast + 1;
+    if (nl == 0) return 1;   /* no view has an operation */
+    D.co_nsum = nl - 1;
+    b->co_desc.assign(n, JDColorDesc{});
+    b->co_blk.assign((size_t)nl * n, 0);
+    std::vector<uint64_t> ctas(nl, 0);
+    for (int i = 0; i < n; i++) {
+        for (uint32_t s = 0; s < nl; s++) b->co_blk[(size_t)s * n + i] = (uint32_t)ctas[s];
+        const JDColorPlan &p = b->co_plans[i];
+        if (b->parse_status[i] != JPEG_SUCCESS || p.nops == 0) continue;
+        JDColorDesc &c = b->co_desc[i];
+        c.off = D.descs_stage[i].out_off; c.pitch = D.descs_stage[i].out_pitch;
+        c.w = b->descs[i].out_w; c.h = b->descs[i].out_h;
+        c.bgr = b->co_bgr[i];
+        c.plan = p;
+        const uint64_t per = ((uint64_t)c.w * c.h + JD_CO_THREADS - 1) / JD_CO_THREADS;
+        for (uint32_t s = 0; s <= p.ncontrast; s++)   /* segment s has operations, or sums for the contrast after it */
+            if (p.seg[s] < p.seg[s + 1] || s < p.ncontrast) ctas[s] += per;
+    }
+    D.co_ctas.assign(nl, 0);
+    for (uint32_t s = 0; s < nl; s++) {
+        if (ctas[s] >= (1ull << 31)) { snprintf(g_err, sizeof(g_err), "colour operations: too many pixels in one job"); return 0; }
+        D.co_ctas[s] = (uint32_t)ctas[s];
+    }
+    CK(b->d_co_desc.alloc(&b->ctx->pool, n));
+    CK(b->d_co_blk.alloc(&b->ctx->pool, (size_t)nl * n));
+    CK(b->d_co_sum.alloc(&b->ctx->pool, D.co_nsum ? (size_t)D.co_nsum * n : 1));
+    CK(cudaMemcpyAsync(b->d_co_desc.p, b->co_desc.data(), sizeof(JDColorDesc) * n, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(b->d_co_blk.p, b->co_blk.data(), sizeof(uint32_t) * nl * n, cudaMemcpyHostToDevice, st));
+    if (D.co_nsum) CK(cudaMemsetAsync(b->d_co_sum.p, 0, sizeof(unsigned long long) * D.co_nsum * n, st));
     return 1;
 }
 
@@ -2071,7 +2157,22 @@ static void run_resize(JPEGB200_BATCH *b, DecodeState &D)
 #undef JD_RS_ARGS
 }
 
-/* timed in the dither slot too, after the resize */
+/* timed in the dither slot too, after the resize: one launch per segment of the operation lists */
+static void run_color(JPEGB200_BATCH *b, DecodeState &D)
+{
+    cudaStream_t st = b->ss.stream;
+    const uint32_t n = (uint32_t)b->n;
+    for (uint32_t s = 0; s < (uint32_t)D.co_ctas.size(); s++) {
+        if (!D.co_ctas[s]) continue;
+        if (b->ptclass == JD_PT_GRAY)
+            jdk_color<1><<<D.co_ctas[s], JD_CO_THREADS, 0, st>>>(b->d_co_desc.p, b->d_co_blk.p + (size_t)s * n, n, s, b->d_co_sum.p, D.co_nsum, D.pipe_out);
+        else
+            jdk_color<4><<<D.co_ctas[s], JD_CO_THREADS, 0, st>>>(b->d_co_desc.p, b->d_co_blk.p + (size_t)s * n, n, s, b->d_co_sum.p, D.co_nsum, D.pipe_out);
+        D.launches++;
+    }
+}
+
+/* timed in the dither slot too, after the resize and the colour operations */
 static void run_tensor(JPEGB200_BATCH *b, DecodeState &D)
 {
     if (!D.tn_ctas) return;
@@ -2104,7 +2205,7 @@ static void set_decode_counters(JPEGB200_BATCH *b, const DecodeState &D)
 }
 
 /* The host pipeline of one job, in stream order.  The events ev[2] .. ev[7] bound the published stage timings
- * (JPEGB200_batchWait): prescan, entropy, stitch, IDCT, and the pixel pass after it (dither, resize, tensor). */
+ * (JPEGB200_batchWait): prescan, entropy, stitch, IDCT, and the pixel pass after it (dither, resize, colour, tensor). */
 extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
 {
     if (!b) return 0;
@@ -2122,6 +2223,7 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
     if (!alloc_prog_planes(b) || !place_outputs(b, D)) return 0;
     /* each stage that writes through scratch redirects the stage before it: tensor <- resize <- IDCT, dither <- IDCT */
     if (b->tensor && !stage_tensor(b, D)) return 0;
+    if (b->color && !stage_color(b, D)) return 0;
     if (b->resize && !stage_resize(b, D)) return 0;
     if (b->dither_bits && !stage_dither(b, D)) return 0;
     CK(cudaMemcpyAsync(b->d_descs.p, D.descs_stage.data(), sizeof(JDImageDesc) * b->n, cudaMemcpyHostToDevice, st));
@@ -2143,6 +2245,7 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
     CK(cudaEventRecord(ev[6], st));
     if (b->dither_bits) run_dither(b, D);
     if (b->resize) run_resize(b, D);
+    if (b->color) run_color(b, D);
     if (b->tensor) run_tensor(b, D);
     CK(cudaEventRecord(ev[7], st));
     CK(cudaGetLastError());
@@ -2360,9 +2463,22 @@ extern "C" int JPEGB200_decodeBatchBox(JPEGB200_CTX *ctx, const uint8_t *const *
                                        const double *reducing_gaps, void *const *outs, const int64_t *pitches,
                                        const int64_t *plane_strides, int flags, int32_t *status)
 {
+    return JPEGB200_decodeBatchColor(ctx, datas, sizes, n, views, pixel_type, options, rois, orients, out_sizes, filter, spec, draft,
+                                     boxes, reducing_gaps, nullptr, outs, pitches, plane_strides, flags, status);
+}
+
+extern "C" int JPEGB200_decodeBatchColor(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                         const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                         const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                         const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
+                                         const double *reducing_gaps, const JPEGB200_ColorOp *color_ops, void *const *outs,
+                                         const int64_t *pitches, const int64_t *plane_strides, int flags, int32_t *status)
+{
     if (!ctx || n <= 0) return 0;
     const int64_t nv = jd_count_views(n, views, "call", g_err, (int)sizeof(g_err));   /* images (views) of the call */
     if (nv < 0) return 0;
+    /* refused for the whole call, not by the first job whose views have operations */
+    if (!jd_check_color(pixel_type, options, nv, color_ops, g_err, (int)sizeof(g_err))) return 0;
     const bool dev_out = (flags & JPEGB200_OUT_DEVICE) != 0;
     if (spec && !dev_out) {
         snprintf(g_err, sizeof(g_err), "tensor output is written to device memory only: call with JPEGB200_OUT_DEVICE");
@@ -2406,10 +2522,11 @@ extern "C" int JPEGB200_decodeBatchBox(JPEGB200_CTX *ctx, const uint8_t *const *
         const int32_t *vi = views ? views + i0 : nullptr;
         int cnt = jd_job_files(n - i0, sizes + i0, vi, maxcnt, limit, nullptr, 0, &cv, &capped);
         auto create = [&](int c) {
-            return JPEGB200_batchCreateBox(ctx, datas + i0, sizes + i0, c, vi, pixel_type, options, rois ? rois + 4 * (size_t)v0 : nullptr,
-                                           orients ? orients + v0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)v0 : nullptr, filter, spec,
-                                           draft ? draft + v0 : nullptr, boxes ? boxes + 4 * (size_t)v0 : nullptr,
-                                           reducing_gaps ? reducing_gaps + v0 : nullptr);
+            return JPEGB200_batchCreateColor(ctx, datas + i0, sizes + i0, c, vi, pixel_type, options, rois ? rois + 4 * (size_t)v0 : nullptr,
+                                             orients ? orients + v0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)v0 : nullptr, filter, spec,
+                                             draft ? draft + v0 : nullptr, boxes ? boxes + 4 * (size_t)v0 : nullptr,
+                                             reducing_gaps ? reducing_gaps + v0 : nullptr,
+                                             color_ops ? color_ops + JPEGB200_COLOR_MAX_OPS * (size_t)v0 : nullptr);
         };
         JPEGB200_BATCH *b = create(cnt);
         if (!b) { rc = 0; break; }

@@ -741,6 +741,44 @@ int jd_check_box(const int32_t *out_sizes, const double *boxes, const double *ga
     return 1;
 }
 
+/* ---- colour operations (JPEGB200_batchCreateColor, jd_color.h) ---- */
+int jd_color_plan(const JPEGB200_ColorOp *row, int gray, JDColorPlan *plan)
+{
+    memset(plan, 0, sizeof(*plan));
+    for (int k = 0; k < JPEGB200_COLOR_MAX_OPS && row[k].op != 0; k++) {
+        const int op = row[k].op;
+        const double a = row[k].arg;
+        if (op < JPEGB200_COLOR_BRIGHTNESS || op > JPEGB200_COLOR_SOLARIZE || !isfinite(a)) return 0;
+        if (op == JPEGB200_COLOR_HUE && !(a >= -0.5 && a <= 0.5)) return 0;   /* torchvision raises there */
+        if (gray && (op == JPEGB200_COLOR_SATURATION || op == JPEGB200_COLOR_HUE || op == JPEGB200_COLOR_GRAYSCALE)) continue;
+        uint32_t bits;
+        if (op == JPEGB200_COLOR_HUE) bits = (uint32_t)(uint8_t)(int32_t)(a * 255.0);   /* np.int32(h * 255).astype(uint8) */
+        else if (op == JPEGB200_COLOR_SOLARIZE) bits = a <= 0.0 ? 0u : a > 255.0 ? 256u : (uint32_t)ceil(a);   /* bytes c < a */
+        else if (op == JPEGB200_COLOR_GRAYSCALE) bits = 0u;
+        else { const float f = (float)a; memcpy(&bits, &f, 4); }   /* ImagingBlend takes the factor as float */
+        if (op == JPEGB200_COLOR_CONTRAST) plan->seg[++plan->ncontrast] = plan->nops;
+        plan->op[plan->nops] = (uint32_t)op;
+        plan->arg[plan->nops] = bits;
+        plan->nops++;
+    }
+    plan->seg[plan->ncontrast + 1] = plan->nops;
+    return 1;
+}
+
+int jd_check_color(int pixel_type, int options, int64_t nv, const JPEGB200_ColorOp *color_ops, char *msg, int msg_len)
+{
+    int any = 0;
+    for (int64_t v = 0; color_ops && v < nv && !any; v++) any = color_ops[v * JPEGB200_COLOR_MAX_OPS].op != 0;
+    if (!any) return 1;
+    const int pt = jd_fold_luma_only(pixel_type, options);
+    const char *why = NULL;
+    if (pt == RGB565_LITTLE_ENDIAN || pt == RGB565_BIG_ENDIAN) why = "RGB565 pixel types (a packed 5/6/5 word has no byte planes)";
+    else if (pt >= FOUR_BIT_DITHERED && pt <= ONE_BIT_DITHERED) why = "dithered pixel types";
+    else if (options & JPEGB200_OPT_PADDED) why = "padded output";
+    if (why) { snprintf(msg, (size_t)msg_len, "colour operations are not supported with %s", why); return 0; }
+    return 1;
+}
+
 /* Pillow's Image.thumbnail(size, BICUBIC, reducing_gap) decision for a W x H JPEG (include/jpegdec_b200.h) */
 int JPEGB200_thumbnailPlan(int width, int height, int req_w, int req_h, double reducing_gap, int *draft, int *out_w, int *out_h,
                            double *box)

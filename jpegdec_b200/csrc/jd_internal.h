@@ -168,6 +168,16 @@ int jd_box_plan(int sw, int sh, int out_w, int out_h, int filter, const double *
 /* Batch-level rule of JPEGB200_batchCreateBox: boxes or reducing_gaps need out_sizes.  0 with a message otherwise. */
 int jd_check_box(const int32_t *out_sizes, const double *boxes, const double *gaps, char *msg, int msg_len);
 
+/* Colour operations of one view (JPEGB200_batchCreateColor, jd_color.h): row = its JPEGB200_COLOR_MAX_OPS entries.  Writes
+ * the plan the kernel runs -- factors as float bits, hue shift bytes, solarize thresholds as the count of bytes below them,
+ * the segments cut at each contrast; on a gray view (gray != 0) saturation, hue and grayscale are dropped.  Returns 0 for
+ * an unknown op, an argument that is not finite, or a hue outside [-0.5, 0.5]. */
+#include "jd_color.h"
+int jd_color_plan(const JPEGB200_ColorOp *row, int gray, JDColorPlan *plan);
+/* Batch-level rule of JPEGB200_batchCreateColor: no operation on RGB565, dithered pixel types or padded output (checked
+ * over the nv rows).  0 with a message otherwise. */
+int jd_check_color(int pixel_type, int options, int64_t nv, const JPEGB200_ColorOp *color_ops, char *msg, int msg_len);
+
 /* Coefficient records an image's entropy walks can address above its record base: the largest JD_REC_INDEX + JD_REC_CAP
  * (jd_core.h) over its restart segments (slots 0 .. nseg - 1, each ending at or before the file's end) and the chunks of a
  * restart-free scan (slots nseg .. nseg + nch - 1, 512 bytes each from scan_offset), computed in 64 bits.  Those indices

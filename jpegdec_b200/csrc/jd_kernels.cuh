@@ -2154,6 +2154,70 @@ __global__ void __launch_bounds__(JD_RS_THREADS) jdk_reduce(const JDResizeDesc *
 }
 
 /* ------------------------------------------------------------------------------------ */
+/* Colour operations (JPEGB200_batchCreateColor, jd_color.h): in place on each view's      */
+/* final uint8 image (the destination, the arena or the tensor staging).  Launch s runs     */
+/* segment s of every view's list (the operations from its s-th contrast to the next one)  */
+/* and, before a contrast, sums L of its output per view: a block reduction and one 64-bit */
+/* atomicAdd per CTA, exact whatever the order.  One thread per pixel.                     */
+/* ------------------------------------------------------------------------------------ */
+#define JD_CO_THREADS 256
+struct JDColorDesc {
+    uint64_t off;              /* the view's image from the launch's base */
+    uint64_t pitch;            /* bytes between its rows */
+    uint32_t w, h;
+    uint32_t bgr;              /* RGB8888 stored as B, G, R, A */
+    uint32_t pad;
+    JDColorPlan plan;
+};
+
+/* cblk: this launch's first CTA of every view (views without CTAs share the next one's); sums: ncontrast slots per view */
+template <int BPP>
+__global__ void __launch_bounds__(JD_CO_THREADS) jdk_color(const JDColorDesc *cd, const uint32_t *cblk, uint32_t n, uint32_t s,
+                                                           unsigned long long *sums, uint32_t nsum, uint8_t *base)
+{
+    uint32_t lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (cblk[mid] <= blockIdx.x) lo = mid; else hi = mid - 1;
+    }
+    const uint32_t v = lo;
+    const JDColorDesc &d = cd[v];
+    const uint64_t npx = (uint64_t)d.w * d.h;
+    const uint64_t item = (uint64_t)(blockIdx.x - cblk[v]) * JD_CO_THREADS + threadIdx.x;
+    const uint32_t k0 = d.plan.seg[s], k1 = d.plan.seg[s + 1];
+    const uint32_t mean = s > 0 ? jd_co_mean(sums[(uint64_t)v * nsum + s - 1], npx) : 0u;
+    uint32_t l = 0;
+    if (item < npx) {
+        const uint32_t y = (uint32_t)(item / d.w), x = (uint32_t)(item % d.w);
+        uint8_t *px = base + d.off + (uint64_t)y * d.pitch + (uint64_t)x * BPP;
+        if (BPP == 4) {
+            const uint32_t w = *reinterpret_cast<const uint32_t *>(px);
+            uint32_t r = d.bgr ? (w >> 16) & 255u : w & 255u, g = (w >> 8) & 255u, b = d.bgr ? w & 255u : (w >> 16) & 255u;
+            for (uint32_t k = k0; k < k1; k++) jd_co_apply3(d.plan.op[k], d.plan.arg[k], mean, &r, &g, &b);
+            if (k1 > k0)
+                *reinterpret_cast<uint32_t *>(px) = (w & 0xFF000000u) | (d.bgr ? (r << 16) | (g << 8) | b : (b << 16) | (g << 8) | r);
+            l = jd_co_luma(r, g, b);
+        } else {
+            uint32_t c = *px;
+            for (uint32_t k = k0; k < k1; k++) c = jd_co_apply1(d.plan.op[k], d.plan.arg[k], mean, c);
+            if (k1 > k0) *px = (uint8_t)c;
+            l = c;
+        }
+    }
+    if (s >= d.plan.ncontrast) return;   /* the same for every thread of the CTA: one view */
+    __shared__ uint32_t part[JD_CO_THREADS / 32];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) l += __shfl_down_sync(0xFFFFFFFFu, l, o);
+    if ((threadIdx.x & 31u) == 0) part[threadIdx.x >> 5] = l;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned long long t = 0;
+        for (int k = 0; k < JD_CO_THREADS / 32; k++) t += part[k];
+        atomicAdd(&sums[(uint64_t)v * nsum + s], t);
+    }
+}
+
+/* ------------------------------------------------------------------------------------ */
 /* Tensor output (JPEGB200_batchCreateTensor): the pipeline has written each image's uint8  */
 /* output U tightly into the staging buffer; jdk_tensor looks every byte up in the C x 256  */
 /* table the host computed (jd_tensor_table) and stores the elements in CHW or HWC order.   */
