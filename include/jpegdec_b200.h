@@ -364,30 +364,40 @@ int JPEGB200_thumbnailPlan(int width, int height, int req_w, int req_h, double r
  *                     trip itself changes pixels, so h = 0 is not the identity (it is torchvision's adjust_hue(img, 0)).
  *       GRAYSCALE     to_grayscale(img, 3): R = G = B = L (arg ignored)
  *       SOLARIZE t    ImageOps.solarize(img, t): c < t ? c : 255 - c, t compared as a double
+ *       GAUSSIAN_BLUR r  img.filter(ImageFilter.GaussianBlur(r)) (Pillow's extended box filter, three passes per direction,
+ *                     edges replicated; DESIGN.md 4.2.10).  R, G and B are blurred independently, so the byte order does
+ *                     not matter; the alpha byte is kept.  r = 0 is the identity and is dropped; r < 0 gives the bytes of
+ *                     |r|.  Flips commute with the blur (symmetric window, clamped edges), so a recipe that blurs before
+ *                     its flip gets the same bytes from the orientation in the pixel stores.
  *     with L = (19595 R + 38470 G + 7471 B + 0x8000) >> 16 (convert("L")) and blend(a, b, f) = Image.blend: t = (float)a +
  *     (float)f * (float)(b - a) in float32; (uint8)t for 0 <= f <= 1, else clamped to 0 .. 255 and truncated.
- *   - 8-bit gray output (EIGHT_BIT_GRAYSCALE, JPEG_LUMA_ONLY) is a Pillow "L" image: brightness, contrast (m over the bytes)
- *     and solarize apply; saturation, hue and grayscale leave it unchanged, as in Pillow and torchvision.
+ *   - 8-bit gray output (EIGHT_BIT_GRAYSCALE, JPEG_LUMA_ONLY) is a Pillow "L" image: brightness, contrast (m over the bytes),
+ *     solarize and the blur apply; saturation, hue and grayscale leave it unchanged, as in Pillow and torchvision.
  *   - color_ops = NULL is JPEGB200_batchCreateBox, which forwards here.  A view whose row is empty stores F_v.  Factor 1
  *     and a solarize threshold above 255 store F_v too.  Status, batchErrMcu, the walked intervals, sizes, output bytes and
  *     the destination rules are those of the same call without operations; only the image's own bytes are rewritten.
  *   - Returns NULL with a message for RGB565, dithered pixel types and padded output when any view has an operation.  A view
- *     with an unknown op, an argument that is not finite or HUE outside [-0.5, 0.5] gets JPEG_INVALID_PARAMETER alone.
+ *     with an unknown op, an argument that is not finite, HUE outside [-0.5, 0.5] or a blur radius whose float32 magnitude
+ *     is 2^31 or more (|r| >= 2147483584; Pillow's box radius overflows there) gets JPEG_INVALID_PARAMETER alone.
  *     Negative factors are accepted: Pillow extrapolates.
  *   - Device work: the operations run in place on each view's uint8 result (the destination, the arena or the tensor
- *     staging).  A view's list is cut at each CONTRAST; each piece is one jdk_color launch over all views, and a piece
- *     before a contrast also sums L per view (exact, in 64 bits).  1 + the most CONTRAST operations of any view launches,
- *     none when no view has an operation; timed in the JPEGB200_T_DITHER slot and counted in JPEGB200_C_LAUNCHES. */
+ *     staging).  A view's list is cut at each CONTRAST and each GAUSSIAN_BLUR; at cut index s (0 = the list's start) the
+ *     call makes, over all views, the blur pair jdk_blur_h + jdk_blur_v when some view blurs there, then one jdk_color
+ *     launch when some view has a per-pixel operation before its next cut or a CONTRAST at it (that launch sums L per view,
+ *     exact in 64 bits).  Without blurs that is 1 + the most CONTRAST operations of any view; none when no view has an
+ *     operation.  The blur pair goes through a scratch copy of the blurred views (w x h x 4 or 1 bytes each), counted in the
+ *     one-call path's per-job scratch bound.  Timed in the JPEGB200_T_DITHER slot, counted in JPEGB200_C_LAUNCHES. */
 #define JPEGB200_COLOR_BRIGHTNESS 1
 #define JPEGB200_COLOR_CONTRAST   2
 #define JPEGB200_COLOR_SATURATION 3
 #define JPEGB200_COLOR_HUE        4
 #define JPEGB200_COLOR_GRAYSCALE  5
 #define JPEGB200_COLOR_SOLARIZE   6
+#define JPEGB200_COLOR_GAUSSIAN_BLUR 16
 #define JPEGB200_COLOR_MAX_OPS    8
 typedef struct {
     int32_t op;                        /* JPEGB200_COLOR_*, 0 = end of the view's list */
-    double arg;                        /* factor, hue shift (-0.5 .. 0.5) or solarize threshold */
+    double arg;                        /* factor, hue shift (-0.5 .. 0.5), solarize threshold or blur radius */
 } JPEGB200_ColorOp;
 JPEGB200_BATCH *JPEGB200_batchCreateColor(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
                                           const int32_t *views, int pixel_type, int options, const int32_t *rois,
@@ -494,8 +504,8 @@ int JPEGB200_decodeBatchBox(JPEGB200_CTX *ctx, const uint8_t *const *datas, cons
                             const double *reducing_gaps, void *const *outs, const int64_t *pitches, const int64_t *plane_strides,
                             int flags, int32_t *status);
 /* The same with colour operations per view (color_ops: V x JPEGB200_COLOR_MAX_OPS, semantics of JPEGB200_batchCreateColor;
- * NULL = JPEGB200_decodeBatchBox, which forwards here).  The jobs are those of the call without operations: the
- * operations need no scratch beyond 8 bytes per view and contrast. */
+ * NULL = JPEGB200_decodeBatchBox, which forwards here).  Without blurs the jobs are those of the call without operations
+ * (8 bytes of scratch per view and contrast); a blurred view's scratch copy counts in the per-job scratch bound. */
 int JPEGB200_decodeBatchColor(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
                               const int32_t *views, int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
                               const int32_t *out_sizes, int filter, const JPEGB200_TensorSpec *spec, const uint8_t *draft,

@@ -38,6 +38,7 @@ LAYOUT_CHW, LAYOUT_HWC = 0, 1
 SCALE_NONE, SCALE_DIV255, SCALE_MUL255 = 0, 1, 2
 # colour operations (JPEGB200_ColorOp): torchvision's ColorJitter / RandomGrayscale / RandomSolarize on PIL images
 COLOR_BRIGHTNESS, COLOR_CONTRAST, COLOR_SATURATION, COLOR_HUE, COLOR_GRAYSCALE, COLOR_SOLARIZE = 1, 2, 3, 4, 5, 6
+COLOR_GAUSSIAN_BLUR = 16   # (COLOR_GAUSSIAN_BLUR, r): Pillow's img.filter(ImageFilter.GaussianBlur(r))
 COLOR_MAX_OPS = 8
 TIMING_NAMES = ["h2d", "prescan", "entropy", "stitch", "idct", "dither", "d2h", "total"]
 COUNTER_NAMES = ["launches", "segments", "blocks", "events", "compressed_bytes", "output_bytes",

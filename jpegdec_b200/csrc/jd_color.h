@@ -1,7 +1,7 @@
 /*
  * jd_color.h -- torchvision's photometric transforms on PIL images (ColorJitter's adjust_brightness / _contrast /
  * _saturation / _hue, RandomGrayscale, RandomSolarize), restated per pixel as Pillow 12 computes them.  Shared by the kernel
- * (jd_kernels.cuh: jdk_color), the host plan (jd_host.c: jd_color_plan) and the CPU stepper (tests/colorsim).  DESIGN.md
+ * (jd_kernels.cuh: jdk_color), the host plan (jd_host.c: jd_color_plan) and the CPU steppers (tests/colorsim, tests/blursim).  DESIGN.md
  * 4.2.9 has the derivation and the probes.
  *
  *   L (convert("L")):     (19595 R + 38470 G + 7471 B + 0x8000) >> 16
@@ -13,6 +13,7 @@
  *   hue (shift byte d):   Pillow's RGB->HSV, H += d mod 256, Pillow's HSV->RGB (both below, exact over all 2^24 inputs)
  *   grayscale:            R = G = B = L
  *   solarize (threshold): c < thr ? c : 255 - c, thr = the number of bytes below the double threshold
+ *   Gaussian blur r:      ImageFilter.GaussianBlur(r), jd_blur.h (not a per-pixel operation: run by its own kernels)
  *
  * On a gray ("L") image brightness, contrast (m over the bytes themselves) and solarize apply; saturation, hue and grayscale
  * leave it alone, as they do in Pillow and torchvision.  Every float and double operation on the device goes through the
@@ -54,6 +55,7 @@
 #define JD_CO_HUE        4
 #define JD_CO_GRAYSCALE  5
 #define JD_CO_SOLARIZE   6
+#define JD_CO_BLUR       16   /* ImageFilter.GaussianBlur: run by jdk_blur (jd_blur.h); jd_co_apply3 / _apply1 skip it */
 #define JD_CO_MAX_OPS    8
 
 JD_CO_HD float jd_co_float(uint32_t bits)
@@ -160,14 +162,24 @@ JD_CO_HD uint32_t jd_co_apply1(uint32_t op, uint32_t arg, uint32_t mean, uint32_
     return c;
 }
 
-/* One view's list as the kernel runs it: ops cut into segments at each contrast.  Segment k (k = 0 .. ncontrast) is
- * op[seg[k] .. seg[k + 1]); segment k >= 1 starts with the contrast whose mean is sum k - 1, the sum of L over the output
- * of segment k - 1. */
+/* One view's list as the kernels run it: ops cut into segments at each contrast and each blur; ncontrast counts those
+ * cuts (without blurs every cut is a contrast, hence the name).  Segment k (k = 0 .. ncontrast) is op[seg[k] .. seg[k + 1]);
+ * segment k >= 1 starts with a contrast, whose mean is sum k - 1, the sum of L over the output of segment k - 1, or with a
+ * blur, which the blur kernels run before jdk_color runs the rest of the segment. */
 typedef struct {
     uint32_t nops, ncontrast;
     uint32_t op[JD_CO_MAX_OPS];
     uint32_t arg[JD_CO_MAX_OPS];
     uint32_t seg[JD_CO_MAX_OPS + 2];
 } JDColorPlan;
+
+/* A blur's integer constants (jd_blur.h), per op slot of the plan: box half-width ri and the 24-bit weights ww (inside the
+ * box) and fw (the two pixels just outside it) */
+typedef struct {
+    uint32_t ri, ww, fw;
+} JDBlur;
+typedef struct {
+    JDBlur b[JD_CO_MAX_OPS];
+} JDBlurPlan;
 
 #endif

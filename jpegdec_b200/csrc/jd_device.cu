@@ -179,6 +179,14 @@ struct JPEGB200_BATCH {
      * uint8 image in place, before jdk_tensor */
     bool color = false;
     std::vector<JDColorPlan> co_plans;
+    std::vector<JDBlurPlan> co_blur;        /* per view: each blur's constants at its op slot */
+    std::vector<int64_t> bl_scratch;        /* per view: its scratch copy's bytes when it blurs (256-byte aligned), else 0 */
+    int64_t bl_scratch_total = 0;
+    std::vector<JDBlurDesc> bl_desc;        /* per blur launch pair, per view blurring there */
+    std::vector<uint32_t> bl_blk;           /* the same entries: first CTA of the horizontal, then of the vertical kernel */
+    DevBuf<JDBlurDesc> d_bl_desc;
+    DevBuf<uint32_t> d_bl_blk;
+    DevBuf<uint8_t> d_bl;                   /* the scratch copies */
     std::vector<uint8_t> co_bgr;
     std::vector<JDColorDesc> co_desc;
     std::vector<uint32_t> co_blk;           /* per launch, per view: its first CTA */
@@ -615,7 +623,7 @@ static void init_batch(JPEGB200_BATCH *b, JPEGB200_CTX *ctx, const CreatePlan &P
     b->box = P.boxes != nullptr || P.gaps != nullptr;
     if (b->box) b->bx_plans.assign(nv, JDBoxPlan{});
     b->color = P.color != nullptr;
-    if (b->color) { b->co_plans.assign(nv, JDColorPlan{}); b->co_bgr.assign(nv, 0); }
+    if (b->color) { b->co_plans.assign(nv, JDColorPlan{}); b->co_blur.assign(nv, JDBlurPlan{}); b->bl_scratch.assign(nv, 0); b->co_bgr.assign(nv, 0); }
     b->lj = (options & JPEGB200_OPT_LIBJPEG) != 0;
     if (b->lj) { b->lj_desc.assign(nv, JDLjDesc{}); b->lj_plane.assign(nv, 0); }
     b->tensor = P.spec != nullptr;
@@ -797,7 +805,7 @@ static uint32_t plan_views(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int 
         bool dropped = false;
         for (int i = v0; i < v0 + nvf; i++) {
             if (!P.vok[i]) continue;
-            if (!jd_color_plan(P.color + JPEGB200_COLOR_MAX_OPS * (size_t)i, b->ptclass == JD_PT_GRAY, &b->co_plans[i])) {
+            if (!jd_color_plan_blur(P.color + JPEGB200_COLOR_MAX_OPS * (size_t)i, b->ptclass == JD_PT_GRAY, &b->co_plans[i], &b->co_blur[i])) {
                 P.vok[i] = 0;
                 dropped = true;
             }
@@ -1015,8 +1023,16 @@ static int plan_view_output(JPEGB200_BATCH *b, CreatePlan &P, int f, int i)
         const bool bgr = !b->lj && jd_rgb8888_is_bgr(b->ctx->arith, b->sshift, inf.ncomp, inf.subsample) != 0;
         b->tn_swap[i] = (uint8_t)(b->tn_nc == 3 && bgr != (b->tn_spec.bgr != 0));
     }
-    if (b->color)   /* the colour operations read true R, G, B: a libjpeg decode stores R, G, B for every file */
+    if (b->color) {   /* the colour operations read true R, G, B: a libjpeg decode stores R, G, B for every file */
         b->co_bgr[i] = (uint8_t)(b->ptclass == JD_PT_8888 && !b->lj && jd_rgb8888_is_bgr(b->ctx->arith, b->sshift, inf.ncomp, inf.subsample));
+        const JDColorPlan &cp = b->co_plans[i];
+        bool blurs = false;
+        for (uint32_t k = 0; k < cp.nops; k++) blurs = blurs || cp.op[k] == JD_CO_BLUR;
+        if (blurs) {
+            b->bl_scratch[i] = (int64_t)align256((size_t)vd.out_w * vd.out_h * bytes_per_pixel_class(b->ptclass));
+            b->bl_scratch_total += b->bl_scratch[i];
+        }
+    }
     size_t pitch;
     if (b->tensor) pitch = (size_t)vd.out_w * (b->tn_spec.layout == JPEGB200_LAYOUT_HWC ? b->tn_nc : 1) * b->tn_elt;
     else if (b->dither_bits) {
@@ -1529,7 +1545,9 @@ struct DecodeState {
     uint32_t tn_ctas = 0, rs_ctas[4] = {0u, 0u, 0u, 0u};
     uint32_t bx_ctas[2] = {0u, 0u};         /* box batches: jdk_resize_coeffs_box, jdk_reduce */
     std::vector<uint32_t> co_ctas;          /* colour operations: CTAs of each jdk_color launch */
-    uint32_t co_nsum = 0;                   /* sum slots per view: the most contrasts of any view */
+    std::vector<uint32_t> bl_first;         /* blurs: the first bl_desc entry of each cut index (one past the last at nl) */
+    std::vector<uint32_t> bl_ctas;          /* CTAs of each cut index's jdk_blur pair: horizontal, vertical */
+    uint32_t co_nsum = 0;                   /* sum slots per view: the most cuts (contrasts and blurs) of any view */
     int launches = 0;
 };
 
@@ -1643,7 +1661,8 @@ static int stage_tensor(JPEGB200_BATCH *b, DecodeState &D)
 }
 
 /* colour operations: where each view's final uint8 image lies before the resize and dither stages redirect the stages
- * before them (D.pipe_out + out_off, out_pitch).  Uploads co_desc, the per-launch CTA starts and zeroed contrast sums. */
+ * before them (D.pipe_out + out_off, out_pitch).  Uploads co_desc, the per-launch CTA starts and zeroed contrast sums, and
+ * for the blurs bl_desc (the views blurring at each cut index, in cut order) with their CTA starts. */
 static int stage_color(JPEGB200_BATCH *b, DecodeState &D)
 {
     const int n = b->n;
@@ -1666,8 +1685,46 @@ static int stage_color(JPEGB200_BATCH *b, DecodeState &D)
         c.bgr = b->co_bgr[i];
         c.plan = p;
         const uint64_t per = ((uint64_t)c.w * c.h + JD_CO_THREADS - 1) / JD_CO_THREADS;
-        for (uint32_t s = 0; s <= p.ncontrast; s++)   /* segment s has operations, or sums for the contrast after it */
-            if (p.seg[s] < p.seg[s + 1] || s < p.ncontrast) ctas[s] += per;
+        for (uint32_t s = 0; s <= p.ncontrast; s++) {
+            /* segment s has per-pixel operations after its blur, or sums L for the contrast after it */
+            const uint32_t k0 = p.seg[s] + (p.seg[s] < p.seg[s + 1] && p.op[p.seg[s]] == JD_CO_BLUR ? 1u : 0u);
+            if (k0 < p.seg[s + 1] || (s < p.ncontrast && p.op[p.seg[s + 1]] == JD_CO_CONTRAST)) ctas[s] += per;
+        }
+    }
+    /* blurs: at cut index s, the views whose segment s starts with one */
+    b->bl_desc.clear();
+    D.bl_first.assign(nl + 1, 0);
+    D.bl_ctas.assign(2 * (size_t)nl, 0);
+    std::vector<uint32_t> hblk, vblk;
+    uint64_t soff = 0;
+    std::vector<uint64_t> soffs(n, 0);
+    for (int i = 0; i < n; i++)
+        if (b->bl_scratch[i] && b->parse_status[i] == JPEG_SUCCESS) { soffs[i] = soff; soff += (uint64_t)b->bl_scratch[i]; }
+    for (uint32_t s = 1; s < nl; s++) {
+        D.bl_first[s] = (uint32_t)b->bl_desc.size();
+        for (int i = 0; i < n; i++) {
+            const JDColorPlan &p = b->co_plans[i];
+            if (b->parse_status[i] != JPEG_SUCCESS || s > p.ncontrast || p.op[p.seg[s]] != JD_CO_BLUR) continue;
+            JDBlurDesc x{};
+            x.off = b->co_desc[i].off; x.pitch = b->co_desc[i].pitch; x.soff = soffs[i];
+            x.w = b->co_desc[i].w; x.h = b->co_desc[i].h;
+            x.k = b->co_blur[i].b[p.seg[s]];
+            b->bl_desc.push_back(x);
+            hblk.push_back(D.bl_ctas[2 * s]); vblk.push_back(D.bl_ctas[2 * s + 1]);
+            D.bl_ctas[2 * s] += (x.h + JD_BL_THREADS / 32 - 1) / (JD_BL_THREADS / 32);   /* 8 rows per CTA */
+            D.bl_ctas[2 * s + 1] += (x.w + 31) / 32;                                       /* 32 columns per CTA */
+        }
+    }
+    D.bl_first[nl] = (uint32_t)b->bl_desc.size();
+    if (!b->bl_desc.empty()) {
+        const size_t m = b->bl_desc.size();
+        b->bl_blk = hblk;
+        b->bl_blk.insert(b->bl_blk.end(), vblk.begin(), vblk.end());
+        CK(b->d_bl_desc.alloc(&b->ctx->pool, m));
+        CK(b->d_bl_blk.alloc(&b->ctx->pool, 2 * m));
+        CK(b->d_bl.alloc(&b->ctx->pool, soff));
+        CK(cudaMemcpyAsync(b->d_bl_desc.p, b->bl_desc.data(), sizeof(JDBlurDesc) * m, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(b->d_bl_blk.p, b->bl_blk.data(), sizeof(uint32_t) * 2 * m, cudaMemcpyHostToDevice, st));
     }
     D.co_ctas.assign(nl, 0);
     for (uint32_t s = 0; s < nl; s++) {
@@ -2157,12 +2214,27 @@ static void run_resize(JPEGB200_BATCH *b, DecodeState &D)
 #undef JD_RS_ARGS
 }
 
-/* timed in the dither slot too, after the resize: one launch per segment of the operation lists */
+/* timed in the dither slot too, after the resize: per cut index of the operation lists, the blur pair for the views that
+ * blur there, then jdk_color for the per-pixel operations up to the next cut */
 static void run_color(JPEGB200_BATCH *b, DecodeState &D)
 {
     cudaStream_t st = b->ss.stream;
     const uint32_t n = (uint32_t)b->n;
+    const size_t m = b->bl_desc.size();
     for (uint32_t s = 0; s < (uint32_t)D.co_ctas.size(); s++) {
+        const uint32_t f = D.bl_first[s], nb = D.bl_first[s + 1] - f;
+        if (nb) {
+            const JDBlurDesc *bd = b->d_bl_desc.p + f;
+            const uint32_t *hb = b->d_bl_blk.p + f, *vb = b->d_bl_blk.p + m + f;
+            if (b->ptclass == JD_PT_GRAY) {
+                jdk_blur<1, false><<<D.bl_ctas[2 * s], JD_BL_THREADS, 0, st>>>(bd, hb, nb, D.pipe_out, b->d_bl.p);
+                jdk_blur<1, true><<<D.bl_ctas[2 * s + 1], JD_BL_THREADS, 0, st>>>(bd, vb, nb, D.pipe_out, b->d_bl.p);
+            } else {
+                jdk_blur<4, false><<<D.bl_ctas[2 * s], JD_BL_THREADS, 0, st>>>(bd, hb, nb, D.pipe_out, b->d_bl.p);
+                jdk_blur<4, true><<<D.bl_ctas[2 * s + 1], JD_BL_THREADS, 0, st>>>(bd, vb, nb, D.pipe_out, b->d_bl.p);
+            }
+            D.launches += 2;
+        }
         if (!D.co_ctas[s]) continue;
         if (b->ptclass == JD_PT_GRAY)
             jdk_color<1><<<D.co_ctas[s], JD_CO_THREADS, 0, st>>>(b->d_co_desc.p, b->d_co_blk.p + (size_t)s * n, n, s, b->d_co_sum.p, D.co_nsum, D.pipe_out);
@@ -2548,13 +2620,15 @@ extern "C" int JPEGB200_decodeBatchColor(JPEGB200_CTX *ctx, const uint8_t *const
                 }
             }
         }
-        if ((b->resize || b->tensor || b->pplane_total || b->lj) && cnt > 1 &&
-            b->rs_scratch_total + b->tn_stage_total + b->pplane_total + b->lj_plane_total > JD_JOB_RESIZE_SCRATCH) {
+        if ((b->resize || b->tensor || b->pplane_total || b->lj || b->bl_scratch_total) && cnt > 1 &&
+            b->rs_scratch_total + b->tn_stage_total + b->pplane_total + b->lj_plane_total + b->bl_scratch_total > JD_JOB_RESIZE_SCRATCH) {
             /* scratch of a job (resize: S + the reduced image of a box batch + intermediate; tensor: the uint8 staging; libjpeg decodes: the sample planes;
-             * progressive files: the coefficient plane, counted on the file's first view): at most JD_JOB_RESIZE_SCRATCH, or
+             * progressive files: the coefficient plane, counted on the file's first view; blurs: the scratch copy): at most JD_JOB_RESIZE_SCRATCH, or
              * one file with all of its views */
             std::vector<int64_t> sc(cv);
-            for (int i = 0; i < cv; i++) sc[i] = (b->resize ? b->rs_scratch[i] : 0) + (b->tensor ? b->tn_stage[i] : 0) + (b->lj ? b->lj_plane[i] : 0);
+            for (int i = 0; i < cv; i++)
+                sc[i] = (b->resize ? b->rs_scratch[i] : 0) + (b->tensor ? b->tn_stage[i] : 0) + (b->lj ? b->lj_plane[i] : 0) +
+                        (b->color ? b->bl_scratch[i] : 0);
             for (int i = 0; i < cv; i++) if (i == 0 || file_of(b, i) != file_of(b, i - 1)) sc[i] += b->pplane[file_of(b, i)];
             int32_t cv3 = 0, capped3 = 0;
             const int c = jd_job_files(cnt, sizes + i0, vi, INT64_MAX, INT64_MAX, sc.data(), JD_JOB_RESIZE_SCRATCH, &cv3, &capped3);

@@ -742,15 +742,51 @@ int jd_check_box(const int32_t *out_sizes, const double *boxes, const double *ga
 }
 
 /* ---- colour operations (JPEGB200_batchCreateColor, jd_color.h) ---- */
+/* GaussianBlur(r)'s box constants (DESIGN.md 4.2.10): every step in float32, as probing Pillow 12.2 pins it (the same steps
+ * in double miss).  r = |radius| as float, 0 < r < 2^31. */
+int jd_blur_consts(float r, JDBlur *out)
+{
+    const float s2 = r * r / 3.0f;
+    const float L = sqrtf(12.0f * s2 + 1.0f);
+    const float l = floorf((L - 1.0f) / 2.0f);
+    const float a = (2.0f * l + 1.0f) * (l * (l + 1.0f) - 3.0f * s2) / (6.0f * (s2 - (l + 1.0f) * (l + 1.0f)));
+    const float rb = l + a;
+    if (!(rb >= 0.0f && rb < 2147483648.0f)) return 0;
+    out->ri = (uint32_t)(int32_t)rb;
+    out->ww = (uint32_t)(16777216.0f / (2.0f * rb + 1.0f));
+    out->fw = (uint32_t)((16777216ull - (2ull * out->ri + 1ull) * out->ww) / 2ull);
+    return 1;
+}
+
 int jd_color_plan(const JPEGB200_ColorOp *row, int gray, JDColorPlan *plan)
 {
+    return jd_color_plan_blur(row, gray, plan, NULL);
+}
+
+int jd_color_plan_blur(const JPEGB200_ColorOp *row, int gray, JDColorPlan *plan, JDBlurPlan *blur)
+{
     memset(plan, 0, sizeof(*plan));
+    if (blur) memset(blur, 0, sizeof(*blur));
     for (int k = 0; k < JPEGB200_COLOR_MAX_OPS && row[k].op != 0; k++) {
         const int op = row[k].op;
         const double a = row[k].arg;
-        if (op < JPEGB200_COLOR_BRIGHTNESS || op > JPEGB200_COLOR_SOLARIZE || !isfinite(a)) return 0;
+        if ((op < JPEGB200_COLOR_BRIGHTNESS || op > JPEGB200_COLOR_SOLARIZE) && op != JPEGB200_COLOR_GAUSSIAN_BLUR) return 0;
+        if (!isfinite(a)) return 0;
         if (op == JPEGB200_COLOR_HUE && !(a >= -0.5 && a <= 0.5)) return 0;   /* torchvision raises there */
         if (gray && (op == JPEGB200_COLOR_SATURATION || op == JPEGB200_COLOR_HUE || op == JPEGB200_COLOR_GRAYSCALE)) continue;
+        if (op == JPEGB200_COLOR_GAUSSIAN_BLUR) {
+            /* Pillow takes the radius as a float: |r| rounding to 2^31 or more overflows its int box radius */
+            const float r = fabsf((float)a);
+            JDBlur c;
+            if (!(r < 2147483648.0f) || !jd_blur_consts(r, &c)) return 0;
+            if (r == 0.0f) continue;   /* the identity */
+            if (blur) blur->b[plan->nops] = c;
+            plan->seg[++plan->ncontrast] = plan->nops;
+            plan->op[plan->nops] = (uint32_t)op;
+            plan->arg[plan->nops] = 0u;
+            plan->nops++;
+            continue;
+        }
         uint32_t bits;
         if (op == JPEGB200_COLOR_HUE) bits = (uint32_t)(uint8_t)(int32_t)(a * 255.0);   /* np.int32(h * 255).astype(uint8) */
         else if (op == JPEGB200_COLOR_SOLARIZE) bits = a <= 0.0 ? 0u : a > 255.0 ? 256u : (uint32_t)ceil(a);   /* bytes c < a */

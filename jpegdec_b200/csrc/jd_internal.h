@@ -169,11 +169,16 @@ int jd_box_plan(int sw, int sh, int out_w, int out_h, int filter, const double *
 int jd_check_box(const int32_t *out_sizes, const double *boxes, const double *gaps, char *msg, int msg_len);
 
 /* Colour operations of one view (JPEGB200_batchCreateColor, jd_color.h): row = its JPEGB200_COLOR_MAX_OPS entries.  Writes
- * the plan the kernel runs -- factors as float bits, hue shift bytes, solarize thresholds as the count of bytes below them,
- * the segments cut at each contrast; on a gray view (gray != 0) saturation, hue and grayscale are dropped.  Returns 0 for
- * an unknown op, an argument that is not finite, or a hue outside [-0.5, 0.5]. */
+ * the plan the kernels run -- factors as float bits, hue shift bytes, solarize thresholds as the count of bytes below them,
+ * the segments cut at each contrast and each blur; on a gray view (gray != 0) saturation, hue and grayscale are dropped.
+ * Blurs of radius 0 are dropped, negative radii planned as |r|, and each blur's constants written to blur (when not NULL)
+ * at its op slot.  Returns 0 for an unknown op, an argument that is not finite, a hue outside [-0.5, 0.5], or a blur
+ * radius whose float32 magnitude is 2^31 or more.  jd_color_plan is the same without the blur constants. */
 #include "jd_color.h"
+int jd_color_plan_blur(const JPEGB200_ColorOp *row, int gray, JDColorPlan *plan, JDBlurPlan *blur);
 int jd_color_plan(const JPEGB200_ColorOp *row, int gray, JDColorPlan *plan);
+/* GaussianBlur(r)'s box half-width and 24-bit weights for r = |radius| as float32, 0 < r < 2^31 (0 past that) */
+int jd_blur_consts(float r, JDBlur *out);
 /* Batch-level rule of JPEGB200_batchCreateColor: no operation on RGB565, dithered pixel types or padded output (checked
  * over the nv rows).  0 with a message otherwise. */
 int jd_check_color(int pixel_type, int options, int64_t nv, const JPEGB200_ColorOp *color_ops, char *msg, int msg_len);

@@ -2218,6 +2218,82 @@ __global__ void __launch_bounds__(JD_CO_THREADS) jdk_color(const JDColorDesc *cd
 }
 
 /* ------------------------------------------------------------------------------------ */
+/* Gaussian blur (JPEGB200_COLOR_GAUSSIAN_BLUR, jd_blur.h): one launch pair per cut index   */
+/* at which some view blurs, over those views only.  jdk_blur<BPP, false> runs the three    */
+/* horizontal passes image -> scratch -> image -> scratch, jdk_blur<BPP, true> the three    */
+/* vertical ones scratch -> image -> scratch -> image: the image ends blurred, and only its */
+/* row bytes are written.  A CTA owns whole lines (8 rows or 32 columns), so its passes     */
+/* need no grid-wide order; each line is cut into G chunks, one per thread (32 per row, 8   */
+/* per column, so a warp reads 32 adjacent columns of one row).                             */
+/* ------------------------------------------------------------------------------------ */
+#include "jd_blur.h"
+#define JD_BL_THREADS 256
+struct JDBlurDesc {
+    uint64_t off;              /* the view's image from the launch's base */
+    uint64_t pitch;            /* bytes between its rows */
+    uint64_t soff;             /* its scratch copy (rows w * BPP bytes apart) from the scratch base */
+    uint32_t w, h;
+    JDBlur k;
+    uint32_t pad;
+};
+
+/* cblk: this launch's first CTA of every blurred view (ceil(h / 8) CTAs each horizontally, ceil(w / 32) vertically) */
+template <int BPP, bool VERT>
+__global__ void __launch_bounds__(JD_BL_THREADS) jdk_blur(const JDBlurDesc *bd, const uint32_t *cblk, uint32_t n, uint8_t *base,
+                                                          uint8_t *scratch)
+{
+    constexpr uint32_t G = VERT ? 8u : 32u, LINES = JD_BL_THREADS / G;
+    constexpr int NC = JD_BL_NC(BPP);
+    uint32_t lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (cblk[mid] <= blockIdx.x) lo = mid; else hi = mid - 1;
+    }
+    const JDBlurDesc &d = bd[lo];
+    const uint32_t li = VERT ? threadIdx.x % LINES : threadIdx.x / G, ch = VERT ? threadIdx.x / LINES : threadIdx.x % G;
+    const uint32_t line = (blockIdx.x - cblk[lo]) * LINES + li;
+    const uint32_t len = VERT ? d.h : d.w;
+    const bool live = line < (VERT ? d.w : d.h);
+    const uint64_t spitch = (uint64_t)d.w * BPP;
+    uint8_t *pi = base + d.off + (VERT ? (uint64_t)line * BPP : (uint64_t)line * d.pitch);
+    uint8_t *ps = scratch + d.soff + (VERT ? (uint64_t)line * BPP : (uint64_t)line * spitch);
+    const int64_t istep = VERT ? (int64_t)d.pitch : BPP, sstep = VERT ? (int64_t)spitch : BPP;
+    const uint32_t C = (len + G - 1) / G, c0 = min(len, ch * C), c1 = min(len, c0 + C);
+    __shared__ uint32_t part[NC][G][LINES];   /* chunk totals per channel (below 2^24: 65535 x 255) */
+    for (int pass = 0; pass < 3; pass++) {
+        const bool from_img = VERT ? (pass & 1) != 0 : (pass & 1) == 0;
+        const uint8_t *src = from_img ? pi : ps;
+        uint8_t *dst = from_img ? ps : pi;
+        const int64_t ss = from_img ? istep : sstep, ds = from_img ? sstep : istep;
+        uint64_t acc[NC];
+        for (int c = 0; c < NC; c++) acc[c] = 0;
+        if (live) jd_bl_sum<BPP>(src, ss, c0, c1, acc);
+        for (int c = 0; c < NC; c++) part[c][ch][li] = (uint32_t)acc[c];
+        __syncthreads();
+        if (live && c0 < c1) {
+            /* the chunk totals before the window's two ends */
+            const uint32_t wlo = c0 > d.k.ri ? c0 - d.k.ri : 0u;
+            const uint64_t e = (uint64_t)c0 + d.k.ri + 1u;
+            const uint32_t qlo = wlo / C, qhi = (e > len ? len : (uint32_t)e) / C;
+            uint32_t pre_lo[NC], pre_hi[NC];
+            for (int c = 0; c < NC; c++) {
+                uint32_t t = 0;
+                for (uint32_t q = 0; q < G; q++) {
+                    if (q == qlo) pre_lo[c] = t;
+                    if (q == qhi) pre_hi[c] = t;
+                    t += part[c][q][li];
+                }
+                if (qhi >= G) pre_hi[c] = t;
+            }
+            uint64_t S[NC];
+            jd_bl_start<BPP>(src, ss, len, c0, d.k.ri, C, pre_lo, pre_hi, S);
+            jd_bl_run<BPP>(src, ss, dst, ds, len, c0, c1, S, d.k);
+        }
+        __syncthreads();
+    }
+}
+
+/* ------------------------------------------------------------------------------------ */
 /* Tensor output (JPEGB200_batchCreateTensor): the pipeline has written each image's uint8  */
 /* output U tightly into the staging buffer; jdk_tensor looks every byte up in the C x 256  */
 /* table the host computed (jd_tensor_table) and stores the elements in CHW or HWC order.   */
