@@ -527,31 +527,11 @@ class Batch:
         self._draft = _draft_array(draft, n)
         self._box, self._gap = _box_array(box, n), _gap_array(reducing_gap, n)
         self._color = _color_array(color, n)
-        if color is not None:
-            self._spec = spec
-            self.h = lib().JPEGB200_batchCreateColor(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
-                                                     self._rois, self._orients, self._out_sizes, int(filter),
-                                                     C.byref(spec) if spec is not None else None, self._draft, self._box,
-                                                     self._gap, self._color)
-        elif box is not None or reducing_gap is not None:
-            self._spec = spec
-            self.h = lib().JPEGB200_batchCreateBox(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
-                                                   self._rois, self._orients, self._out_sizes, int(filter),
-                                                   C.byref(spec) if spec is not None else None, self._draft, self._box,
-                                                   self._gap)
-        elif draft is not None:
-            self._spec = spec
-            self.h = lib().JPEGB200_batchCreateDraft(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
-                                                     self._rois, self._orients, self._out_sizes, int(filter),
-                                                     C.byref(spec) if spec is not None else None, self._draft)
-        elif spec is None and views is None:
-            self.h = lib().JPEGB200_batchCreateResized(ctx.h, self._ptrs, self._sizes, n, pixel_type, options, self._rois,
-                                                       self._orients, self._out_sizes, int(filter))
-        else:   # views and / or a TensorSpec (device outputs only): JPEGB200_batchCreateViews
-            self._spec = spec
-            self.h = lib().JPEGB200_batchCreateViews(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
-                                                     self._rois, self._orients, self._out_sizes, int(filter),
-                                                     C.byref(spec) if spec is not None else None)
+        self._spec = spec
+        self.h = lib().JPEGB200_batchCreateColor(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
+                                                 self._rois, self._orients, self._out_sizes, int(filter),
+                                                 C.byref(spec) if spec is not None else None, self._draft, self._box,
+                                                 self._gap, self._color)
         if not self.h:
             raise RuntimeError("batchCreate failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
 
@@ -645,28 +625,10 @@ def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flag
     oa = (C.c_void_p * n)(*outs)
     pi = (C.c_int64 * n)(*pitches) if pitches is not None else None
     st = (C.c_int32 * n)()
-    if color is not None:
-        rc = lib().JPEGB200_decodeBatchColor(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
-                                             _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None,
-                                             _draft_array(draft, n), _box_array(box, n), _gap_array(reducing_gap, n),
-                                             _color_array(color, n), oa, pi, None, flags, st)
-    elif box is not None or reducing_gap is not None:
-        rc = lib().JPEGB200_decodeBatchBox(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
-                                           _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None,
-                                           _draft_array(draft, n), _box_array(box, n), _gap_array(reducing_gap, n), oa, pi,
-                                           None, flags, st)
-    elif draft is not None:
-        rc = lib().JPEGB200_decodeBatchDraft(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
-                                             _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None,
-                                             _draft_array(draft, n), oa, pi, None, flags, st)
-    elif views is None:
-        rc = lib().JPEGB200_decodeBatchResized(ctx.h, pa, sa, n, pixel_type, options, _roi_array(rois, n),
-                                               _orient_array(orients, n), _size_array(out_sizes, n), int(filter), oa, pi, flags,
-                                               st)
-    else:
-        rc = lib().JPEGB200_decodeBatchViews(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
-                                             _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None, oa, pi,
-                                             None, flags, st)
+    rc = lib().JPEGB200_decodeBatchColor(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
+                                         _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None,
+                                         _draft_array(draft, n), _box_array(box, n), _gap_array(reducing_gap, n),
+                                         _color_array(color, n), oa, pi, None, flags, st)
     cnt = (C.c_int64 * len(COUNTER_NAMES))()
     lib().JPEGB200_lastCallCounters(ctx.h, cnt)
     return rc, list(st), dict(zip(COUNTER_NAMES, list(cnt)))

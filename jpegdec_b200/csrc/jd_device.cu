@@ -141,11 +141,10 @@ struct DevBuf {
 struct JPEGB200_BATCH {
     JPEGB200_CTX *ctx = nullptr;
     int n = 0;                      /* images (views with JPEGB200_batchCreateViews): everything per image is per view */
-    /* views (JPEGB200_batchCreateViews): nf files, each walked once through its entropy-facing descriptor fdescs[f]
-     * (d_fdescs); descs[i] is view i's descriptor for the IDCT and after it, carrying its file's seg / blk / rec bases.
-     * Without views nf = n and descs serves both (fdescs and vfile stay empty). */
+    /* nf files, each walked once through its entropy-facing descriptor fdescs[f] (d_fdescs), where the kernels write its
+     * status; descs[i] is view i's descriptor for the IDCT and after it, carrying its file's seg / blk / rec bases.
+     * Without views every file has one view: n = nf and vfile[i] = i. */
     int nf = 0;
-    bool views = false;
     std::vector<int32_t> vfile;     /* per view: its file */
     std::vector<JDImageDesc> fdescs;
     DevBuf<JDImageDesc> d_fdescs;
@@ -284,11 +283,6 @@ struct JPEGB200_BATCH {
 };
 
 static char *ctx_err() { return g_err; }
-
-/* the file of image (view) i, and the entropy-facing descriptors (one per file) on the host and the device */
-static inline int file_of(const JPEGB200_BATCH *b, int i) { return b->views ? b->vfile[i] : i; }
-static inline std::vector<JDImageDesc> &file_descs(JPEGB200_BATCH *b) { return b->views ? b->fdescs : b->descs; }
-static inline JDImageDesc *file_descs_dev(JPEGB200_BATCH *b) { return b->views ? b->d_fdescs.p : b->d_descs.p; }
 
 #define JD_EVENT_CAP (1u << 20)
 #define JD_CHUNK_PASSES 6     /* restart-free scans: entry-state passes per decode (from the third on only moved chunks are parsed; the last one verifies) */
@@ -568,7 +562,8 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateTensor(JPEGB200_CTX *ctx, const u
  * one file's steps hand to the next file's. ---- */
 struct CreatePlan {
     const uint8_t *const *datas = nullptr;
-    const int32_t *sizes = nullptr, *views = nullptr, *rois = nullptr, *out_sizes = nullptr;
+    const int32_t *sizes = nullptr, *rois = nullptr, *out_sizes = nullptr;
+    const int32_t *views = nullptr;     /* per file: its view count (all ones for a call without views) */
     const uint8_t *orients = nullptr;
     const JPEGB200_TensorSpec *spec = nullptr;
     const uint8_t *draft = nullptr;     /* per view: draft scale denominator (JPEGB200_batchCreateDraft), NULL = 1 */
@@ -601,7 +596,6 @@ static void init_batch(JPEGB200_BATCH *b, JPEGB200_CTX *ctx, const CreatePlan &P
     b->ctx = ctx;
     b->n = nv;
     b->nf = n;
-    b->views = P.views != nullptr;
     b->roi = P.rois != nullptr || P.orients != nullptr;
     b->plans.assign(nv, JDRoiPlan{});   /* read with rois or orients only */
     b->exif_tag.assign(nv, 0);
@@ -643,11 +637,9 @@ static void init_batch(JPEGB200_BATCH *b, JPEGB200_CTX *ctx, const CreatePlan &P
     b->datas.assign(P.datas, P.datas + n);
     b->sizes.assign(P.sizes, P.sizes + n);
     b->descs.resize(nv);
-    if (b->views) {
-        b->fdescs.resize(n);
-        b->vfile.resize(nv);
-        for (int f = 0, i = 0; f < n; f++) for (int k = 0; k < P.views[f]; k++) b->vfile[i++] = f;
-    }
+    b->fdescs.resize(n);
+    b->vfile.resize(nv);
+    for (int f = 0, i = 0; f < n; f++) for (int k = 0; k < P.views[f]; k++) b->vfile[i++] = f;
     b->quant.assign((size_t)nv * 192, 0);   /* per view: the IDCT kernels index it by their descriptor's index */
     b->outs.assign(nv, nullptr);
     b->pitches.assign(nv, 0);
@@ -835,12 +827,11 @@ static void size_file_walk(const JPEGB200_BATCH *b, int f, FileAdmit &a)
 /* a file that is not walked: harmless empty descriptors for it and its views */
 static void fill_refused_descs(JPEGB200_BATCH *b, const CreatePlan &P, int f, int v0, int nvf, int status)
 {
-    JDImageDesc &d = file_descs(b)[f];
+    JDImageDesc &d = b->fdescs[f];
     d.nseg = 0; d.seg_base = P.seg; d.blk_base = (uint32_t)P.blk; d.status = (uint32_t)status;
     for (int i = v0; i < v0 + nvf; i++) {
-        JDImageDesc &vd = b->descs[i];
-        if (b->views) vd = d;
-        vd.status = (uint32_t)b->parse_status[i];
+        b->descs[i] = d;
+        b->descs[i].status = (uint32_t)b->parse_status[i];
     }
 }
 
@@ -881,7 +872,7 @@ static uint32_t lut_set_for(JPEGB200_BATCH *b, CreatePlan &P, int f)
 static void fill_file_desc(JPEGB200_BATCH *b, const CreatePlan &P, int f, const FileAdmit &a, uint32_t walk, uint32_t lutset)
 {
     const JDInfo &inf = b->infos[f];
-    JDImageDesc &d = file_descs(b)[f];
+    JDImageDesc &d = b->fdescs[f];
     d.scan_off = (uint32_t)(b->comp_off[f] + inf.scan_offset);
     d.scan_end = (uint32_t)(b->comp_off[f] + b->sizes[f]);
     d.width = (uint16_t)inf.width; d.height = (uint16_t)inf.height;
@@ -945,21 +936,20 @@ static void add_prog_file(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int n
 
 /* View i of admitted file f: the file's descriptor (its walk, blocks and records) with the view's rectangle, orientation and
  * output.  Writes descs[i], pitches[i], arena_off[i] and the view's libjpeg box, resize plan + scratch and tensor staging;
- * advances P.out_total / P.gray_total.  The file's own descriptor keeps roi_mcu_end = 0: jdk_stitch reports its first
- * error, jd_view_err_mcu judges it per view.  0 with a message when the resize cannot be planned. */
+ * advances P.out_total / P.gray_total.  roi_mcu_end goes into the view's descriptor only: jdk_stitch reports the file's
+ * first error, jd_view_err_mcu (JPEGB200_batchErrMcu) judges it per view.  0 with a message when the resize cannot be
+ * planned. */
 static int plan_view_output(JPEGB200_BATCH *b, CreatePlan &P, int f, int i)
 {
     const JDInfo &inf = b->infos[f];
     const int s = b->lj ? (int)b->lj_desc[i].shift : b->sshift;   /* a libjpeg batch scales per view (draft) */
     JDImageDesc &vd = b->descs[i];
-    if (b->views) {
-        if (b->parse_status[i] != JPEG_SUCCESS) {   /* an invalid view of a walked file: empty, like a refused image */
-            memset(&vd, 0, sizeof(vd));
-            vd.seg_base = P.seg; vd.blk_base = (uint32_t)P.blk; vd.status = (uint32_t)b->parse_status[i];
-            return 1;
-        }
-        vd = b->fdescs[f];
+    if (b->parse_status[i] != JPEG_SUCCESS) {   /* an invalid view of a walked file: empty, like a refused image */
+        memset(&vd, 0, sizeof(vd));
+        vd.seg_base = P.seg; vd.blk_base = (uint32_t)P.blk; vd.status = (uint32_t)b->parse_status[i];
+        return 1;
     }
+    vd = b->fdescs[f];
     vd.out_w = (uint32_t)((inf.width + (1 << s) - 1) >> s);
     vd.out_h = (uint32_t)((inf.height + (1 << s) - 1) >> s);
     if (b->padded) {
@@ -1066,7 +1056,7 @@ static void sort_prog_waves(JPEGB200_BATCH *b)
 static void build_work_list(JPEGB200_BATCH *b)
 {
     b->seg_img.resize(b->nseg ? b->nseg : 1);
-    const std::vector<JDImageDesc> &fd = file_descs(b);
+    const std::vector<JDImageDesc> &fd = b->fdescs;
     for (uint32_t li = 0; li < (b->nlut ? b->nlut : 1); li++) {
         for (int i = 0; i < b->nf; i++) {
             const JDImageDesc &d = fd[i];
@@ -1085,10 +1075,10 @@ static void build_work_list(JPEGB200_BATCH *b)
  * the batch as a whole is refused. */
 static int plan_files(JPEGB200_BATCH *b, CreatePlan &P)
 {
-    for (int f = 0, v0 = 0; f < b->nf; v0 += P.views ? P.views[f] : 1, f++) {
-        const int nvf = P.views ? P.views[f] : 1;   /* the file's views (images) are v0 .. v0 + nvf - 1 */
+    for (int f = 0, v0 = 0; f < b->nf; v0 += P.views[f], f++) {
+        const int nvf = P.views[f];   /* the file's views (images) are v0 .. v0 + nvf - 1 */
         const JDInfo &inf = b->infos[f];
-        memset(&file_descs(b)[f], 0, sizeof(JDImageDesc));
+        memset(&b->fdescs[f], 0, sizeof(JDImageDesc));
         FileAdmit a = admit_file(b, P, f);
         const int file_ok = a.ok;
         resolve_orients(b, P, f, v0, nvf);
@@ -1108,7 +1098,7 @@ static int plan_files(JPEGB200_BATCH *b, CreatePlan &P)
         else P.rec_total += (uint64_t)JD_REC_PER_BYTE * (uint64_t)(((size_t)b->sizes[f] + 15) & ~(size_t)15) + (uint64_t)JD_REC_SLOT_SLACK * (a.nseg + a.nch + 1u);
         for (int i = v0; i < v0 + nvf; i++) if (!plan_view_output(b, P, f, i)) return 0;
         P.seg += a.nseg;
-        b->nseg_walk += file_descs(b)[f].nseg_walk;
+        b->nseg_walk += b->fdescs[f].nseg_walk;
         P.blk += (uint64_t)a.total_mcus * inf.bpm;
         if (P.blk >= (1ull << 32)) { snprintf(g_err, sizeof(g_err), "batch too large (block count)"); return 0; }
     }
@@ -1162,6 +1152,8 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateColor(JPEGB200_CTX *ctx, const ui
         !jd_check_draft(options, draft, g_err, (int)sizeof(g_err)) || !jd_check_box(out_sizes, boxes, reducing_gaps, g_err, (int)sizeof(g_err)) ||
         !jd_check_color(pixel_type, options, nv, color_ops, g_err, (int)sizeof(g_err)))
         return nullptr;
+    std::vector<int32_t> one_each;   /* views NULL: one view per file, the same batch as views of ones */
+    if (!views) { one_each.assign((size_t)n, 1); views = one_each.data(); }
     JPEGB200_BATCH *b = new (std::nothrow) JPEGB200_BATCH();
     if (!b) return nullptr;
     CreatePlan P;
@@ -1194,7 +1186,7 @@ extern "C" int JPEGB200_batchImageInfo(JPEGB200_BATCH *b, int i, int32_t *width,
                                        int32_t *out_w, int32_t *out_h, int32_t *status)
 {
     if (!b || i < 0 || i >= b->n) return 0;
-    const JDInfo &inf = b->infos[file_of(b, i)];
+    const JDInfo &inf = b->infos[b->vfile[i]];
     if (width) *width = inf.width;
     if (height) *height = inf.height;
     if (subsample) *subsample = inf.subsample;
@@ -1283,7 +1275,7 @@ extern "C" int JPEGB200_batchUpload(JPEGB200_BATCH *b)
     const int n = b->n, nf = b->nf;
     CK(b->d_comp.alloc(&b->ctx->pool, b->comp_total + 256));
     CK(b->d_descs.alloc(&b->ctx->pool, n));
-    if (b->views) CK(b->d_fdescs.alloc(&b->ctx->pool, nf));
+    CK(b->d_fdescs.alloc(&b->ctx->pool, nf));
     CK(b->d_quant.alloc(&b->ctx->pool, (size_t)n * 192));
     CK(b->d_luts.alloc(&b->ctx->pool, b->luts.size() ? b->luts.size() : 1));
     CK(b->d_work.alloc(&b->ctx->pool, b->work.size() ? b->work.size() : 1));
@@ -1313,8 +1305,9 @@ extern "C" int JPEGB200_batchUpload(JPEGB200_BATCH *b)
         for (int i = 0; i < nf; i++)
             CK(cudaMemcpyAsync(b->d_comp.p + b->comp_off[i], b->datas[i], (size_t)b->sizes[i], cudaMemcpyHostToDevice, st));
     }
-    /* the entropy-facing descriptors; view descriptors go up with their output placement in batchDecode */
-    CK(cudaMemcpyAsync(file_descs_dev(b), file_descs(b).data(), sizeof(JDImageDesc) * nf, cudaMemcpyHostToDevice, st));
+    /* the entropy-facing descriptors, once: the kernels rewrite only their status and err_mcu, on every decode.  View
+     * descriptors go up with their output placement in batchDecode. */
+    CK(cudaMemcpyAsync(b->d_fdescs.p, b->fdescs.data(), sizeof(JDImageDesc) * nf, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(b->d_quant.p, b->quant.data(), sizeof(int32_t) * 192 * n, cudaMemcpyHostToDevice, st));
     if (b->luts.size()) CK(cudaMemcpyAsync(b->d_luts.p, b->luts.data(), b->luts.size() * 2, cudaMemcpyHostToDevice, st));
     if (b->work.size()) CK(cudaMemcpyAsync(b->d_work.p, b->work.data(), b->work.size() * 4, cudaMemcpyHostToDevice, st));
@@ -1564,7 +1557,7 @@ static int alloc_prog_planes(JPEGB200_BATCH *b)
         const int f = (int)pf.file;
         if (b->d_pplane[f].alloc(&b->ctx->pool, (size_t)b->pplane[f] / 2) != cudaSuccess) {
             cudaGetLastError();
-            for (int i = 0; i < b->n; i++) if (file_of(b, i) == f) b->parse_status[i] = JPEG_ERROR_MEMORY;
+            for (int i = 0; i < b->n; i++) if (b->vfile[i] == f) b->parse_status[i] = JPEG_ERROR_MEMORY;
             continue;
         }
         b->pplane_ptr[f] = b->d_pplane[f].p;
@@ -1825,7 +1818,7 @@ static int stage_dither(JPEGB200_BATCH *b, DecodeState &D)
     size_t go = 0, eo = 0;
     b->errinit.clear();
     for (int i = 0; i < n; i++) {
-        const JDInfo &inf = b->infos[i];
+        const JDInfo &inf = b->infos[b->vfile[i]];
         gray_off[i] = go; err_off[i] = (uint32_t)eo;
         gray_off[(size_t)n + i] = D.descs_stage[i].out_off;         /* where jdk_dither writes the packed rows ... */
         gray_off[2 * (size_t)n + i] = D.descs_stage[i].out_pitch;   /* ... and their pitch: the caller's, or tight in the arena */
@@ -1880,7 +1873,7 @@ static int run_entropy(JPEGB200_BATCH *b, DecodeState &D)
 {
     if (b->work.empty()) return 1;
     cudaStream_t st = b->ss.stream;
-    JDImageDesc *const fdev = file_descs_dev(b);
+    JDImageDesc *const fdev = b->d_fdescs.p;
     JDEntropyArgs ea;
     ea.data = b->d_comp.p; ea.imgs = fdev; ea.luts = b->d_luts.p; ea.work = b->d_work.p; ea.cta_lut = b->d_cta_lut.p;
     ea.seg_img = b->d_seg_img.p; ea.seg_start = b->d_seg_start.p; ea.blk_hdr = b->d_blk_hdr.p; ea.rec = b->d_rec.p;
@@ -1935,7 +1928,7 @@ static int run_chunks(JPEGB200_BATCH *b, DecodeState &D)
     if (!b->nchunks) return 1;
     cudaStream_t st = b->ss.stream;
     JDChunkArgs ca;
-    ca.comp = b->d_comp.p; ca.filt = b->d_filt.p; ca.imgs = file_descs_dev(b); ca.luts = b->d_luts.p;
+    ca.comp = b->d_comp.p; ca.filt = b->d_filt.p; ca.imgs = b->d_fdescs.p; ca.luts = b->d_luts.p;
     ca.cimg_list = b->d_cimg_list.p; ca.ncimg = (uint32_t)b->cimg_list.size(); ca.flen = b->d_flen.p;
     ca.nchunks = b->nchunks;
     ca.cn = b->d_cn.p; ca.cpre = b->d_cpre.p; ca.cjmap = b->d_cjmap.p; ca.cstatus = b->d_cstatus.p; ca.cnown = b->d_cnown.p;
@@ -2003,7 +1996,7 @@ static void run_prog_waves(JPEGB200_BATCH *b, DecodeState &D)
 static void run_stitch_patch_pack(JPEGB200_BATCH *b, DecodeState &D)
 {
     cudaStream_t st = b->ss.stream;
-    JDImageDesc *const fdev = file_descs_dev(b);
+    JDImageDesc *const fdev = b->d_fdescs.p;
     const int nf = b->nf;
     jdk_stitch<<<(nf + 127) / 128, 128, 0, st>>>(fdev, (uint32_t)nf, b->d_seg_jmap.p, b->d_seg_status.p, b->d_seg_phase.p, b->d_seg_nrec.p,
                                                reinterpret_cast<unsigned long long *>(b->d_counters.p + 4));
@@ -2089,7 +2082,7 @@ static int run_lj(JPEGB200_BATCH *b, DecodeState &D)
 static int launch_idct_run(JPEGB200_BATCH *b, const DecodeState &D, int i0, uint32_t nimg, uint32_t max_mx, uint32_t max_my, uint32_t orc)
 {
     cudaStream_t st = b->ss.stream;
-    const JDInfo &f = b->infos[file_of(b, i0)];
+    const JDInfo &f = b->infos[b->vfile[i0]];
     if (b->sshift >= 2) {
         JDScaledArgs sa;
         sa.imgs = b->d_descs.p; sa.blk_hdr = b->d_blk_hdr.p; sa.rec = b->d_rec.p; sa.quant = b->d_quant.p;
@@ -2123,11 +2116,11 @@ static int run_idct(JPEGB200_BATCH *b, DecodeState &D)
     const int n = b->n;
     for (int i0 = 0; i0 < n;) {
         if (b->parse_status[i0] != JPEG_SUCCESS) { i0++; continue; }
-        const JDInfo &f = b->infos[file_of(b, i0)];
+        const JDInfo &f = b->infos[b->vfile[i0]];
         int i1 = i0 + 1;
         uint32_t max_mx = f.mcus_x, max_my = f.mcus_y;
         while (i1 < n && i1 - i0 < 65535 && b->parse_status[i1] == JPEG_SUCCESS) {
-            const JDInfo &g = b->infos[file_of(b, i1)];
+            const JDInfo &g = b->infos[b->vfile[i1]];
             if (g.subsample != f.subsample || g.ncomp != f.ncomp || (b->sshift < 2 && (g.width != f.width || g.height != f.height))) break;
             if ((uint32_t)g.mcus_x > max_mx) max_mx = g.mcus_x;
             if ((uint32_t)g.mcus_y > max_my) max_my = g.mcus_y;
@@ -2304,7 +2297,7 @@ extern "C" int JPEGB200_batchDecode(JPEGB200_BATCH *b, int flags)
 
     /* prescan, entropy walk, stitch and patch: one entropy-facing descriptor per file (its views share them) */
     CK(cudaEventRecord(ev[2], st));
-    jdk_prescan<<<b->nf, 256, 0, st>>>(b->d_comp.p, file_descs_dev(b), b->d_seg_start.p);
+    jdk_prescan<<<b->nf, 256, 0, st>>>(b->d_comp.p, b->d_fdescs.p, b->d_seg_start.p);
     D.launches++;
     CK(cudaEventRecord(ev[3], st));
     if (!run_entropy(b, D) || !run_chunks(b, D)) return 0;
@@ -2365,7 +2358,7 @@ extern "C" int JPEGB200_batchDownload(JPEGB200_BATCH *b)
         if (!b->descs_dl) { snprintf(g_err, sizeof(g_err), "pinned status buffer allocation failed"); return 0; }
         b->h_counters = (uint32_t *)(b->descs_dl + b->nf);
     }
-    CK(cudaMemcpyAsync(b->descs_dl, file_descs_dev(b), sizeof(JDImageDesc) * b->nf, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(b->descs_dl, b->d_fdescs.p, sizeof(JDImageDesc) * b->nf, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(b->h_counters, b->d_counters.p, 32, cudaMemcpyDeviceToHost, st));
     b->downloaded = true;
     bytes += (int64_t)sizeof(JDImageDesc) * b->nf + 32;
@@ -2397,7 +2390,7 @@ extern "C" int JPEGB200_batchWait(JPEGB200_BATCH *b, int32_t *status)
     if (ev_overflow) snprintf(g_err, sizeof(g_err), "%u window-truncation events exceed the event buffer (%u): job rejected", b->h_counters[0], JD_EVENT_CAP);
     for (int i = 0; i < b->n; i++) {
         int st = b->parse_status[i];
-        if (st == JPEG_SUCCESS && b->downloaded && (b->views ? JPEGB200_batchErrMcu(b, i) >= 0 : b->descs_dl[i].status != 0))
+        if (st == JPEG_SUCCESS && JPEGB200_batchErrMcu(b, i) >= 0)
             st = JPEG_DECODE_ERROR; /* jpeg.inl:5354 */
         if (st == JPEG_SUCCESS && ev_overflow) st = JPEG_DECODE_ERROR;
         if (status) status[i] = st;
@@ -2425,13 +2418,9 @@ extern "C" int JPEGB200_batchWait(JPEGB200_BATCH *b, int32_t *status)
 extern "C" int JPEGB200_batchErrMcu(JPEGB200_BATCH *b, int i)
 {
     if (!b || i < 0 || i >= b->n) return -1;
-    if (!b->downloaded) return -1;
-    if (b->views) {
-        if (b->parse_status[i] != JPEG_SUCCESS) return -1;
-        const JDImageDesc &fd = b->descs_dl[b->vfile[i]];
-        return jd_view_err_mcu(fd.status, fd.err_mcu, b->descs[i].roi_mcu_end);
-    }
-    return b->descs_dl[i].status ? (int)b->descs_dl[i].err_mcu : -1;
+    if (!b->downloaded || b->parse_status[i] != JPEG_SUCCESS) return -1;
+    const JDImageDesc &fd = b->descs_dl[b->vfile[i]];
+    return jd_view_err_mcu(fd.status, fd.err_mcu, b->descs[i].roi_mcu_end);
 }
 
 extern "C" int JPEGB200_batchOrientation(JPEGB200_BATCH *b, int i, int32_t *exif_tag, int32_t *applied)
@@ -2629,7 +2618,7 @@ extern "C" int JPEGB200_decodeBatchColor(JPEGB200_CTX *ctx, const uint8_t *const
             for (int i = 0; i < cv; i++)
                 sc[i] = (b->resize ? b->rs_scratch[i] : 0) + (b->tensor ? b->tn_stage[i] : 0) + (b->lj ? b->lj_plane[i] : 0) +
                         (b->color ? b->bl_scratch[i] : 0);
-            for (int i = 0; i < cv; i++) if (i == 0 || file_of(b, i) != file_of(b, i - 1)) sc[i] += b->pplane[file_of(b, i)];
+            for (int i = 0; i < cv; i++) if (i == 0 || b->vfile[i] != b->vfile[i - 1]) sc[i] += b->pplane[b->vfile[i]];
             int32_t cv3 = 0, capped3 = 0;
             const int c = jd_job_files(cnt, sizes + i0, vi, INT64_MAX, INT64_MAX, sc.data(), JD_JOB_RESIZE_SCRATCH, &cv3, &capped3);
             JPEGB200_batchDestroy(b);

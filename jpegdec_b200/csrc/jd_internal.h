@@ -79,8 +79,9 @@ typedef struct {
     /* region of interest (JPEGB200_batchCreateROI); out_w / out_h above are then its size */
     uint16_t roi_x, roi_y;  /* its origin in output pixels (0, 0 without one) */
     uint16_t mcu_x0, mcu_y0;/* first MCU column / row it touches: the IDCT grid starts there */
-    uint32_t roi_mcu_end;   /* 1 + the last MCU (full-image raster index) of the last MCU row it touches; 0 = no rectangle.
-                             * An error at or past this MCU is not reported (the reference's crop decode stops above it). */
+    uint32_t roi_mcu_end;   /* view descriptors only: 1 + the last MCU (full-image raster index) of the last MCU row it
+                             * touches; 0 = no rectangle.  JPEGB200_batchErrMcu does not report a file error at or past this
+                             * MCU (jd_view_err_mcu).  File descriptors keep 0: no kernel reads it. */
     uint32_t orient;        /* EXIF transform 1-8 applied by the stores (JPEGB200_batchCreateOriented; 0 / 1 = none).  With
                              * it, roi_x / roi_y and the MCU box are those of the rectangle in the STORED frame, while out_w /
                              * out_h stay the output (upright) size: swapped against the stored rectangle for 5-8. */
@@ -117,11 +118,12 @@ int jd_orient_plan(int width, int height, int subsample, int restart_interval, i
  * valid views (all nseg intervals for a view of a batch without rois and orients), 0 if no view is valid. */
 int jd_views_plan(int width, int height, int subsample, int restart_interval, int sshift, int nv, const int32_t *rois,
                   const uint8_t *ks, const int32_t *out_sizes, JDRoiPlan *plans, int32_t *srects, int32_t *ok);
-/* Views (JPEGB200_batchCreateViews): the first undecodable MCU a view reports, -1 for none.  file_status / file_err_mcu:
- * what jdk_stitch wrote for the view's file, whose walk reaches the deepest view and has no rectangle rule; mcu_end: the
- * view's JDRoiPlan.mcu_end (0 = no rectangle).  The view reports the file's error when it has no rectangle or the error lies
- * before mcu_end: the rule jdk_stitch applies to a single-view batch, because a view's walked intervals are a prefix of its
- * file's and every MCU before its mcu_end lies in that prefix. */
+/* The first undecodable MCU an image (view) reports, -1 for none.  file_status / file_err_mcu: what jdk_stitch (or
+ * jdk_prog_pack) wrote for the view's file, whose walk reaches the deepest of its views; mcu_end: the view's
+ * JDRoiPlan.mcu_end (0 = no rectangle).  The view reports the file's error when it has no rectangle or the error lies before
+ * mcu_end, as the reference's crop decode, which stops parsing after the rectangle's last MCU row.  A view alone in its file
+ * gets the same answer as with several: a view's walked intervals are a prefix of its file's and every MCU before its
+ * mcu_end lies in that prefix.  The chunk path's error MCU is judged the same way, wherever its chunk lies. */
 int32_t jd_view_err_mcu(uint32_t file_status, uint32_t file_err_mcu, uint32_t mcu_end);
 /* How many files, from the first, the next job of JPEGB200_decodeBatchViews takes: always the first, then each next file
  * while the job keeps at most max_views views, at most max_bytes compressed bytes (a negative size counts 0) and, with

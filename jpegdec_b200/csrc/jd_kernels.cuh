@@ -377,9 +377,8 @@ __global__ void jdk_stitch(JDImageDesc *imgs, uint32_t nimg, const uint32_t *__r
         const uint32_t st = seg_status[g];
         if (st != 0u && status == 0u) { status = st >> 28; err_mcu = s * im.mcus_per_seg + (st & 0x0FFFFFFFu); }
     }
-    /* a region of interest reports an error only above or in its last MCU row, as the reference's crop decode, which stops
-     * parsing after that row (the chunk path's error MCU is judged the same way, wherever its chunk lies) */
-    if (im.roi_mcu_end != 0u && err_mcu >= im.roi_mcu_end) { status = 0; err_mcu = 0; }
+    /* the file's first error among its walked intervals; each view judges it against its own rectangle on the host
+     * (jd_view_err_mcu) */
     im.status = status;
     im.err_mcu = err_mcu;
     if (nrec) atomicAdd(rec_count, nrec);
@@ -2447,7 +2446,7 @@ struct JDProgPackArgs {
 /* One CTA per file: 256 blocks at a time are counted, placed by a block-wide prefix sum and written as block headers and
  * records from the image's rec_base.  An image whose records would pass its budget gets empty headers from there on and
  * an error status instead of an overwrite.  Then the file's status: JPEG_DECODE_ERROR from the first undecodable MCU row
- * of its scans, under the region-of-interest rule of jdk_stitch. */
+ * of its scans, judged per view as jdk_stitch's is. */
 __global__ void __launch_bounds__(256) jdk_prog_pack(const JDProgPackArgs a)
 {
     __shared__ uint8_t s_tpos[64];
@@ -2496,7 +2495,6 @@ __global__ void __launch_bounds__(256) jdk_prog_pack(const JDProgPackArgs a)
         const uint32_t r = a.err_row[pf.file];
         if (r != JD_PROG_NONE) { status = JD_SEG_BADCODE; err_mcu = r * (uint32_t)im.mcus_x; }
         else if (over) status = JD_SEG_OVERFLOW;
-        if (im.roi_mcu_end != 0u && err_mcu >= im.roi_mcu_end) { status = 0; err_mcu = 0; }
         im.status = status;
         im.err_mcu = err_mcu;
         if (base) atomicAdd(a.rec_count, (unsigned long long)base);
