@@ -394,10 +394,39 @@ int JPEGB200_thumbnailPlan(int width, int height, int req_w, int req_h, double r
 #define JPEGB200_COLOR_GRAYSCALE  5
 #define JPEGB200_COLOR_SOLARIZE   6
 #define JPEGB200_COLOR_GAUSSIAN_BLUR 16
+/* The auto-augment operations of torchvision's RandAugment / TrivialAugmentWide / AutoAugment on a PIL image (the arg is the
+ * magnitude torchvision's _apply_op receives; Brightness / Color / Contrast / Solarize / Identity are the ops above):
+ *       SHARPNESS f    F.adjust_sharpness(img, f): blend(SMOOTH(img), img, f), SMOOTH's border pixels unchanged
+ *       POSTERIZE b    F.posterize(img, b), b an integer 0 .. 8
+ *       AUTOCONTRAST   F.autocontrast(img), per channel (arg ignored)
+ *       EQUALIZE       F.equalize(img), per channel (arg ignored)
+ *       INVERT         F.invert(img) (arg ignored)
+ *       SHEAR_X m, SHEAR_Y m, TRANSLATE_X m, TRANSLATE_Y m (int(m) pixels), ROTATE m (degrees, counter-clockwise):
+ *                      _apply_op(img, "ShearX" .. "Rotate", m, NEAREST, fill=None); the view keeps its size, pixels from
+ *                      outside the image are 0 (alpha kept).
+ *   They apply to gray views too, on the one channel.  A posterize argument that is not an integer in 0 .. 8, or a
+ *   geometric op on a view wider or taller than 1024 pixels (the sizes pinned against Pillow) or whose fixed-point mapping
+ *   does not fit 32 bits, gives that view JPEG_INVALID_PARAMETER.  The list is also cut at each SHARPNESS, AUTOCONTRAST,
+ *   EQUALIZE and geometric op: at such a cut index the call makes jdk_augment + jdk_augment_copy when some view sharpens
+ *   or moves pixels there (through the blur's scratch copy).  A cut index where some view posterizes, inverts, applies an
+ *   AUTOCONTRAST / EQUALIZE or counts the histogram for one runs jdk_color_lut in place of jdk_color: the launch before an
+ *   AUTOCONTRAST or EQUALIZE counts per-view histograms (768 64-bit counts per op, counted in the one-call path's scratch
+ *   bound), from which the next one builds the LUT.  Lists without these ops make the same launches as before.
+ *   DESIGN.md 4.2.11. */
+#define JPEGB200_COLOR_SHARPNESS    20
+#define JPEGB200_COLOR_POSTERIZE    21
+#define JPEGB200_COLOR_AUTOCONTRAST 22
+#define JPEGB200_COLOR_EQUALIZE     23
+#define JPEGB200_COLOR_INVERT       24
+#define JPEGB200_COLOR_SHEAR_X      25
+#define JPEGB200_COLOR_SHEAR_Y      26
+#define JPEGB200_COLOR_TRANSLATE_X  27
+#define JPEGB200_COLOR_TRANSLATE_Y  28
+#define JPEGB200_COLOR_ROTATE       29
 #define JPEGB200_COLOR_MAX_OPS    8
 typedef struct {
     int32_t op;                        /* JPEGB200_COLOR_*, 0 = end of the view's list */
-    double arg;                        /* factor, hue shift (-0.5 .. 0.5), solarize threshold or blur radius */
+    double arg;                        /* factor, hue shift (-0.5 .. 0.5), solarize threshold, blur radius or magnitude */
 } JPEGB200_ColorOp;
 JPEGB200_BATCH *JPEGB200_batchCreateColor(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
                                           const int32_t *views, int pixel_type, int options, const int32_t *rois,

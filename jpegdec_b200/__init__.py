@@ -39,6 +39,9 @@ SCALE_NONE, SCALE_DIV255, SCALE_MUL255 = 0, 1, 2
 # colour operations (JPEGB200_ColorOp): torchvision's ColorJitter / RandomGrayscale / RandomSolarize on PIL images
 COLOR_BRIGHTNESS, COLOR_CONTRAST, COLOR_SATURATION, COLOR_HUE, COLOR_GRAYSCALE, COLOR_SOLARIZE = 1, 2, 3, 4, 5, 6
 COLOR_GAUSSIAN_BLUR = 16   # (COLOR_GAUSSIAN_BLUR, r): Pillow's img.filter(ImageFilter.GaussianBlur(r))
+# torchvision's auto-augment operations on PIL images (include/jpegdec_b200.h; auto_augment_ops draws them)
+COLOR_SHARPNESS, COLOR_POSTERIZE, COLOR_AUTOCONTRAST, COLOR_EQUALIZE, COLOR_INVERT = 20, 21, 22, 23, 24
+COLOR_SHEAR_X, COLOR_SHEAR_Y, COLOR_TRANSLATE_X, COLOR_TRANSLATE_Y, COLOR_ROTATE = 25, 26, 27, 28, 29
 COLOR_MAX_OPS = 8
 TIMING_NAMES = ["h2d", "prescan", "entropy", "stitch", "idct", "dither", "d2h", "total"]
 COUNTER_NAMES = ["launches", "segments", "blocks", "events", "compressed_bytes", "output_bytes",
@@ -473,6 +476,64 @@ def color_jitter_ops(params):
         v = (b, c, s, h)[fn]
         if v is not None:
             ops.append(((COLOR_BRIGHTNESS, COLOR_CONTRAST, COLOR_SATURATION, COLOR_HUE)[fn], float(v)))
+    return ops
+
+
+_AUTO_AUGMENT_OPS = {
+    "ShearX": lambda m: [(COLOR_SHEAR_X, m)], "ShearY": lambda m: [(COLOR_SHEAR_Y, m)],
+    "TranslateX": lambda m: [(COLOR_TRANSLATE_X, m)], "TranslateY": lambda m: [(COLOR_TRANSLATE_Y, m)],
+    "Rotate": lambda m: [(COLOR_ROTATE, m)], "Brightness": lambda m: [(COLOR_BRIGHTNESS, 1.0 + m)],
+    "Color": lambda m: [(COLOR_SATURATION, 1.0 + m)], "Contrast": lambda m: [(COLOR_CONTRAST, 1.0 + m)],
+    "Sharpness": lambda m: [(COLOR_SHARPNESS, 1.0 + m)], "Posterize": lambda m: [(COLOR_POSTERIZE, float(int(m)))],
+    "Solarize": lambda m: [(COLOR_SOLARIZE, m)], "AutoContrast": lambda m: [COLOR_AUTOCONTRAST],
+    "Equalize": lambda m: [COLOR_EQUALIZE], "Invert": lambda m: [COLOR_INVERT], "Identity": lambda m: [],
+}
+
+
+def auto_augment_ops(t, size):
+    """One view's operation list for torchvision's RandAugment, TrivialAugmentWide or AutoAugment `t` on a PIL image of
+    size = (w, h): the same draws from torch's global generator, in the same order and with the same calls, as t.forward,
+    so under one torch.manual_seed the list gives torchvision's image (and leaves the generator where forward does).
+    ValueError for an interpolation other than NEAREST or a non-zero fill, whose bytes the operations do not pin."""
+    import torch
+    from torchvision import transforms as TV
+    from torchvision.transforms import InterpolationMode
+    if not isinstance(t, (TV.RandAugment, TV.TrivialAugmentWide, TV.AutoAugment)):
+        raise TypeError("auto_augment_ops: a RandAugment, TrivialAugmentWide or AutoAugment")
+    if t.interpolation != InterpolationMode.NEAREST:
+        raise ValueError("auto_augment_ops: only interpolation=NEAREST is supported")
+    fill = t.fill
+    if fill is not None and any(float(f) != 0.0 for f in (fill if isinstance(fill, (list, tuple)) else [fill])):
+        raise ValueError("auto_augment_ops: only fill None or 0 is supported")
+    w, h = size
+    ops = []
+    if isinstance(t, TV.RandAugment):
+        meta = t._augmentation_space(t.num_magnitude_bins, (h, w))
+        for _ in range(t.num_ops):
+            name = list(meta.keys())[int(torch.randint(len(meta), (1,)).item())]
+            mags, signed = meta[name]
+            m = float(mags[t.magnitude].item()) if mags.ndim > 0 else 0.0
+            if signed and torch.randint(2, (1,)):
+                m *= -1.0
+            ops += _AUTO_AUGMENT_OPS[name](m)
+    elif isinstance(t, TV.TrivialAugmentWide):
+        meta = t._augmentation_space(t.num_magnitude_bins)
+        name = list(meta.keys())[int(torch.randint(len(meta), (1,)).item())]
+        mags, signed = meta[name]
+        m = float(mags[torch.randint(len(mags), (1,), dtype=torch.long)].item()) if mags.ndim > 0 else 0.0
+        if signed and torch.randint(2, (1,)):
+            m *= -1.0
+        ops += _AUTO_AUGMENT_OPS[name](m)
+    else:
+        pid, probs, signs = t.get_params(len(t.policies))
+        meta = t._augmentation_space(10, (h, w))
+        for i, (name, p, mid) in enumerate(t.policies[pid]):
+            if probs[i] <= p:
+                mags, signed = meta[name]
+                m = float(mags[mid].item()) if mid is not None else 0.0
+                if signed and signs[i] == 0:
+                    m *= -1.0
+                ops += _AUTO_AUGMENT_OPS[name](m)
     return ops
 
 

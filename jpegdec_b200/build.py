@@ -19,7 +19,7 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 C_SOURCES = ["jd_host.c", "jd_api.c"]
 CU_SOURCES = ["jd_device.cu"]
-HEADERS = ["jd_core.h", "jd_chunk.h", "jd_internal.h", "jd_kernels.cuh", "jd_resize.h", "jd_reduce.h", "jd_color.h", "jd_blur.h", "jd_prog.h", "jd_ljpeg.h",
+HEADERS = ["jd_core.h", "jd_chunk.h", "jd_internal.h", "jd_kernels.cuh", "jd_resize.h", "jd_reduce.h", "jd_color.h", "jd_blur.h", "jd_augment.h", "jd_prog.h", "jd_ljpeg.h",
            os.path.join("..", "..", "include", "JPEGDEC.h"),
            os.path.join("..", "..", "include", "jpegdec_b200.h")]
 
@@ -47,7 +47,8 @@ def build(force=False, verbose=False):
         s = os.path.join(CSRC, src)
         o = os.path.join(BUILD, src + ".o")
         if force or _stale(o, [s] + hdrs):
-            _run(["gcc", "-c", "-O2", "-fPIC", "-Wall", "-pthread", s, "-o", o])
+            # no FMA contraction: the geometric ops' matrices (jd_host.c) round each double operation as Python does
+            _run(["gcc", "-c", "-O2", "-fPIC", "-Wall", "-pthread", "-ffp-contract=off", s, "-o", o])
         objs.append(o)
     for src in CU_SOURCES:
         s = os.path.join(CSRC, src)

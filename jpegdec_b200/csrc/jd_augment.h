@@ -1,0 +1,114 @@
+/*
+ * jd_augment.h -- the auto-augment operations of torchvision's RandAugment / TrivialAugmentWide / AutoAugment on PIL images
+ * that are not per-pixel blends (adjust_sharpness, autocontrast, equalize, and ShearX / ShearY / TranslateX / TranslateY /
+ * Rotate with NEAREST and fill 0), restated as probing Pillow 12.2 pins them.  Shared by the kernels (jd_kernels.cuh:
+ * jdk_augment, jdk_color's LUT step), the host plan (jd_host.c: jd_color_plan_aug) and the CPU stepper (tests/augsim).
+ * DESIGN.md 4.2.11 has the probes.  Posterize and invert are per pixel: jd_color.h.
+ *
+ *   SMOOTH (ImageFilter.SMOOTH): inner pixels (S + 6) / 13, S = the 8 neighbours + 5 x the centre; the border, and an
+ *                       image under 3 pixels on a side, unchanged.  Sharpness f = blend(SMOOTH, img, f) (jd_co_blend).
+ *   autocontrast:       per channel lo / hi = the lowest / highest non-empty bin; hi <= lo: unchanged; else in double
+ *                       scale = 255 / (hi - lo), offset = -lo * scale, lut[i] = clamp(int(i * scale + offset), 0, 255).
+ *   equalize:           per channel, fewer than 2 non-empty bins: unchanged; step = (sum h - h[last non-empty]) / 255 (integer);
+ *                       step 0: unchanged; else lut[i] = min(255, (step / 2 + sum_{j < i} h[j]) / step).  64-bit counts.
+ *   geometric (NEAREST): Pillow's inverse matrix (a, b, c, d, e, f) in 16.16 fixed point, R(v) = floor(v * 65536 + 0.5):
+ *                       output (x, y) reads source ((X0 + y R(b) + x R(a)) >> 16, (Y0 + y R(e) + x R(d)) >> 16) with
+ *                       X0 = R(a / 2 + b / 2 + c), Y0 = R(d / 2 + e / 2 + f); outside the image: fill 0 (alpha kept 0xFF).
+ *                       The host computes the six integers (jd_color_plan_aug) and checks that every value over the view
+ *                       fits 32 bits, so the device stays integer-only.
+ * Plain C, C++ or CUDA.
+ */
+#ifndef JD_AUGMENT_H
+#define JD_AUGMENT_H
+
+#include <stdint.h>
+
+#include "jd_color.h"
+
+/* views with a geometric op: sides up to this many pixels (the sizes the CPU tier pins; larger views are refused) */
+#define JD_AU_MAX_SIDE 1024
+#define JD_AU_HIST     768   /* histogram words per view and cut: 3 channels x 256 bins (gray uses the first 256) */
+
+/* A geometric op's source mapping: source x = (x0 + y * bx + x * ax) >> 16, source y = (y0 + y * by + x * ay) >> 16 */
+typedef struct {
+    int32_t x0, y0, ax, ay, bx, by;
+} JDAffine;
+typedef struct {
+    JDAffine a[JD_CO_MAX_OPS];   /* per op slot of the plan */
+} JDAugPlan;
+
+/* ImageFilter.SMOOTH of one channel at an inner pixel: c = the centre, nb = the sum of its 8 neighbours */
+JD_CO_HD uint32_t jd_au_smooth(uint32_t c, uint32_t nb) { return (nb + 5u * c + 6u) / 13u; }
+
+/* the source pixel of output (x, y), or -1 for fill */
+JD_CO_HD int64_t jd_au_source(const JDAffine *m, uint32_t x, uint32_t y, uint32_t w, uint32_t h)
+{
+    /* modulo 2^32: the host checked that the values at the view's corners, hence everywhere, fit int32 */
+    const int32_t X = (int32_t)((uint32_t)m->x0 + y * (uint32_t)m->bx + x * (uint32_t)m->ax);
+    const int32_t Y = (int32_t)((uint32_t)m->y0 + y * (uint32_t)m->by + x * (uint32_t)m->ay);
+    const int32_t sx = X >> 16, sy = Y >> 16;   /* arithmetic shifts: floor */
+    if (sx < 0 || sy < 0 || (uint32_t)sx >= w || (uint32_t)sy >= h) return -1;
+    return (int64_t)sy * w + sx;
+}
+
+/* jd_co_apply3 / _apply1 with the per-pixel auto-augment ops: posterize (arg: the kept-bits mask,
+ * c & ~(2^(8 - bits) - 1), ImageOps.posterize) and invert (255 - c, ImageOps.invert).  Kept apart from jd_color.h so that
+ * lists without them run jdk_color as before. */
+JD_CO_HD void jd_au_apply3(uint32_t op, uint32_t arg, uint32_t mean, uint32_t *r, uint32_t *g, uint32_t *b)
+{
+    if (op == JD_CO_POSTERIZE) { *r &= arg; *g &= arg; *b &= arg; }
+    else if (op == JD_CO_INVERT) { *r = 255u - *r; *g = 255u - *g; *b = 255u - *b; }
+    else jd_co_apply3(op, arg, mean, r, g, b);
+}
+
+JD_CO_HD uint32_t jd_au_apply1(uint32_t op, uint32_t arg, uint32_t mean, uint32_t c)
+{
+    if (op == JD_CO_POSTERIZE) return c & arg;
+    if (op == JD_CO_INVERT) return 255u - c;
+    return jd_co_apply1(op, arg, mean, c);
+}
+
+/* autocontrast's entry i for the non-empty bin range lo < hi */
+JD_CO_HD uint32_t jd_au_ac_entry(uint32_t lo, uint32_t hi, uint32_t i)
+{
+    const double scale = JD_CO_DDIV(255.0, (double)(hi - lo));
+    const double offset = JD_CO_DMUL(-(double)lo, scale);
+    const int v = (int)JD_CO_DADD(JD_CO_DMUL((double)i, scale), offset);
+    return v < 0 ? 0u : v > 255 ? 255u : (uint32_t)v;
+}
+
+/* equalize's entry for a bin whose lower bins hold below pixels, step > 0 */
+JD_CO_HD uint32_t jd_au_eq_entry(uint64_t step, uint64_t below)
+{
+    const uint64_t v = (step / 2u + below) / step;
+    return v > 255u ? 255u : (uint32_t)v;
+}
+
+/* Entry i of the LUT of autocontrast or equalize (op) for one channel, from its histogram's summary: lo / hi its lowest /
+ * highest non-empty bin, nz its non-empty bins, total its count, last = h[hi], below = the count of the bins under i.  The
+ * rules, the "unchanged" cases included, live here alone: the serial builder below (host, CPU stepper) and the kernels'
+ * block-wide builder (jd_kernels.cuh: jd_co_build_lut) both call it. */
+JD_CO_HD uint32_t jd_au_lut_entry(uint32_t op, uint32_t lo, uint32_t hi, uint32_t nz, uint64_t total, uint64_t last, uint64_t below,
+                                  uint32_t i)
+{
+    if (op == JD_CO_AUTOCONTRAST) return nz > 0u && hi > lo ? jd_au_ac_entry(lo, hi, i) : i;
+    if (nz < 2u) return i;
+    const uint64_t step = (total - last) / 255u;
+    return step ? jd_au_eq_entry(step, below) : i;
+}
+
+/* the LUT of autocontrast or equalize (op) from one channel's 256-bin histogram */
+JD_CO_HD void jd_au_lut(uint32_t op, const uint64_t *h, uint8_t *lut)
+{
+    uint32_t lo = 256u, hi = 0u, nz = 0u;
+    uint64_t total = 0u;
+    for (uint32_t i = 0; i < 256u; i++)
+        if (h[i]) { if (lo == 256u) lo = i; hi = i; nz++; total += h[i]; }
+    uint64_t below = 0u;
+    for (uint32_t i = 0; i < 256u; i++) {
+        lut[i] = (uint8_t)jd_au_lut_entry(op, lo, hi, nz, total, h[hi], below, i);
+        below += h[i];
+    }
+}
+
+#endif

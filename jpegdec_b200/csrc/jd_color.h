@@ -14,6 +14,7 @@
  *   grayscale:            R = G = B = L
  *   solarize (threshold): c < thr ? c : 255 - c, thr = the number of bytes below the double threshold
  *   Gaussian blur r:      ImageFilter.GaussianBlur(r), jd_blur.h (not a per-pixel operation: run by its own kernels)
+ *   posterize, invert, sharpness, autocontrast, equalize, shear, translate, rotate: jd_augment.h
  *
  * On a gray ("L") image brightness, contrast (m over the bytes themselves) and solarize apply; saturation, hue and grayscale
  * leave it alone, as they do in Pillow and torchvision.  Every float and double operation on the device goes through the
@@ -56,7 +57,24 @@
 #define JD_CO_GRAYSCALE  5
 #define JD_CO_SOLARIZE   6
 #define JD_CO_BLUR       16   /* ImageFilter.GaussianBlur: run by jdk_blur (jd_blur.h); jd_co_apply3 / _apply1 skip it */
+/* the auto-augment operations (jd_augment.h); jd_co_apply3 / _apply1 skip them.  Posterize (arg: the kept-bits mask) and
+ * invert are per pixel (jd_au_apply3 / _apply1), sharpness and the geometric ops are run by jdk_augment, autocontrast and
+ * equalize by jdk_color_lut's LUT step at the start of a segment */
+#define JD_CO_SHARPNESS    20
+#define JD_CO_POSTERIZE    21
+#define JD_CO_AUTOCONTRAST 22
+#define JD_CO_EQUALIZE     23
+#define JD_CO_INVERT       24
+#define JD_CO_SHEAR_X      25
+#define JD_CO_SHEAR_Y      26
+#define JD_CO_TRANSLATE_X  27
+#define JD_CO_TRANSLATE_Y  28
+#define JD_CO_ROTATE       29
 #define JD_CO_MAX_OPS    8
+#define JD_CO_GEOMETRIC(op) ((op) >= JD_CO_SHEAR_X && (op) <= JD_CO_ROTATE)
+#define JD_CO_LUT(op)       ((op) == JD_CO_AUTOCONTRAST || (op) == JD_CO_EQUALIZE)
+/* ops a kernel of their own runs at a cut, before jdk_color runs the rest of the segment */
+#define JD_CO_OWN_KERNEL(op) ((op) == JD_CO_BLUR || (op) == JD_CO_SHARPNESS || JD_CO_GEOMETRIC(op))
 
 JD_CO_HD float jd_co_float(uint32_t bits)
 {
@@ -162,10 +180,11 @@ JD_CO_HD uint32_t jd_co_apply1(uint32_t op, uint32_t arg, uint32_t mean, uint32_
     return c;
 }
 
-/* One view's list as the kernels run it: ops cut into segments at each contrast and each blur; ncontrast counts those
- * cuts (without blurs every cut is a contrast, hence the name).  Segment k (k = 0 .. ncontrast) is op[seg[k] .. seg[k + 1]);
- * segment k >= 1 starts with a contrast, whose mean is sum k - 1, the sum of L over the output of segment k - 1, or with a
- * blur, which the blur kernels run before jdk_color runs the rest of the segment. */
+/* One view's list as the kernels run it: ops cut into segments at each contrast, blur, sharpness, autocontrast, equalize
+ * and geometric op; ncontrast counts those cuts (without the others every cut is a contrast, hence the name).  Segment k
+ * (k = 0 .. ncontrast) is op[seg[k] .. seg[k + 1]); segment k >= 1 starts with a contrast, whose mean is sum k - 1, the sum
+ * of L over the output of segment k - 1; with an autocontrast or equalize, whose LUT comes from histogram k - 1 of that
+ * output; or with an op of its own kernel (JD_CO_OWN_KERNEL), run before jdk_color runs the rest of the segment. */
 typedef struct {
     uint32_t nops, ncontrast;
     uint32_t op[JD_CO_MAX_OPS];

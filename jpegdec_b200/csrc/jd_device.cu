@@ -179,13 +179,18 @@ struct JPEGB200_BATCH {
     bool color = false;
     std::vector<JDColorPlan> co_plans;
     std::vector<JDBlurPlan> co_blur;        /* per view: each blur's constants at its op slot */
-    std::vector<int64_t> bl_scratch;        /* per view: its scratch copy's bytes when it blurs (256-byte aligned), else 0 */
+    std::vector<JDAugPlan> co_aug;          /* per view: each geometric op's mapping at its op slot */
+    std::vector<int64_t> bl_scratch;        /* per view: its scratch copy's bytes when it blurs, sharpens or moves pixels
+                                               (256-byte aligned), plus JD_AU_HIST counts per autocontrast / equalize */
     int64_t bl_scratch_total = 0;
     std::vector<JDBlurDesc> bl_desc;        /* per blur launch pair, per view blurring there */
     std::vector<uint32_t> bl_blk;           /* the same entries: first CTA of the horizontal, then of the vertical kernel */
     DevBuf<JDBlurDesc> d_bl_desc;
     DevBuf<uint32_t> d_bl_blk;
     DevBuf<uint8_t> d_bl;                   /* the scratch copies */
+    std::vector<JDAugDesc> au_desc;         /* per jdk_augment launch pair, per view sharpening or moving pixels there */
+    DevBuf<JDAugDesc> d_au_desc;
+    DevBuf<uint32_t> d_co_hslot;            /* per cut index and view: its histogram slot (the slots follow the scratch copies in d_bl) */
     std::vector<uint8_t> co_bgr;
     std::vector<JDColorDesc> co_desc;
     std::vector<uint32_t> co_blk;           /* per launch, per view: its first CTA */
@@ -617,7 +622,7 @@ static void init_batch(JPEGB200_BATCH *b, JPEGB200_CTX *ctx, const CreatePlan &P
     b->box = P.boxes != nullptr || P.gaps != nullptr;
     if (b->box) b->bx_plans.assign(nv, JDBoxPlan{});
     b->color = P.color != nullptr;
-    if (b->color) { b->co_plans.assign(nv, JDColorPlan{}); b->co_blur.assign(nv, JDBlurPlan{}); b->bl_scratch.assign(nv, 0); b->co_bgr.assign(nv, 0); }
+    if (b->color) { b->co_plans.assign(nv, JDColorPlan{}); b->co_blur.assign(nv, JDBlurPlan{}); b->co_aug.assign(nv, JDAugPlan{}); b->bl_scratch.assign(nv, 0); b->co_bgr.assign(nv, 0); }
     b->lj = (options & JPEGB200_OPT_LIBJPEG) != 0;
     if (b->lj) { b->lj_desc.assign(nv, JDLjDesc{}); b->lj_plane.assign(nv, 0); }
     b->tensor = P.spec != nullptr;
@@ -797,7 +802,12 @@ static uint32_t plan_views(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int 
         bool dropped = false;
         for (int i = v0; i < v0 + nvf; i++) {
             if (!P.vok[i]) continue;
-            if (!jd_color_plan_blur(P.color + JPEGB200_COLOR_MAX_OPS * (size_t)i, b->ptclass == JD_PT_GRAY, &b->co_plans[i], &b->co_blur[i])) {
+            /* the view's final size, which the geometric ops' mappings depend on (padded output takes no operations) */
+            const int s = b->lj ? (int)b->lj_desc[i].shift : b->sshift;
+            const uint32_t w = b->resize ? (uint32_t)P.out_sizes[2 * (size_t)i] : b->roi ? (uint32_t)b->plans[i].out_w : (uint32_t)((inf.width + (1 << s) - 1) >> s);
+            const uint32_t h = b->resize ? (uint32_t)P.out_sizes[2 * (size_t)i + 1] : b->roi ? (uint32_t)b->plans[i].out_h : (uint32_t)((inf.height + (1 << s) - 1) >> s);
+            if (!jd_color_plan_aug(P.color + JPEGB200_COLOR_MAX_OPS * (size_t)i, b->ptclass == JD_PT_GRAY, w, h, &b->co_plans[i],
+                                   &b->co_blur[i], &b->co_aug[i])) {
                 P.vok[i] = 0;
                 dropped = true;
             }
@@ -1016,12 +1026,12 @@ static int plan_view_output(JPEGB200_BATCH *b, CreatePlan &P, int f, int i)
     if (b->color) {   /* the colour operations read true R, G, B: a libjpeg decode stores R, G, B for every file */
         b->co_bgr[i] = (uint8_t)(b->ptclass == JD_PT_8888 && !b->lj && jd_rgb8888_is_bgr(b->ctx->arith, b->sshift, inf.ncomp, inf.subsample));
         const JDColorPlan &cp = b->co_plans[i];
-        bool blurs = false;
-        for (uint32_t k = 0; k < cp.nops; k++) blurs = blurs || cp.op[k] == JD_CO_BLUR;
-        if (blurs) {
-            b->bl_scratch[i] = (int64_t)align256((size_t)vd.out_w * vd.out_h * bytes_per_pixel_class(b->ptclass));
-            b->bl_scratch_total += b->bl_scratch[i];
-        }
+        bool own = false;
+        int64_t nlut = 0;
+        for (uint32_t k = 0; k < cp.nops; k++) { own = own || JD_CO_OWN_KERNEL(cp.op[k]); nlut += JD_CO_LUT(cp.op[k]) ? 1 : 0; }
+        if (own) b->bl_scratch[i] = (int64_t)align256((size_t)vd.out_w * vd.out_h * bytes_per_pixel_class(b->ptclass));
+        b->bl_scratch[i] += nlut * JD_AU_HIST * (int64_t)sizeof(unsigned long long);
+        b->bl_scratch_total += b->bl_scratch[i];
     }
     size_t pitch;
     if (b->tensor) pitch = (size_t)vd.out_w * (b->tn_spec.layout == JPEGB200_LAYOUT_HWC ? b->tn_nc : 1) * b->tn_elt;
@@ -1540,6 +1550,11 @@ struct DecodeState {
     std::vector<uint32_t> co_ctas;          /* colour operations: CTAs of each jdk_color launch */
     std::vector<uint32_t> bl_first;         /* blurs: the first bl_desc entry of each cut index (one past the last at nl) */
     std::vector<uint32_t> bl_ctas;          /* CTAs of each cut index's jdk_blur pair: horizontal, vertical */
+    std::vector<uint32_t> au_first;         /* sharpness and geometric ops: the first au_desc entry of each cut index */
+    std::vector<uint32_t> au_ctas;          /* CTAs of each cut index's jdk_augment pair */
+    std::vector<uint8_t> co_lut;            /* per cut index: some view posterizes, inverts, applies a LUT or counts a
+                                               histogram there (jdk_color_lut) */
+    unsigned long long *co_hist = nullptr;  /* the histogram slots */
     uint32_t co_nsum = 0;                   /* sum slots per view: the most cuts (contrasts and blurs) of any view */
     int launches = 0;
 };
@@ -1668,6 +1683,9 @@ static int stage_color(JPEGB200_BATCH *b, DecodeState &D)
     b->co_desc.assign(n, JDColorDesc{});
     b->co_blk.assign((size_t)nl * n, 0);
     std::vector<uint64_t> ctas(nl, 0);
+    D.co_lut.assign(nl, 0);
+    std::vector<uint32_t> hslot((size_t)nl * n, 0);
+    uint32_t nslots = 0;
     for (int i = 0; i < n; i++) {
         for (uint32_t s = 0; s < nl; s++) b->co_blk[(size_t)s * n + i] = (uint32_t)ctas[s];
         const JDColorPlan &p = b->co_plans[i];
@@ -1679,9 +1697,14 @@ static int stage_color(JPEGB200_BATCH *b, DecodeState &D)
         c.plan = p;
         const uint64_t per = ((uint64_t)c.w * c.h + JD_CO_THREADS - 1) / JD_CO_THREADS;
         for (uint32_t s = 0; s <= p.ncontrast; s++) {
-            /* segment s has per-pixel operations after its blur, or sums L for the contrast after it */
-            const uint32_t k0 = p.seg[s] + (p.seg[s] < p.seg[s + 1] && p.op[p.seg[s]] == JD_CO_BLUR ? 1u : 0u);
-            if (k0 < p.seg[s + 1] || (s < p.ncontrast && p.op[p.seg[s + 1]] == JD_CO_CONTRAST)) ctas[s] += per;
+            /* segment s has per-pixel operations after its own-kernel op, or sums L for the contrast after it, or counts
+             * the histogram for the autocontrast or equalize after it */
+            const uint32_t k0 = p.seg[s] + (p.seg[s] < p.seg[s + 1] && JD_CO_OWN_KERNEL(p.op[p.seg[s]]) ? 1u : 0u);
+            const uint32_t next = s < p.ncontrast ? p.op[p.seg[s + 1]] : 0u;
+            if (k0 < p.seg[s + 1] || next == JD_CO_CONTRAST || JD_CO_LUT(next)) ctas[s] += per;
+            if (JD_CO_LUT(next)) { hslot[(size_t)s * n + i] = nslots++; D.co_lut[s] = 1; }
+            for (uint32_t k = p.seg[s]; k < p.seg[s + 1]; k++)
+                if (JD_CO_LUT(p.op[k]) || p.op[k] == JD_CO_POSTERIZE || p.op[k] == JD_CO_INVERT) D.co_lut[s] = 1;
         }
     }
     /* blurs: at cut index s, the views whose segment s starts with one */
@@ -1691,8 +1714,15 @@ static int stage_color(JPEGB200_BATCH *b, DecodeState &D)
     std::vector<uint32_t> hblk, vblk;
     uint64_t soff = 0;
     std::vector<uint64_t> soffs(n, 0);
-    for (int i = 0; i < n; i++)
-        if (b->bl_scratch[i] && b->parse_status[i] == JPEG_SUCCESS) { soffs[i] = soff; soff += (uint64_t)b->bl_scratch[i]; }
+    for (int i = 0; i < n; i++) {   /* the scratch copies first, then the histogram slots */
+        if (b->parse_status[i] != JPEG_SUCCESS) continue;
+        const JDColorPlan &p = b->co_plans[i];
+        uint64_t nlut = 0;
+        for (uint32_t k = 0; k < p.nops; k++) nlut += JD_CO_LUT(p.op[k]) ? 1u : 0u;
+        const uint64_t img = (uint64_t)b->bl_scratch[i] - nlut * JD_AU_HIST * sizeof(unsigned long long);
+        if (img) { soffs[i] = soff; soff += img; }
+    }
+    const uint64_t hbytes = (uint64_t)nslots * JD_AU_HIST * sizeof(unsigned long long);
     for (uint32_t s = 1; s < nl; s++) {
         D.bl_first[s] = (uint32_t)b->bl_desc.size();
         for (int i = 0; i < n; i++) {
@@ -1709,13 +1739,47 @@ static int stage_color(JPEGB200_BATCH *b, DecodeState &D)
         }
     }
     D.bl_first[nl] = (uint32_t)b->bl_desc.size();
+    /* sharpness and geometric ops: at cut index s, the views whose segment s starts with one */
+    b->au_desc.clear();
+    D.au_first.assign(nl + 1, 0);
+    D.au_ctas.assign(nl, 0);
+    for (uint32_t s = 1; s < nl; s++) {
+        D.au_first[s] = (uint32_t)b->au_desc.size();
+        for (int i = 0; i < n; i++) {
+            const JDColorPlan &p = b->co_plans[i];
+            if (b->parse_status[i] != JPEG_SUCCESS || s > p.ncontrast) continue;
+            const uint32_t op = p.op[p.seg[s]];
+            if (op != JD_CO_SHARPNESS && !JD_CO_GEOMETRIC(op)) continue;
+            JDAugDesc x{};
+            x.off = b->co_desc[i].off; x.pitch = b->co_desc[i].pitch; x.soff = soffs[i];
+            x.w = b->co_desc[i].w; x.h = b->co_desc[i].h;
+            x.op = op; x.arg = p.arg[p.seg[s]];
+            x.m = b->co_aug[i].a[p.seg[s]];
+            x.blk = D.au_ctas[s];
+            const uint64_t c = D.au_ctas[s] + ((uint64_t)x.w * x.h + JD_AU_THREADS - 1) / JD_AU_THREADS;
+            if (c >= (1ull << 31)) { snprintf(g_err, sizeof(g_err), "colour operations: too many pixels in one job"); return 0; }
+            D.au_ctas[s] = (uint32_t)c;
+            b->au_desc.push_back(x);
+        }
+    }
+    D.au_first[nl] = (uint32_t)b->au_desc.size();
+    if (soff + hbytes) CK(b->d_bl.alloc(&b->ctx->pool, soff + hbytes));
+    if (!b->au_desc.empty()) {
+        CK(b->d_au_desc.alloc(&b->ctx->pool, b->au_desc.size()));
+        CK(cudaMemcpyAsync(b->d_au_desc.p, b->au_desc.data(), sizeof(JDAugDesc) * b->au_desc.size(), cudaMemcpyHostToDevice, st));
+    }
+    if (nslots) {   /* soff is 256-byte aligned: the slots are 64-bit aligned */
+        D.co_hist = reinterpret_cast<unsigned long long *>(b->d_bl.p + soff);
+        CK(cudaMemsetAsync(D.co_hist, 0, hbytes, st));
+        CK(b->d_co_hslot.alloc(&b->ctx->pool, (size_t)nl * n));
+        CK(cudaMemcpyAsync(b->d_co_hslot.p, hslot.data(), sizeof(uint32_t) * nl * n, cudaMemcpyHostToDevice, st));
+    }
     if (!b->bl_desc.empty()) {
         const size_t m = b->bl_desc.size();
         b->bl_blk = hblk;
         b->bl_blk.insert(b->bl_blk.end(), vblk.begin(), vblk.end());
         CK(b->d_bl_desc.alloc(&b->ctx->pool, m));
         CK(b->d_bl_blk.alloc(&b->ctx->pool, 2 * m));
-        CK(b->d_bl.alloc(&b->ctx->pool, soff));
         CK(cudaMemcpyAsync(b->d_bl_desc.p, b->bl_desc.data(), sizeof(JDBlurDesc) * m, cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(b->d_bl_blk.p, b->bl_blk.data(), sizeof(uint32_t) * 2 * m, cudaMemcpyHostToDevice, st));
     }
@@ -2208,7 +2272,8 @@ static void run_resize(JPEGB200_BATCH *b, DecodeState &D)
 }
 
 /* timed in the dither slot too, after the resize: per cut index of the operation lists, the blur pair for the views that
- * blur there, then jdk_color for the per-pixel operations up to the next cut */
+ * blur there, the jdk_augment pair for the views that sharpen or move pixels there, then jdk_color for the per-pixel
+ * operations up to the next cut */
 static void run_color(JPEGB200_BATCH *b, DecodeState &D)
 {
     cudaStream_t st = b->ss.stream;
@@ -2228,11 +2293,29 @@ static void run_color(JPEGB200_BATCH *b, DecodeState &D)
             }
             D.launches += 2;
         }
+        const uint32_t fa = D.au_first[s], na = D.au_first[s + 1] - fa;
+        if (na) {
+            const JDAugDesc *ad = b->d_au_desc.p + fa;
+            if (b->ptclass == JD_PT_GRAY) {
+                jdk_augment<1><<<D.au_ctas[s], JD_AU_THREADS, 0, st>>>(ad, na, D.pipe_out, b->d_bl.p);
+                jdk_augment_copy<1><<<D.au_ctas[s], JD_AU_THREADS, 0, st>>>(ad, na, D.pipe_out, b->d_bl.p);
+            } else {
+                jdk_augment<4><<<D.au_ctas[s], JD_AU_THREADS, 0, st>>>(ad, na, D.pipe_out, b->d_bl.p);
+                jdk_augment_copy<4><<<D.au_ctas[s], JD_AU_THREADS, 0, st>>>(ad, na, D.pipe_out, b->d_bl.p);
+            }
+            D.launches += 2;
+        }
         if (!D.co_ctas[s]) continue;
-        if (b->ptclass == JD_PT_GRAY)
-            jdk_color<1><<<D.co_ctas[s], JD_CO_THREADS, 0, st>>>(b->d_co_desc.p, b->d_co_blk.p + (size_t)s * n, n, s, b->d_co_sum.p, D.co_nsum, D.pipe_out);
+        const uint32_t *cblk = b->d_co_blk.p + (size_t)s * n;
+        if (D.co_lut[s]) {
+            if (b->ptclass == JD_PT_GRAY)
+                jdk_color_lut<1><<<D.co_ctas[s], JD_CO_THREADS, 0, st>>>(b->d_co_desc.p, cblk, n, s, b->d_co_sum.p, D.co_nsum, D.pipe_out, D.co_hist, b->d_co_hslot.p);
+            else
+                jdk_color_lut<4><<<D.co_ctas[s], JD_CO_THREADS, 0, st>>>(b->d_co_desc.p, cblk, n, s, b->d_co_sum.p, D.co_nsum, D.pipe_out, D.co_hist, b->d_co_hslot.p);
+        } else if (b->ptclass == JD_PT_GRAY)
+            jdk_color<1><<<D.co_ctas[s], JD_CO_THREADS, 0, st>>>(b->d_co_desc.p, cblk, n, s, b->d_co_sum.p, D.co_nsum, D.pipe_out);
         else
-            jdk_color<4><<<D.co_ctas[s], JD_CO_THREADS, 0, st>>>(b->d_co_desc.p, b->d_co_blk.p + (size_t)s * n, n, s, b->d_co_sum.p, D.co_nsum, D.pipe_out);
+            jdk_color<4><<<D.co_ctas[s], JD_CO_THREADS, 0, st>>>(b->d_co_desc.p, cblk, n, s, b->d_co_sum.p, D.co_nsum, D.pipe_out);
         D.launches++;
     }
 }

@@ -765,15 +765,106 @@ int jd_color_plan(const JPEGB200_ColorOp *row, int gray, JDColorPlan *plan)
 
 int jd_color_plan_blur(const JPEGB200_ColorOp *row, int gray, JDColorPlan *plan, JDBlurPlan *blur)
 {
+    return jd_color_plan_aug(row, gray, 0, 0, plan, blur, NULL);
+}
+
+double jd_round15(double x)
+{
+    /* CPython rounds to 15 decimals through the correctly rounded decimal string; glibc's printf is exact as well */
+    char s[400];
+    snprintf(s, sizeof(s), "%.15f", x);
+    return strtod(s, NULL);
+}
+
+void jd_aug_matrix(int op, double m, uint32_t w, uint32_t h, double *mat)
+{
+    const double deg2rad = M_PI / 180.0, rad2deg = 180.0 / M_PI;   /* math.radians / math.degrees */
+    if (op == JPEGB200_COLOR_ROTATE) {
+        /* Image.rotate(m): angle % 360 as Python takes it, the matrix rounded to 15 decimals, the centre kept */
+        double ang = fmod(m, 360.0);
+        if (ang != 0.0 && ang < 0.0) ang += 360.0;
+        else if (ang == 0.0) ang = 0.0;
+        const double t = -(ang * deg2rad);
+        mat[0] = jd_round15(cos(t)); mat[1] = jd_round15(sin(t)); mat[2] = 0.0;
+        mat[3] = jd_round15(-sin(t)); mat[4] = jd_round15(cos(t)); mat[5] = 0.0;
+        const double cx = w / 2.0, cy = h / 2.0;
+        mat[2] = mat[0] * -cx + mat[1] * -cy + mat[2] + cx;
+        mat[5] = mat[3] * -cx + mat[4] * -cy + mat[5] + cy;
+        return;
+    }
+    /* torchvision's _get_inverse_affine_matrix(center, 0, translate, 1, shear), step for step */
+    double sx = 0.0, sy = 0.0, cx = w * 0.5, cy = h * 0.5, tx = 0.0, ty = 0.0;
+    if (op == JPEGB200_COLOR_SHEAR_X) { sx = (atan(m) * rad2deg) * deg2rad; cx = cy = 0.0; }
+    else if (op == JPEGB200_COLOR_SHEAR_Y) { sy = (atan(m) * rad2deg) * deg2rad; cx = cy = 0.0; }
+    else if (op == JPEGB200_COLOR_TRANSLATE_X) tx = trunc(m);   /* int(magnitude), exact for every finite m */
+    else ty = trunc(m);
+    const double rot = 0.0 * deg2rad;
+    const double a = cos(rot - sy) / cos(sy);
+    const double b = -cos(rot - sy) * tan(sx) / cos(sy) - sin(rot);
+    const double c = sin(rot - sy) / cos(sy);
+    const double d = -sin(rot - sy) * tan(sx) / cos(sy) + cos(rot);
+    mat[0] = d / 1.0; mat[1] = -b / 1.0; mat[2] = 0.0 / 1.0; mat[3] = -c / 1.0; mat[4] = a / 1.0; mat[5] = 0.0 / 1.0;
+    mat[2] += mat[0] * (-cx - tx) + mat[1] * (-cy - ty);
+    mat[5] += mat[3] * (-cx - tx) + mat[4] * (-cy - ty);
+    mat[2] += cx;
+    mat[5] += cy;
+}
+
+/* R(v) = floor(v * 65536 + 0.5) into *out; 0 when it does not fit int32 */
+static int jd_aug_fixed(double v, int64_t *out)
+{
+    const double f = floor(v * 65536.0 + 0.5);
+    if (!(f >= -2147483648.0 && f <= 2147483647.0)) return 0;
+    *out = (int64_t)f;
+    return 1;
+}
+
+/* the 16.16 mapping of a geometric op on a w x h view; 0 when a value over the view leaves int32 */
+static int jd_aug_affine(int op, double m, uint32_t w, uint32_t h, JDAffine *out)
+{
+    double mat[6];
+    jd_aug_matrix(op, m, w, h, mat);
+    int64_t x0, y0, ax, ay, bx, by;
+    if (!jd_aug_fixed(mat[0] * 0.5 + mat[1] * 0.5 + mat[2], &x0) || !jd_aug_fixed(mat[3] * 0.5 + mat[4] * 0.5 + mat[5], &y0) ||
+        !jd_aug_fixed(mat[0], &ax) || !jd_aug_fixed(mat[3], &ay) || !jd_aug_fixed(mat[1], &bx) || !jd_aug_fixed(mat[4], &by))
+        return 0;
+    for (int k = 0; k < 4; k++) {   /* the corners bound every pixel's value: the map is affine */
+        const int64_t x = (k & 1) ? (int64_t)w - 1 : 0, y = (k & 2) ? (int64_t)h - 1 : 0;
+        const int64_t X = x0 + y * bx + x * ax, Y = y0 + y * by + x * ay;
+        if (X < INT32_MIN || X > INT32_MAX || Y < INT32_MIN || Y > INT32_MAX) return 0;
+    }
+    out->x0 = (int32_t)x0; out->y0 = (int32_t)y0; out->ax = (int32_t)ax; out->ay = (int32_t)ay; out->bx = (int32_t)bx; out->by = (int32_t)by;
+    return 1;
+}
+
+int jd_color_plan_aug(const JPEGB200_ColorOp *row, int gray, uint32_t w, uint32_t h, JDColorPlan *plan, JDBlurPlan *blur,
+                      JDAugPlan *aug)
+{
     memset(plan, 0, sizeof(*plan));
     if (blur) memset(blur, 0, sizeof(*blur));
+    if (aug) memset(aug, 0, sizeof(*aug));
     for (int k = 0; k < JPEGB200_COLOR_MAX_OPS && row[k].op != 0; k++) {
         const int op = row[k].op;
         const double a = row[k].arg;
-        if ((op < JPEGB200_COLOR_BRIGHTNESS || op > JPEGB200_COLOR_SOLARIZE) && op != JPEGB200_COLOR_GAUSSIAN_BLUR) return 0;
+        if ((op < JPEGB200_COLOR_BRIGHTNESS || op > JPEGB200_COLOR_SOLARIZE) && op != JPEGB200_COLOR_GAUSSIAN_BLUR &&
+            (op < JPEGB200_COLOR_SHARPNESS || op > JPEGB200_COLOR_ROTATE)) return 0;
         if (!isfinite(a)) return 0;
         if (op == JPEGB200_COLOR_HUE && !(a >= -0.5 && a <= 0.5)) return 0;   /* torchvision raises there */
+        if (op == JPEGB200_COLOR_POSTERIZE && !(a >= 0.0 && a <= 8.0 && a == floor(a))) return 0;   /* and there */
         if (gray && (op == JPEGB200_COLOR_SATURATION || op == JPEGB200_COLOR_HUE || op == JPEGB200_COLOR_GRAYSCALE)) continue;
+        if (op >= JPEGB200_COLOR_SHARPNESS) {
+            uint32_t bits = 0u;
+            if (op == JPEGB200_COLOR_SHARPNESS) { const float f = (float)a; memcpy(&bits, &f, 4); }
+            else if (op == JPEGB200_COLOR_POSTERIZE) bits = 255u & ~((1u << (8 - (int)a)) - 1u);
+            else if (JD_CO_GEOMETRIC(op) && aug) {
+                if (w > JD_AU_MAX_SIDE || h > JD_AU_MAX_SIDE || !jd_aug_affine(op, a, w, h, &aug->a[plan->nops])) return 0;
+            }
+            if (op != JPEGB200_COLOR_POSTERIZE && op != JPEGB200_COLOR_INVERT) plan->seg[++plan->ncontrast] = plan->nops;
+            plan->op[plan->nops] = (uint32_t)op;
+            plan->arg[plan->nops] = bits;
+            plan->nops++;
+            continue;
+        }
         if (op == JPEGB200_COLOR_GAUSSIAN_BLUR) {
             /* Pillow takes the radius as a float: |r| rounding to 2^31 or more overflows its int box radius */
             const float r = fabsf((float)a);

@@ -175,10 +175,23 @@ int jd_check_box(const int32_t *out_sizes, const double *boxes, const double *ga
  * the segments cut at each contrast and each blur; on a gray view (gray != 0) saturation, hue and grayscale are dropped.
  * Blurs of radius 0 are dropped, negative radii planned as |r|, and each blur's constants written to blur (when not NULL)
  * at its op slot.  Returns 0 for an unknown op, an argument that is not finite, a hue outside [-0.5, 0.5], or a blur
- * radius whose float32 magnitude is 2^31 or more.  jd_color_plan is the same without the blur constants. */
+ * radius whose float32 magnitude is 2^31 or more.  jd_color_plan is the same without the blur constants.
+ * jd_color_plan_aug also plans the auto-augment operations (jd_augment.h) of a w x h view: the list is cut before each
+ * sharpness, autocontrast, equalize and geometric op; posterize is planned as its mask; each geometric op's 16.16 mapping
+ * goes to aug (when not NULL) at its op slot.  It also returns 0 for a posterize argument that is not an integer in 0 .. 8,
+ * and, when aug is not NULL, for a geometric op on a view with a side above JD_AU_MAX_SIDE or whose mapping does not fit
+ * 32 bits.  jd_color_plan_blur is jd_color_plan_aug with aug NULL. */
 #include "jd_color.h"
+#include "jd_augment.h"
+int jd_color_plan_aug(const JPEGB200_ColorOp *row, int gray, uint32_t w, uint32_t h, JDColorPlan *plan, JDBlurPlan *blur,
+                      JDAugPlan *aug);
 int jd_color_plan_blur(const JPEGB200_ColorOp *row, int gray, JDColorPlan *plan, JDBlurPlan *blur);
 int jd_color_plan(const JPEGB200_ColorOp *row, int gray, JDColorPlan *plan);
+/* the inverse matrix Pillow's transform gets for geometric op `op` with magnitude m on a w x h image (torchvision's
+ * _apply_op: _get_inverse_affine_matrix, or Image.rotate's matrix) */
+void jd_aug_matrix(int op, double m, uint32_t w, uint32_t h, double *mat);
+/* Python's round(x, 15) */
+double jd_round15(double x);
 /* GaussianBlur(r)'s box half-width and 24-bit weights for r = |radius| as float32, 0 < r < 2^31 (0 past that) */
 int jd_blur_consts(float r, JDBlur *out);
 /* Batch-level rule of JPEGB200_batchCreateColor: no operation on RGB565, dithered pixel types or padded output (checked

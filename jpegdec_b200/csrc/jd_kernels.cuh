@@ -2169,11 +2169,52 @@ struct JDColorDesc {
     JDColorPlan plan;
 };
 
-/* cblk: this launch's first CTA of every view (views without CTAs share the next one's); sums: ncontrast slots per view */
-template <int BPP>
-__global__ void __launch_bounds__(JD_CO_THREADS) jdk_color(const JDColorDesc *cd, const uint32_t *cblk, uint32_t n, uint32_t s,
-                                                           unsigned long long *sums, uint32_t nsum, uint8_t *base)
+/* This CTA's LUT of autocontrast or equalize (op) from the view's histogram h (channel c at h + 256 c), one bin per thread:
+ * block-wide reductions give each channel's lowest and highest non-empty bin, its non-empty bins and its count, and an
+ * exclusive prefix sum the count below each bin; jd_au_lut_entry (jd_augment.h, which the CPU tier pins through the serial
+ * jd_au_lut) turns them into the entry. */
+template <int NC>
+__device__ void jd_co_build_lut(const unsigned long long *h, uint32_t op, uint8_t (*lut)[256])
 {
+    static_assert(JD_CO_THREADS == 256, "one thread per histogram bin");
+    __shared__ unsigned long long wsum[JD_CO_THREADS / 32];
+    __shared__ uint32_t lohi[2], nz;
+    const uint32_t t = threadIdx.x, lane = t & 31u, wid = t >> 5;
+    for (int c = 0; c < NC; c++) {
+        const unsigned long long hv = h[256 * c + t];
+        unsigned long long inc = hv;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long u = __shfl_up_sync(0xFFFFFFFFu, inc, o);
+            if (lane >= (uint32_t)o) inc += u;
+        }
+        if (t == 0) { lohi[0] = 256u; lohi[1] = 0u; nz = 0u; }
+        if (lane == 31u) wsum[wid] = inc;
+        __syncthreads();
+        if (hv) { atomicMin(&lohi[0], t); atomicMax(&lohi[1], t); atomicAdd(&nz, 1u); }
+        unsigned long long below = inc - hv, total = 0;
+        for (uint32_t k = 0; k < JD_CO_THREADS / 32; k++) {
+            if (k < wid) below += wsum[k];
+            total += wsum[k];
+        }
+        __syncthreads();
+        const uint32_t lo = lohi[0], hi = lohi[1];
+        lut[c][t] = (uint8_t)jd_au_lut_entry(op, lo, hi, nz, total, h[256 * c + (hi & 255u)], below, t);
+        __syncthreads();
+    }
+}
+
+/* One launch of the colour operations.  AUG: the launch also serves the per-pixel auto-augment steps -- posterize and
+ * invert (jd_au_apply3 / _apply1); a view whose segment s starts with an autocontrast / equalize looks its pixels up in the
+ * LUT built from histogram slot hslot[(s - 1) n + v]; a view whose next cut is one counts its output into slot
+ * hslot[s n + v] (shared-memory bins, then one 64-bit atomicAdd per non-empty bin).  The host picks AUG per cut index, so
+ * lists without those ops run jdk_color, the AUG = false code, as before. */
+template <int BPP, bool AUG>
+__device__ __forceinline__ void jd_co_run(const JDColorDesc *cd, const uint32_t *cblk, uint32_t n, uint32_t s,
+                                          unsigned long long *sums, uint32_t nsum, uint8_t *base, unsigned long long *hist,
+                                          const uint32_t *hslot)
+{
+    constexpr int NC = BPP == 4 ? 3 : 1;
     uint32_t lo = 0, hi = n - 1;
     while (lo < hi) {
         const uint32_t mid = (lo + hi + 1) >> 1;
@@ -2185,6 +2226,22 @@ __global__ void __launch_bounds__(JD_CO_THREADS) jdk_color(const JDColorDesc *cd
     const uint64_t item = (uint64_t)(blockIdx.x - cblk[v]) * JD_CO_THREADS + threadIdx.x;
     const uint32_t k0 = d.plan.seg[s], k1 = d.plan.seg[s + 1];
     const uint32_t mean = s > 0 ? jd_co_mean(sums[(uint64_t)v * nsum + s - 1], npx) : 0u;
+    /* one view per CTA: both conditions are the same for all its threads */
+    const bool lut_op = AUG && s > 0 && k0 < k1 && JD_CO_LUT(d.plan.op[k0]);
+    const bool count = AUG && s < d.plan.ncontrast && JD_CO_LUT(d.plan.op[k1]);
+    uint8_t (*lut)[256] = nullptr;
+    uint32_t (*bins)[256] = nullptr;
+    if constexpr (AUG) {
+        static_assert(JD_CO_THREADS == 256, "one thread per histogram bin");
+        __shared__ uint8_t lut_s[NC][256];
+        __shared__ uint32_t bins_s[NC][256];
+        lut = lut_s; bins = bins_s;
+        if (lut_op) jd_co_build_lut<NC>(hist + (uint64_t)hslot[(uint64_t)(s - 1) * n + v] * JD_AU_HIST, d.plan.op[k0], lut);
+        if (count) {
+            for (int c = 0; c < NC; c++) bins[c][threadIdx.x] = 0u;
+            __syncthreads();
+        }
+    }
     uint32_t l = 0;
     if (item < npx) {
         const uint32_t y = (uint32_t)(item / d.w), x = (uint32_t)(item % d.w);
@@ -2192,16 +2249,33 @@ __global__ void __launch_bounds__(JD_CO_THREADS) jdk_color(const JDColorDesc *cd
         if (BPP == 4) {
             const uint32_t w = *reinterpret_cast<const uint32_t *>(px);
             uint32_t r = d.bgr ? (w >> 16) & 255u : w & 255u, g = (w >> 8) & 255u, b = d.bgr ? w & 255u : (w >> 16) & 255u;
-            for (uint32_t k = k0; k < k1; k++) jd_co_apply3(d.plan.op[k], d.plan.arg[k], mean, &r, &g, &b);
+            if (lut_op) { r = lut[0][r]; g = lut[1][g]; b = lut[2][b]; }
+            for (uint32_t k = k0; k < k1; k++) {
+                if constexpr (AUG) jd_au_apply3(d.plan.op[k], d.plan.arg[k], mean, &r, &g, &b);
+                else jd_co_apply3(d.plan.op[k], d.plan.arg[k], mean, &r, &g, &b);
+            }
             if (k1 > k0)
                 *reinterpret_cast<uint32_t *>(px) = (w & 0xFF000000u) | (d.bgr ? (r << 16) | (g << 8) | b : (b << 16) | (g << 8) | r);
             l = jd_co_luma(r, g, b);
+            if (count) { atomicAdd(&bins[0][r], 1u); atomicAdd(&bins[1][g], 1u); atomicAdd(&bins[2][b], 1u); }
         } else {
             uint32_t c = *px;
-            for (uint32_t k = k0; k < k1; k++) c = jd_co_apply1(d.plan.op[k], d.plan.arg[k], mean, c);
+            if (lut_op) c = lut[0][c];
+            for (uint32_t k = k0; k < k1; k++) {
+                if constexpr (AUG) c = jd_au_apply1(d.plan.op[k], d.plan.arg[k], mean, c);
+                else c = jd_co_apply1(d.plan.op[k], d.plan.arg[k], mean, c);
+            }
             if (k1 > k0) *px = (uint8_t)c;
             l = c;
+            if (count) atomicAdd(&bins[0][c], 1u);
         }
+    }
+    if (count) {
+        __syncthreads();
+        unsigned long long *g = hist + (uint64_t)hslot[(uint64_t)s * n + v] * JD_AU_HIST;
+        for (int c = 0; c < NC; c++)
+            if (bins[c][threadIdx.x]) atomicAdd(&g[256 * c + threadIdx.x], (unsigned long long)bins[c][threadIdx.x]);
+        return;
     }
     if (s >= d.plan.ncontrast) return;   /* the same for every thread of the CTA: one view */
     __shared__ uint32_t part[JD_CO_THREADS / 32];
@@ -2214,6 +2288,24 @@ __global__ void __launch_bounds__(JD_CO_THREADS) jdk_color(const JDColorDesc *cd
         for (int k = 0; k < JD_CO_THREADS / 32; k++) t += part[k];
         atomicAdd(&sums[(uint64_t)v * nsum + s], t);
     }
+}
+
+/* cblk: this launch's first CTA of every view (views without CTAs share the next one's); sums: ncontrast slots per view */
+template <int BPP>
+__global__ void __launch_bounds__(JD_CO_THREADS) jdk_color(const JDColorDesc *cd, const uint32_t *cblk, uint32_t n, uint32_t s,
+                                                           unsigned long long *sums, uint32_t nsum, uint8_t *base)
+{
+    jd_co_run<BPP, false>(cd, cblk, n, s, sums, nsum, base, nullptr, nullptr);
+}
+
+/* the same at a cut index where some view posterizes, inverts, applies an autocontrast / equalize LUT or counts a
+ * histogram for one; hist: the histogram slots (JD_AU_HIST words each), hslot: per cut index and view its slot */
+template <int BPP>
+__global__ void __launch_bounds__(JD_CO_THREADS) jdk_color_lut(const JDColorDesc *cd, const uint32_t *cblk, uint32_t n, uint32_t s,
+                                                               unsigned long long *sums, uint32_t nsum, uint8_t *base,
+                                                               unsigned long long *hist, const uint32_t *hslot)
+{
+    jd_co_run<BPP, true>(cd, cblk, n, s, sums, nsum, base, hist, hslot);
 }
 
 /* ------------------------------------------------------------------------------------ */
@@ -2290,6 +2382,84 @@ __global__ void __launch_bounds__(JD_BL_THREADS) jdk_blur(const JDBlurDesc *bd, 
         }
         __syncthreads();
     }
+}
+
+/* ------------------------------------------------------------------------------------ */
+/* Sharpness and the geometric ops (jd_augment.h): one launch pair per cut index at which   */
+/* some view sharpens or moves pixels, over those views only.  jdk_augment writes the new   */
+/* image into the view's scratch copy (rows w * BPP bytes apart), reading only the image;   */
+/* jdk_augment_copy copies it back, writing only the image's row bytes.  One thread per     */
+/* pixel in both, the same CTAs per view.                                                   */
+/* ------------------------------------------------------------------------------------ */
+#include "jd_augment.h"
+#define JD_AU_THREADS 256
+struct JDAugDesc {
+    uint64_t off;              /* the view's image from the launch's base */
+    uint64_t pitch;            /* bytes between its rows */
+    uint64_t soff;             /* its scratch copy from the scratch base */
+    uint32_t w, h;
+    uint32_t op;               /* JD_CO_SHARPNESS or a geometric op */
+    uint32_t arg;              /* sharpness: the factor's float bits (each channel on its own: the byte order is moot) */
+    uint32_t blk;              /* first CTA of this view */
+    JDAffine m;                /* geometric ops: the source mapping */
+};
+
+__device__ __forceinline__ const JDAugDesc &jd_au_find(const JDAugDesc *ad, uint32_t n, uint32_t b)
+{
+    uint32_t lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (ad[mid].blk <= b) lo = mid; else hi = mid - 1;
+    }
+    return ad[lo];
+}
+
+template <int BPP>
+__global__ void __launch_bounds__(JD_AU_THREADS) jdk_augment(const JDAugDesc *ad, uint32_t n, const uint8_t *base, uint8_t *scratch)
+{
+    const JDAugDesc &d = jd_au_find(ad, n, blockIdx.x);
+    const uint64_t item = (uint64_t)(blockIdx.x - d.blk) * JD_AU_THREADS + threadIdx.x;
+    if (item >= (uint64_t)d.w * d.h) return;
+    const uint32_t y = (uint32_t)(item / d.w), x = (uint32_t)(item % d.w);
+    const uint8_t *img = base + d.off;
+    uint32_t o;
+    if (d.op == JD_CO_SHARPNESS) {
+        const uint32_t c = jd_bl_load<BPP>(img + (uint64_t)y * d.pitch + (uint64_t)x * BPP);
+        o = c;
+        if (x > 0 && y > 0 && x + 1 < d.w && y + 1 < d.h) {   /* SMOOTH leaves the border alone */
+            const float f = jd_co_float(d.arg);
+            uint32_t nb[JD_BL_NC(BPP)] = {};
+            for (int dy = -1; dy <= 1; dy++)
+                for (int dx = -1; dx <= 1; dx++) {
+                    if (dx == 0 && dy == 0) continue;
+                    const uint32_t q = jd_bl_load<BPP>(img + (uint64_t)(y + dy) * d.pitch + (uint64_t)(x + dx) * BPP);
+                    for (int k = 0; k < JD_BL_NC(BPP); k++) nb[k] += (q >> (8 * k)) & 255u;
+                }
+            o = BPP == 4 ? c & 0xFF000000u : 0u;
+            for (int k = 0; k < JD_BL_NC(BPP); k++) {
+                const uint32_t ck = (c >> (8 * k)) & 255u;
+                o |= jd_co_blend(jd_au_smooth(ck, nb[k]), ck, f) << (8 * k);
+            }
+        }
+    } else {
+        const int64_t src = jd_au_source(&d.m, x, y, d.w, d.h);
+        o = src < 0 ? (BPP == 4 ? 0xFF000000u : 0u)
+                    : jd_bl_load<BPP>(img + (uint64_t)(src / d.w) * d.pitch + (uint64_t)(src % d.w) * BPP);
+    }
+    if (BPP == 4) reinterpret_cast<uint32_t *>(scratch + d.soff)[item] = o;
+    else scratch[d.soff + item] = (uint8_t)o;
+}
+
+template <int BPP>
+__global__ void __launch_bounds__(JD_AU_THREADS) jdk_augment_copy(const JDAugDesc *ad, uint32_t n, uint8_t *base, const uint8_t *scratch)
+{
+    const JDAugDesc &d = jd_au_find(ad, n, blockIdx.x);
+    const uint64_t item = (uint64_t)(blockIdx.x - d.blk) * JD_AU_THREADS + threadIdx.x;
+    if (item >= (uint64_t)d.w * d.h) return;
+    const uint32_t y = (uint32_t)(item / d.w), x = (uint32_t)(item % d.w);
+    uint8_t *px = base + d.off + (uint64_t)y * d.pitch + (uint64_t)x * BPP;
+    if (BPP == 4) *reinterpret_cast<uint32_t *>(px) = reinterpret_cast<const uint32_t *>(scratch + d.soff)[item];
+    else *px = scratch[d.soff + item];
 }
 
 /* ------------------------------------------------------------------------------------ */
