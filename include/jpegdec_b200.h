@@ -423,6 +423,15 @@ int JPEGB200_thumbnailPlan(int width, int height, int req_w, int req_h, double r
 #define JPEGB200_COLOR_TRANSLATE_X  27
 #define JPEGB200_COLOR_TRANSLATE_Y  28
 #define JPEGB200_COLOR_ROTATE       29
+/* A filter flag OR'd into one of the five geometric codes (25 .. 29), e.g. JPEGB200_COLOR_ROTATE | JPEGB200_COLOR_BILINEAR:
+ * the op is _apply_op(img, "ShearX" .. "Rotate", m, BILINEAR or BICUBIC, fill=None) instead, the same argument, size, fill
+ * and refusals (a view side above 1024, a non-finite argument).  R, G and B are resampled on their own; gray views too.
+ * Both flags together, a flag on any other code or on its own is an unknown op (that view gets JPEG_INVALID_PARAMETER).
+ * At a cut index where some view resamples, the call adds jdk_augment_rs, which writes the view's scratch copy, and the
+ * jdk_augment_copy that copies it back (one copy launch serves the NEAREST and sharpness views there too).
+ * DESIGN.md 4.2.12. */
+#define JPEGB200_COLOR_BILINEAR     0x100
+#define JPEGB200_COLOR_BICUBIC      0x200
 #define JPEGB200_COLOR_MAX_OPS    8
 typedef struct {
     int32_t op;                        /* JPEGB200_COLOR_*, 0 = end of the view's list */

@@ -42,6 +42,8 @@ COLOR_GAUSSIAN_BLUR = 16   # (COLOR_GAUSSIAN_BLUR, r): Pillow's img.filter(Image
 # torchvision's auto-augment operations on PIL images (include/jpegdec_b200.h; auto_augment_ops draws them)
 COLOR_SHARPNESS, COLOR_POSTERIZE, COLOR_AUTOCONTRAST, COLOR_EQUALIZE, COLOR_INVERT = 20, 21, 22, 23, 24
 COLOR_SHEAR_X, COLOR_SHEAR_Y, COLOR_TRANSLATE_X, COLOR_TRANSLATE_Y, COLOR_ROTATE = 25, 26, 27, 28, 29
+# OR'd into a geometric code: that op resamples with BILINEAR or BICUBIC instead of NEAREST
+COLOR_BILINEAR, COLOR_BICUBIC = 0x100, 0x200
 COLOR_MAX_OPS = 8
 TIMING_NAMES = ["h2d", "prescan", "entropy", "stitch", "idct", "dither", "d2h", "total"]
 COUNTER_NAMES = ["launches", "segments", "blocks", "events", "compressed_bytes", "output_bytes",
@@ -489,24 +491,37 @@ _AUTO_AUGMENT_OPS = {
     "Equalize": lambda m: [COLOR_EQUALIZE], "Invert": lambda m: [COLOR_INVERT], "Identity": lambda m: [],
 }
 
+_GEOMETRIC = ("ShearX", "ShearY", "TranslateX", "TranslateY", "Rotate")
 
-def auto_augment_ops(t, size):
+
+def auto_augment_ops(t, size, *, resample=False):
     """One view's operation list for torchvision's RandAugment, TrivialAugmentWide or AutoAugment `t` on a PIL image of
     size = (w, h): the same draws from torch's global generator, in the same order and with the same calls, as t.forward,
     so under one torch.manual_seed the list gives torchvision's image (and leaves the generator where forward does).
-    ValueError for an interpolation other than NEAREST or a non-zero fill, whose bytes the operations do not pin."""
+    With resample=True a BILINEAR or BICUBIC `t` gets its geometric ops with COLOR_BILINEAR / COLOR_BICUBIC.
+    ValueError for any other interpolation than NEAREST (or, with resample=True, BILINEAR and BICUBIC) or a non-zero fill,
+    whose bytes the operations do not pin."""
     import torch
     from torchvision import transforms as TV
     from torchvision.transforms import InterpolationMode
     if not isinstance(t, (TV.RandAugment, TV.TrivialAugmentWide, TV.AutoAugment)):
         raise TypeError("auto_augment_ops: a RandAugment, TrivialAugmentWide or AutoAugment")
-    if t.interpolation != InterpolationMode.NEAREST:
-        raise ValueError("auto_augment_ops: only interpolation=NEAREST is supported")
+    flags = {InterpolationMode.NEAREST: 0}
+    if resample:
+        flags.update({InterpolationMode.BILINEAR: COLOR_BILINEAR, InterpolationMode.BICUBIC: COLOR_BICUBIC})
+    if t.interpolation not in flags:
+        raise ValueError("auto_augment_ops: interpolation %s is not supported%s"
+                         % (t.interpolation, "" if resample else " without resample=True"))
+    flag = flags[t.interpolation]
     fill = t.fill
     if fill is not None and any(float(f) != 0.0 for f in (fill if isinstance(fill, (list, tuple)) else [fill])):
         raise ValueError("auto_augment_ops: only fill None or 0 is supported")
     w, h = size
     ops = []
+
+    def op_list(name, m):
+        return [(o[0] | flag, o[1]) if name in _GEOMETRIC else o for o in _AUTO_AUGMENT_OPS[name](m)]
+
     if isinstance(t, TV.RandAugment):
         meta = t._augmentation_space(t.num_magnitude_bins, (h, w))
         for _ in range(t.num_ops):
@@ -515,7 +530,7 @@ def auto_augment_ops(t, size):
             m = float(mags[t.magnitude].item()) if mags.ndim > 0 else 0.0
             if signed and torch.randint(2, (1,)):
                 m *= -1.0
-            ops += _AUTO_AUGMENT_OPS[name](m)
+            ops += op_list(name, m)
     elif isinstance(t, TV.TrivialAugmentWide):
         meta = t._augmentation_space(t.num_magnitude_bins)
         name = list(meta.keys())[int(torch.randint(len(meta), (1,)).item())]
@@ -523,7 +538,7 @@ def auto_augment_ops(t, size):
         m = float(mags[torch.randint(len(mags), (1,), dtype=torch.long)].item()) if mags.ndim > 0 else 0.0
         if signed and torch.randint(2, (1,)):
             m *= -1.0
-        ops += _AUTO_AUGMENT_OPS[name](m)
+        ops += op_list(name, m)
     else:
         pid, probs, signs = t.get_params(len(t.policies))
         meta = t._augmentation_space(10, (h, w))
@@ -533,7 +548,7 @@ def auto_augment_ops(t, size):
                 m = float(mags[mid].item()) if mid is not None else 0.0
                 if signed and signs[i] == 0:
                     m *= -1.0
-                ops += _AUTO_AUGMENT_OPS[name](m)
+                ops += op_list(name, m)
     return ops
 
 

@@ -1,9 +1,10 @@
 /*
  * jd_augment.h -- the auto-augment operations of torchvision's RandAugment / TrivialAugmentWide / AutoAugment on PIL images
  * that are not per-pixel blends (adjust_sharpness, autocontrast, equalize, and ShearX / ShearY / TranslateX / TranslateY /
- * Rotate with NEAREST and fill 0), restated as probing Pillow 12.2 pins them.  Shared by the kernels (jd_kernels.cuh:
- * jdk_augment, jdk_color's LUT step), the host plan (jd_host.c: jd_color_plan_aug) and the CPU stepper (tests/augsim).
- * DESIGN.md 4.2.11 has the probes.  Posterize and invert are per pixel: jd_color.h.
+ * Rotate with NEAREST, BILINEAR or BICUBIC and fill 0), restated as probing Pillow 12.2 pins them.  Shared by the kernels
+ * (jd_kernels.cuh: jdk_augment, jdk_augment_rs, jdk_color's LUT step), the host plan (jd_host.c: jd_color_plan_aug) and the
+ * CPU steppers (tests/augsim, tests/augrssim).  DESIGN.md 4.2.11 and 4.2.12 have the probes.  Posterize and invert are
+ * per pixel: jd_color.h.
  *
  *   SMOOTH (ImageFilter.SMOOTH): inner pixels (S + 6) / 13, S = the 8 neighbours + 5 x the centre; the border, and an
  *                       image under 3 pixels on a side, unchanged.  Sharpness f = blend(SMOOTH, img, f) (jd_co_blend).
@@ -16,6 +17,15 @@
  *                       X0 = R(a / 2 + b / 2 + c), Y0 = R(d / 2 + e / 2 + f); outside the image: fill 0 (alpha kept 0xFF).
  *                       The host computes the six integers (jd_color_plan_aug) and checks that every value over the view
  *                       fits 32 bits, so the device stays integer-only.
+ *   geometric (BILINEAR / BICUBIC, JD_CO_BILINEAR / _BICUBIC OR'd into the code): the same matrix (a .. f) in double, each
+ *                       output pixel computed on its own, every step one IEEE double operation (no FMA):
+ *                       xin = (a (x + 0.5) + b (y + 0.5)) + c, yin = (d (x + 0.5) + e (y + 0.5)) + f; outside [0, w) x [0, h):
+ *                       fill 0 (alpha kept 0xFF); else xin -= 0.5, yin -= 0.5, x0 = floor(xin), dx = xin - x0 (y alike),
+ *                       neighbour indices clamped to the image.  BILINEAR: lerp(p, q, t) = p + (q - p) t along x on rows
+ *                       y0 and y0 + 1, then along y.  BICUBIC: cubic(v1 .. v4, t) = v2 + t (p2 + t (p3 + t p4)),
+ *                       p2 = -v1 + v3, p3 = 2 (v1 - v2) + v3 - v4, p4 = -v1 + v2 - v3 + v4 (the a = -1 kernel) along x on rows
+ *                       y0 - 1 .. y0 + 2 (columns x0 - 1 .. x0 + 2), then along y.  Both: clamped to [0, 255], truncated.
+ *                       jd_au_resample; the host plan stores the six doubles (JDResamplePlan).
  * Plain C, C++ or CUDA.
  */
 #ifndef JD_AUGMENT_H
@@ -36,6 +46,10 @@ typedef struct {
 typedef struct {
     JDAffine a[JD_CO_MAX_OPS];   /* per op slot of the plan */
 } JDAugPlan;
+/* A BILINEAR / BICUBIC geometric op's matrix (jd_aug_matrix), per op slot of the plan */
+typedef struct {
+    double mat[JD_CO_MAX_OPS][6];
+} JDResamplePlan;
 
 /* ImageFilter.SMOOTH of one channel at an inner pixel: c = the centre, nb = the sum of its 8 neighbours */
 JD_CO_HD uint32_t jd_au_smooth(uint32_t c, uint32_t nb) { return (nb + 5u * c + 6u) / 13u; }
@@ -49,6 +63,55 @@ JD_CO_HD int64_t jd_au_source(const JDAffine *m, uint32_t x, uint32_t y, uint32_
     const int32_t sx = X >> 16, sy = Y >> 16;   /* arithmetic shifts: floor */
     if (sx < 0 || sy < 0 || (uint32_t)sx >= w || (uint32_t)sy >= h) return -1;
     return (int64_t)sy * w + sx;
+}
+
+JD_CO_HD double jd_au_lerp(double p, double q, double t) { return JD_CO_DADD(p, JD_CO_DMUL(JD_CO_DSUB(q, p), t)); }
+
+JD_CO_HD double jd_au_cubic(double v1, double v2, double v3, double v4, double t)
+{
+    const double p2 = JD_CO_DADD(-v1, v3);
+    const double p3 = JD_CO_DSUB(JD_CO_DADD(JD_CO_DMUL(2.0, JD_CO_DSUB(v1, v2)), v3), v4);
+    const double p4 = JD_CO_DADD(JD_CO_DSUB(JD_CO_DADD(-v1, v2), v3), v4);
+    return JD_CO_DADD(v2, JD_CO_DMUL(t, JD_CO_DADD(p2, JD_CO_DMUL(t, JD_CO_DADD(p3, JD_CO_DMUL(t, p4))))));
+}
+
+JD_CO_HD uint32_t jd_au_clamp8(double v) { return v <= 0.0 ? 0u : v >= 255.0 ? 255u : (uint32_t)v; }
+
+/* Output (x, y) of a BILINEAR (bicubic = 0) or BICUBIC geometric op with matrix m on the w x h image img (rows pitch bytes
+ * apart, bpp 4 = RGB8888 words, each of the first 3 bytes resampled on its own, or 1 = gray): its resampled bytes into
+ * out[0 .. 2] or out[0]; 0 (out untouched) for a fill pixel.  A NaN coordinate, which no finite matrix gives, is fill. */
+JD_CO_HD int jd_au_resample(const double *m, uint32_t bicubic, uint32_t x, uint32_t y, uint32_t w, uint32_t h,
+                            const uint8_t *img, uint64_t pitch, uint32_t bpp, uint8_t *out)
+{
+    const double xx = JD_CO_DADD((double)x, 0.5), yy = JD_CO_DADD((double)y, 0.5);
+    const double xin = JD_CO_DADD(JD_CO_DADD(JD_CO_DMUL(m[0], xx), JD_CO_DMUL(m[1], yy)), m[2]);
+    const double yin = JD_CO_DADD(JD_CO_DADD(JD_CO_DMUL(m[3], xx), JD_CO_DMUL(m[4], yy)), m[5]);
+    if (!(xin >= 0.0 && xin < (double)w && yin >= 0.0 && yin < (double)h)) return 0;
+    const double sx = JD_CO_DSUB(xin, 0.5), sy = JD_CO_DSUB(yin, 0.5);
+    const double fx = floor(sx), fy = floor(sy);
+    const double dx = JD_CO_DSUB(sx, fx), dy = JD_CO_DSUB(sy, fy);
+    const int x0 = (int)fx, y0 = (int)fy;   /* -1 .. w - 1, -1 .. h - 1 */
+    uint64_t xo[4], yo[4];   /* byte offsets of columns x0 - 1 .. x0 + 2 and rows y0 - 1 .. y0 + 2, clamped */
+    for (int j = 0; j < 4; j++) {
+        const int xj = x0 - 1 + j, yj = y0 - 1 + j;
+        xo[j] = (uint64_t)(xj < 0 ? 0 : xj >= (int)w ? (int)w - 1 : xj) * bpp;
+        yo[j] = (uint64_t)(yj < 0 ? 0 : yj >= (int)h ? (int)h - 1 : yj) * pitch;
+    }
+    const uint32_t nc = bpp == 4u ? 3u : 1u;
+    for (uint32_t k = 0; k < nc; k++) {
+        const uint8_t *p = img + k;
+        double v;
+        if (bicubic) {
+            double r[4];
+            for (int j = 0; j < 4; j++)
+                r[j] = jd_au_cubic(p[yo[j] + xo[0]], p[yo[j] + xo[1]], p[yo[j] + xo[2]], p[yo[j] + xo[3]], dx);
+            v = jd_au_cubic(r[0], r[1], r[2], r[3], dy);
+        } else {
+            v = jd_au_lerp(jd_au_lerp(p[yo[1] + xo[1]], p[yo[1] + xo[2]], dx), jd_au_lerp(p[yo[2] + xo[1]], p[yo[2] + xo[2]], dx), dy);
+        }
+        out[k] = (uint8_t)jd_au_clamp8(v);
+    }
+    return 1;
 }
 
 /* jd_co_apply3 / _apply1 with the per-pixel auto-augment ops: posterize (arg: the kept-bits mask,

@@ -70,11 +70,15 @@
 #define JD_CO_TRANSLATE_X  27
 #define JD_CO_TRANSLATE_Y  28
 #define JD_CO_ROTATE       29
+/* a geometric op's resampling filter, OR'd into its code (the plan holds only valid combinations): run by jdk_augment_rs */
+#define JD_CO_BILINEAR     0x100
+#define JD_CO_BICUBIC      0x200
 #define JD_CO_MAX_OPS    8
 #define JD_CO_GEOMETRIC(op) ((op) >= JD_CO_SHEAR_X && (op) <= JD_CO_ROTATE)
+#define JD_CO_RESAMPLE(op)  (((op) & (JD_CO_BILINEAR | JD_CO_BICUBIC)) != 0)
 #define JD_CO_LUT(op)       ((op) == JD_CO_AUTOCONTRAST || (op) == JD_CO_EQUALIZE)
 /* ops a kernel of their own runs at a cut, before jdk_color runs the rest of the segment */
-#define JD_CO_OWN_KERNEL(op) ((op) == JD_CO_BLUR || (op) == JD_CO_SHARPNESS || JD_CO_GEOMETRIC(op))
+#define JD_CO_OWN_KERNEL(op) ((op) == JD_CO_BLUR || (op) == JD_CO_SHARPNESS || JD_CO_GEOMETRIC(op) || JD_CO_RESAMPLE(op))
 
 JD_CO_HD float jd_co_float(uint32_t bits)
 {

@@ -180,6 +180,7 @@ struct JPEGB200_BATCH {
     std::vector<JDColorPlan> co_plans;
     std::vector<JDBlurPlan> co_blur;        /* per view: each blur's constants at its op slot */
     std::vector<JDAugPlan> co_aug;          /* per view: each geometric op's mapping at its op slot */
+    std::vector<JDResamplePlan> co_rs;      /* per view: each BILINEAR / BICUBIC geometric op's matrix at its op slot */
     std::vector<int64_t> bl_scratch;        /* per view: its scratch copy's bytes when it blurs, sharpens or moves pixels
                                                (256-byte aligned), plus JD_AU_HIST counts per autocontrast / equalize */
     int64_t bl_scratch_total = 0;
@@ -188,8 +189,10 @@ struct JPEGB200_BATCH {
     DevBuf<JDBlurDesc> d_bl_desc;
     DevBuf<uint32_t> d_bl_blk;
     DevBuf<uint8_t> d_bl;                   /* the scratch copies */
-    std::vector<JDAugDesc> au_desc;         /* per jdk_augment launch pair, per view sharpening or moving pixels there */
+    std::vector<JDAugDesc> au_desc;         /* per cut index, per view sharpening or moving pixels there (jdk_augment, _rs, _copy) */
     DevBuf<JDAugDesc> d_au_desc;
+    std::vector<JDAugMat> au_mat;           /* the same entries: the BILINEAR / BICUBIC ops' matrices (zero for the others) */
+    DevBuf<JDAugMat> d_au_mat;
     DevBuf<uint32_t> d_co_hslot;            /* per cut index and view: its histogram slot (the slots follow the scratch copies in d_bl) */
     std::vector<uint8_t> co_bgr;
     std::vector<JDColorDesc> co_desc;
@@ -622,7 +625,7 @@ static void init_batch(JPEGB200_BATCH *b, JPEGB200_CTX *ctx, const CreatePlan &P
     b->box = P.boxes != nullptr || P.gaps != nullptr;
     if (b->box) b->bx_plans.assign(nv, JDBoxPlan{});
     b->color = P.color != nullptr;
-    if (b->color) { b->co_plans.assign(nv, JDColorPlan{}); b->co_blur.assign(nv, JDBlurPlan{}); b->co_aug.assign(nv, JDAugPlan{}); b->bl_scratch.assign(nv, 0); b->co_bgr.assign(nv, 0); }
+    if (b->color) { b->co_plans.assign(nv, JDColorPlan{}); b->co_blur.assign(nv, JDBlurPlan{}); b->co_aug.assign(nv, JDAugPlan{}); b->co_rs.assign(nv, JDResamplePlan{}); b->bl_scratch.assign(nv, 0); b->co_bgr.assign(nv, 0); }
     b->lj = (options & JPEGB200_OPT_LIBJPEG) != 0;
     if (b->lj) { b->lj_desc.assign(nv, JDLjDesc{}); b->lj_plane.assign(nv, 0); }
     b->tensor = P.spec != nullptr;
@@ -806,8 +809,8 @@ static uint32_t plan_views(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int 
             const int s = b->lj ? (int)b->lj_desc[i].shift : b->sshift;
             const uint32_t w = b->resize ? (uint32_t)P.out_sizes[2 * (size_t)i] : b->roi ? (uint32_t)b->plans[i].out_w : (uint32_t)((inf.width + (1 << s) - 1) >> s);
             const uint32_t h = b->resize ? (uint32_t)P.out_sizes[2 * (size_t)i + 1] : b->roi ? (uint32_t)b->plans[i].out_h : (uint32_t)((inf.height + (1 << s) - 1) >> s);
-            if (!jd_color_plan_aug(P.color + JPEGB200_COLOR_MAX_OPS * (size_t)i, b->ptclass == JD_PT_GRAY, w, h, &b->co_plans[i],
-                                   &b->co_blur[i], &b->co_aug[i])) {
+            if (!jd_color_plan_rs(P.color + JPEGB200_COLOR_MAX_OPS * (size_t)i, b->ptclass == JD_PT_GRAY, w, h, &b->co_plans[i],
+                                  &b->co_blur[i], &b->co_aug[i], &b->co_rs[i])) {
                 P.vok[i] = 0;
                 dropped = true;
             }
@@ -1551,7 +1554,8 @@ struct DecodeState {
     std::vector<uint32_t> bl_first;         /* blurs: the first bl_desc entry of each cut index (one past the last at nl) */
     std::vector<uint32_t> bl_ctas;          /* CTAs of each cut index's jdk_blur pair: horizontal, vertical */
     std::vector<uint32_t> au_first;         /* sharpness and geometric ops: the first au_desc entry of each cut index */
-    std::vector<uint32_t> au_ctas;          /* CTAs of each cut index's jdk_augment pair */
+    std::vector<uint32_t> au_ctas;          /* CTAs of each cut index's jdk_augment_copy (jdk_augment's, then jdk_augment_rs's) */
+    std::vector<uint32_t> au_nn;            /* per cut index: the entries and CTAs of jdk_augment (the rest resample) */
     std::vector<uint8_t> co_lut;            /* per cut index: some view posterizes, inverts, applies a LUT or counts a
                                                histogram there (jdk_color_lut) */
     unsigned long long *co_hist = nullptr;  /* the histogram slots */
@@ -1739,27 +1743,38 @@ static int stage_color(JPEGB200_BATCH *b, DecodeState &D)
         }
     }
     D.bl_first[nl] = (uint32_t)b->bl_desc.size();
-    /* sharpness and geometric ops: at cut index s, the views whose segment s starts with one */
+    /* sharpness and geometric ops: at cut index s, the views whose segment s starts with one -- first those that sharpen or
+     * move pixels with NEAREST (jdk_augment), then those that resample (jdk_augment_rs), each with its matrix in au_mat */
     b->au_desc.clear();
+    b->au_mat.clear();
     D.au_first.assign(nl + 1, 0);
     D.au_ctas.assign(nl, 0);
+    D.au_nn.assign(2 * (size_t)nl, 0);
+    bool any_rs = false;
     for (uint32_t s = 1; s < nl; s++) {
         D.au_first[s] = (uint32_t)b->au_desc.size();
-        for (int i = 0; i < n; i++) {
-            const JDColorPlan &p = b->co_plans[i];
-            if (b->parse_status[i] != JPEG_SUCCESS || s > p.ncontrast) continue;
-            const uint32_t op = p.op[p.seg[s]];
-            if (op != JD_CO_SHARPNESS && !JD_CO_GEOMETRIC(op)) continue;
-            JDAugDesc x{};
-            x.off = b->co_desc[i].off; x.pitch = b->co_desc[i].pitch; x.soff = soffs[i];
-            x.w = b->co_desc[i].w; x.h = b->co_desc[i].h;
-            x.op = op; x.arg = p.arg[p.seg[s]];
-            x.m = b->co_aug[i].a[p.seg[s]];
-            x.blk = D.au_ctas[s];
-            const uint64_t c = D.au_ctas[s] + ((uint64_t)x.w * x.h + JD_AU_THREADS - 1) / JD_AU_THREADS;
-            if (c >= (1ull << 31)) { snprintf(g_err, sizeof(g_err), "colour operations: too many pixels in one job"); return 0; }
-            D.au_ctas[s] = (uint32_t)c;
-            b->au_desc.push_back(x);
+        for (int rs = 0; rs < 2; rs++) {
+            for (int i = 0; i < n; i++) {
+                const JDColorPlan &p = b->co_plans[i];
+                if (b->parse_status[i] != JPEG_SUCCESS || s > p.ncontrast) continue;
+                const uint32_t op = p.op[p.seg[s]];
+                if (rs ? !JD_CO_RESAMPLE(op) : op != JD_CO_SHARPNESS && !JD_CO_GEOMETRIC(op)) continue;
+                JDAugDesc x{};
+                x.off = b->co_desc[i].off; x.pitch = b->co_desc[i].pitch; x.soff = soffs[i];
+                x.w = b->co_desc[i].w; x.h = b->co_desc[i].h;
+                x.op = op; x.arg = p.arg[p.seg[s]];
+                x.m = b->co_aug[i].a[p.seg[s]];
+                x.blk = D.au_ctas[s];
+                const uint64_t c = D.au_ctas[s] + ((uint64_t)x.w * x.h + JD_AU_THREADS - 1) / JD_AU_THREADS;
+                if (c >= (1ull << 31)) { snprintf(g_err, sizeof(g_err), "colour operations: too many pixels in one job"); return 0; }
+                D.au_ctas[s] = (uint32_t)c;
+                b->au_desc.push_back(x);
+                JDAugMat mt;
+                memcpy(mt.m, b->co_rs[i].mat[p.seg[s]], sizeof(mt.m));
+                b->au_mat.push_back(mt);
+                any_rs = any_rs || rs;
+            }
+            if (!rs) { D.au_nn[2 * s] = (uint32_t)b->au_desc.size() - D.au_first[s]; D.au_nn[2 * s + 1] = D.au_ctas[s]; }
         }
     }
     D.au_first[nl] = (uint32_t)b->au_desc.size();
@@ -1767,6 +1782,10 @@ static int stage_color(JPEGB200_BATCH *b, DecodeState &D)
     if (!b->au_desc.empty()) {
         CK(b->d_au_desc.alloc(&b->ctx->pool, b->au_desc.size()));
         CK(cudaMemcpyAsync(b->d_au_desc.p, b->au_desc.data(), sizeof(JDAugDesc) * b->au_desc.size(), cudaMemcpyHostToDevice, st));
+    }
+    if (any_rs) {
+        CK(b->d_au_mat.alloc(&b->ctx->pool, b->au_mat.size()));
+        CK(cudaMemcpyAsync(b->d_au_mat.p, b->au_mat.data(), sizeof(JDAugMat) * b->au_mat.size(), cudaMemcpyHostToDevice, st));
     }
     if (nslots) {   /* soff is 256-byte aligned: the slots are 64-bit aligned */
         D.co_hist = reinterpret_cast<unsigned long long *>(b->d_bl.p + soff);
@@ -2272,8 +2291,8 @@ static void run_resize(JPEGB200_BATCH *b, DecodeState &D)
 }
 
 /* timed in the dither slot too, after the resize: per cut index of the operation lists, the blur pair for the views that
- * blur there, the jdk_augment pair for the views that sharpen or move pixels there, then jdk_color for the per-pixel
- * operations up to the next cut */
+ * blur there, jdk_augment for the views that sharpen or move pixels with NEAREST there and jdk_augment_rs for those that
+ * resample, then one jdk_augment_copy for both, then jdk_color for the per-pixel operations up to the next cut */
 static void run_color(JPEGB200_BATCH *b, DecodeState &D)
 {
     cudaStream_t st = b->ss.stream;
@@ -2295,15 +2314,19 @@ static void run_color(JPEGB200_BATCH *b, DecodeState &D)
         }
         const uint32_t fa = D.au_first[s], na = D.au_first[s + 1] - fa;
         if (na) {
+            /* the NEAREST / sharpness entries first (nn of them, in nc CTAs), then the BILINEAR / BICUBIC ones */
             const JDAugDesc *ad = b->d_au_desc.p + fa;
+            const uint32_t nn = D.au_nn[2 * s], nc = D.au_nn[2 * s + 1];
             if (b->ptclass == JD_PT_GRAY) {
-                jdk_augment<1><<<D.au_ctas[s], JD_AU_THREADS, 0, st>>>(ad, na, D.pipe_out, b->d_bl.p);
+                if (nn) jdk_augment<1><<<nc, JD_AU_THREADS, 0, st>>>(ad, nn, D.pipe_out, b->d_bl.p);
+                if (nn < na) jdk_augment_rs<1><<<D.au_ctas[s] - nc, JD_AU_THREADS, 0, st>>>(ad + nn, b->d_au_mat.p + fa + nn, na - nn, nc, D.pipe_out, b->d_bl.p);
                 jdk_augment_copy<1><<<D.au_ctas[s], JD_AU_THREADS, 0, st>>>(ad, na, D.pipe_out, b->d_bl.p);
             } else {
-                jdk_augment<4><<<D.au_ctas[s], JD_AU_THREADS, 0, st>>>(ad, na, D.pipe_out, b->d_bl.p);
+                if (nn) jdk_augment<4><<<nc, JD_AU_THREADS, 0, st>>>(ad, nn, D.pipe_out, b->d_bl.p);
+                if (nn < na) jdk_augment_rs<4><<<D.au_ctas[s] - nc, JD_AU_THREADS, 0, st>>>(ad + nn, b->d_au_mat.p + fa + nn, na - nn, nc, D.pipe_out, b->d_bl.p);
                 jdk_augment_copy<4><<<D.au_ctas[s], JD_AU_THREADS, 0, st>>>(ad, na, D.pipe_out, b->d_bl.p);
             }
-            D.launches += 2;
+            D.launches += 1 + (nn ? 1 : 0) + (nn < na ? 1 : 0);
         }
         if (!D.co_ctas[s]) continue;
         const uint32_t *cblk = b->d_co_blk.p + (size_t)s * n;

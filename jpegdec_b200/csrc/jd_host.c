@@ -840,14 +840,24 @@ static int jd_aug_affine(int op, double m, uint32_t w, uint32_t h, JDAffine *out
 int jd_color_plan_aug(const JPEGB200_ColorOp *row, int gray, uint32_t w, uint32_t h, JDColorPlan *plan, JDBlurPlan *blur,
                       JDAugPlan *aug)
 {
+    return jd_color_plan_rs(row, gray, w, h, plan, blur, aug, NULL);
+}
+
+int jd_color_plan_rs(const JPEGB200_ColorOp *row, int gray, uint32_t w, uint32_t h, JDColorPlan *plan, JDBlurPlan *blur,
+                     JDAugPlan *aug, JDResamplePlan *rs)
+{
     memset(plan, 0, sizeof(*plan));
     if (blur) memset(blur, 0, sizeof(*blur));
     if (aug) memset(aug, 0, sizeof(*aug));
+    if (rs) memset(rs, 0, sizeof(*rs));
     for (int k = 0; k < JPEGB200_COLOR_MAX_OPS && row[k].op != 0; k++) {
         const int op = row[k].op;
         const double a = row[k].arg;
-        if ((op < JPEGB200_COLOR_BRIGHTNESS || op > JPEGB200_COLOR_SOLARIZE) && op != JPEGB200_COLOR_GAUSSIAN_BLUR &&
-            (op < JPEGB200_COLOR_SHARPNESS || op > JPEGB200_COLOR_ROTATE)) return 0;
+        /* a filter flag: exactly one, on a geometric op, for a caller that takes the matrices */
+        const int filt = op & (JPEGB200_COLOR_BILINEAR | JPEGB200_COLOR_BICUBIC), base = op & ~filt;
+        if (filt && (!rs || filt == (JPEGB200_COLOR_BILINEAR | JPEGB200_COLOR_BICUBIC) || !JD_CO_GEOMETRIC(base))) return 0;
+        if ((base < JPEGB200_COLOR_BRIGHTNESS || base > JPEGB200_COLOR_SOLARIZE) && base != JPEGB200_COLOR_GAUSSIAN_BLUR &&
+            (base < JPEGB200_COLOR_SHARPNESS || base > JPEGB200_COLOR_ROTATE)) return 0;
         if (!isfinite(a)) return 0;
         if (op == JPEGB200_COLOR_HUE && !(a >= -0.5 && a <= 0.5)) return 0;   /* torchvision raises there */
         if (op == JPEGB200_COLOR_POSTERIZE && !(a >= 0.0 && a <= 8.0 && a == floor(a))) return 0;   /* and there */
@@ -858,6 +868,9 @@ int jd_color_plan_aug(const JPEGB200_ColorOp *row, int gray, uint32_t w, uint32_
             else if (op == JPEGB200_COLOR_POSTERIZE) bits = 255u & ~((1u << (8 - (int)a)) - 1u);
             else if (JD_CO_GEOMETRIC(op) && aug) {
                 if (w > JD_AU_MAX_SIDE || h > JD_AU_MAX_SIDE || !jd_aug_affine(op, a, w, h, &aug->a[plan->nops])) return 0;
+            } else if (filt) {
+                if (w > JD_AU_MAX_SIDE || h > JD_AU_MAX_SIDE) return 0;
+                jd_aug_matrix(base, a, w, h, rs->mat[plan->nops]);
             }
             if (op != JPEGB200_COLOR_POSTERIZE && op != JPEGB200_COLOR_INVERT) plan->seg[++plan->ncontrast] = plan->nops;
             plan->op[plan->nops] = (uint32_t)op;

@@ -180,9 +180,15 @@ int jd_check_box(const int32_t *out_sizes, const double *boxes, const double *ga
  * sharpness, autocontrast, equalize and geometric op; posterize is planned as its mask; each geometric op's 16.16 mapping
  * goes to aug (when not NULL) at its op slot.  It also returns 0 for a posterize argument that is not an integer in 0 .. 8,
  * and, when aug is not NULL, for a geometric op on a view with a side above JD_AU_MAX_SIDE or whose mapping does not fit
- * 32 bits.  jd_color_plan_blur is jd_color_plan_aug with aug NULL. */
+ * 32 bits.  jd_color_plan_blur is jd_color_plan_aug with aug NULL.
+ * jd_color_plan_rs also plans the geometric ops flagged JPEGB200_COLOR_BILINEAR or _BICUBIC: cut like the NEAREST ones,
+ * each one's matrix (jd_aug_matrix) into rs at its op slot.  It returns 0 for a flag that is not exactly one of the two on
+ * a geometric code, and for a flagged op on a view with a side above JD_AU_MAX_SIDE.  jd_color_plan_aug is
+ * jd_color_plan_rs with rs NULL, which refuses every flagged op, as the plans without rs always have. */
 #include "jd_color.h"
 #include "jd_augment.h"
+int jd_color_plan_rs(const JPEGB200_ColorOp *row, int gray, uint32_t w, uint32_t h, JDColorPlan *plan, JDBlurPlan *blur,
+                     JDAugPlan *aug, JDResamplePlan *rs);
 int jd_color_plan_aug(const JPEGB200_ColorOp *row, int gray, uint32_t w, uint32_t h, JDColorPlan *plan, JDBlurPlan *blur,
                       JDAugPlan *aug);
 int jd_color_plan_blur(const JPEGB200_ColorOp *row, int gray, JDColorPlan *plan, JDBlurPlan *blur);

@@ -2462,6 +2462,28 @@ __global__ void __launch_bounds__(JD_AU_THREADS) jdk_augment_copy(const JDAugDes
     else *px = scratch[d.soff + item];
 }
 
+/* The BILINEAR / BICUBIC geometric ops (jd_au_resample): like jdk_augment, into the view's scratch copy, one thread per
+ * output pixel.  ad / mats: this launch's views and their matrices, entry for entry; their first CTAs (blk) count from
+ * b0, the CTAs of the jdk_augment launch before them at the same cut index, so jdk_augment_copy serves both sets. */
+struct JDAugMat {
+    double m[6];
+};
+
+template <int BPP>
+__global__ void __launch_bounds__(JD_AU_THREADS) jdk_augment_rs(const JDAugDesc *ad, const JDAugMat *mats, uint32_t n, uint32_t b0,
+                                                                const uint8_t *base, uint8_t *scratch)
+{
+    const uint32_t b = blockIdx.x + b0;
+    const JDAugDesc &d = jd_au_find(ad, n, b);
+    const uint64_t item = (uint64_t)(b - d.blk) * JD_AU_THREADS + threadIdx.x;
+    if (item >= (uint64_t)d.w * d.h) return;
+    const uint32_t y = (uint32_t)(item / d.w), x = (uint32_t)(item % d.w);
+    uint8_t o[4] = {0u, 0u, 0u, 0xFFu};   /* fill 0, alpha kept */
+    jd_au_resample(mats[&d - ad].m, (d.op & JD_CO_BICUBIC) != 0u, x, y, d.w, d.h, base + d.off, d.pitch, BPP, o);
+    if (BPP == 4) reinterpret_cast<uint32_t *>(scratch + d.soff)[item] = o[0] | (uint32_t)o[1] << 8 | (uint32_t)o[2] << 16 | (uint32_t)o[3] << 24;
+    else scratch[d.soff + item] = o[0];
+}
+
 /* ------------------------------------------------------------------------------------ */
 /* Tensor output (JPEGB200_batchCreateTensor): the pipeline has written each image's uint8  */
 /* output U tightly into the staging buffer; jdk_tensor looks every byte up in the C x 256  */

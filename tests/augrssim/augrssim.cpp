@@ -1,0 +1,99 @@
+/*
+ * tests/augrssim/augrssim.cpp -- CPU stepper of the auto-augment operations with the BILINEAR / BICUBIC geometric ops
+ * (a geometric code | JPEGB200_COLOR_BILINEAR or _BICUBIC; test infrastructure, not linked into the library).  It runs the
+ * host plan with the resampling matrices (jd_color_plan_rs) and one view's list cut index by cut index as the kernels run
+ * it: tests/augsim's steps, plus jdk_augment_rs (jd_au_resample into a scratch copy) and jdk_augment_copy back at the cut
+ * of a resampling op, so tests/test_augment_resample_host.py can check it against Pillow and torchvision without a GPU.
+ */
+#include "../augsim/augsim.cpp"
+
+/* jdk_augment_rs then jdk_augment_copy on one view: op is a geometric code with its filter flag, mat its matrix */
+static void resample_view(uint8_t *img, int w, int h, int64_t pitch, int bpp, uint32_t op, const double *mat)
+{
+    std::vector<uint8_t> scr((size_t)w * h * bpp);
+    for (int y = 0; y < h; y++)
+        for (int x = 0; x < w; x++) {
+            uint8_t *o = scr.data() + ((size_t)y * w + x) * bpp;
+            memset(o, 0, (size_t)bpp);   /* fill 0, alpha kept */
+            if (bpp == 4) o[3] = 255;
+            jd_au_resample(mat, (op & JD_CO_BICUBIC) != 0, (uint32_t)x, (uint32_t)y, (uint32_t)w, (uint32_t)h, img, (uint64_t)pitch,
+                           (uint32_t)bpp, o);
+        }
+    for (int y = 0; y < h; y++) memcpy(img + (int64_t)y * pitch, scr.data() + (size_t)y * w * bpp, (size_t)w * bpp);
+}
+
+extern "C" {
+
+/* jd_color_plan_rs for a w x h view: the plan (28 words) into o, the 6 mapping words of each of the 8 op slots into oa,
+ * the 6 matrix doubles of each op slot into om.  0 = refused. */
+int augrssim_plan(const JPEGB200_ColorOp *row, int gray, uint32_t w, uint32_t h, uint32_t *o, int32_t *oa, double *om)
+{
+    JDColorPlan p;
+    JDBlurPlan bp;
+    JDAugPlan ap;
+    JDResamplePlan rp;
+    if (!jd_color_plan_rs(row, gray, w, h, &p, &bp, &ap, &rp)) return 0;
+    memcpy(o, &p, sizeof(p));
+    memcpy(oa, &ap, sizeof(ap));
+    memcpy(om, &rp, sizeof(rp));
+    return 1;
+}
+
+/* one BILINEAR (bicubic 0) or BICUBIC resampling with the matrix mat, in place, as jdk_augment_rs + jdk_augment_copy */
+void augrssim_resample(uint8_t *img, int w, int h, int64_t pitch, int bpp, int bicubic, const double *mat)
+{
+    resample_view(img, w, h, pitch, bpp, bicubic ? JD_CO_BICUBIC : JD_CO_BILINEAR, mat);
+}
+
+/* augsim_apply with the resampling ops: one view's operations in place on img (h rows of w pixels, bpp 4 = RGB8888 words
+ * in the byte order bgr says, or 1 = gray bytes, rows pitch bytes apart), cut index by cut index as the kernels run them.
+ * 0 when the plan refuses the row. */
+int augrssim_apply(uint8_t *img, int w, int h, int64_t pitch, int bpp, int bgr, const JPEGB200_ColorOp *row)
+{
+    JDColorPlan p;
+    JDBlurPlan bp;
+    JDAugPlan ap;
+    JDResamplePlan rp;
+    if (!jd_color_plan_rs(row, bpp == 1, (uint32_t)w, (uint32_t)h, &p, &bp, &ap, &rp)) return 0;
+    const int nc = bpp == 4 ? 3 : 1;
+    const int ch[3] = {bgr ? 2 : 0, 1, bgr ? 0 : 2};   /* byte of R, G, B */
+    uint64_t sums[JD_CO_MAX_OPS] = {0};
+    std::vector<uint64_t> hist((size_t)JD_CO_MAX_OPS * JD_AU_HIST, 0);
+    const uint64_t npx = (uint64_t)w * h;
+    for (uint32_t s = 0; s <= p.ncontrast; s++) {
+        const uint32_t k0 = p.seg[s], k1 = p.seg[s + 1];
+        const uint32_t first = k0 < k1 ? p.op[k0] : 0u;
+        if (s > 0 && first == JD_CO_BLUR) blur_view(img, w, h, pitch, bpp, bp.b[k0]);
+        if (s > 0 && (first == JD_CO_SHARPNESS || JD_CO_GEOMETRIC(first))) augment_view(img, w, h, pitch, bpp, first, p.arg[k0], &ap.a[k0]);
+        if (s > 0 && JD_CO_RESAMPLE(first)) resample_view(img, w, h, pitch, bpp, first, rp.mat[k0]);
+        uint8_t lut[3][256];
+        const bool lut_op = s > 0 && JD_CO_LUT(first);
+        for (int c = 0; lut_op && c < nc; c++) augsim_lut(first == JD_CO_EQUALIZE, &hist[(size_t)(s - 1) * JD_AU_HIST + 256 * c], lut[c]);
+        const bool count = s < p.ncontrast && JD_CO_LUT(p.op[k1]);
+        const uint32_t mean = s > 0 ? jd_co_mean(sums[s - 1], npx) : 0u;
+        for (int y = 0; y < h; y++)
+            for (int x = 0; x < w; x++) {
+                uint8_t *px = img + (int64_t)y * pitch + (int64_t)x * bpp;
+                uint32_t l;
+                if (bpp == 4) {
+                    uint32_t r = px[ch[0]], g = px[ch[1]], b = px[ch[2]];
+                    if (lut_op) { r = lut[0][r]; g = lut[1][g]; b = lut[2][b]; }
+                    for (uint32_t k = k0; k < k1; k++) jd_au_apply3(p.op[k], p.arg[k], mean, &r, &g, &b);
+                    px[ch[0]] = (uint8_t)r; px[ch[1]] = (uint8_t)g; px[ch[2]] = (uint8_t)b;
+                    l = jd_co_luma(r, g, b);
+                    if (count) { hist[(size_t)s * JD_AU_HIST + r]++; hist[(size_t)s * JD_AU_HIST + 256 + g]++; hist[(size_t)s * JD_AU_HIST + 512 + b]++; }
+                } else {
+                    uint32_t c = *px;
+                    if (lut_op) c = lut[0][c];
+                    for (uint32_t k = k0; k < k1; k++) c = jd_au_apply1(p.op[k], p.arg[k], mean, c);
+                    *px = (uint8_t)c;
+                    l = c;
+                    if (count) hist[(size_t)s * JD_AU_HIST + c]++;
+                }
+                if (s < p.ncontrast) sums[s] += l;
+            }
+    }
+    return 1;
+}
+
+}

@@ -6,7 +6,9 @@ auto-augment operations) against the same calls with empty lists, and against Pi
 Workload (seeded, generated in the process): n 1920x1080 4:2:0 q75 files with a restart marker per MCU row (64 unique files
 repeated), JPEGB200_OPT_LIBJPEG, one 224 view per file (RandomResizedCrop's draw, flip, bilinear resize), one Batch per step
 into device memory (uint8 RGB8888), with J.auto_augment_ops draws per view:
-  - ta: TrivialAugmentWide(); ra: RandAugment(); none: the same calls with empty lists (alternated step by step).  Median
+  - ta: TrivialAugmentWide(); ra: RandAugment(); ta_bilinear / ra_bilinear / ta_bicubic / ra_bicubic: the same with
+    interpolation=BILINEAR / BICUBIC (geometric ops flagged J.COLOR_BILINEAR / _BICUBIC; the resize stays bilinear, so
+    the arms differ in their operations only); none: the same calls with empty lists (alternated step by step).  Median
     device step time (CUDA events, JPEGB200_T_TOTAL) and of the slot after the IDCT (JPEGB200_T_DITHER: resize and
     operations).
   - cpu: Image.open + convert + RandomResizedCrop + flip + TrivialAugmentWide on every usable host CPU, views per second.
@@ -53,12 +55,13 @@ def plan(n, aug):
         k = 2 if torch.rand(1) < 0.5 else 1
         rois.append((1920 - j - w, i, w, h) if k == 2 else (j, i, w, h))
         ks.append(k)
-        color.append(J.auto_augment_ops(aug, (S, S)))
+        color.append(J.auto_augment_ops(aug, (S, S), resample=True))
     return rois, ks, color
 
 
 def main():
     from torchvision import transforms as TV
+    from torchvision.transforms import InterpolationMode as IM
     a = dict(n=1024, steps=5, warmup=2)
     args = sys.argv[1:]
     for k in a:
@@ -71,6 +74,10 @@ def main():
     _, _, ra = plan(len(files), TV.RandAugment())
     base = dict(rois=rois, orients=ks, out_sizes=[(S, S)] * len(files), filter=J.RESIZE_BILINEAR)
     arms = {"ta": dict(base, color=ta), "ra": dict(base, color=ra), "none": dict(base, color=[[] for _ in files])}
+    for f in ("bilinear", "bicubic"):
+        interp = IM.BILINEAR if f == "bilinear" else IM.BICUBIC
+        arms["ta_" + f] = dict(base, color=plan(len(files), TV.TrivialAugmentWide(interpolation=interp))[2])
+        arms["ra_" + f] = dict(base, color=plan(len(files), TV.RandAugment(interpolation=interp))[2])
     ctx = J.Context(0, J.JPEG_ARITH_SSE2)
     res = {k: [] for k in arms}
     for k in range(a["warmup"] + a["steps"]):
@@ -85,7 +92,7 @@ def main():
     for name in res:
         out[name] = {"ms_per_step": float(np.median([t["total"] for t in res[name]])),
                      "dither_slot_ms": float(np.median([t["dither"] for t in res[name]]))}
-    for name in ("ta", "ra"):
+    for name in ("ta", "ra", "ta_bilinear", "ra_bilinear", "ta_bicubic", "ra_bicubic"):
         out[name + "_ops_ms"] = out[name]["dither_slot_ms"] - out["none"]["dither_slot_ms"]
     ncpu = len(os.sched_getaffinity(0))
     from PIL import Image
