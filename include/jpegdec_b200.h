@@ -432,16 +432,48 @@ int JPEGB200_thumbnailPlan(int width, int height, int req_w, int req_h, double r
  * DESIGN.md 4.2.12. */
 #define JPEGB200_COLOR_BILINEAR     0x100
 #define JPEGB200_COLOR_BICUBIC      0x200
+/* Pillow's Image.transform(size, AFFINE or PERSPECTIVE, data, resample, fillcolor) on the view's final image, the size
+ * kept: torchvision's RandomAffine, RandomRotation (expand=False) and RandomPerspective on a PIL image (jpegdec_b200's
+ * geometric_ops draws them).  Only through JPEGB200_batchCreateWarp / JPEGB200_decodeBatchWarp, whose warp_args entry
+ * (v, k) holds op (v, k)'s data (6 coefficients for AFFINE, 8 for PERSPECTIVE) and fill.  A bare code is NEAREST; OR in
+ * JPEGB200_COLOR_BILINEAR or _BICUBIC for those filters.  R, G and B are warped on their own; gray views too (fill[0]).
+ * Fill values are clamped to 0 .. 255, as Pillow clamps them, and land in the view's own byte order; the alpha byte of a
+ * filled RGB8888 pixel is 0xFF.  A view gets JPEG_INVALID_PARAMETER for a non-finite coefficient, both filter flags, a
+ * side above 1024 pixels (the sizes pinned against Pillow), or a NEAREST affine with b or d non-zero outside Pillow's 16.16
+ * fixed-point range: |x a + y b + c| or |x d + y e + f| at least 32768 at a corner (x = 0 or w, y = 0 or h) of the view
+ * (Pillow switches to another form there, which is not pinned).  NEAREST AFFINE with b = d = 0
+ * (scale and translate only) follows Pillow's own path for that case.  Through the Color calls both codes are unknown ops.
+ * At a cut index where some view warps, the call adds jdk_warp, which writes the view's scratch copy, and the shared
+ * jdk_augment_copy.  DESIGN.md 4.2.13. */
+#define JPEGB200_COLOR_AFFINE       40
+#define JPEGB200_COLOR_PERSPECTIVE  41
 #define JPEGB200_COLOR_MAX_OPS    8
 typedef struct {
     int32_t op;                        /* JPEGB200_COLOR_*, 0 = end of the view's list */
     double arg;                        /* factor, hue shift (-0.5 .. 0.5), solarize threshold, blur radius or magnitude */
 } JPEGB200_ColorOp;
+/* the arguments of an AFFINE or PERSPECTIVE op */
+typedef struct {
+    double coeffs[8];                  /* Pillow's data: a, b, c, d, e, f (AFFINE) and g, h (PERSPECTIVE); the rest unread */
+    int32_t fill[3];                   /* true R, G, B (a gray view uses fill[0]), each clamped to 0 .. 255 */
+} JPEGB200_WarpArgs;
+/* Image.rotate(angle, center=center)'s matrix for a w x h image (center NULL = (w / 2, h / 2)): angle % 360 as Python takes
+ * it, the rotation rounded to 15 decimals, the centre kept; the AFFINE data of RandomRotation's draw.  0 for mat NULL. */
+int JPEGB200_rotateMatrix(double angle, int w, int h, const double *center, double mat[6]);
 JPEGB200_BATCH *JPEGB200_batchCreateColor(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
                                           const int32_t *views, int pixel_type, int options, const int32_t *rois,
                                           const uint8_t *orients, const int32_t *out_sizes, int filter,
                                           const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
                                           const double *reducing_gaps, const JPEGB200_ColorOp *color_ops);
+/* The same with the AFFINE / PERSPECTIVE arguments: warp_args has V x JPEGB200_COLOR_MAX_OPS entries, parallel to
+ * color_ops; entry (v, k) is read only when op (v, k) is AFFINE or PERSPECTIVE.  warp_args = NULL is
+ * JPEGB200_batchCreateColor, which forwards here. */
+JPEGB200_BATCH *JPEGB200_batchCreateWarp(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                         const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                         const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                         const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
+                                         const double *reducing_gaps, const JPEGB200_ColorOp *color_ops,
+                                         const JPEGB200_WarpArgs *warp_args);
 void JPEGB200_batchDestroy(JPEGB200_BATCH *b);
 int JPEGB200_batchCount(JPEGB200_BATCH *b);
 /* per-image facts after batchCreate: status is JPEG_SUCCESS or the open() error the reference would give */
@@ -550,6 +582,14 @@ int JPEGB200_decodeBatchColor(JPEGB200_CTX *ctx, const uint8_t *const *datas, co
                               const double *boxes, const double *reducing_gaps, const JPEGB200_ColorOp *color_ops,
                               void *const *outs, const int64_t *pitches, const int64_t *plane_strides, int flags,
                               int32_t *status);
+/* The same with the AFFINE / PERSPECTIVE arguments (warp_args: semantics of JPEGB200_batchCreateWarp; NULL =
+ * JPEGB200_decodeBatchColor, which forwards here).  A warped view's scratch copy counts in the per-job scratch bound. */
+int JPEGB200_decodeBatchWarp(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                             const int32_t *views, int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
+                             const int32_t *out_sizes, int filter, const JPEGB200_TensorSpec *spec, const uint8_t *draft,
+                             const double *boxes, const double *reducing_gaps, const JPEGB200_ColorOp *color_ops,
+                             const JPEGB200_WarpArgs *warp_args, void *const *outs, const int64_t *pitches,
+                             const int64_t *plane_strides, int flags, int32_t *status);
 /* JPEGB200_NUM_COUNTERS counters summed over the jobs of the last JPEGB200_decodeBatch on this context */
 int JPEGB200_lastCallCounters(JPEGB200_CTX *ctx, int64_t *counters);
 /* CUDA-event stage times (JPEGB200_NUM_TIMINGS, ms) summed over those jobs, and how many jobs there were.  Jobs overlap

@@ -44,6 +44,9 @@ COLOR_SHARPNESS, COLOR_POSTERIZE, COLOR_AUTOCONTRAST, COLOR_EQUALIZE, COLOR_INVE
 COLOR_SHEAR_X, COLOR_SHEAR_Y, COLOR_TRANSLATE_X, COLOR_TRANSLATE_Y, COLOR_ROTATE = 25, 26, 27, 28, 29
 # OR'd into a geometric code: that op resamples with BILINEAR or BICUBIC instead of NEAREST
 COLOR_BILINEAR, COLOR_BICUBIC = 0x100, 0x200
+# Pillow's Image.transform(size, AFFINE / PERSPECTIVE, coeffs, resample, fillcolor): (op, coeffs, fill) entries, NEAREST bare
+# or with COLOR_BILINEAR / COLOR_BICUBIC OR'd in (geometric_ops draws them for RandomAffine / RandomRotation / RandomPerspective)
+COLOR_AFFINE, COLOR_PERSPECTIVE = 40, 41
 COLOR_MAX_OPS = 8
 TIMING_NAMES = ["h2d", "prescan", "entropy", "stitch", "idct", "dither", "d2h", "total"]
 COUNTER_NAMES = ["launches", "segments", "blocks", "events", "compressed_bytes", "output_bytes",
@@ -60,6 +63,11 @@ class TensorSpec(C.Structure):
 class ColorOp(C.Structure):
     """JPEGB200_ColorOp (include/jpegdec_b200.h)"""
     _fields_ = [("op", C.c_int32), ("arg", C.c_double)]
+
+
+class WarpArgs(C.Structure):
+    """JPEGB200_WarpArgs (include/jpegdec_b200.h)"""
+    _fields_ = [("coeffs", C.c_double * 8), ("fill", C.c_int32 * 3)]
 
 
 class JPEGDRAW(C.Structure):
@@ -158,6 +166,11 @@ def lib():
     L.JPEGB200_decodeBatchColor.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, i32p, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
                                             i32p, C.c_int, C.POINTER(TensorSpec), C.POINTER(C.c_uint8), dp, dp, cop,
                                             C.POINTER(vp), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int, i32p]
+    wap = C.POINTER(WarpArgs)
+    L.JPEGB200_batchCreateWarp.argtypes = L.JPEGB200_batchCreateColor.argtypes + [wap]
+    L.JPEGB200_batchCreateWarp.restype = vp
+    L.JPEGB200_decodeBatchWarp.argtypes = L.JPEGB200_decodeBatchColor.argtypes[:16] + [wap] + L.JPEGB200_decodeBatchColor.argtypes[16:]
+    L.JPEGB200_rotateMatrix.argtypes = [C.c_double, C.c_int, C.c_int, dp, dp]
     L.JPEGB200_thumbnailPlan.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, ip, ip, ip, dp]
     L.JPEGB200_batchSetOutputTensor.argtypes = [vp, C.c_int, vp, C.c_int64, C.c_int64]
     L.JPEGB200_decodeBatchTensor.argtypes = [vp, C.POINTER(vp), i32p, C.c_int, C.c_int, C.c_int, i32p, C.POINTER(C.c_uint8),
@@ -445,28 +458,70 @@ def thumbnail_plan(width, height, size, reducing_gap=2.0):
 def _color_array(color, n):
     """one sequence of operations for every image, or one list of them per image -> ColorOp[n * COLOR_MAX_OPS] (None stays
     None).  An operation is a tuple (op, arg), or the bare constant for an op without an argument (COLOR_GRAYSCALE)."""
+    return _color_arrays(color, n)[0]
+
+
+def _warp_fill(fill):
+    """an (op, coeffs, fill) entry's fill -> 3 ints in R, G, B order: None = 0, an int for every channel, or 3 values"""
+    if fill is None:
+        return (0, 0, 0)
+    if isinstance(fill, (int, np.integer)):
+        return (int(fill),) * 3
+    fill = tuple(int(f) for f in fill)
+    if len(fill) != 3:
+        raise ValueError("color: a warp fill is None, an int or 3 ints (R, G, B)")
+    return fill
+
+
+def _is_warp(o):
+    """an (op, coeffs, fill) entry: a 3-tuple whose second item is a sequence of numbers other than an (op, arg) pair.  A
+    row written as a tuple -- three bare ops, or ops and (op, arg) pairs -- stays a row."""
+    if not (isinstance(o, tuple) and len(o) == 3 and isinstance(o[1], (list, tuple, np.ndarray)) and len(o[1]) != 2):
+        return False
+    return all(isinstance(v, (int, float, np.integer, np.floating)) for v in o[1])
+
+
+def _color_arrays(color, n):
+    """_color_array, plus the WarpArgs[n * COLOR_MAX_OPS] of the (op, coeffs, fill) entries (COLOR_AFFINE /
+    COLOR_PERSPECTIVE, coeffs 6 or 8 numbers, fill as _warp_fill takes it), or None when there is none"""
     if color is None:
-        return None
+        return None, None
     color = list(color)
     def row(ops):
         out = []
         for o in ops:
             o = (o, 0.0) if isinstance(o, (int, np.integer)) else tuple(o)
-            out.append((int(o[0]), float(o[1])))
+            if _is_warp(o):
+                c = [float(v) for v in o[1]]
+                if len(c) not in (6, 8):
+                    raise ValueError("color: warp coefficients are 6 (AFFINE) or 8 (PERSPECTIVE) numbers")
+                out.append((int(o[0]), 0.0, c, _warp_fill(o[2])))
+            else:
+                out.append((int(o[0]), float(o[1]), None, None))
         if len(out) > COLOR_MAX_OPS:
             raise ValueError("color: at most %d operations per image (view)" % COLOR_MAX_OPS)
         return out
     def is_op(o):
-        return isinstance(o, (int, np.integer)) or (isinstance(o, tuple) and len(o) == 2 and isinstance(o[0], (int, np.integer)))
+        return isinstance(o, (int, np.integer)) or (isinstance(o, tuple) and isinstance(o[0] if o else None, (int, np.integer)) and
+                                                    (len(o) == 2 or _is_warp(o)))
     rows = [row(color)] * n if all(is_op(o) for o in color) else [row(r) for r in color]
     if len(rows) != n:
         raise ValueError("color: one sequence of (op, arg) for every image, or one per image (view)")
     a = (ColorOp * (n * COLOR_MAX_OPS))()
+    wa = None
     for v, r in enumerate(rows):
-        for k, (op, arg) in enumerate(r):
+        for k, (op, arg, coeffs, fill) in enumerate(r):
             a[v * COLOR_MAX_OPS + k].op = op
             a[v * COLOR_MAX_OPS + k].arg = arg
-    return a
+            if coeffs is not None:
+                if wa is None:
+                    wa = (WarpArgs * (n * COLOR_MAX_OPS))()
+                w = wa[v * COLOR_MAX_OPS + k]
+                for j, c in enumerate(coeffs):
+                    w.coeffs[j] = c
+                for j in range(3):
+                    w.fill[j] = max(-2 ** 31, min(2 ** 31 - 1, fill[j]))
+    return a, wa
 
 
 def color_jitter_ops(params):
@@ -552,6 +607,61 @@ def auto_augment_ops(t, size, *, resample=False):
     return ops
 
 
+def rotate_matrix(angle, size, center=None):
+    """Image.rotate(angle, center=center)'s AFFINE data for an image of size = (w, h) (JPEGB200_rotateMatrix)"""
+    m = (C.c_double * 6)()
+    c = (C.c_double * 2)(*[float(v) for v in center]) if center is not None else None
+    if not lib().JPEGB200_rotateMatrix(float(angle), int(size[0]), int(size[1]), c, m):
+        raise ValueError("rotate_matrix: a size of at least 0 x 0")
+    return list(m)
+
+
+def geometric_ops(t, size, mode="RGB"):
+    """One view's operation list (none or one (op, coeffs, fill) entry) for torchvision's RandomAffine, RandomRotation or
+    RandomPerspective `t` on a PIL image of size = (w, h) and `mode` ("RGB" or "L"): the same draws from torch's global
+    generator as t.forward (t.get_params, and RandomPerspective's torch.rand(1) < p), so under one torch.manual_seed the list
+    gives torchvision's image and leaves the generator where forward does.  The data come from torchvision's own
+    _get_inverse_affine_matrix (centre (w / 2, h / 2) unless t.center) and _get_perspective_coeffs, or from rotate_matrix;
+    the fill from torchvision's _parse_fill.  The list runs on the view's final image, which keeps its size.  ValueError for
+    RandomRotation(expand=True), which changes the size, and for interpolations Pillow's transform does not take."""
+    import torch
+    from PIL import Image
+    from torchvision import transforms as TV
+    from torchvision.transforms import InterpolationMode
+    from torchvision.transforms import functional as F
+    from torchvision.transforms._functional_pil import _parse_fill
+    if not isinstance(t, (TV.RandomAffine, TV.RandomRotation, TV.RandomPerspective)):
+        raise TypeError("geometric_ops: a RandomAffine, RandomRotation or RandomPerspective")
+    flags = {InterpolationMode.NEAREST: 0, InterpolationMode.BILINEAR: COLOR_BILINEAR, InterpolationMode.BICUBIC: COLOR_BICUBIC}
+    if t.interpolation not in flags:
+        raise ValueError("geometric_ops: interpolation %s is not supported (NEAREST, BILINEAR or BICUBIC)" % t.interpolation)
+    if isinstance(t, TV.RandomRotation) and t.expand:
+        raise ValueError("geometric_ops: RandomRotation(expand=True) changes the image's size")
+    if mode not in ("RGB", "L"):
+        raise ValueError("geometric_ops: mode 'RGB' or 'L'")
+    flag = flags[t.interpolation]
+
+    def fill():   # after the draws, as forward parses it
+        return _parse_fill(t.fill, Image.new(mode, (1, 1)))["fillcolor"]
+
+    w, h = int(size[0]), int(size[1])
+    if isinstance(t, TV.RandomAffine):
+        angle, translate, scale, shear = t.get_params(t.degrees, t.translate, t.scale, t.shear, [w, h])
+        # F.affine's normalisation of the draw, then its PIL branch
+        angle = float(angle) if isinstance(angle, int) else angle
+        translate = list(translate) if isinstance(translate, tuple) else translate
+        shear = list(shear) if isinstance(shear, tuple) else shear
+        center = t.center if t.center is not None else [w * 0.5, h * 0.5]
+        return [(COLOR_AFFINE | flag, F._get_inverse_affine_matrix(center, angle, translate, scale, shear), fill())]
+    if isinstance(t, TV.RandomRotation):
+        angle = t.get_params(t.degrees)
+        return [(COLOR_AFFINE | flag, rotate_matrix(angle, (w, h), t.center), fill())]
+    if torch.rand(1) < t.p:
+        startpoints, endpoints = t.get_params(w, h, t.distortion_scale)
+        return [(COLOR_PERSPECTIVE | flag, F._get_perspective_coeffs(startpoints, endpoints), fill())]
+    return []
+
+
 def _orient_array(orients, n):
     """n EXIF transforms (0 = from the file, 1-8) -> uint8[n] for the C ABI (None stays None = no orientation)"""
     if orients is None:
@@ -587,7 +697,9 @@ class Batch:
     doubles for every image or one per image, and reducing_gap: one value or one per image (None = Pillow's None): the
     resize is then Pillow's resize(out_size, filter, box=box, reducing_gap=gap) of the unresized output
     (JPEGB200_batchCreateBox; needs out_sizes).  color: one sequence of (op, arg) (COLOR_*) for every image or one per
-    image, run on each final uint8 image as torchvision's PIL transforms do (JPEGB200_batchCreateColor), or None."""
+    image, run on each final uint8 image as torchvision's PIL transforms do (JPEGB200_batchCreateColor), or None.  An
+    operation may also be (COLOR_AFFINE / COLOR_PERSPECTIVE [| COLOR_BILINEAR / _BICUBIC], coeffs, fill): Pillow's
+    Image.transform of the view with those 6 / 8 coefficients and fill (None, an int, or R, G, B; JPEGB200_batchCreateWarp)."""
 
     def __init__(self, ctx, ptrs, sizes, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
                  filter=RESIZE_BILINEAR, spec=None, views=None, draft=None, box=None, reducing_gap=None, color=None):
@@ -602,12 +714,12 @@ class Batch:
         self.ctx = ctx
         self._draft = _draft_array(draft, n)
         self._box, self._gap = _box_array(box, n), _gap_array(reducing_gap, n)
-        self._color = _color_array(color, n)
+        self._color, self._warp = _color_arrays(color, n)
         self._spec = spec
-        self.h = lib().JPEGB200_batchCreateColor(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
-                                                 self._rois, self._orients, self._out_sizes, int(filter),
-                                                 C.byref(spec) if spec is not None else None, self._draft, self._box,
-                                                 self._gap, self._color)
+        self.h = lib().JPEGB200_batchCreateWarp(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
+                                                self._rois, self._orients, self._out_sizes, int(filter),
+                                                C.byref(spec) if spec is not None else None, self._draft, self._box,
+                                                self._gap, self._color, self._warp)
         if not self.h:
             raise RuntimeError("batchCreate failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
 
@@ -691,7 +803,7 @@ def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flag
     views: one view count per file, or None; outs, pitches and the per-image lists are then per view.  Returns (rc,
     per-image status list, counters summed over the internal jobs).  draft: one scale denominator per image (view), or
     None (JPEGB200_decodeBatchDraft).  box / reducing_gap: as in Batch (JPEGB200_decodeBatchBox).  color: as in Batch
-    (JPEGB200_decodeBatchColor)."""
+    (JPEGB200_decodeBatchWarp)."""
     nf = len(ptrs)
     va, n = _views_array(views, nf)
     pa = (C.c_void_p * nf)(*ptrs)
@@ -701,10 +813,11 @@ def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flag
     oa = (C.c_void_p * n)(*outs)
     pi = (C.c_int64 * n)(*pitches) if pitches is not None else None
     st = (C.c_int32 * n)()
-    rc = lib().JPEGB200_decodeBatchColor(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
-                                         _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None,
-                                         _draft_array(draft, n), _box_array(box, n), _gap_array(reducing_gap, n),
-                                         _color_array(color, n), oa, pi, None, flags, st)
+    ca, wa = _color_arrays(color, n)
+    rc = lib().JPEGB200_decodeBatchWarp(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
+                                        _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None,
+                                        _draft_array(draft, n), _box_array(box, n), _gap_array(reducing_gap, n),
+                                        ca, wa, oa, pi, None, flags, st)
     cnt = (C.c_int64 * len(COUNTER_NAMES))()
     lib().JPEGB200_lastCallCounters(ctx.h, cnt)
     return rc, list(st), dict(zip(COUNTER_NAMES, list(cnt)))
@@ -783,7 +896,7 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     images are then the views: rois / orients / out_sizes / out and the result ([V, C, H, W], or a list) are per view.
     draft: one scale denominator (1, 2, 4, 8) per image (view), Pillow's draft() at that scale (JPEGB200_decodeBatchDraft),
     or None.  box / reducing_gap: as in Batch (JPEGB200_decodeBatchBox).  color: as in Batch, before the conversion
-    (JPEGB200_decodeBatchColor)."""
+    (JPEGB200_decodeBatchWarp)."""
     import torch
     dtype = torch.float32 if dtype is None else dtype
     spec = tensor_spec(dtype, layout, scale, mean, std, bgr)
@@ -838,10 +951,11 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     st = (C.c_int32 * n)()
     with torch.cuda.device(dev):
         torch.cuda.current_stream(dev).synchronize()   # the library's streams do not order against torch's
-        rc = lib().JPEGB200_decodeBatchColor(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
-                                             _orient_array(orients, n), _size_array(out_sizes, n), int(filter),
-                                             C.byref(spec), _draft_array(draft, n), _box_array(box, n),
-                                             _gap_array(reducing_gap, n), _color_array(color, n), (C.c_void_p * n)(*ptr_l),
+        ca, wa = _color_arrays(color, n)
+        rc = lib().JPEGB200_decodeBatchWarp(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
+                                            _orient_array(orients, n), _size_array(out_sizes, n), int(filter),
+                                            C.byref(spec), _draft_array(draft, n), _box_array(box, n),
+                                            _gap_array(reducing_gap, n), ca, wa, (C.c_void_p * n)(*ptr_l),
                                              (C.c_int64 * n)(*pitch_l), (C.c_int64 * n)(*plane_l), JPEGB200_OUT_DEVICE, st)
     if rc == 0:
         raise RuntimeError("decodeBatchViews failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())

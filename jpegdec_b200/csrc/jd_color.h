@@ -73,12 +73,18 @@
 /* a geometric op's resampling filter, OR'd into its code (the plan holds only valid combinations): run by jdk_augment_rs */
 #define JD_CO_BILINEAR     0x100
 #define JD_CO_BICUBIC      0x200
+/* Pillow's Image.transform(size, AFFINE or PERSPECTIVE, data, resample, fillcolor) with the caller's coefficients and fill
+ * (jd_augment.h: jd_au_warp), a bare code for NEAREST or with one filter flag OR'd in: run by jdk_warp */
+#define JD_CO_AFFINE       40
+#define JD_CO_PERSPECTIVE  41
 #define JD_CO_MAX_OPS    8
 #define JD_CO_GEOMETRIC(op) ((op) >= JD_CO_SHEAR_X && (op) <= JD_CO_ROTATE)
+#define JD_CO_WARP(op)      (((op) & 0xFFu) == JD_CO_AFFINE || ((op) & 0xFFu) == JD_CO_PERSPECTIVE)
+/* a flagged geometric op 25 .. 29 (jdk_augment_rs); a flagged warp op matches too, so callers test JD_CO_WARP first */
 #define JD_CO_RESAMPLE(op)  (((op) & (JD_CO_BILINEAR | JD_CO_BICUBIC)) != 0)
 #define JD_CO_LUT(op)       ((op) == JD_CO_AUTOCONTRAST || (op) == JD_CO_EQUALIZE)
 /* ops a kernel of their own runs at a cut, before jdk_color runs the rest of the segment */
-#define JD_CO_OWN_KERNEL(op) ((op) == JD_CO_BLUR || (op) == JD_CO_SHARPNESS || JD_CO_GEOMETRIC(op) || JD_CO_RESAMPLE(op))
+#define JD_CO_OWN_KERNEL(op) ((op) == JD_CO_BLUR || (op) == JD_CO_SHARPNESS || JD_CO_GEOMETRIC(op) || JD_CO_RESAMPLE(op) || JD_CO_WARP(op))
 
 JD_CO_HD float jd_co_float(uint32_t bits)
 {

@@ -181,6 +181,8 @@ struct JPEGB200_BATCH {
     std::vector<JDBlurPlan> co_blur;        /* per view: each blur's constants at its op slot */
     std::vector<JDAugPlan> co_aug;          /* per view: each geometric op's mapping at its op slot */
     std::vector<JDResamplePlan> co_rs;      /* per view: each BILINEAR / BICUBIC geometric op's matrix at its op slot */
+    std::vector<JDWarpPlan> co_warp;        /* per view, for a batch created with warp arguments: each AFFINE / PERSPECTIVE
+                                               op's coefficients and fill at its op slot */
     std::vector<int64_t> bl_scratch;        /* per view: its scratch copy's bytes when it blurs, sharpens or moves pixels
                                                (256-byte aligned), plus JD_AU_HIST counts per autocontrast / equalize */
     int64_t bl_scratch_total = 0;
@@ -193,6 +195,10 @@ struct JPEGB200_BATCH {
     DevBuf<JDAugDesc> d_au_desc;
     std::vector<JDAugMat> au_mat;           /* the same entries: the BILINEAR / BICUBIC ops' matrices (zero for the others) */
     DevBuf<JDAugMat> d_au_mat;
+    std::vector<JDWarpDesc> au_warp;        /* the same entries: the AFFINE / PERSPECTIVE ops' coefficients and fill (zero for the others) */
+    DevBuf<JDWarpDesc> d_au_warp;
+    std::vector<int16_t> au_tab;            /* the walk tables of the NEAREST affines with b = d = 0 (jd_au_walk_table) */
+    DevBuf<int16_t> d_au_tab;
     DevBuf<uint32_t> d_co_hslot;            /* per cut index and view: its histogram slot (the slots follow the scratch copies in d_bl) */
     std::vector<uint8_t> co_bgr;
     std::vector<JDColorDesc> co_desc;
@@ -577,6 +583,7 @@ struct CreatePlan {
     const uint8_t *draft = nullptr;     /* per view: draft scale denominator (JPEGB200_batchCreateDraft), NULL = 1 */
     const double *boxes = nullptr, *gaps = nullptr;   /* per view: resize box and reducing gap (JPEGB200_batchCreateBox) */
     const JPEGB200_ColorOp *color = nullptr;          /* per view: JPEGB200_COLOR_MAX_OPS operations (JPEGB200_batchCreateColor) */
+    const JPEGB200_WarpArgs *warp = nullptr;          /* per view: their AFFINE / PERSPECTIVE arguments (JPEGB200_batchCreateWarp) */
     /* where the next file's restart segments, blocks and records start; where the next view's output and gray stage start */
     uint32_t seg = 0;
     uint64_t blk = 0, rec_total = 0;
@@ -626,6 +633,7 @@ static void init_batch(JPEGB200_BATCH *b, JPEGB200_CTX *ctx, const CreatePlan &P
     if (b->box) b->bx_plans.assign(nv, JDBoxPlan{});
     b->color = P.color != nullptr;
     if (b->color) { b->co_plans.assign(nv, JDColorPlan{}); b->co_blur.assign(nv, JDBlurPlan{}); b->co_aug.assign(nv, JDAugPlan{}); b->co_rs.assign(nv, JDResamplePlan{}); b->bl_scratch.assign(nv, 0); b->co_bgr.assign(nv, 0); }
+    if (b->color && P.warp) b->co_warp.assign(nv, JDWarpPlan{});
     b->lj = (options & JPEGB200_OPT_LIBJPEG) != 0;
     if (b->lj) { b->lj_desc.assign(nv, JDLjDesc{}); b->lj_plane.assign(nv, 0); }
     b->tensor = P.spec != nullptr;
@@ -809,8 +817,9 @@ static uint32_t plan_views(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int 
             const int s = b->lj ? (int)b->lj_desc[i].shift : b->sshift;
             const uint32_t w = b->resize ? (uint32_t)P.out_sizes[2 * (size_t)i] : b->roi ? (uint32_t)b->plans[i].out_w : (uint32_t)((inf.width + (1 << s) - 1) >> s);
             const uint32_t h = b->resize ? (uint32_t)P.out_sizes[2 * (size_t)i + 1] : b->roi ? (uint32_t)b->plans[i].out_h : (uint32_t)((inf.height + (1 << s) - 1) >> s);
-            if (!jd_color_plan_rs(P.color + JPEGB200_COLOR_MAX_OPS * (size_t)i, b->ptclass == JD_PT_GRAY, w, h, &b->co_plans[i],
-                                  &b->co_blur[i], &b->co_aug[i], &b->co_rs[i])) {
+            if (!jd_color_plan_warp(P.color + JPEGB200_COLOR_MAX_OPS * (size_t)i, P.warp ? P.warp + JPEGB200_COLOR_MAX_OPS * (size_t)i : nullptr,
+                                    b->ptclass == JD_PT_GRAY, w, h, &b->co_plans[i], &b->co_blur[i], &b->co_aug[i], &b->co_rs[i],
+                                    P.warp ? &b->co_warp[i] : nullptr)) {
                 P.vok[i] = 0;
                 dropped = true;
             }
@@ -1158,6 +1167,17 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateColor(JPEGB200_CTX *ctx, const ui
                                                      const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
                                                      const double *reducing_gaps, const JPEGB200_ColorOp *color_ops)
 {
+    return JPEGB200_batchCreateWarp(ctx, datas, sizes, n, views, pixel_type, options, rois, orients, out_sizes, filter, spec, draft,
+                                    boxes, reducing_gaps, color_ops, nullptr);
+}
+
+extern "C" JPEGB200_BATCH *JPEGB200_batchCreateWarp(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                                    const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                                    const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                                    const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
+                                                    const double *reducing_gaps, const JPEGB200_ColorOp *color_ops,
+                                                    const JPEGB200_WarpArgs *warp_args)
+{
     if (!ctx) { snprintf(g_err, sizeof(g_err), "invalid parameter"); return nullptr; }
     int64_t nv = 0;   /* images of the batch: views */
     if (!jd_check_batch_features(pixel_type, options, n, views, rois != nullptr, orients != nullptr, out_sizes != nullptr, filter, spec,
@@ -1171,7 +1191,7 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateColor(JPEGB200_CTX *ctx, const ui
     if (!b) return nullptr;
     CreatePlan P;
     P.datas = datas; P.sizes = sizes; P.views = views; P.rois = rois; P.orients = orients; P.out_sizes = out_sizes; P.spec = spec;
-    P.draft = draft; P.boxes = boxes; P.gaps = reducing_gaps; P.color = color_ops;
+    P.draft = draft; P.boxes = boxes; P.gaps = reducing_gaps; P.color = color_ops; P.warp = color_ops ? warp_args : nullptr;
     P.srects.assign(4 * (size_t)nv, 0); P.vok.assign((size_t)nv, 0);
     P.ks.assign(orients ? (size_t)nv : 0u, 0);
     if (options & JPEGB200_OPT_PROGRESSIVE) { P.fscans.resize(JD_PROG_MAX_SCANS); P.ftabs.resize(JD_PROG_MAX_TABS); }
@@ -1555,7 +1575,8 @@ struct DecodeState {
     std::vector<uint32_t> bl_ctas;          /* CTAs of each cut index's jdk_blur pair: horizontal, vertical */
     std::vector<uint32_t> au_first;         /* sharpness and geometric ops: the first au_desc entry of each cut index */
     std::vector<uint32_t> au_ctas;          /* CTAs of each cut index's jdk_augment_copy (jdk_augment's, then jdk_augment_rs's) */
-    std::vector<uint32_t> au_nn;            /* per cut index: the entries and CTAs of jdk_augment (the rest resample) */
+    std::vector<uint32_t> au_nn;            /* per cut index: the entries and CTAs of jdk_augment, then those of jdk_augment
+                                               and jdk_augment_rs together (the rest warp) */
     std::vector<uint8_t> co_lut;            /* per cut index: some view posterizes, inverts, applies a LUT or counts a
                                                histogram there (jdk_color_lut) */
     unsigned long long *co_hist = nullptr;  /* the histogram slots */
@@ -1743,22 +1764,25 @@ static int stage_color(JPEGB200_BATCH *b, DecodeState &D)
         }
     }
     D.bl_first[nl] = (uint32_t)b->bl_desc.size();
-    /* sharpness and geometric ops: at cut index s, the views whose segment s starts with one -- first those that sharpen or
-     * move pixels with NEAREST (jdk_augment), then those that resample (jdk_augment_rs), each with its matrix in au_mat */
+    /* sharpness, geometric and warp ops: at cut index s, the views whose segment s starts with one -- first those that
+     * sharpen or move pixels with NEAREST (jdk_augment), then those that resample (jdk_augment_rs), each with its matrix in
+     * au_mat, then those that warp (jdk_warp), each with its coefficients and fill in au_warp */
     b->au_desc.clear();
     b->au_mat.clear();
+    b->au_warp.clear();
+    b->au_tab.clear();
     D.au_first.assign(nl + 1, 0);
     D.au_ctas.assign(nl, 0);
-    D.au_nn.assign(2 * (size_t)nl, 0);
-    bool any_rs = false;
+    D.au_nn.assign(4 * (size_t)nl, 0);
+    bool any_rs = false, any_warp = false;
     for (uint32_t s = 1; s < nl; s++) {
         D.au_first[s] = (uint32_t)b->au_desc.size();
-        for (int rs = 0; rs < 2; rs++) {
+        for (int rs = 0; rs < 3; rs++) {
             for (int i = 0; i < n; i++) {
                 const JDColorPlan &p = b->co_plans[i];
                 if (b->parse_status[i] != JPEG_SUCCESS || s > p.ncontrast) continue;
                 const uint32_t op = p.op[p.seg[s]];
-                if (rs ? !JD_CO_RESAMPLE(op) : op != JD_CO_SHARPNESS && !JD_CO_GEOMETRIC(op)) continue;
+                if (rs == 2 ? !JD_CO_WARP(op) : rs ? !JD_CO_RESAMPLE(op) || JD_CO_WARP(op) : op != JD_CO_SHARPNESS && !JD_CO_GEOMETRIC(op)) continue;
                 JDAugDesc x{};
                 x.off = b->co_desc[i].off; x.pitch = b->co_desc[i].pitch; x.soff = soffs[i];
                 x.w = b->co_desc[i].w; x.h = b->co_desc[i].h;
@@ -1772,9 +1796,24 @@ static int stage_color(JPEGB200_BATCH *b, DecodeState &D)
                 JDAugMat mt;
                 memcpy(mt.m, b->co_rs[i].mat[p.seg[s]], sizeof(mt.m));
                 b->au_mat.push_back(mt);
-                any_rs = any_rs || rs;
+                JDWarpDesc wd{};
+                if (rs == 2) {   /* the fill in the view's byte order, alpha 0xFF */
+                    const JDWarpPlan &wp = b->co_warp[i];
+                    memcpy(wd.c, wp.c[p.seg[s]], sizeof(wd.c));
+                    const uint32_t f = wp.fill[p.seg[s]];
+                    wd.fill = b->ptclass == JD_PT_GRAY ? (f & 255u)
+                            : b->co_bgr[i] ? (f >> 16 & 255u) | (f & 0xFF00u) | (f & 255u) << 16 | 0xFF000000u : f | 0xFF000000u;
+                    if (op == JD_CO_AFFINE && wd.c[1] == 0.0 && wd.c[3] == 0.0) {   /* NEAREST, scale and translate only */
+                        wd.tab = (uint32_t)b->au_tab.size();
+                        b->au_tab.resize(b->au_tab.size() + x.w + x.h);
+                        jd_walk_table(wd.c, x.w, x.h, b->au_tab.data() + wd.tab);
+                    }
+                }
+                b->au_warp.push_back(wd);
+                any_rs = any_rs || rs == 1;
+                any_warp = any_warp || rs == 2;
             }
-            if (!rs) { D.au_nn[2 * s] = (uint32_t)b->au_desc.size() - D.au_first[s]; D.au_nn[2 * s + 1] = D.au_ctas[s]; }
+            if (rs < 2) { D.au_nn[4 * s + 2 * rs] = (uint32_t)b->au_desc.size() - D.au_first[s]; D.au_nn[4 * s + 2 * rs + 1] = D.au_ctas[s]; }
         }
     }
     D.au_first[nl] = (uint32_t)b->au_desc.size();
@@ -1786,6 +1825,14 @@ static int stage_color(JPEGB200_BATCH *b, DecodeState &D)
     if (any_rs) {
         CK(b->d_au_mat.alloc(&b->ctx->pool, b->au_mat.size()));
         CK(cudaMemcpyAsync(b->d_au_mat.p, b->au_mat.data(), sizeof(JDAugMat) * b->au_mat.size(), cudaMemcpyHostToDevice, st));
+    }
+    if (any_warp) {
+        CK(b->d_au_warp.alloc(&b->ctx->pool, b->au_warp.size()));
+        CK(cudaMemcpyAsync(b->d_au_warp.p, b->au_warp.data(), sizeof(JDWarpDesc) * b->au_warp.size(), cudaMemcpyHostToDevice, st));
+    }
+    if (!b->au_tab.empty()) {
+        CK(b->d_au_tab.alloc(&b->ctx->pool, b->au_tab.size()));
+        CK(cudaMemcpyAsync(b->d_au_tab.p, b->au_tab.data(), sizeof(int16_t) * b->au_tab.size(), cudaMemcpyHostToDevice, st));
     }
     if (nslots) {   /* soff is 256-byte aligned: the slots are 64-bit aligned */
         D.co_hist = reinterpret_cast<unsigned long long *>(b->d_bl.p + soff);
@@ -2291,8 +2338,9 @@ static void run_resize(JPEGB200_BATCH *b, DecodeState &D)
 }
 
 /* timed in the dither slot too, after the resize: per cut index of the operation lists, the blur pair for the views that
- * blur there, jdk_augment for the views that sharpen or move pixels with NEAREST there and jdk_augment_rs for those that
- * resample, then one jdk_augment_copy for both, then jdk_color for the per-pixel operations up to the next cut */
+ * blur there, jdk_augment for the views that sharpen or move pixels with NEAREST there, jdk_augment_rs for those that
+ * resample and jdk_warp for those that warp, then one jdk_augment_copy for all of them, then jdk_color for the per-pixel
+ * operations up to the next cut */
 static void run_color(JPEGB200_BATCH *b, DecodeState &D)
 {
     cudaStream_t st = b->ss.stream;
@@ -2314,19 +2362,22 @@ static void run_color(JPEGB200_BATCH *b, DecodeState &D)
         }
         const uint32_t fa = D.au_first[s], na = D.au_first[s + 1] - fa;
         if (na) {
-            /* the NEAREST / sharpness entries first (nn of them, in nc CTAs), then the BILINEAR / BICUBIC ones */
+            /* the NEAREST / sharpness entries first (nn of them, in nc CTAs), then the BILINEAR / BICUBIC ones (up to entry nr,
+             * CTA nrc), then the warps */
             const JDAugDesc *ad = b->d_au_desc.p + fa;
-            const uint32_t nn = D.au_nn[2 * s], nc = D.au_nn[2 * s + 1];
+            const uint32_t nn = D.au_nn[4 * s], nc = D.au_nn[4 * s + 1], nr = D.au_nn[4 * s + 2], nrc = D.au_nn[4 * s + 3];
             if (b->ptclass == JD_PT_GRAY) {
                 if (nn) jdk_augment<1><<<nc, JD_AU_THREADS, 0, st>>>(ad, nn, D.pipe_out, b->d_bl.p);
-                if (nn < na) jdk_augment_rs<1><<<D.au_ctas[s] - nc, JD_AU_THREADS, 0, st>>>(ad + nn, b->d_au_mat.p + fa + nn, na - nn, nc, D.pipe_out, b->d_bl.p);
+                if (nn < nr) jdk_augment_rs<1><<<nrc - nc, JD_AU_THREADS, 0, st>>>(ad + nn, b->d_au_mat.p + fa + nn, nr - nn, nc, D.pipe_out, b->d_bl.p);
+                if (nr < na) jdk_warp<1><<<D.au_ctas[s] - nrc, JD_AU_THREADS, 0, st>>>(ad + nr, b->d_au_warp.p + fa + nr, b->d_au_tab.p, na - nr, nrc, D.pipe_out, b->d_bl.p);
                 jdk_augment_copy<1><<<D.au_ctas[s], JD_AU_THREADS, 0, st>>>(ad, na, D.pipe_out, b->d_bl.p);
             } else {
                 if (nn) jdk_augment<4><<<nc, JD_AU_THREADS, 0, st>>>(ad, nn, D.pipe_out, b->d_bl.p);
-                if (nn < na) jdk_augment_rs<4><<<D.au_ctas[s] - nc, JD_AU_THREADS, 0, st>>>(ad + nn, b->d_au_mat.p + fa + nn, na - nn, nc, D.pipe_out, b->d_bl.p);
+                if (nn < nr) jdk_augment_rs<4><<<nrc - nc, JD_AU_THREADS, 0, st>>>(ad + nn, b->d_au_mat.p + fa + nn, nr - nn, nc, D.pipe_out, b->d_bl.p);
+                if (nr < na) jdk_warp<4><<<D.au_ctas[s] - nrc, JD_AU_THREADS, 0, st>>>(ad + nr, b->d_au_warp.p + fa + nr, b->d_au_tab.p, na - nr, nrc, D.pipe_out, b->d_bl.p);
                 jdk_augment_copy<4><<<D.au_ctas[s], JD_AU_THREADS, 0, st>>>(ad, na, D.pipe_out, b->d_bl.p);
             }
-            D.launches += 1 + (nn ? 1 : 0) + (nn < na ? 1 : 0);
+            D.launches += 1 + (nn ? 1 : 0) + (nn < nr ? 1 : 0) + (nr < na ? 1 : 0);
         }
         if (!D.co_ctas[s]) continue;
         const uint32_t *cblk = b->d_co_blk.p + (size_t)s * n;
@@ -2641,6 +2692,18 @@ extern "C" int JPEGB200_decodeBatchColor(JPEGB200_CTX *ctx, const uint8_t *const
                                          const double *reducing_gaps, const JPEGB200_ColorOp *color_ops, void *const *outs,
                                          const int64_t *pitches, const int64_t *plane_strides, int flags, int32_t *status)
 {
+    return JPEGB200_decodeBatchWarp(ctx, datas, sizes, n, views, pixel_type, options, rois, orients, out_sizes, filter, spec, draft,
+                                    boxes, reducing_gaps, color_ops, nullptr, outs, pitches, plane_strides, flags, status);
+}
+
+extern "C" int JPEGB200_decodeBatchWarp(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                        const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                        const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                        const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
+                                        const double *reducing_gaps, const JPEGB200_ColorOp *color_ops,
+                                        const JPEGB200_WarpArgs *warp_args, void *const *outs, const int64_t *pitches,
+                                        const int64_t *plane_strides, int flags, int32_t *status)
+{
     if (!ctx || n <= 0) return 0;
     const int64_t nv = jd_count_views(n, views, "call", g_err, (int)sizeof(g_err));   /* images (views) of the call */
     if (nv < 0) return 0;
@@ -2689,11 +2752,12 @@ extern "C" int JPEGB200_decodeBatchColor(JPEGB200_CTX *ctx, const uint8_t *const
         const int32_t *vi = views ? views + i0 : nullptr;
         int cnt = jd_job_files(n - i0, sizes + i0, vi, maxcnt, limit, nullptr, 0, &cv, &capped);
         auto create = [&](int c) {
-            return JPEGB200_batchCreateColor(ctx, datas + i0, sizes + i0, c, vi, pixel_type, options, rois ? rois + 4 * (size_t)v0 : nullptr,
-                                             orients ? orients + v0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)v0 : nullptr, filter, spec,
-                                             draft ? draft + v0 : nullptr, boxes ? boxes + 4 * (size_t)v0 : nullptr,
-                                             reducing_gaps ? reducing_gaps + v0 : nullptr,
-                                             color_ops ? color_ops + JPEGB200_COLOR_MAX_OPS * (size_t)v0 : nullptr);
+            return JPEGB200_batchCreateWarp(ctx, datas + i0, sizes + i0, c, vi, pixel_type, options, rois ? rois + 4 * (size_t)v0 : nullptr,
+                                            orients ? orients + v0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)v0 : nullptr, filter, spec,
+                                            draft ? draft + v0 : nullptr, boxes ? boxes + 4 * (size_t)v0 : nullptr,
+                                            reducing_gaps ? reducing_gaps + v0 : nullptr,
+                                            color_ops ? color_ops + JPEGB200_COLOR_MAX_OPS * (size_t)v0 : nullptr,
+                                            color_ops && warp_args ? warp_args + JPEGB200_COLOR_MAX_OPS * (size_t)v0 : nullptr);
         };
         JPEGB200_BATCH *b = create(cnt);
         if (!b) { rc = 0; break; }

@@ -776,20 +776,29 @@ double jd_round15(double x)
     return strtod(s, NULL);
 }
 
+int JPEGB200_rotateMatrix(double angle, int w, int h, const double *center, double mat[6])
+{
+    if (!mat || (!center && (w < 0 || h < 0))) return 0;
+    /* Image.rotate(angle, center=center): angle % 360 as Python takes it, the matrix rounded to 15 decimals, the centre kept */
+    const double deg2rad = M_PI / 180.0;
+    const double cx = center ? center[0] : w / 2.0, cy = center ? center[1] : h / 2.0;
+    double ang = fmod(angle, 360.0);
+    if (ang != 0.0 && ang < 0.0) ang += 360.0;
+    else if (ang == 0.0) ang = 0.0;
+    const double t = -(ang * deg2rad);
+    mat[0] = jd_round15(cos(t)); mat[1] = jd_round15(sin(t)); mat[2] = 0.0;
+    mat[3] = jd_round15(-sin(t)); mat[4] = jd_round15(cos(t)); mat[5] = 0.0;
+    mat[2] = mat[0] * -cx + mat[1] * -cy + mat[2] + cx;
+    mat[5] = mat[3] * -cx + mat[4] * -cy + mat[5] + cy;
+    return 1;
+}
+
 void jd_aug_matrix(int op, double m, uint32_t w, uint32_t h, double *mat)
 {
     const double deg2rad = M_PI / 180.0, rad2deg = 180.0 / M_PI;   /* math.radians / math.degrees */
     if (op == JPEGB200_COLOR_ROTATE) {
-        /* Image.rotate(m): angle % 360 as Python takes it, the matrix rounded to 15 decimals, the centre kept */
-        double ang = fmod(m, 360.0);
-        if (ang != 0.0 && ang < 0.0) ang += 360.0;
-        else if (ang == 0.0) ang = 0.0;
-        const double t = -(ang * deg2rad);
-        mat[0] = jd_round15(cos(t)); mat[1] = jd_round15(sin(t)); mat[2] = 0.0;
-        mat[3] = jd_round15(-sin(t)); mat[4] = jd_round15(cos(t)); mat[5] = 0.0;
-        const double cx = w / 2.0, cy = h / 2.0;
-        mat[2] = mat[0] * -cx + mat[1] * -cy + mat[2] + cx;
-        mat[5] = mat[3] * -cx + mat[4] * -cy + mat[5] + cy;
+        const double c[2] = {w / 2.0, h / 2.0};
+        JPEGB200_rotateMatrix(m, (int)w, (int)h, c, mat);
         return;
     }
     /* torchvision's _get_inverse_affine_matrix(center, 0, translate, 1, shear), step for step */
@@ -819,11 +828,9 @@ static int jd_aug_fixed(double v, int64_t *out)
     return 1;
 }
 
-/* the 16.16 mapping of a geometric op on a w x h view; 0 when a value over the view leaves int32 */
-static int jd_aug_affine(int op, double m, uint32_t w, uint32_t h, JDAffine *out)
+/* the 16.16 mapping of the matrix mat on a w x h view; 0 when a value over the view leaves int32 */
+static int jd_aug_fixed_map(const double *mat, uint32_t w, uint32_t h, JDAffine *out)
 {
-    double mat[6];
-    jd_aug_matrix(op, m, w, h, mat);
     int64_t x0, y0, ax, ay, bx, by;
     if (!jd_aug_fixed(mat[0] * 0.5 + mat[1] * 0.5 + mat[2], &x0) || !jd_aug_fixed(mat[3] * 0.5 + mat[4] * 0.5 + mat[5], &y0) ||
         !jd_aug_fixed(mat[0], &ax) || !jd_aug_fixed(mat[3], &ay) || !jd_aug_fixed(mat[1], &bx) || !jd_aug_fixed(mat[4], &by))
@@ -837,6 +844,14 @@ static int jd_aug_affine(int op, double m, uint32_t w, uint32_t h, JDAffine *out
     return 1;
 }
 
+/* the 16.16 mapping of a geometric op on a w x h view */
+static int jd_aug_affine(int op, double m, uint32_t w, uint32_t h, JDAffine *out)
+{
+    double mat[6];
+    jd_aug_matrix(op, m, w, h, mat);
+    return jd_aug_fixed_map(mat, w, h, out);
+}
+
 int jd_color_plan_aug(const JPEGB200_ColorOp *row, int gray, uint32_t w, uint32_t h, JDColorPlan *plan, JDBlurPlan *blur,
                       JDAugPlan *aug)
 {
@@ -846,15 +861,62 @@ int jd_color_plan_aug(const JPEGB200_ColorOp *row, int gray, uint32_t w, uint32_
 int jd_color_plan_rs(const JPEGB200_ColorOp *row, int gray, uint32_t w, uint32_t h, JDColorPlan *plan, JDBlurPlan *blur,
                      JDAugPlan *aug, JDResamplePlan *rs)
 {
+    return jd_color_plan_warp(row, NULL, gray, w, h, plan, blur, aug, rs, NULL);
+}
+
+void jd_walk_table(const double *c, uint32_t w, uint32_t h, int16_t *tab)
+{
+    jd_au_walk_table(c, w, h, tab);
+}
+
+static uint32_t jd_fill8(int32_t v) { return v < 0 ? 0u : v > 255 ? 255u : (uint32_t)v; }
+
+/* Pillow's own switch to its 16.16 NEAREST affine, as probing pins it: |x a + y b + c| and |x d + y e + f| below 32768 at
+ * the image's corners (0, 0), (w, 0), (0, h) and (w, h) -- one pixel past the last pixel centre, so the 16.16 values can
+ * fit 32 bits while Pillow already takes its other form, which is not pinned */
+static int jd_pillow_fixed_ok(const double *c, uint32_t w, uint32_t h)
+{
+    for (int k = 0; k < 4; k++) {
+        const double x = (k & 1) ? (double)w : 0.0, y = (k & 2) ? (double)h : 0.0;
+        if (!(fabs(x * c[0] + y * c[1] + c[2]) < 32768.0) || !(fabs(x * c[3] + y * c[4] + c[5]) < 32768.0)) return 0;
+    }
+    return 1;
+}
+
+int jd_color_plan_warp(const JPEGB200_ColorOp *row, const JPEGB200_WarpArgs *warp, int gray, uint32_t w, uint32_t h,
+                       JDColorPlan *plan, JDBlurPlan *blur, JDAugPlan *aug, JDResamplePlan *rs, JDWarpPlan *wp)
+{
     memset(plan, 0, sizeof(*plan));
     if (blur) memset(blur, 0, sizeof(*blur));
     if (aug) memset(aug, 0, sizeof(*aug));
     if (rs) memset(rs, 0, sizeof(*rs));
+    if (wp) memset(wp, 0, sizeof(*wp));
     for (int k = 0; k < JPEGB200_COLOR_MAX_OPS && row[k].op != 0; k++) {
         const int op = row[k].op;
         const double a = row[k].arg;
-        /* a filter flag: exactly one, on a geometric op, for a caller that takes the matrices */
+        /* a filter flag: exactly one, on a geometric op (for a caller that takes the matrices) or on a warp op */
         const int filt = op & (JPEGB200_COLOR_BILINEAR | JPEGB200_COLOR_BICUBIC), base = op & ~filt;
+        if (base == JPEGB200_COLOR_AFFINE || base == JPEGB200_COLOR_PERSPECTIVE) {
+            /* Image.transform: only for a caller that passes the warp arguments and takes their plan */
+            if (!warp || !aug || !wp || filt == (JPEGB200_COLOR_BILINEAR | JPEGB200_COLOR_BICUBIC)) return 0;
+            if (w > JD_AU_MAX_SIDE || h > JD_AU_MAX_SIDE) return 0;
+            const int nc = base == JPEGB200_COLOR_AFFINE ? 6 : 8;
+            const double *c = warp[k].coeffs;
+            for (int j = 0; j < nc; j++) {
+                if (!isfinite(c[j])) return 0;
+                wp->c[plan->nops][j] = c[j];
+            }
+            /* NEAREST AFFINE with b or d non-zero: the 16.16 form, only where Pillow takes it */
+            if (base == JPEGB200_COLOR_AFFINE && !filt && !(c[1] == 0.0 && c[3] == 0.0) &&
+                (!jd_pillow_fixed_ok(c, w, h) || !jd_aug_fixed_map(c, w, h, &aug->a[plan->nops])))
+                return 0;
+            wp->fill[plan->nops] = jd_fill8(warp[k].fill[0]) | jd_fill8(warp[k].fill[1]) << 8 | jd_fill8(warp[k].fill[2]) << 16;
+            plan->seg[++plan->ncontrast] = plan->nops;
+            plan->op[plan->nops] = (uint32_t)op;
+            plan->arg[plan->nops] = 0u;
+            plan->nops++;
+            continue;
+        }
         if (filt && (!rs || filt == (JPEGB200_COLOR_BILINEAR | JPEGB200_COLOR_BICUBIC) || !JD_CO_GEOMETRIC(base))) return 0;
         if ((base < JPEGB200_COLOR_BRIGHTNESS || base > JPEGB200_COLOR_SOLARIZE) && base != JPEGB200_COLOR_GAUSSIAN_BLUR &&
             (base < JPEGB200_COLOR_SHARPNESS || base > JPEGB200_COLOR_ROTATE)) return 0;

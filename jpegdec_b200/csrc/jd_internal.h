@@ -184,9 +184,18 @@ int jd_check_box(const int32_t *out_sizes, const double *boxes, const double *ga
  * jd_color_plan_rs also plans the geometric ops flagged JPEGB200_COLOR_BILINEAR or _BICUBIC: cut like the NEAREST ones,
  * each one's matrix (jd_aug_matrix) into rs at its op slot.  It returns 0 for a flag that is not exactly one of the two on
  * a geometric code, and for a flagged op on a view with a side above JD_AU_MAX_SIDE.  jd_color_plan_aug is
- * jd_color_plan_rs with rs NULL, which refuses every flagged op, as the plans without rs always have. */
+ * jd_color_plan_rs with rs NULL, which refuses every flagged op, as the plans without rs always have.
+ * jd_color_plan_warp also plans JPEGB200_COLOR_AFFINE / _PERSPECTIVE (bare or with one filter flag), whose arguments are
+ * warp[k] for op slot k of the row: cut like the geometric ops, the coefficients and the clamped fill into wp, and a
+ * NEAREST affine with b or d non-zero as its 16.16 mapping into aug, at the op's plan slot.  It returns 0 for both filter
+ * flags together, a non-finite coefficient, a view side above JD_AU_MAX_SIDE and such an affine where Pillow does not
+ * take its 16.16 form (|x a + y b + c| or |x d + y e + f| at least 32768 at a corner (0 or w, 0 or h) of the view).  jd_color_plan_rs is jd_color_plan_warp with warp and wp NULL, which refuses both codes. */
 #include "jd_color.h"
 #include "jd_augment.h"
+int jd_color_plan_warp(const JPEGB200_ColorOp *row, const JPEGB200_WarpArgs *warp, int gray, uint32_t w, uint32_t h,
+                       JDColorPlan *plan, JDBlurPlan *blur, JDAugPlan *aug, JDResamplePlan *rs, JDWarpPlan *wp);
+/* jd_au_walk_table, built here without FMA contraction: the table jdk_warp reads for a NEAREST affine with b = d = 0 */
+void jd_walk_table(const double *c, uint32_t w, uint32_t h, int16_t *tab);
 int jd_color_plan_rs(const JPEGB200_ColorOp *row, int gray, uint32_t w, uint32_t h, JDColorPlan *plan, JDBlurPlan *blur,
                      JDAugPlan *aug, JDResamplePlan *rs);
 int jd_color_plan_aug(const JPEGB200_ColorOp *row, int gray, uint32_t w, uint32_t h, JDColorPlan *plan, JDBlurPlan *blur,

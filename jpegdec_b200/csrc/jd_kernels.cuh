@@ -2484,6 +2484,32 @@ __global__ void __launch_bounds__(JD_AU_THREADS) jdk_augment_rs(const JDAugDesc 
     else scratch[d.soff + item] = o[0];
 }
 
+/* Image.transform's AFFINE / PERSPECTIVE (jd_au_warp): like jdk_augment_rs, into the view's scratch copy, one thread per
+ * output pixel, the views' first CTAs counting from b0 (the CTAs of jdk_augment and jdk_augment_rs at the same cut index).
+ * wd: each view's coefficients and its fill word in the view's byte order (alpha 0xFF), entry for entry with ad.  A NEAREST
+ * affine with b or d non-zero reads the 16.16 mapping in ad's m; one with b = d = 0 its walk table at tabs + tab. */
+struct JDWarpDesc {
+    double c[8];
+    uint32_t fill;
+    uint32_t tab;
+};
+
+template <int BPP>
+__global__ void __launch_bounds__(JD_AU_THREADS) jdk_warp(const JDAugDesc *ad, const JDWarpDesc *wd, const int16_t *tabs, uint32_t n,
+                                                          uint32_t b0, const uint8_t *base, uint8_t *scratch)
+{
+    const uint32_t b = blockIdx.x + b0;
+    const JDAugDesc &d = jd_au_find(ad, n, b);
+    const uint64_t item = (uint64_t)(b - d.blk) * JD_AU_THREADS + threadIdx.x;
+    if (item >= (uint64_t)d.w * d.h) return;
+    const uint32_t y = (uint32_t)(item / d.w), x = (uint32_t)(item % d.w);
+    const JDWarpDesc &w = wd[&d - ad];
+    uint8_t o[4] = {(uint8_t)w.fill, (uint8_t)(w.fill >> 8), (uint8_t)(w.fill >> 16), (uint8_t)(w.fill >> 24)};
+    jd_au_warp(d.op, w.c, &d.m, tabs + w.tab, x, y, d.w, d.h, base + d.off, d.pitch, BPP, o);
+    if (BPP == 4) reinterpret_cast<uint32_t *>(scratch + d.soff)[item] = o[0] | (uint32_t)o[1] << 8 | (uint32_t)o[2] << 16 | (uint32_t)o[3] << 24;
+    else scratch[d.soff + item] = o[0];
+}
+
 /* ------------------------------------------------------------------------------------ */
 /* Tensor output (JPEGB200_batchCreateTensor): the pipeline has written each image's uint8  */
 /* output U tightly into the staging buffer; jdk_tensor looks every byte up in the C x 256  */

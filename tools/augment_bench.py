@@ -1,5 +1,6 @@
-"""torchvision's classification preset with RandAugment / TrivialAugmentWide on the GPU (JPEGB200_batchCreateColor with the
-auto-augment operations) against the same calls with empty lists, and against Pillow + torchvision on the host's CPU threads.
+"""torchvision's classification preset with RandAugment / TrivialAugmentWide, or RandomAffine / RandomRotation /
+RandomPerspective, on the GPU (JPEGB200_batchCreateWarp with the auto-augment and warp operations) against the same calls
+with empty lists, and against Pillow + torchvision on the host's CPU threads.
 
     python tools/augment_bench.py [--n 1024] [--steps 5] [--warmup 2]
 
@@ -8,7 +9,10 @@ repeated), JPEGB200_OPT_LIBJPEG, one 224 view per file (RandomResizedCrop's draw
 into device memory (uint8 RGB8888), with J.auto_augment_ops draws per view:
   - ta: TrivialAugmentWide(); ra: RandAugment(); ta_bilinear / ra_bilinear / ta_bicubic / ra_bicubic: the same with
     interpolation=BILINEAR / BICUBIC (geometric ops flagged J.COLOR_BILINEAR / _BICUBIC; the resize stays bilinear, so
-    the arms differ in their operations only); none: the same calls with empty lists (alternated step by step).  Median
+    the arms differ in their operations only); J.geometric_ops draws of affine_nearest / affine_bilinear:
+    RandomAffine(15, (0.1, 0.1), (0.9, 1.1)) in NEAREST / BILINEAR, affine_scale_nearest: RandomAffine(0, (0.1, 0.1),
+    (0.9, 1.1)) (b = d = 0, the walked form), rotation_bilinear: RandomRotation(30, BILINEAR), perspective:
+    RandomPerspective(0.5, p=1.0) (BILINEAR); none: the same calls with empty lists (alternated step by step).  Median
     device step time (CUDA events, JPEGB200_T_TOTAL) and of the slot after the IDCT (JPEGB200_T_DITHER: resize and
     operations).
   - cpu: Image.open + convert + RandomResizedCrop + flip + TrivialAugmentWide on every usable host CPU, views per second.
@@ -55,7 +59,10 @@ def plan(n, aug):
         k = 2 if torch.rand(1) < 0.5 else 1
         rois.append((1920 - j - w, i, w, h) if k == 2 else (j, i, w, h))
         ks.append(k)
-        color.append(J.auto_augment_ops(aug, (S, S), resample=True))
+        if isinstance(aug, (TV.RandomAffine, TV.RandomRotation, TV.RandomPerspective)):
+            color.append(J.geometric_ops(aug, (S, S)))
+        else:
+            color.append(J.auto_augment_ops(aug, (S, S), resample=True))
     return rois, ks, color
 
 
@@ -78,6 +85,13 @@ def main():
         interp = IM.BILINEAR if f == "bilinear" else IM.BICUBIC
         arms["ta_" + f] = dict(base, color=plan(len(files), TV.TrivialAugmentWide(interpolation=interp))[2])
         arms["ra_" + f] = dict(base, color=plan(len(files), TV.RandAugment(interpolation=interp))[2])
+    geo = {"affine_nearest": TV.RandomAffine(15, (0.1, 0.1), (0.9, 1.1)),
+           "affine_bilinear": TV.RandomAffine(15, (0.1, 0.1), (0.9, 1.1), interpolation=IM.BILINEAR),
+           "affine_scale_nearest": TV.RandomAffine(0, (0.1, 0.1), (0.9, 1.1)),
+           "rotation_bilinear": TV.RandomRotation(30, IM.BILINEAR),
+           "perspective": TV.RandomPerspective(0.5, p=1.0)}
+    for name, t in geo.items():
+        arms[name] = dict(base, color=plan(len(files), t)[2])
     ctx = J.Context(0, J.JPEG_ARITH_SSE2)
     res = {k: [] for k in arms}
     for k in range(a["warmup"] + a["steps"]):
@@ -92,7 +106,7 @@ def main():
     for name in res:
         out[name] = {"ms_per_step": float(np.median([t["total"] for t in res[name]])),
                      "dither_slot_ms": float(np.median([t["dither"] for t in res[name]]))}
-    for name in ("ta", "ra", "ta_bilinear", "ra_bilinear", "ta_bicubic", "ra_bicubic"):
+    for name in ("ta", "ra", "ta_bilinear", "ra_bilinear", "ta_bicubic", "ra_bicubic") + tuple(geo):
         out[name + "_ops_ms"] = out[name]["dither_slot_ms"] - out["none"]["dither_slot_ms"]
     ncpu = len(os.sched_getaffinity(0))
     from PIL import Image
