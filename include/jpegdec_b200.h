@@ -141,7 +141,8 @@ int JPEGB200_digestDevice(JPEGB200_CTX *ctx, const void *const *dev_ptrs, const 
 /* Parses the n headers on the host (no GPU work).  datas[i]/sizes[i]: JPEG files in host memory
  * (pinned memory makes the upload a straight DMA; files that sit back to back are uploaded with one copy).
  * pixel_type / options as in JPEGDEC.h.  At most 3 GiB of compressed bytes per batchCreate (JPEGB200_decodeBatch
- * takes any amount and splits it); a single file may be at most 512 MiB.  An image whose coefficient records could
+ * takes any amount and splits it); a single file may be at most 512 MiB.  Within those byte limits a batch may hold
+ * any number of images (or views) up to INT32_MAX.  An image whose coefficient records could
  * pass 2^32 (6 per byte of the file plus 128 per restart interval: a file with very many short restart intervals, e.g.
  * 8-bit gray with DRI 1 and 10 bytes per interval above about 21 M intervals) gets JPEG_UNSUPPORTED_FEATURE; the
  * other images of the batch still decode.

@@ -2068,16 +2068,27 @@ static int run_chunks(JPEGB200_BATCH *b, DecodeState &D)
     ca.seg_phase = b->d_seg_phase.p; ca.seg_jmap = b->d_seg_jmap.p; ca.seg_status = b->d_seg_status.p; ca.nseg_total = b->nseg;
     const unsigned gi = ((unsigned)b->cimg_list.size() * 32 + 127) / 128;
     ca.max_nch = b->max_nch; ca.Ep = b->d_Ep.p; ca.cfirst = b->d_cfirst.p;
-    const dim3 gchunks((b->max_nch + 127) / 128, (unsigned)b->cimg_list.size());
+    /* jdk_unstuff, jdk_chunk_parse and jdk_chunk_emit take their position in cimg_list from blockIdx.y, which a grid caps
+     * at 65 535: a longer list runs in slices of at most that many positions, each with the list offset to its first one.
+     * Every slice of a launch is on the stream before the next launch, so a parse pass still ends before the next begins. */
+    const uint32_t ncimg = (uint32_t)b->cimg_list.size();
+    auto sliced = [&](void (*kernel)(const JDChunkArgs), unsigned gx) {
+        for (uint32_t c0 = 0; c0 < ncimg; c0 += 65535u) {
+            JDChunkArgs s = ca;
+            s.cimg_list = ca.cimg_list + c0;
+            kernel<<<dim3(gx, std::min(ncimg - c0, 65535u)), 128, 0, st>>>(s);
+            D.launches++;
+        }
+    };
+    const unsigned gchunks = (b->max_nch + 127) / 128;
     /* guess: every chunk starts a block at its first bit (exit state of every left neighbour = (0, 0, 0)); no chunk parsed yet */
     CK(cudaMemsetAsync(b->d_E0.p, 0, (size_t)(b->nchunks + 1) * 4, st));
     CK(cudaMemsetAsync(b->d_Ep.p, 0xFE, (size_t)b->nchunks * 4, st));
     {
-        const dim3 gu(((b->max_nch * JD_CHUNK_BYTES + JD_UNSTUFF_PIECE - 1) / JD_UNSTUFF_PIECE + 3) / 4, (unsigned)b->cimg_list.size());
-        jdk_unstuff<false><<<gu, 128, 0, st>>>(ca);
-        jdk_unstuff<true><<<gu, 128, 0, st>>>(ca);
+        const unsigned gu = ((b->max_nch * JD_CHUNK_BYTES + JD_UNSTUFF_PIECE - 1) / JD_UNSTUFF_PIECE + 3) / 4;
+        sliced(jdk_unstuff<false>, gu);
+        sliced(jdk_unstuff<true>, gu);
     }
-    D.launches += 2;
     uint32_t *Xin = b->d_E0.p, *Xout = b->d_E1.p;
     int passes = 0;
     /* The entry states reach their fix point in 2-4 passes on real streams (a chunk re-synchronises well inside its 512
@@ -2093,8 +2104,8 @@ static int run_chunks(JPEGB200_BATCH *b, DecodeState &D)
         for (int k = 0; k < burst; k++) {
             if (k == burst - 1) CK(cudaMemsetAsync(b->d_counters.p + 2, 0, 4, st));
             ca.X_in = Xin; ca.X_out = Xout;
-            jdk_chunk_parse<<<gchunks, 128, 0, st>>>(ca);
-            D.launches++; passes++;
+            sliced(jdk_chunk_parse, gchunks);
+            passes++;
             uint32_t *tmp = Xin; Xin = Xout; Xout = tmp;
         }
         if (fixed) break;
@@ -2104,9 +2115,9 @@ static int run_chunks(JPEGB200_BATCH *b, DecodeState &D)
     }
     ca.X_in = Xin; ca.X_out = Xout;
     jdk_chunk_prefix<<<gi, 128, 0, st>>>(ca);
-    jdk_chunk_emit<<<gchunks, 128, 0, st>>>(ca);
+    sliced(jdk_chunk_emit, gchunks);
     jdk_chunk_stitch<<<gi, 128, 0, st>>>(ca);
-    D.launches += 3;
+    D.launches += 2;
     return 1;
 }
 
@@ -2279,6 +2290,10 @@ static int run_idct(JPEGB200_BATCH *b, DecodeState &D)
         else if (!any_tr) classes[nclass++] = JD_ORC_NONE;
         if (any_tr) classes[nclass++] = JD_ORC_TRANSPOSE;
         for (int ci = 0; ci < nclass; ci++) {
+            /* A failed launch only leaves its error pending, and cudaFuncSetAttribute (the IDCT launchers' first-use carveout
+             * calls) returns cudaSuccess and clears it (measured on an H100, CUDA runtime 12.9).  So every launch enqueued so far --
+             * entropy, chunks, stitch, earlier runs -- is checked here, before the next launcher can clear its error. */
+            CK(cudaGetLastError());
             if (!launch_idct_run(b, D, i0, (uint32_t)(i1 - i0), max_mx, max_my, classes[ci])) return 0;
             D.launches++;
         }
