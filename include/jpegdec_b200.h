@@ -448,6 +448,26 @@ int JPEGB200_thumbnailPlan(int width, int height, int req_w, int req_h, double r
  * jdk_augment_copy.  DESIGN.md 4.2.13. */
 #define JPEGB200_COLOR_AFFINE       40
 #define JPEGB200_COLOR_PERSPECTIVE  41
+/* The JPEG round trip: Pillow's img.save(buf, "JPEG", quality=q) then Image.open(buf), which is torchvision's
+ * v2.functional.jpeg(img, q) on a PIL image and on a uint8 tensor alike (jpegdec_b200's jpeg_ops draws v2.JPEG's q).
+ *       JPEG q       an RGB view is compressed as Pillow compresses an "RGB" image -- YCbCr, 4:2:0, the baseline tables of
+ *                    quality q, islow forward DCT -- and decoded as libjpeg-turbo decodes by default (islow, fancy
+ *                    upsampling); a gray view is an "L" image, one component with the luminance table
+ *       JPEG_444 q   the same with subsampling=0 (4:4:4)
+ *       JPEG_422 q   the same with subsampling=1 (4:2:2)
+ *   R, G, B are taken in the view's byte order and the alpha byte is kept.  No file is made: the entropy coding is lossless,
+ *   so the quantized coefficients go straight back through the decoder's arithmetic.  A q that is not finite or not an
+ *   integer in 1 .. 100 gives that view JPEG_INVALID_PARAMETER alone; any view size is accepted (sides above 65 500,
+ *   which libjpeg's encoder and so Pillow's save refuse, get the same arithmetic).  The list is cut at each
+ *   JPEG op, as at a blur: the ops before it see the pixels before compression, those after it the decoded pixels.  At a
+ *   cut index where some view compresses, the call makes jdk_jq_fwd (one thread per 8 x 8 block: the forward half and the
+ *   inverse DCT) over those views, then on RGB output jdk_jq_color (upsampling and colour conversion, in place); a gray
+ *   view's blocks are written back in place by jdk_jq_fwd.  The decoded sample planes of an RGB view (its MCUs x blocks per
+ *   MCU x 64 bytes) take the blur's scratch, counted in the one-call path's per-job scratch bound.  Lists without these
+ *   ops make the same launches as before.  DESIGN.md 4.2.15. */
+#define JPEGB200_COLOR_JPEG         31
+#define JPEGB200_COLOR_JPEG_444     32
+#define JPEGB200_COLOR_JPEG_422     33
 #define JPEGB200_COLOR_MAX_OPS    8
 typedef struct {
     int32_t op;                        /* JPEGB200_COLOR_*, 0 = end of the view's list */

@@ -47,6 +47,9 @@ COLOR_BILINEAR, COLOR_BICUBIC = 0x100, 0x200
 # Pillow's Image.transform(size, AFFINE / PERSPECTIVE, coeffs, resample, fillcolor): (op, coeffs, fill) entries, NEAREST bare
 # or with COLOR_BILINEAR / COLOR_BICUBIC OR'd in (geometric_ops draws them for RandomAffine / RandomRotation / RandomPerspective)
 COLOR_AFFINE, COLOR_PERSPECTIVE = 40, 41
+# the JPEG round trip (COLOR_JPEG, q): Pillow's save(buf, "JPEG", quality=q) + Image.open(buf), i.e. torchvision's
+# v2.functional.jpeg; _444 / _422 are Pillow's subsampling=0 / 1 (jpeg_ops draws v2.JPEG's q)
+COLOR_JPEG, COLOR_JPEG_444, COLOR_JPEG_422 = 31, 32, 33
 COLOR_MAX_OPS = 8
 TIMING_NAMES = ["h2d", "prescan", "entropy", "stitch", "idct", "dither", "d2h", "total"]
 COUNTER_NAMES = ["launches", "segments", "blocks", "events", "compressed_bytes", "output_bytes",
@@ -605,6 +608,18 @@ def auto_augment_ops(t, size, *, resample=False):
                     m *= -1.0
                 ops += op_list(name, m)
     return ops
+
+
+def jpeg_ops(t):
+    """One view's operation list [(COLOR_JPEG, q)] for torchvision's v2.JPEG `t`: q drawn from torch's global generator as
+    t.make_params draws it, so under one torch.manual_seed the list gives torchvision's image (PIL or uint8 tensor, which
+    agree) and leaves the generator where forward does."""
+    import torch
+    from torchvision.transforms import v2
+    if not isinstance(t, v2.JPEG):
+        raise TypeError("jpeg_ops: a torchvision.transforms.v2.JPEG")
+    lo, hi = t.quality
+    return [(COLOR_JPEG, float(torch.randint(lo, hi + 1, ()).item()))]
 
 
 def rotate_matrix(angle, size, center=None):

@@ -19,7 +19,7 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 C_SOURCES = ["jd_host.c", "jd_api.c"]
 CU_SOURCES = ["jd_device.cu"]
-HEADERS = ["jd_core.h", "jd_chunk.h", "jd_internal.h", "jd_kernels.cuh", "jd_resize.h", "jd_reduce.h", "jd_color.h", "jd_blur.h", "jd_augment.h", "jd_prog.h", "jd_ljpeg.h",
+HEADERS = ["jd_core.h", "jd_chunk.h", "jd_internal.h", "jd_kernels.cuh", "jd_resize.h", "jd_reduce.h", "jd_color.h", "jd_blur.h", "jd_augment.h", "jd_prog.h", "jd_ljpeg.h", "jd_jpegop.h",
            os.path.join("..", "..", "include", "JPEGDEC.h"),
            os.path.join("..", "..", "include", "jpegdec_b200.h")]
 

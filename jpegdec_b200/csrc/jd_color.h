@@ -15,6 +15,7 @@
  *   solarize (threshold): c < thr ? c : 255 - c, thr = the number of bytes below the double threshold
  *   Gaussian blur r:      ImageFilter.GaussianBlur(r), jd_blur.h (not a per-pixel operation: run by its own kernels)
  *   posterize, invert, sharpness, autocontrast, equalize, shear, translate, rotate: jd_augment.h
+ *   JPEG round trip q:    save(buf, "JPEG", quality=q) + Image.open, jd_jpegop.h (run by its own kernels)
  *
  * On a gray ("L") image brightness, contrast (m over the bytes themselves) and solarize apply; saturation, hue and grayscale
  * leave it alone, as they do in Pillow and torchvision.  Every float and double operation on the device goes through the
@@ -77,14 +78,21 @@
  * (jd_augment.h: jd_au_warp), a bare code for NEAREST or with one filter flag OR'd in: run by jdk_warp */
 #define JD_CO_AFFINE       40
 #define JD_CO_PERSPECTIVE  41
+/* the JPEG round trip at quality q (arg: q), 4:2:0, 4:4:4 or 4:2:2 on RGB views (jd_jpegop.h): run by jdk_jq_fwd and
+ * jdk_jq_color */
+#define JD_CO_JPEG         31
+#define JD_CO_JPEG_444     32
+#define JD_CO_JPEG_422     33
 #define JD_CO_MAX_OPS    8
 #define JD_CO_GEOMETRIC(op) ((op) >= JD_CO_SHEAR_X && (op) <= JD_CO_ROTATE)
 #define JD_CO_WARP(op)      (((op) & 0xFFu) == JD_CO_AFFINE || ((op) & 0xFFu) == JD_CO_PERSPECTIVE)
 /* a flagged geometric op 25 .. 29 (jdk_augment_rs); a flagged warp op matches too, so callers test JD_CO_WARP first */
 #define JD_CO_RESAMPLE(op)  (((op) & (JD_CO_BILINEAR | JD_CO_BICUBIC)) != 0)
 #define JD_CO_LUT(op)       ((op) == JD_CO_AUTOCONTRAST || (op) == JD_CO_EQUALIZE)
+#define JD_CO_JQ(op)        ((op) >= JD_CO_JPEG && (op) <= JD_CO_JPEG_422)
 /* ops a kernel of their own runs at a cut, before jdk_color runs the rest of the segment */
-#define JD_CO_OWN_KERNEL(op) ((op) == JD_CO_BLUR || (op) == JD_CO_SHARPNESS || JD_CO_GEOMETRIC(op) || JD_CO_RESAMPLE(op) || JD_CO_WARP(op))
+#define JD_CO_OWN_KERNEL(op) ((op) == JD_CO_BLUR || (op) == JD_CO_SHARPNESS || JD_CO_GEOMETRIC(op) || JD_CO_RESAMPLE(op) || JD_CO_WARP(op) || \
+                              JD_CO_JQ(op))
 
 JD_CO_HD float jd_co_float(uint32_t bits)
 {

@@ -199,6 +199,10 @@ struct JPEGB200_BATCH {
     DevBuf<JDWarpDesc> d_au_warp;
     std::vector<int16_t> au_tab;            /* the walk tables of the NEAREST affines with b = d = 0 (jd_au_walk_table) */
     DevBuf<int16_t> d_au_tab;
+    std::vector<JDJqDesc> jq_desc;          /* per cut index, per view compressing there (jdk_jq_fwd, jdk_jq_color) */
+    DevBuf<JDJqDesc> d_jq_desc;
+    std::vector<uint16_t> jq_tab;           /* the table pair of each distinct quality in the batch (jd_jq_tables) */
+    DevBuf<uint16_t> d_jq_tab;
     DevBuf<uint32_t> d_co_hslot;            /* per cut index and view: its histogram slot (the slots follow the scratch copies in d_bl) */
     std::vector<uint8_t> co_bgr;
     std::vector<JDColorDesc> co_desc;
@@ -1040,8 +1044,17 @@ static int plan_view_output(JPEGB200_BATCH *b, CreatePlan &P, int f, int i)
         const JDColorPlan &cp = b->co_plans[i];
         bool own = false;
         int64_t nlut = 0;
-        for (uint32_t k = 0; k < cp.nops; k++) { own = own || JD_CO_OWN_KERNEL(cp.op[k]); nlut += JD_CO_LUT(cp.op[k]) ? 1 : 0; }
+        uint64_t jq = 0;   /* a JPEG op on an RGB view: its decoded planes (a gray view's blocks are written back in place) */
+        for (uint32_t k = 0; k < cp.nops; k++) {
+            if (JD_CO_JQ(cp.op[k])) {
+                uint32_t hs, vs;
+                jd_jq_factors(cp.op[k], &hs, &vs);
+                if (b->ptclass != JD_PT_GRAY) jq = std::max(jq, jd_jq_scratch(jd_jq_geo(vd.out_w, vd.out_h, hs, vs)));
+            } else own = own || JD_CO_OWN_KERNEL(cp.op[k]);
+            nlut += JD_CO_LUT(cp.op[k]) ? 1 : 0;
+        }
         if (own) b->bl_scratch[i] = (int64_t)align256((size_t)vd.out_w * vd.out_h * bytes_per_pixel_class(b->ptclass));
+        if ((int64_t)align256((size_t)jq) > b->bl_scratch[i]) b->bl_scratch[i] = (int64_t)align256((size_t)jq);
         b->bl_scratch[i] += nlut * JD_AU_HIST * (int64_t)sizeof(unsigned long long);
         b->bl_scratch_total += b->bl_scratch[i];
     }
@@ -1577,6 +1590,8 @@ struct DecodeState {
     std::vector<uint32_t> au_ctas;          /* CTAs of each cut index's jdk_augment_copy (jdk_augment's, then jdk_augment_rs's) */
     std::vector<uint32_t> au_nn;            /* per cut index: the entries and CTAs of jdk_augment, then those of jdk_augment
                                                and jdk_augment_rs together (the rest warp) */
+    std::vector<uint32_t> jq_first;         /* JPEG ops: the first jq_desc entry of each cut index (one past the last at nl) */
+    std::vector<uint32_t> jq_ctas;          /* CTAs of each cut index's jdk_jq_fwd, then of its jdk_jq_color */
     std::vector<uint8_t> co_lut;            /* per cut index: some view posterizes, inverts, applies a LUT or counts a
                                                histogram there (jdk_color_lut) */
     unsigned long long *co_hist = nullptr;  /* the histogram slots */
@@ -1817,6 +1832,48 @@ static int stage_color(JPEGB200_BATCH *b, DecodeState &D)
         }
     }
     D.au_first[nl] = (uint32_t)b->au_desc.size();
+    /* JPEG ops: at cut index s, the views whose segment s starts with one; one table pair per distinct quality */
+    b->jq_desc.clear();
+    b->jq_tab.clear();
+    D.jq_first.assign(nl + 1, 0);
+    D.jq_ctas.assign(2 * (size_t)nl, 0);
+    int32_t tab_of[101];
+    for (int q = 0; q <= 100; q++) tab_of[q] = -1;
+    for (uint32_t s = 1; s < nl; s++) {
+        D.jq_first[s] = (uint32_t)b->jq_desc.size();
+        uint64_t cf = 0, cc = 0;
+        for (int i = 0; i < n; i++) {
+            const JDColorPlan &p = b->co_plans[i];
+            if (b->parse_status[i] != JPEG_SUCCESS || s > p.ncontrast || !JD_CO_JQ(p.op[p.seg[s]])) continue;
+            const uint32_t q = p.arg[p.seg[s]];
+            if (tab_of[q] < 0) {
+                tab_of[q] = (int32_t)(b->jq_tab.size() / 128);
+                b->jq_tab.resize(b->jq_tab.size() + 128);
+                jd_jq_tables((int)q, b->jq_tab.data() + b->jq_tab.size() - 128);
+            }
+            const bool gray = b->ptclass == JD_PT_GRAY;
+            uint32_t hs = 1u, vs = 1u;
+            if (!gray) jd_jq_factors(p.op[p.seg[s]], &hs, &vs);
+            JDJqDesc x{};
+            x.off = b->co_desc[i].off; x.pitch = b->co_desc[i].pitch; x.soff = soffs[i];
+            x.g = jd_jq_geo(b->co_desc[i].w, b->co_desc[i].h, hs, vs);
+            x.bgr = b->co_bgr[i];
+            x.tab = (uint32_t)tab_of[q];
+            x.blk = (uint32_t)cf; x.cblk = (uint32_t)cc;
+            cf += ((uint64_t)x.g.nmx * x.g.nmy * jd_jq_bpm(hs, vs, gray) + JD_JQ_THREADS - 1) / JD_JQ_THREADS;
+            if (!gray) cc += ((uint64_t)x.g.w * x.g.h + JD_CO_THREADS - 1) / JD_CO_THREADS;
+            if (cf >= (1ull << 31) || cc >= (1ull << 31)) { snprintf(g_err, sizeof(g_err), "colour operations: too many pixels in one job"); return 0; }
+            b->jq_desc.push_back(x);
+        }
+        D.jq_ctas[2 * s] = (uint32_t)cf; D.jq_ctas[2 * s + 1] = (uint32_t)cc;
+    }
+    D.jq_first[nl] = (uint32_t)b->jq_desc.size();
+    if (!b->jq_desc.empty()) {
+        CK(b->d_jq_desc.alloc(&b->ctx->pool, b->jq_desc.size()));
+        CK(cudaMemcpyAsync(b->d_jq_desc.p, b->jq_desc.data(), sizeof(JDJqDesc) * b->jq_desc.size(), cudaMemcpyHostToDevice, st));
+        CK(b->d_jq_tab.alloc(&b->ctx->pool, b->jq_tab.size()));
+        CK(cudaMemcpyAsync(b->d_jq_tab.p, b->jq_tab.data(), sizeof(uint16_t) * b->jq_tab.size(), cudaMemcpyHostToDevice, st));
+    }
     if (soff + hbytes) CK(b->d_bl.alloc(&b->ctx->pool, soff + hbytes));
     if (!b->au_desc.empty()) {
         CK(b->d_au_desc.alloc(&b->ctx->pool, b->au_desc.size()));
@@ -2354,8 +2411,8 @@ static void run_resize(JPEGB200_BATCH *b, DecodeState &D)
 
 /* timed in the dither slot too, after the resize: per cut index of the operation lists, the blur pair for the views that
  * blur there, jdk_augment for the views that sharpen or move pixels with NEAREST there, jdk_augment_rs for those that
- * resample and jdk_warp for those that warp, then one jdk_augment_copy for all of them, then jdk_color for the per-pixel
- * operations up to the next cut */
+ * resample and jdk_warp for those that warp, then one jdk_augment_copy for all of them, jdk_jq_fwd (and on RGB output
+ * jdk_jq_color) for the views that compress there, then jdk_color for the per-pixel operations up to the next cut */
 static void run_color(JPEGB200_BATCH *b, DecodeState &D)
 {
     cudaStream_t st = b->ss.stream;
@@ -2393,6 +2450,18 @@ static void run_color(JPEGB200_BATCH *b, DecodeState &D)
                 jdk_augment_copy<4><<<D.au_ctas[s], JD_AU_THREADS, 0, st>>>(ad, na, D.pipe_out, b->d_bl.p);
             }
             D.launches += 1 + (nn ? 1 : 0) + (nn < nr ? 1 : 0) + (nr < na ? 1 : 0);
+        }
+        const uint32_t fj = D.jq_first[s], nj = D.jq_first[s + 1] - fj;
+        if (nj) {
+            const JDJqDesc *jd = b->d_jq_desc.p + fj;
+            if (b->ptclass == JD_PT_GRAY) {
+                jdk_jq_fwd<1><<<D.jq_ctas[2 * s], JD_JQ_THREADS, 0, st>>>(jd, nj, b->d_jq_tab.p, D.pipe_out, b->d_bl.p);
+                D.launches++;
+            } else {
+                jdk_jq_fwd<4><<<D.jq_ctas[2 * s], JD_JQ_THREADS, 0, st>>>(jd, nj, b->d_jq_tab.p, D.pipe_out, b->d_bl.p);
+                jdk_jq_color<<<D.jq_ctas[2 * s + 1], JD_CO_THREADS, 0, st>>>(jd, nj, D.pipe_out, b->d_bl.p);
+                D.launches += 2;
+            }
         }
         if (!D.co_ctas[s]) continue;
         const uint32_t *cblk = b->d_co_blk.p + (size_t)s * n;

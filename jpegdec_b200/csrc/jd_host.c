@@ -918,6 +918,15 @@ int jd_color_plan_warp(const JPEGB200_ColorOp *row, const JPEGB200_WarpArgs *war
             continue;
         }
         if (filt && (!rs || filt == (JPEGB200_COLOR_BILINEAR | JPEGB200_COLOR_BICUBIC) || !JD_CO_GEOMETRIC(base))) return 0;
+        if (!filt && op >= JPEGB200_COLOR_JPEG && op <= JPEGB200_COLOR_JPEG_422) {
+            /* Pillow's quality: an integer 1 .. 100 (the tables of q are built by the device plan, jd_jq_tables) */
+            if (!(a >= 1.0 && a <= 100.0 && a == floor(a))) return 0;
+            plan->seg[++plan->ncontrast] = plan->nops;
+            plan->op[plan->nops] = (uint32_t)op;
+            plan->arg[plan->nops] = (uint32_t)a;
+            plan->nops++;
+            continue;
+        }
         if ((base < JPEGB200_COLOR_BRIGHTNESS || base > JPEGB200_COLOR_SOLARIZE) && base != JPEGB200_COLOR_GAUSSIAN_BLUR &&
             (base < JPEGB200_COLOR_SHARPNESS || base > JPEGB200_COLOR_ROTATE)) return 0;
         if (!isfinite(a)) return 0;

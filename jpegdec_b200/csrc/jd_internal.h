@@ -181,6 +181,8 @@ int jd_check_box(const int32_t *out_sizes, const double *boxes, const double *ga
  * goes to aug (when not NULL) at its op slot.  It also returns 0 for a posterize argument that is not an integer in 0 .. 8,
  * and, when aug is not NULL, for a geometric op on a view with a side above JD_AU_MAX_SIDE or whose mapping does not fit
  * 32 bits.  jd_color_plan_blur is jd_color_plan_aug with aug NULL.
+ * Every variant plans the JPEG ops (JPEGB200_COLOR_JPEG, _444, _422; jd_jpegop.h) as a cut with arg q, and returns 0 for a
+ * q that is not an integer in 1 .. 100.
  * jd_color_plan_rs also plans the geometric ops flagged JPEGB200_COLOR_BILINEAR or _BICUBIC: cut like the NEAREST ones,
  * each one's matrix (jd_aug_matrix) into rs at its op slot.  It returns 0 for a flag that is not exactly one of the two on
  * a geometric code, and for a flagged op on a view with a side above JD_AU_MAX_SIDE.  jd_color_plan_aug is

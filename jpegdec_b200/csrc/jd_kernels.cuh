@@ -2511,6 +2511,76 @@ __global__ void __launch_bounds__(JD_AU_THREADS) jdk_warp(const JDAugDesc *ad, c
 }
 
 /* ------------------------------------------------------------------------------------ */
+/* JPEG round trip (JPEGB200_COLOR_JPEG, _444, _422; jd_jpegop.h): at a cut index where some */
+/* view compresses, jdk_jq_fwd runs one thread per 8 x 8 block of those views (the threads  */
+/* of an MCU's blocks side by side): it reads the view, runs the forward half and the       */
+/* inverse DCT in registers, and writes the decoded samples to the view's planes in the     */
+/* scratch (RGB) or back into the view (gray: its blocks are disjoint and read only their   */
+/* own pixels).  jdk_jq_color then upsamples and converts every pixel of the RGB views in   */
+/* place, keeping the alpha byte.  One view per CTA in both; a CTA stages its view's table  */
+/* pair in shared memory.                                                                   */
+/* ------------------------------------------------------------------------------------ */
+#include "jd_jpegop.h"
+#define JD_JQ_THREADS 128
+struct JDJqDesc {
+    uint64_t off;              /* the view's image from the launch's base */
+    uint64_t pitch;            /* bytes between its rows */
+    uint64_t soff;             /* its decoded planes from the scratch base (RGB views) */
+    JDJqGeo g;                 /* size, luma factors (1 x 1 on gray views) and MCUs */
+    uint32_t bgr;              /* RGB8888 stored as B, G, R, A */
+    uint32_t tab;              /* its table pair: tables + 128 tab (jd_jq_tables) */
+    uint32_t blk;              /* first CTA of this view in jdk_jq_fwd */
+    uint32_t cblk;             /* first CTA of this view in jdk_jq_color */
+};
+
+__device__ __forceinline__ const JDJqDesc &jd_jq_find(const JDJqDesc *jd, uint32_t n, uint32_t b, bool color)
+{
+    uint32_t lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if ((color ? jd[mid].cblk : jd[mid].blk) <= b) lo = mid; else hi = mid - 1;
+    }
+    return jd[lo];
+}
+
+template <int BPP>
+__global__ void __launch_bounds__(JD_JQ_THREADS) jdk_jq_fwd(const JDJqDesc *jd, uint32_t n, const uint16_t *tables, uint8_t *base,
+                                                            uint8_t *scratch)
+{
+    static_assert(JD_JQ_THREADS == 128, "one thread per table entry");
+    const JDJqDesc &d = jd_jq_find(jd, n, blockIdx.x, false);
+    __shared__ uint16_t tab[128];
+    tab[threadIdx.x] = tables[128u * d.tab + threadIdx.x];
+    __syncthreads();
+    const uint64_t b = (uint64_t)(blockIdx.x - d.blk) * JD_JQ_THREADS + threadIdx.x;
+    if (b >= (uint64_t)d.g.nmx * d.g.nmy * jd_jq_bpm(d.g.hs, d.g.vs, BPP == 1)) return;
+    int32_t c[64];
+    uint32_t o[16], px, py;
+    const uint32_t comp = jd_jq_fwd_block(base + d.off, d.pitch, BPP, d.bgr, d.g, (uint32_t)b, tab, c, o, nullptr, nullptr, &px, &py);
+    if (BPP == 1) {
+        uint8_t *dst = base + d.off + (uint64_t)py * d.pitch + px;
+        for (uint32_t r = 0; r < 8u && py + r < d.g.h; r++)
+            for (uint32_t k = 0; k < 8u && px + k < d.g.w; k++) dst[(uint64_t)r * d.pitch + k] = (uint8_t)(o[2 * r + k / 4] >> (8 * (k % 4)));
+    } else {
+        uint32_t pp;
+        uint8_t *dst = scratch + d.soff + jd_jq_plane_off(d.g, comp, px, py, &pp);
+#pragma unroll
+        for (uint32_t r = 0; r < 8u; r++) *reinterpret_cast<uint2 *>(dst + (uint64_t)r * pp) = make_uint2(o[2 * r], o[2 * r + 1]);
+    }
+}
+
+__global__ void __launch_bounds__(JD_CO_THREADS) jdk_jq_color(const JDJqDesc *jd, uint32_t n, uint8_t *base, const uint8_t *scratch)
+{
+    const JDJqDesc &d = jd_jq_find(jd, n, blockIdx.x, true);
+    const uint64_t item = (uint64_t)(blockIdx.x - d.cblk) * JD_CO_THREADS + threadIdx.x;
+    if (item >= (uint64_t)d.g.w * d.g.h) return;
+    const uint32_t y = (uint32_t)(item / d.g.w), x = (uint32_t)(item % d.g.w);
+    const uint32_t v = jd_jq_rgb(scratch + d.soff, d.g, x, y);
+    uint32_t *p = reinterpret_cast<uint32_t *>(base + d.off + (uint64_t)y * d.pitch + (uint64_t)x * 4u);
+    *p = (*p & 0xFF000000u) | (d.bgr ? ((v & 255u) << 16) | (v & 0xFF00u) | ((v >> 16) & 255u) : v);
+}
+
+/* ------------------------------------------------------------------------------------ */
 /* Tensor output (JPEGB200_batchCreateTensor): the pipeline has written each image's uint8  */
 /* output U tightly into the staging buffer; jdk_tensor looks every byte up in the C x 256  */
 /* table the host computed (jd_tensor_table) and stores the elements in CHW or HWC order.   */
