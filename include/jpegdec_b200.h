@@ -495,6 +495,30 @@ JPEGB200_BATCH *JPEGB200_batchCreateWarp(JPEGB200_CTX *ctx, const uint8_t *const
                                          const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
                                          const double *reducing_gaps, const JPEGB200_ColorOp *color_ops,
                                          const JPEGB200_WarpArgs *warp_args);
+/* Crop after the resize: torchvision's evaluation preset (Resize -> CenterCrop), FiveCrop, TenCrop and RandomCrop.  The
+ * arguments of JPEGB200_batchCreateWarp plus windows: V x {x, y, w, h}, one per view (windows = NULL is
+ * JPEGB200_batchCreateWarp, which forwards here).  Let R_v be what the same call without windows has after its resize and
+ * before its colour list (rectangle, orientation, draft, box / reduce, resize; uint8).  View v is then Pillow's
+ * R_v.crop((x, y, x + w, y + h)) of every byte plane: the window may reach past R_v on any side or lie wholly outside it,
+ * and its pixels outside R_v are 0 (RGB8888: R = G = B = 0, alpha 0xFF; gray 0).  Without out_sizes R_v is the unresized
+ * image itself, so a window is a rectangle that may pad.  The colour list then runs on the w x h window, and the tensor
+ * conversion follows; JPEGB200_batchImageInfo, _batchOutputBytes, the arena, JPEGB200_C_OUTPUT_BYTES and the tensor shape
+ * follow w x h.  A w or h outside 1..65535 gives that view alone JPEG_INVALID_PARAMETER; RGB565, dithered pixel types and
+ * padded output return NULL, as for out_sizes.
+ * The resize reads only the window's support: the rectangle of the unresized image from the first in-image output's
+ * first tap to the last one's last tap per resampled axis (the window's in-image span along an axis Pillow does not
+ * resample; 1 x 1 at the origin when the window reads no pixel).  The view decodes that rectangle alone, through the
+ * region-of-interest decode, inside its own rois rectangle.  So its status and JPEGB200_batchErrMcu follow the
+ * JPEGB200_batchCreateROI rule for the support rectangle: a corrupt scan below the support leaves the view at JPEG_SUCCESS,
+ * and restart intervals below it are not walked.  A boxed view (boxes or reducing_gaps) decodes all of its rectangle.
+ * The passes (which axes, vertical first) are Pillow's choice for the full sizes, so the bytes are those of the full
+ * resize.  DESIGN.md 4.2.16. */
+JPEGB200_BATCH *JPEGB200_batchCreateWindow(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                           const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                           const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                           const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
+                                           const double *reducing_gaps, const JPEGB200_ColorOp *color_ops,
+                                           const JPEGB200_WarpArgs *warp_args, const int32_t *windows);
 void JPEGB200_batchDestroy(JPEGB200_BATCH *b);
 int JPEGB200_batchCount(JPEGB200_BATCH *b);
 /* per-image facts after batchCreate: status is JPEG_SUCCESS or the open() error the reference would give */
@@ -611,6 +635,14 @@ int JPEGB200_decodeBatchWarp(JPEGB200_CTX *ctx, const uint8_t *const *datas, con
                              const double *boxes, const double *reducing_gaps, const JPEGB200_ColorOp *color_ops,
                              const JPEGB200_WarpArgs *warp_args, void *const *outs, const int64_t *pitches,
                              const int64_t *plane_strides, int flags, int32_t *status);
+/* The same with a window per view (semantics of JPEGB200_batchCreateWindow; NULL = JPEGB200_decodeBatchWarp, which forwards
+ * here).  The per-job scratch bound counts each view's support, not its whole unresized image. */
+int JPEGB200_decodeBatchWindow(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                               const int32_t *views, int pixel_type, int options, const int32_t *rois, const uint8_t *orients,
+                               const int32_t *out_sizes, int filter, const JPEGB200_TensorSpec *spec, const uint8_t *draft,
+                               const double *boxes, const double *reducing_gaps, const JPEGB200_ColorOp *color_ops,
+                               const JPEGB200_WarpArgs *warp_args, const int32_t *windows, void *const *outs,
+                               const int64_t *pitches, const int64_t *plane_strides, int flags, int32_t *status);
 /* JPEGB200_NUM_COUNTERS counters summed over the jobs of the last JPEGB200_decodeBatch on this context */
 int JPEGB200_lastCallCounters(JPEGB200_CTX *ctx, int64_t *counters);
 /* CUDA-event stage times (JPEGB200_NUM_TIMINGS, ms) summed over those jobs, and how many jobs there were.  Jobs overlap

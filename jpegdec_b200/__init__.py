@@ -173,6 +173,9 @@ def lib():
     L.JPEGB200_batchCreateWarp.argtypes = L.JPEGB200_batchCreateColor.argtypes + [wap]
     L.JPEGB200_batchCreateWarp.restype = vp
     L.JPEGB200_decodeBatchWarp.argtypes = L.JPEGB200_decodeBatchColor.argtypes[:16] + [wap] + L.JPEGB200_decodeBatchColor.argtypes[16:]
+    L.JPEGB200_batchCreateWindow.argtypes = L.JPEGB200_batchCreateWarp.argtypes + [i32p]
+    L.JPEGB200_batchCreateWindow.restype = vp
+    L.JPEGB200_decodeBatchWindow.argtypes = L.JPEGB200_decodeBatchWarp.argtypes[:17] + [i32p] + L.JPEGB200_decodeBatchWarp.argtypes[17:]
     L.JPEGB200_rotateMatrix.argtypes = [C.c_double, C.c_int, C.c_int, dp, dp]
     L.JPEGB200_thumbnailPlan.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, ip, ip, ip, dp]
     L.JPEGB200_batchSetOutputTensor.argtypes = [vp, C.c_int, vp, C.c_int64, C.c_int64]
@@ -677,6 +680,155 @@ def geometric_ops(t, size, mode="RGB"):
     return []
 
 
+def resized_size(size_wh, size, max_size=None):
+    """(W, H) of torchvision's Resize(size, max_size=max_size) on a w x h image (F._compute_resized_output_size): an int
+    sets the shorter side, a 1-sequence likewise, an (h, w) pair is taken as it is."""
+    from torchvision.transforms import functional as F
+    w, h = int(size_wh[0]), int(size_wh[1])
+    size = [int(size)] if isinstance(size, int) else [int(v) for v in size]
+    oh, ow = F._compute_resized_output_size((h, w), size, max_size)
+    return int(ow), int(oh)
+
+
+def _crop_hw(crop):
+    """torchvision's output_size: an int or a 1-sequence is square, else (h, w)"""
+    if isinstance(crop, int):
+        return int(crop), int(crop)
+    crop = [int(v) for v in crop]
+    return (crop[0], crop[0]) if len(crop) == 1 else (crop[0], crop[1])
+
+
+def center_crop_window(size_wh, crop):
+    """The window (x, y, w, h) of torchvision's F.center_crop(img, crop) on a w x h image: zero padding where the crop is
+    larger (floor half before, ceil half after), then round() placement, which rounds halves to even as Python does."""
+    w, h = int(size_wh[0]), int(size_wh[1])
+    ch, cw = _crop_hw(crop)
+    x = -((cw - w) // 2) if cw > w else int(round((w - cw) / 2.0))
+    y = -((ch - h) // 2) if ch > h else int(round((h - ch) / 2.0))
+    return (x, y, cw, ch)
+
+
+def five_crop_windows(size_wh, crop):
+    """The windows of torchvision's F.five_crop(img, crop) on a w x h image, in its order: top-left, top-right,
+    bottom-left, bottom-right, centre.  ValueError where five_crop raises (a crop larger than the image)."""
+    w, h = int(size_wh[0]), int(size_wh[1])
+    ch, cw = _crop_hw(crop)
+    if cw > w or ch > h:
+        raise ValueError("five_crop_windows: requested crop size %s is bigger than input size %s" % ((ch, cw), (h, w)))
+    return [(0, 0, cw, ch), (w - cw, 0, cw, ch), (0, h - ch, cw, ch), (w - cw, h - ch, cw, ch),
+            center_crop_window((w, h), (ch, cw))]
+
+
+def flip_op(size_wh, vertical=False):
+    """The colour-list entry that flips a w x h view: Pillow's NEAREST AFFINE transform with (-1, 0, w, 0, 1, 0), or
+    (1, 0, 0, 0, -1, h) with vertical=True, which equals Image.transpose(FLIP_LEFT_RIGHT / FLIP_TOP_BOTTOM) pixel for
+    pixel.  A flip after a crop (RandomHorizontalFlip after RandomCrop or CenterCrop) is this op on the window.  Views
+    with a side above 1024 are refused, as for every warp."""
+    w, h = int(size_wh[0]), int(size_wh[1])
+    return (COLOR_AFFINE, [1.0, 0.0, 0.0, 0.0, -1.0, float(h)] if vertical else [-1.0, 0.0, float(w), 0.0, 1.0, 0.0], None)
+
+
+def ten_crop_views(size_wh, crop, vertical_flip=False):
+    """(windows, color) for torchvision's F.ten_crop(img, crop, vertical_flip) on a w x h image: ten views of one file.
+    The first five are five_crop_windows.  The crop of the flipped image at a window is the flip of the crop at the
+    mirrored window, so the second five are the mirrored windows with flip_op in their colour list.  Exact for any resize
+    before it: the resize never sees a flipped image.  Append further operations to the colour lists."""
+    w, h = int(size_wh[0]), int(size_wh[1])
+    first = five_crop_windows(size_wh, crop)
+    if vertical_flip:
+        second = [(x, h - y - ch, cw, ch) for x, y, cw, ch in first]
+    else:
+        second = [(w - x - cw, y, cw, ch) for x, y, cw, ch in first]
+    ch, cw = _crop_hw(crop)
+    return first + second, [[] for _ in range(5)] + [[flip_op((cw, ch), vertical_flip)] for _ in range(5)]
+
+
+def random_crop_window(t, size_wh):
+    """The window of torchvision's RandomCrop `t` on a w x h image: its padding, pad_if_needed and get_params, with the
+    same draws from torch's global generator as t.forward, so that under one torch.manual_seed it gives forward's crop and
+    leaves the generator where forward does.  ValueError for a padding_mode or fill other than constant 0."""
+    import numbers
+    import torch
+    from torchvision import transforms as TV
+    if not isinstance(t, TV.RandomCrop):
+        raise TypeError("random_crop_window: a torchvision.transforms.RandomCrop")
+    fills = t.fill if isinstance(t.fill, (list, tuple)) else [t.fill]
+    if t.padding_mode != "constant" or any(f != 0 for f in fills):
+        raise ValueError("random_crop_window: only padding_mode='constant' with fill 0 is supported")
+    w, h = int(size_wh[0]), int(size_wh[1])
+    left = top = 0
+    if t.padding is not None:
+        p = t.padding
+        if isinstance(p, numbers.Number):
+            p = [int(p)] * 4
+        elif len(p) == 1:
+            p = [int(p[0])] * 4
+        elif len(p) == 2:
+            p = [int(p[0]), int(p[1]), int(p[0]), int(p[1])]
+        else:
+            p = [int(v) for v in p]
+        if any(v < 0 for v in p):
+            raise ValueError("random_crop_window: negative padding crops, which is not supported")
+        left, top = p[0], p[1]
+        w, h = w + p[0] + p[2], h + p[1] + p[3]
+    th, tw = t.size
+    if t.pad_if_needed and w < tw:
+        left += tw - w
+        w += 2 * (tw - w)
+    if t.pad_if_needed and h < th:
+        top += th - h
+        h += 2 * (th - h)
+    i, j, ch, cw = t.get_params(torch.empty((1, 1, 1), dtype=torch.uint8).expand(1, h, w), t.size)
+    return (int(j) - left, int(i) - top, int(cw), int(ch))
+
+
+def eval_plan(t, size_wh):
+    """The decode arguments of torchvision's evaluation transform `t` for one w x h file: t is
+    transforms._presets.ImageClassification (what weights.transforms() returns) or a v1 / v2
+    Compose([Resize, CenterCrop, ToTensor | PILToTensor + ConvertImageDtype(float32) | ToImage + ToDtype(float32,
+    scale=True), Normalize]).  Returns dict(out_size=(W, H), window=(x, y, w, h), filter, scale, mean, std): the file's
+    out_sizes entry, its windows entry, and the arguments of decode_batch_tensor.  A Resize's max_size is applied as
+    torchvision applies it.  ValueError for a transform of another shape or an interpolation the resize does not take
+    (NEAREST, LANCZOS, ...)."""
+    import torch
+    from torchvision import transforms as TV
+    from torchvision.transforms import InterpolationMode
+    from torchvision.transforms import v2
+    from torchvision.transforms._presets import ImageClassification
+    filters = {InterpolationMode.BILINEAR: RESIZE_BILINEAR, InterpolationMode.BICUBIC: RESIZE_BICUBIC,
+               InterpolationMode.BOX: RESIZE_BOX}
+
+    def plan(resize, max_size, interp, crop, scale, mean, std):
+        if interp not in filters:
+            raise ValueError("eval_plan: interpolation %s is not supported (BILINEAR, BICUBIC or BOX)" % interp)
+        out = resized_size(size_wh, resize, max_size)
+        return dict(out_size=out, window=center_crop_window(out, crop), filter=filters[interp], scale=scale,
+                    mean=tuple(float(v) for v in mean), std=tuple(float(v) for v in std))
+
+    if isinstance(t, ImageClassification):
+        return plan(t.resize_size, None, t.interpolation, t.crop_size, "div255", t.mean, t.std)
+    if not isinstance(t, (TV.Compose, v2.Compose)):
+        raise ValueError("eval_plan: an ImageClassification preset or a Compose")
+    ts = list(t.transforms)
+    if len(ts) < 4 or not isinstance(ts[0], (TV.Resize, v2.Resize)) or not isinstance(ts[1], (TV.CenterCrop, v2.CenterCrop)) \
+            or not isinstance(ts[-1], (TV.Normalize, v2.Normalize)):
+        raise ValueError("eval_plan: Compose([Resize, CenterCrop, <to float tensor>, Normalize])")
+    conv = ts[2:-1]
+    if len(conv) == 1 and isinstance(conv[0], TV.ToTensor):
+        scale = "div255"
+    elif len(conv) == 2 and isinstance(conv[0], TV.PILToTensor) and isinstance(conv[1], TV.ConvertImageDtype) \
+            and conv[1].dtype == torch.float32:
+        scale = "div255"
+    elif len(conv) == 2 and isinstance(conv[0], (v2.ToImage, v2.PILToTensor)) and isinstance(conv[1], v2.ToDtype) \
+            and conv[1].scale and conv[1].dtype == torch.float32:
+        scale = "mul255"
+    else:
+        raise ValueError("eval_plan: the conversion must be ToTensor, PILToTensor + ConvertImageDtype(float32) or "
+                         "ToImage + ToDtype(float32, scale=True)")
+    rs, cc, nm = ts[0], ts[1], ts[-1]
+    return plan(rs.size, rs.max_size, rs.interpolation, cc.size, scale, nm.mean, nm.std)
+
+
 def _orient_array(orients, n):
     """n EXIF transforms (0 = from the file, 1-8) -> uint8[n] for the C ABI (None stays None = no orientation)"""
     if orients is None:
@@ -699,6 +851,18 @@ def _size_array(out_sizes, n):
     return (C.c_int32 * (2 * n))(*flat)
 
 
+def _window_array(windows, n):
+    """n (x, y, w, h) windows -> int32[4n] for the C ABI (None stays None = no windows).  x and y may be negative."""
+    if windows is None:
+        return None
+    flat = [int(v) for r in windows for v in r]
+    if len(flat) != 4 * n:
+        raise ValueError("windows: one (x, y, w, h) per image")
+    if any(v < -(1 << 31) or v >= (1 << 31) for v in flat):
+        raise ValueError("windows: values are int32")
+    return (C.c_int32 * (4 * n))(*flat)
+
+
 class Batch:
     """A decode job over n JPEG files that live in host memory at (ptr, size) pairs.  rois: one (x, y, w, h) rectangle
     in output pixels per image (JPEGB200_batchCreateROI), or None for whole images.  orients: one EXIF transform per
@@ -714,10 +878,13 @@ class Batch:
     (JPEGB200_batchCreateBox; needs out_sizes).  color: one sequence of (op, arg) (COLOR_*) for every image or one per
     image, run on each final uint8 image as torchvision's PIL transforms do (JPEGB200_batchCreateColor), or None.  An
     operation may also be (COLOR_AFFINE / COLOR_PERSPECTIVE [| COLOR_BILINEAR / _BICUBIC], coeffs, fill): Pillow's
-    Image.transform of the view with those 6 / 8 coefficients and fill (None, an int, or R, G, B; JPEGB200_batchCreateWarp)."""
+    Image.transform of the view with those 6 / 8 coefficients and fill (None, an int, or R, G, B; JPEGB200_batchCreateWarp).
+    windows: one (x, y, w, h) per image, or None: each output is then Pillow's crop((x, y, x + w, y + h)) of the resized
+    (or, without out_sizes, the unresized) image, 0 outside it, before `color` (JPEGB200_batchCreateWindow)."""
 
     def __init__(self, ctx, ptrs, sizes, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
-                 filter=RESIZE_BILINEAR, spec=None, views=None, draft=None, box=None, reducing_gap=None, color=None):
+                 filter=RESIZE_BILINEAR, spec=None, views=None, draft=None, box=None, reducing_gap=None, color=None,
+                 windows=None):
         nf = len(ptrs)
         self._views, n = _views_array(views, nf)
         self.n = n
@@ -731,10 +898,11 @@ class Batch:
         self._box, self._gap = _box_array(box, n), _gap_array(reducing_gap, n)
         self._color, self._warp = _color_arrays(color, n)
         self._spec = spec
-        self.h = lib().JPEGB200_batchCreateWarp(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
-                                                self._rois, self._orients, self._out_sizes, int(filter),
-                                                C.byref(spec) if spec is not None else None, self._draft, self._box,
-                                                self._gap, self._color, self._warp)
+        self._windows = _window_array(windows, n)
+        self.h = lib().JPEGB200_batchCreateWindow(ctx.h, self._ptrs, self._sizes, nf, self._views, pixel_type, options,
+                                                  self._rois, self._orients, self._out_sizes, int(filter),
+                                                  C.byref(spec) if spec is not None else None, self._draft, self._box,
+                                                  self._gap, self._color, self._warp, self._windows)
         if not self.h:
             raise RuntimeError("batchCreate failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
 
@@ -811,14 +979,15 @@ class Batch:
 
 
 def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flags=0, rois=None, orients=None,
-                 out_sizes=None, filter=RESIZE_BILINEAR, views=None, draft=None, box=None, reducing_gap=None, color=None):
+                 out_sizes=None, filter=RESIZE_BILINEAR, views=None, draft=None, box=None, reducing_gap=None, color=None,
+                 windows=None):
     """JPEGB200_decodeBatch(ROI / Oriented / Resized / Views): one call for n files (host pointers) -> n outputs (host
     pointers, or device pointers with JPEGB200_OUT_DEVICE); rois: one (x, y, w, h) per image or None; orients: one EXIF
     transform per image (0 = from the file) or None; out_sizes: one (W, H) per image (resized with `filter`) or None.
     views: one view count per file, or None; outs, pitches and the per-image lists are then per view.  Returns (rc,
     per-image status list, counters summed over the internal jobs).  draft: one scale denominator per image (view), or
-    None (JPEGB200_decodeBatchDraft).  box / reducing_gap: as in Batch (JPEGB200_decodeBatchBox).  color: as in Batch
-    (JPEGB200_decodeBatchWarp)."""
+    None (JPEGB200_decodeBatchDraft).  box / reducing_gap: as in Batch (JPEGB200_decodeBatchBox).  color / windows: as
+    in Batch (JPEGB200_decodeBatchWindow)."""
     nf = len(ptrs)
     va, n = _views_array(views, nf)
     pa = (C.c_void_p * nf)(*ptrs)
@@ -829,26 +998,27 @@ def decode_batch(ctx, ptrs, sizes, pixel_type, options, outs, pitches=None, flag
     pi = (C.c_int64 * n)(*pitches) if pitches is not None else None
     st = (C.c_int32 * n)()
     ca, wa = _color_arrays(color, n)
-    rc = lib().JPEGB200_decodeBatchWarp(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
-                                        _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None,
-                                        _draft_array(draft, n), _box_array(box, n), _gap_array(reducing_gap, n),
-                                        ca, wa, oa, pi, None, flags, st)
+    rc = lib().JPEGB200_decodeBatchWindow(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
+                                          _orient_array(orients, n), _size_array(out_sizes, n), int(filter), None,
+                                          _draft_array(draft, n), _box_array(box, n), _gap_array(reducing_gap, n),
+                                          ca, wa, _window_array(windows, n), oa, pi, None, flags, st)
     cnt = (C.c_int64 * len(COUNTER_NAMES))()
     lib().JPEGB200_lastCallCounters(ctx.h, cnt)
     return rc, list(st), dict(zip(COUNTER_NAMES, list(cnt)))
 
 
 def decode_batch_to_host(ctx, jpegs, pixel_type, options=0, rois=None, orients=None, out_sizes=None,
-                         filter=RESIZE_BILINEAR, views=None, draft=None, box=None, reducing_gap=None, color=None):
+                         filter=RESIZE_BILINEAR, views=None, draft=None, box=None, reducing_gap=None, color=None,
+                         windows=None):
     """Convenience: list of bytes -> list of numpy arrays [out_h, pitch_bytes] (uint8).
     One public-API call per batch with HOST buffers on both sides.  rois: one (x, y, w, h) per image (the arrays are then
     h rows of w pixels), or None.  orients: one EXIF transform per image (0 = from the file), or None.  out_sizes: one
     (W, H) per image (the arrays are then H rows of W pixels, resized with `filter`), or None.  views: one view count
     per file, or None; the lists (and rois / orients / out_sizes) are then per view.  draft: one scale denominator per
-    image (view), or None.  box / reducing_gap / color: as in Batch."""
+    image (view), or None.  box / reducing_gap / color / windows: as in Batch (the arrays are then h rows of w pixels)."""
     bufs = [np.frombuffer(j, dtype=np.uint8) for j in jpegs]
     b = Batch(ctx, [x.ctypes.data for x in bufs], [len(x) for x in bufs], pixel_type, options, rois, orients, out_sizes,
-              filter, views=views, draft=draft, box=box, reducing_gap=reducing_gap, color=color)
+              filter, views=views, draft=draft, box=box, reducing_gap=reducing_gap, color=color, windows=windows)
     try:
         outs = []
         for i in range(b.n):
@@ -897,7 +1067,7 @@ def tensor_spec(dtype, layout="CHW", scale="div255", mean=(0.0, 0.0, 0.0), std=(
 def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, orients=None, out_sizes=None,
                         filter=RESIZE_BILINEAR, dtype=None, layout="CHW", scale="div255", mean=(0.0, 0.0, 0.0),
                         std=(1.0, 1.0, 1.0), bgr=False, out=None, views=None, draft=None, box=None, reducing_gap=None,
-                        color=None):
+                        color=None, windows=None):
     """JPEGB200_decodeBatchTensor: list of bytes -> the model's input tensor on the context's GPU, and the status list.
 
     Image i becomes a C x H x W (layout "CHW") or H x W x C ("HWC") tensor of `dtype` (torch.float32 by default, float16,
@@ -911,7 +1081,7 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     images are then the views: rois / orients / out_sizes / out and the result ([V, C, H, W], or a list) are per view.
     draft: one scale denominator (1, 2, 4, 8) per image (view), Pillow's draft() at that scale (JPEGB200_decodeBatchDraft),
     or None.  box / reducing_gap: as in Batch (JPEGB200_decodeBatchBox).  color: as in Batch, before the conversion
-    (JPEGB200_decodeBatchWarp)."""
+    (JPEGB200_decodeBatchWarp).  windows: as in Batch; the shapes are then the windows' (JPEGB200_decodeBatchWindow)."""
     import torch
     dtype = torch.float32 if dtype is None else dtype
     spec = tensor_spec(dtype, layout, scale, mean, std, bgr)
@@ -920,7 +1090,9 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     bufs = [np.frombuffer(j, dtype=np.uint8) for j in jpegs]
     ptrs, sizes = [x.ctypes.data for x in bufs], [len(x) for x in bufs]
     C_ = 3 if pixel_type == RGB8888 and not (options & JPEG_LUMA_ONLY) else 1
-    if out_sizes is not None:
+    if windows is not None:
+        hw = [(int(r[3]), int(r[2])) for r in windows]
+    elif out_sizes is not None:
         hw = [(int(h), int(w)) for w, h in out_sizes]
     elif rois is not None:
         hw = [(int(r[3]), int(r[2])) for r in rois]
@@ -967,11 +1139,11 @@ def decode_batch_tensor(ctx, jpegs, pixel_type=RGB8888, options=0, rois=None, or
     with torch.cuda.device(dev):
         torch.cuda.current_stream(dev).synchronize()   # the library's streams do not order against torch's
         ca, wa = _color_arrays(color, n)
-        rc = lib().JPEGB200_decodeBatchWarp(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
-                                            _orient_array(orients, n), _size_array(out_sizes, n), int(filter),
-                                            C.byref(spec), _draft_array(draft, n), _box_array(box, n),
-                                            _gap_array(reducing_gap, n), ca, wa, (C.c_void_p * n)(*ptr_l),
-                                             (C.c_int64 * n)(*pitch_l), (C.c_int64 * n)(*plane_l), JPEGB200_OUT_DEVICE, st)
+        rc = lib().JPEGB200_decodeBatchWindow(ctx.h, pa, sa, nf, va, pixel_type, options, _roi_array(rois, n),
+                                              _orient_array(orients, n), _size_array(out_sizes, n), int(filter),
+                                              C.byref(spec), _draft_array(draft, n), _box_array(box, n),
+                                              _gap_array(reducing_gap, n), ca, wa, _window_array(windows, n), (C.c_void_p * n)(*ptr_l),
+                                              (C.c_int64 * n)(*pitch_l), (C.c_int64 * n)(*plane_l), JPEGB200_OUT_DEVICE, st)
     if rc == 0:
         raise RuntimeError("decodeBatchViews failed: " + lib().JPEGB200_lastErrorString(ctx.h).decode())
     return out, list(st)

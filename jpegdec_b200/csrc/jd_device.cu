@@ -174,6 +174,13 @@ struct JPEGB200_BATCH {
     std::vector<JDBoxPlan> bx_plans;
     std::vector<JDBoxDesc> bx_desc;
     DevBuf<JDBoxDesc> d_bx_desc;
+    /* windows (JPEGB200_batchCreateWindow): every view resizes (to S's own size without out_sizes) into its window.  Per
+     * view its plan, its window and the full S (before the decode is narrowed to the support) */
+    bool window = false;
+    std::vector<JDWindowPlan> wn_plans;
+    std::vector<int32_t> wn_full;       /* 2 per view */
+    std::vector<int32_t> wn_out;        /* 2 per view: R's size */
+    std::vector<int32_t> wn_win;        /* 4 per view: the window */
     /* colour operations (JPEGB200_batchCreateColor): per view its plan and byte order; jdk_color rewrites the view's final
      * uint8 image in place, before jdk_tensor */
     bool color = false;
@@ -588,6 +595,11 @@ struct CreatePlan {
     const double *boxes = nullptr, *gaps = nullptr;   /* per view: resize box and reducing gap (JPEGB200_batchCreateBox) */
     const JPEGB200_ColorOp *color = nullptr;          /* per view: JPEGB200_COLOR_MAX_OPS operations (JPEGB200_batchCreateColor) */
     const JPEGB200_WarpArgs *warp = nullptr;          /* per view: their AFFINE / PERSPECTIVE arguments (JPEGB200_batchCreateWarp) */
+    const int32_t *windows = nullptr;                 /* per view: x, y, w, h (JPEGB200_batchCreateWindow) */
+    /* with windows: the rectangles the views decode (the caller's rois narrowed to each window's support; rois points here)
+     * and without out_sizes the resize targets (S's own size; out_sizes points here) */
+    std::vector<int32_t> wn_rois, wn_sizes;
+    const int32_t *caller_rois = nullptr;
     /* where the next file's restart segments, blocks and records start; where the next view's output and gray stage start */
     uint32_t seg = 0;
     uint64_t blk = 0, rec_total = 0;
@@ -627,8 +639,14 @@ static void init_batch(JPEGB200_BATCH *b, JPEGB200_CTX *ctx, const CreatePlan &P
     b->gray_out = pixel_type >= EIGHT_BIT_GRAYSCALE;
     b->ptclass = (pixel_type == RGB8888) ? JD_PT_8888 : (b->gray_out ? JD_PT_GRAY : JD_PT_565);
     b->dither_bits = (pixel_type == FOUR_BIT_DITHERED) ? 4 : (pixel_type == TWO_BIT_DITHERED) ? 2 : (pixel_type == ONE_BIT_DITHERED) ? 1 : 0;
-    b->resize = P.out_sizes != nullptr;
+    b->resize = P.out_sizes != nullptr || P.windows != nullptr;
     b->rs_filter = filter;
+    b->window = P.windows != nullptr;
+    if (b->window) {
+        b->wn_plans.assign(nv, JDWindowPlan{});
+        b->wn_full.assign(2 * (size_t)nv, 0); b->wn_out.assign(2 * (size_t)nv, 0);
+        b->wn_win.assign(P.windows, P.windows + 4 * (size_t)nv);
+    }
     if (b->resize) {
         b->rs_plans.assign(nv, JDResizePlan{});
         b->rs_src_w.assign(nv, 0); b->rs_src_h.assign(nv, 0); b->rs_scratch.assign(nv, 0);
@@ -760,10 +778,46 @@ static uint32_t kept_walk(const JPEGB200_BATCH *b, const CreatePlan &P, int v0, 
 /* The views' own arguments (no such transform, a rectangle outside the output, a resize target outside 1..65535) and how
  * deep the file is walked: down to the deepest last MCU row among its valid views.  Writes plans, P.srects and P.vok;
  * returns the restart intervals to walk, 0 when no view is valid. */
+/* With windows, before the views are planned: each view's full S (what the call without windows resizes), its window plan,
+ * and the rectangle it decodes: its support, inside the caller's rectangle (boxed views keep the whole S).  A view whose
+ * own arguments are refused keeps them, so that jd_views_plan refuses it; a refused window clears wn_ok. */
+static void plan_windows(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int nvf, std::vector<int32_t> &wn_ok)
+{
+    const JDInfo &inf = b->infos[f];
+    for (int i = v0; i < v0 + nvf; i++) {
+        int32_t *r = &P.wn_rois[4 * (size_t)i];
+        const int32_t *cr = P.caller_rois ? P.caller_rois + 4 * (size_t)i : nullptr;
+        const int s = P.draft ? jd_draft_shift(P.draft[i]) : b->sshift;
+        const int k = P.orients ? P.ks[i] : 1;
+        int W = (inf.width + (1 << (s < 0 ? 0 : s)) - 1) >> (s < 0 ? 0 : s), H = (inf.height + (1 << (s < 0 ? 0 : s)) - 1) >> (s < 0 ? 0 : s);
+        if (k >= 5 && k <= 8) std::swap(W, H);
+        if (cr) { r[0] = cr[0]; r[1] = cr[1]; r[2] = cr[2]; r[3] = cr[3]; }
+        else { r[0] = 0; r[1] = 0; r[2] = W; r[3] = H; }
+        const bool ok = s >= 0 && k >= 1 && k <= 8 && r[0] >= 0 && r[1] >= 0 && r[2] >= 1 && r[3] >= 1 &&
+                        (int64_t)r[0] + r[2] <= W && (int64_t)r[1] + r[3] <= H;
+        const int32_t sw = ok ? r[2] : 1, sh = ok ? r[3] : 1;
+        b->wn_full[2 * (size_t)i] = sw; b->wn_full[2 * (size_t)i + 1] = sh;
+        if (P.wn_sizes.size()) { P.wn_sizes[2 * (size_t)i] = sw; P.wn_sizes[2 * (size_t)i + 1] = sh; }
+        wn_ok[i - v0] = 1;
+        b->wn_out[2 * (size_t)i] = P.out_sizes[2 * (size_t)i]; b->wn_out[2 * (size_t)i + 1] = P.out_sizes[2 * (size_t)i + 1];
+        if (b->box || !ok) continue;   /* a box reads all of S; a refused view is refused by jd_views_plan */
+        const int32_t *os = &P.out_sizes[2 * (size_t)i];
+        if (os[0] < 1 || os[1] < 1 || os[0] > 65535 || os[1] > 65535) continue;
+        JDWindowPlan &wp = b->wn_plans[i];
+        if (!jd_window_plan(sw, sh, os[0], os[1], b->rs_filter, P.windows + 4 * (size_t)i, bytes_per_pixel_class(b->ptclass), &wp)) {
+            wn_ok[i - v0] = 0;
+            continue;
+        }
+        r[0] += wp.sx; r[1] += wp.sy; r[2] = wp.sw; r[3] = wp.sh;
+    }
+}
+
 static uint32_t plan_views(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int nvf)
 {
     const JDInfo &inf = b->infos[f];
     uint32_t walk = 0;
+    std::vector<int32_t> wn_ok;
+    if (b->window) { wn_ok.assign((size_t)nvf, 1); plan_windows(b, P, f, v0, nvf, wn_ok); }
     if (!P.draft) {
         walk = (uint32_t)jd_views_plan(inf.width, inf.height, inf.subsample, inf.restart_interval, b->sshift, nvf,
                                        P.rois ? P.rois + 4 * (size_t)v0 : nullptr, P.orients ? &P.ks[v0] : nullptr,
@@ -782,6 +836,11 @@ static uint32_t plan_views(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int 
             b->lj_desc[i].shift = (uint32_t)sh;
             if (w > walk) walk = w;
         }
+    }
+    if (walk != 0 && b->window) {
+        bool dropped = false;
+        for (int i = v0; i < v0 + nvf; i++) if (P.vok[i] && !wn_ok[i - v0]) { P.vok[i] = 0; dropped = true; }
+        if (dropped) walk = kept_walk(b, P, v0, nvf, walk);
     }
     if (walk != 0 && b->lj && b->roi) {
         /* what libjpeg's fancy upsampling reads around each rectangle */
@@ -805,7 +864,9 @@ static uint32_t plan_views(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int 
             const double whole[4] = {0.0, 0.0, (double)sw, (double)sh};
             if (!jd_box_plan(sw, sh, P.out_sizes[2 * (size_t)i], P.out_sizes[2 * (size_t)i + 1], b->rs_filter,
                              P.boxes ? P.boxes + 4 * (size_t)i : whole, P.gaps ? P.gaps[i] : 0.0, bytes_per_pixel_class(b->ptclass),
-                             &b->bx_plans[i])) {
+                             &b->bx_plans[i]) ||
+                (b->window && !jd_window_box(&b->bx_plans[i], P.out_sizes[2 * (size_t)i], P.out_sizes[2 * (size_t)i + 1],
+                                             P.windows + 4 * (size_t)i, bytes_per_pixel_class(b->ptclass), &b->wn_plans[i]))) {
                 P.vok[i] = 0;
                 dropped = true;
             }
@@ -819,8 +880,9 @@ static uint32_t plan_views(JPEGB200_BATCH *b, CreatePlan &P, int f, int v0, int 
             if (!P.vok[i]) continue;
             /* the view's final size, which the geometric ops' mappings depend on (padded output takes no operations) */
             const int s = b->lj ? (int)b->lj_desc[i].shift : b->sshift;
-            const uint32_t w = b->resize ? (uint32_t)P.out_sizes[2 * (size_t)i] : b->roi ? (uint32_t)b->plans[i].out_w : (uint32_t)((inf.width + (1 << s) - 1) >> s);
-            const uint32_t h = b->resize ? (uint32_t)P.out_sizes[2 * (size_t)i + 1] : b->roi ? (uint32_t)b->plans[i].out_h : (uint32_t)((inf.height + (1 << s) - 1) >> s);
+            uint32_t w = b->resize ? (uint32_t)P.out_sizes[2 * (size_t)i] : b->roi ? (uint32_t)b->plans[i].out_w : (uint32_t)((inf.width + (1 << s) - 1) >> s);
+            uint32_t h = b->resize ? (uint32_t)P.out_sizes[2 * (size_t)i + 1] : b->roi ? (uint32_t)b->plans[i].out_h : (uint32_t)((inf.height + (1 << s) - 1) >> s);
+            if (b->window) { w = (uint32_t)P.windows[4 * (size_t)i + 2]; h = (uint32_t)P.windows[4 * (size_t)i + 3]; }
             if (!jd_color_plan_warp(P.color + JPEGB200_COLOR_MAX_OPS * (size_t)i, P.warp ? P.warp + JPEGB200_COLOR_MAX_OPS * (size_t)i : nullptr,
                                     b->ptclass == JD_PT_GRAY, w, h, &b->co_plans[i], &b->co_blur[i], &b->co_aug[i], &b->co_rs[i],
                                     P.warp ? &b->co_warp[i] : nullptr)) {
@@ -1018,8 +1080,11 @@ static int plan_view_output(JPEGB200_BATCH *b, CreatePlan &P, int f, int i)
         /* S = what the same call without out_sizes stores; the descriptor carries the resized size from here on */
         const int bp = bytes_per_pixel_class(b->ptclass);
         JDResizePlan &rp = b->rs_plans[i];
-        const int32_t rw = P.out_sizes[2 * (size_t)i], rh = P.out_sizes[2 * (size_t)i + 1];
-        if (b->box) rp = b->bx_plans[i].rp;   /* planned with the box by plan_views */
+        int32_t rw = P.out_sizes[2 * (size_t)i], rh = P.out_sizes[2 * (size_t)i + 1];
+        if (b->window) {   /* planned by plan_windows (or with the box by plan_views); S is the support */
+            rp = b->wn_plans[i].rp;
+            rw = P.windows[4 * (size_t)i + 2]; rh = P.windows[4 * (size_t)i + 3];
+        } else if (b->box) rp = b->bx_plans[i].rp;   /* planned with the box by plan_views */
         else if (!jd_resize_plan((int)vd.out_w, (int)vd.out_h, rw, rh, b->rs_filter, bp, &rp)) {
             snprintf(g_err, sizeof(g_err), "resize plan failed for image %d", i);
             return 0;
@@ -1191,10 +1256,31 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateWarp(JPEGB200_CTX *ctx, const uin
                                                     const double *reducing_gaps, const JPEGB200_ColorOp *color_ops,
                                                     const JPEGB200_WarpArgs *warp_args)
 {
+    return JPEGB200_batchCreateWindow(ctx, datas, sizes, n, views, pixel_type, options, rois, orients, out_sizes, filter, spec, draft,
+                                      boxes, reducing_gaps, color_ops, warp_args, nullptr);
+}
+
+extern "C" JPEGB200_BATCH *JPEGB200_batchCreateWindow(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                                      const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                                      const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                                      const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
+                                                      const double *reducing_gaps, const JPEGB200_ColorOp *color_ops,
+                                                      const JPEGB200_WarpArgs *warp_args, const int32_t *windows)
+{
     if (!ctx) { snprintf(g_err, sizeof(g_err), "invalid parameter"); return nullptr; }
     int64_t nv = 0;   /* images of the batch: views */
-    if (!jd_check_batch_features(pixel_type, options, n, views, rois != nullptr, orients != nullptr, out_sizes != nullptr, filter, spec,
-                                 &nv, g_err, (int)sizeof(g_err)) ||
+    /* a window resizes (to S's own size without out_sizes): the resize's refusals (RGB565, dithered, padded) apply, named
+     * for the windows */
+    const int rs_filter = out_sizes ? filter : JPEGB200_RESIZE_BILINEAR;
+    if (windows) {
+        const int pt = jd_fold_luma_only(pixel_type, options);
+        const char *why = (pt == RGB565_LITTLE_ENDIAN || pt == RGB565_BIG_ENDIAN) ? "RGB565 pixel types"
+                          : (pt >= FOUR_BIT_DITHERED && pt <= ONE_BIT_DITHERED) ? "dithered pixel types"
+                          : (options & JPEGB200_OPT_PADDED) ? "padded output" : nullptr;
+        if (why) { snprintf(g_err, sizeof(g_err), "windows are not supported with %s", why); return nullptr; }
+    }
+    if (!jd_check_batch_features(pixel_type, options, n, views, rois != nullptr, orients != nullptr,
+                                 out_sizes != nullptr || windows != nullptr, rs_filter, spec, &nv, g_err, (int)sizeof(g_err)) ||
         !jd_check_draft(options, draft, g_err, (int)sizeof(g_err)) || !jd_check_box(out_sizes, boxes, reducing_gaps, g_err, (int)sizeof(g_err)) ||
         !jd_check_color(pixel_type, options, nv, color_ops, g_err, (int)sizeof(g_err)))
         return nullptr;
@@ -1208,7 +1294,14 @@ extern "C" JPEGB200_BATCH *JPEGB200_batchCreateWarp(JPEGB200_CTX *ctx, const uin
     P.srects.assign(4 * (size_t)nv, 0); P.vok.assign((size_t)nv, 0);
     P.ks.assign(orients ? (size_t)nv : 0u, 0);
     if (options & JPEGB200_OPT_PROGRESSIVE) { P.fscans.resize(JD_PROG_MAX_SCANS); P.ftabs.resize(JD_PROG_MAX_TABS); }
-    init_batch(b, ctx, P, n, (int)nv, pixel_type, options, filter);
+    if (windows) {
+        P.windows = windows;
+        P.caller_rois = rois;
+        P.wn_rois.assign(4 * (size_t)nv, 0);
+        P.rois = P.wn_rois.data();
+        if (!out_sizes) { P.wn_sizes.assign(2 * (size_t)nv, 1); P.out_sizes = P.wn_sizes.data(); }
+    }
+    init_batch(b, ctx, P, n, (int)nv, pixel_type, options, rs_filter);
     if (!layout_input(b) || !plan_files(b, P)) { delete b; return nullptr; }
     sort_prog_waves(b);
     build_work_list(b);
@@ -1941,6 +2034,16 @@ static int stage_resize(JPEGB200_BATCH *b, DecodeState &D)
         r.ksize_h = (uint32_t)rp.ksize_h; r.ksize_v = (uint32_t)rp.ksize_v;
         r.ybox0 = (uint32_t)rp.ybox0; r.rows = (uint32_t)rp.rows;
         r.flags = (rp.need_h ? 1u : 0u) | (rp.need_v ? 2u : 0u) | (rp.vfirst ? 4u : 0u);
+        r.in_w = sw; r.in_h = sh; r.full_w = r.dst_w; r.full_h = r.dst_h;
+        r.wx1 = r.dst_w; r.wy1 = r.dst_h;
+        if (b->window) {
+            const JDWindowPlan &wp = b->wn_plans[i];
+            r.in_w = (uint32_t)b->wn_full[2 * (size_t)i]; r.in_h = (uint32_t)b->wn_full[2 * (size_t)i + 1];
+            r.full_w = (uint32_t)b->wn_out[2 * (size_t)i]; r.full_h = (uint32_t)b->wn_out[2 * (size_t)i + 1];
+            r.sx = (uint32_t)wp.sx; r.sy = (uint32_t)wp.sy;
+            r.wx0 = (uint32_t)wp.x0; r.wx1 = (uint32_t)wp.x1; r.wy0 = (uint32_t)wp.y0; r.wy1 = (uint32_t)wp.y1;
+            r.win_x = b->wn_win[4 * (size_t)i]; r.win_y = b->wn_win[4 * (size_t)i + 1];
+        }
         r.src_off = so;
         so += align256((size_t)sw * sh * bp);
         if (b->box) {
@@ -1952,6 +2055,7 @@ static int stage_resize(JPEGB200_BATCH *b, DecodeState &D)
             x.rx0 = (uint32_t)p.rx0; x.ry0 = (uint32_t)p.ry0; x.rbw = (uint32_t)(p.rx1 - p.rx0); x.rbh = (uint32_t)(p.ry1 - p.ry0);
             x.fx = (uint32_t)p.fx; x.fy = (uint32_t)p.fy;
             r.src_w = (uint32_t)p.rw; r.src_h = (uint32_t)p.rh;
+            r.in_w = r.src_w; r.in_h = r.src_h;
             if (p.fx > 1 || p.fy > 1) {
                 r.src_off = so;
                 so += align256((size_t)r.src_w * r.src_h * bp);
@@ -2788,6 +2892,18 @@ extern "C" int JPEGB200_decodeBatchWarp(JPEGB200_CTX *ctx, const uint8_t *const 
                                         const JPEGB200_WarpArgs *warp_args, void *const *outs, const int64_t *pitches,
                                         const int64_t *plane_strides, int flags, int32_t *status)
 {
+    return JPEGB200_decodeBatchWindow(ctx, datas, sizes, n, views, pixel_type, options, rois, orients, out_sizes, filter, spec, draft,
+                                      boxes, reducing_gaps, color_ops, warp_args, nullptr, outs, pitches, plane_strides, flags, status);
+}
+
+extern "C" int JPEGB200_decodeBatchWindow(JPEGB200_CTX *ctx, const uint8_t *const *datas, const int32_t *sizes, int n,
+                                          const int32_t *views, int pixel_type, int options, const int32_t *rois,
+                                          const uint8_t *orients, const int32_t *out_sizes, int filter,
+                                          const JPEGB200_TensorSpec *spec, const uint8_t *draft, const double *boxes,
+                                          const double *reducing_gaps, const JPEGB200_ColorOp *color_ops,
+                                          const JPEGB200_WarpArgs *warp_args, const int32_t *windows, void *const *outs,
+                                          const int64_t *pitches, const int64_t *plane_strides, int flags, int32_t *status)
+{
     if (!ctx || n <= 0) return 0;
     const int64_t nv = jd_count_views(n, views, "call", g_err, (int)sizeof(g_err));   /* images (views) of the call */
     if (nv < 0) return 0;
@@ -2836,12 +2952,13 @@ extern "C" int JPEGB200_decodeBatchWarp(JPEGB200_CTX *ctx, const uint8_t *const 
         const int32_t *vi = views ? views + i0 : nullptr;
         int cnt = jd_job_files(n - i0, sizes + i0, vi, maxcnt, limit, nullptr, 0, &cv, &capped);
         auto create = [&](int c) {
-            return JPEGB200_batchCreateWarp(ctx, datas + i0, sizes + i0, c, vi, pixel_type, options, rois ? rois + 4 * (size_t)v0 : nullptr,
+            return JPEGB200_batchCreateWindow(ctx, datas + i0, sizes + i0, c, vi, pixel_type, options, rois ? rois + 4 * (size_t)v0 : nullptr,
                                             orients ? orients + v0 : nullptr, out_sizes ? out_sizes + 2 * (size_t)v0 : nullptr, filter, spec,
                                             draft ? draft + v0 : nullptr, boxes ? boxes + 4 * (size_t)v0 : nullptr,
                                             reducing_gaps ? reducing_gaps + v0 : nullptr,
                                             color_ops ? color_ops + JPEGB200_COLOR_MAX_OPS * (size_t)v0 : nullptr,
-                                            color_ops && warp_args ? warp_args + JPEGB200_COLOR_MAX_OPS * (size_t)v0 : nullptr);
+                                            color_ops && warp_args ? warp_args + JPEGB200_COLOR_MAX_OPS * (size_t)v0 : nullptr,
+                                            windows ? windows + 4 * (size_t)v0 : nullptr);
         };
         JPEGB200_BATCH *b = create(cnt);
         if (!b) { rc = 0; break; }

@@ -680,6 +680,70 @@ int jd_resize_plan(int src_w, int src_h, int out_w, int out_h, int filter, int b
     return 1;
 }
 
+/* window columns (or rows) [*i0, *i1) of a window (start ws, length wl) inside an axis of n samples; 0 when none */
+static int jd_win_span(int64_t ws, int64_t wl, int64_t n, int32_t *i0, int32_t *i1)
+{
+    const int64_t a = ws < 0 ? -ws : 0, b = ws + wl < n ? wl : n - ws;
+    if (a >= b) { *i0 = *i1 = 0; return 0; }
+    *i0 = (int32_t)a; *i1 = (int32_t)b;
+    return 1;
+}
+
+/* the window's intermediate and tables (rp's passes and strides already set; rows = the source rows held) */
+static void jd_win_sizes(JDResizePlan *rp, int w, int h, int src_w, int src_h, int bytes_per_pixel)
+{
+    rp->ybox0 = 0;
+    rp->rows = src_h;
+    if (rp->vfirst) rp->mid_bytes = (int64_t)h * src_w * bytes_per_pixel;
+    else rp->mid_bytes = rp->need_h ? (int64_t)src_h * w * bytes_per_pixel : 0;
+    rp->coef_words = (rp->need_h ? (int64_t)w * (rp->ksize_h + 2) : 0) + (rp->need_v ? (int64_t)h * (rp->ksize_v + 2) : 0);
+}
+
+/* Window plan (JDWindowPlan) */
+int jd_window_plan(int src_w, int src_h, int out_w, int out_h, int filter, const int32_t *window, int bytes_per_pixel,
+                   JDWindowPlan *plan)
+{
+    if (!jd_resize_plan(src_w, src_h, out_w, out_h, filter, bytes_per_pixel, &plan->rp)) return 0;
+    const int w = window[2], h = window[3];
+    if (w < 1 || h < 1 || w > 65535 || h > 65535) return 0;
+    const int in_x = jd_win_span(window[0], w, out_w, &plan->x0, &plan->x1);
+    const int in_y = jd_win_span(window[1], h, out_h, &plan->y0, &plan->y1);
+    plan->sx = plan->sy = 0;
+    plan->sw = plan->sh = 1;
+    if (!in_x || !in_y) { plan->x0 = plan->x1 = plan->y0 = plan->y1 = 0; }
+    else {
+        /* first and last in-image output of each axis, in R */
+        const int64_t gx0 = (int64_t)window[0] + plan->x0, gx1 = (int64_t)window[0] + plan->x1 - 1;
+        const int64_t gy0 = (int64_t)window[1] + plan->y0, gy1 = (int64_t)window[1] + plan->y1 - 1;
+        int32_t a, na, b, nb;
+        if (plan->rp.need_h) {
+            jd_rs_bounds(src_w, out_w, filter, (int)gx0, &a, &na);
+            jd_rs_bounds(src_w, out_w, filter, (int)gx1, &b, &nb);
+            plan->sx = a; plan->sw = b + nb - a;
+        } else { plan->sx = (int32_t)gx0; plan->sw = (int32_t)(gx1 - gx0 + 1); }
+        if (plan->rp.need_v) {
+            jd_rs_bounds(src_h, out_h, filter, (int)gy0, &a, &na);
+            jd_rs_bounds(src_h, out_h, filter, (int)gy1, &b, &nb);
+            plan->sy = a; plan->sh = b + nb - a;
+        } else { plan->sy = (int32_t)gy0; plan->sh = (int32_t)(gy1 - gy0 + 1); }
+    }
+    jd_win_sizes(&plan->rp, w, h, plan->sw, plan->sh, bytes_per_pixel);
+    return 1;
+}
+
+int jd_window_box(const JDBoxPlan *box, int out_w, int out_h, const int32_t *window, int bytes_per_pixel, JDWindowPlan *plan)
+{
+    const int w = window[2], h = window[3];
+    if (w < 1 || h < 1 || w > 65535 || h > 65535) return 0;
+    plan->rp = box->rp;
+    if (!jd_win_span(window[0], w, out_w, &plan->x0, &plan->x1) || !jd_win_span(window[1], h, out_h, &plan->y0, &plan->y1))
+        plan->x0 = plan->x1 = plan->y0 = plan->y1 = 0;
+    plan->sx = plan->sy = 0;
+    plan->sw = box->rw; plan->sh = box->rh;
+    jd_win_sizes(&plan->rp, w, h, box->rw, box->rh, bytes_per_pixel);
+    return 1;
+}
+
 /* Box plan (JDBoxPlan): Image.resize's Python steps in double (jd_internal.h), then the C resize's pass choice and row box
  * for the float box, like jd_resize_plan */
 int jd_box_plan(int sw, int sh, int out_w, int out_h, int filter, const double *box, double gap, int bytes_per_pixel, JDBoxPlan *p)

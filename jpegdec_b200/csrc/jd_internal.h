@@ -149,6 +149,23 @@ typedef struct {
 /* Returns 0 for a filter other than JPEGB200_RESIZE_* or a size outside 1..65535. */
 int jd_resize_plan(int src_w, int src_h, int out_w, int out_h, int filter, int bytes_per_pixel, JDResizePlan *plan);
 
+/* Window of one view (JPEGB200_batchCreateWindow): the crop (x, y, w, h) of R, the resize of S (src_w x src_h) to out_w x
+ * out_h, as Pillow's R.crop((x, y, x + w, y + h)).  Window columns x0 .. x1 - 1 and rows y0 .. y1 - 1 lie inside R; the
+ * others are fill (all four 0 when the window reads no pixel of R).  The support (sx, sy, sw, sh) is the rectangle of S the
+ * in-image outputs read: along a resampled axis from the first one's xmin to the last one's xmin + taps (jd_rs_bounds with
+ * the full sizes), along an axis Pillow does not resample the window's in-image span; 1 x 1 at S's origin when the window
+ * reads nothing.  rp holds the passes: need_h, need_v, vfirst and the strides on the full sizes (Pillow decides there, and
+ * the order changes the rounding), ybox0 = 0 and rows = sh (every support row), and the intermediate and coefficient tables
+ * for the window only. */
+typedef struct {
+    int32_t sx, sy, sw, sh;
+    int32_t x0, x1, y0, y1;
+    JDResizePlan rp;
+} JDWindowPlan;
+/* Returns 0 for what jd_resize_plan refuses and for a window side outside 1..65535. */
+int jd_window_plan(int src_w, int src_h, int out_w, int out_h, int filter, const int32_t *window, int bytes_per_pixel,
+                   JDWindowPlan *plan);
+
 /* Box resize of one view (JPEGB200_batchCreateBox): Pillow's resize(out, filter, box, reducing_gap) of S (sw x sh) as its
  * Python code decides it, in double: factor = int(box extent / out / gap) or 1 per axis; with a factor above 1 the region
  * _get_safe_box(out, filter, box) of S is reduced (jd_reduce.h) and the box carried into the reduced frame; then the C
@@ -167,6 +184,9 @@ typedef struct {
  * reduce to an empty image or of boxes of 2^23 pixels or more, and for jd_resize_plan's refusals.  The box is checked in
  * S's frame: one past the edge is refused even where Pillow's reduce would carry it inside the reduced image. */
 int jd_box_plan(int sw, int sh, int out_w, int out_h, int filter, const double *box, double gap, int bytes_per_pixel, JDBoxPlan *plan);
+/* The window of a boxed view: box->rp's passes, the whole resize source as the support (no narrowing), the intermediate and
+ * tables for the window.  0 for a window side outside 1..65535. */
+int jd_window_box(const JDBoxPlan *box, int out_w, int out_h, const int32_t *window, int bytes_per_pixel, JDWindowPlan *plan);
 /* Batch-level rule of JPEGB200_batchCreateBox: boxes or reducing_gaps need out_sizes.  0 with a message otherwise. */
 int jd_check_box(const int32_t *out_sizes, const double *boxes, const double *gaps, char *msg, int msg_len);
 

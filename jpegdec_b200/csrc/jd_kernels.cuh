@@ -1913,6 +1913,13 @@ struct JDResizeDesc {
     uint32_t ybox0, rows;      /* source rows the horizontal pass reads (horizontal pass first) */
     uint32_t flags;            /* bit 0: horizontal pass, bit 1: vertical pass, bit 2: vertical pass first */
     uint32_t blk_c, blk_h, blk_v, blk_h2;  /* first CTA of this image in jdk_resize_coeffs, _h<_, 0>, _v, _h<_, 1> */
+    /* window (JPEGB200_batchCreateWindow, JDWindowPlan): dst_w x dst_h is the window at (win_x, win_y) of the full resize
+     * R (full_w x full_h) of the full source (in_w x in_h); S above is its support, at (sx, sy) of the full source.  Window
+     * columns wx0 .. wx1 - 1 and rows wy0 .. wy1 - 1 lie in R, the last pass stores fill elsewhere.  Without a window
+     * win = s = 0, in = src, full = dst and the spans are the whole output: the same arithmetic as before. */
+    uint32_t in_w, in_h, full_w, full_h, sx, sy;
+    uint32_t wx0, wx1, wy0, wy1;
+    int32_t win_x, win_y;
 };
 
 template <int F>
@@ -1933,16 +1940,19 @@ __global__ void __launch_bounds__(JD_RS_THREADS) jdk_resize_coeffs(const JDResiz
     const JDResizeDesc &r = rd[jd_rs_find<0>(rd, n, blockIdx.x)];
     const uint32_t item = (blockIdx.x - r.blk_c) * JD_RS_THREADS + threadIdx.x;
     const uint32_t nh = (r.flags & 1u) ? r.dst_w : 0u, nv = (r.flags & 2u) ? r.dst_h : 0u;
+    /* window column / row i (jd_rs_win_coeffs): output win + i of the full axis, xmin relative to the support */
     int32_t xmin;
     if (item < nh) {
         int32_t *tab = coef + r.coef_h;
-        const int taps = jd_rs_coeffs((int)r.src_w, (int)r.dst_w, filter, (int)item, &xmin, tab + 2 * (uint64_t)r.dst_w + item, r.dst_w);
+        const int taps = jd_rs_win_coeffs((int)r.in_w, (int)r.full_w, filter, r.win_x, item, r.wx0, r.wx1, (int32_t)r.sx,
+                                          (int32_t)r.src_w, &xmin, tab + 2 * (uint64_t)r.dst_w + item, r.dst_w);
         tab[2 * item] = xmin;
         tab[2 * item + 1] = taps;
     } else if (item < nh + nv) {
         const uint32_t yy = item - nh;
         int32_t *tab = coef + r.coef_v + (uint64_t)yy * (r.ksize_v + 2);
-        const int taps = jd_rs_coeffs((int)r.src_h, (int)r.dst_h, filter, (int)yy, &xmin, tab + 2, 1);
+        const int taps = jd_rs_win_coeffs((int)r.in_h, (int)r.full_h, filter, r.win_y, yy, r.wy0, r.wy1, (int32_t)r.sy,
+                                          (int32_t)r.src_h, &xmin, tab + 2, 1);
         tab[0] = xmin;
         tab[1] = taps;
     }
@@ -1974,8 +1984,9 @@ __global__ void __launch_bounds__(JD_RS_THREADS) jdk_resize_h(const JDResizeDesc
         const uint8_t *row = VFIRST ? scratch + r.mid_off + (uint64_t)y * r.src_w * BPP
                                     : scratch + r.src_off + (uint64_t)(r.ybox0 + y) * r.src_w * BPP;
         uint8_t *dst = VFIRST ? out + r.dst_off + (uint64_t)y * r.dst_pitch + (uint64_t)x * BPP : scratch + r.mid_off + item * BPP;
-        if (BPP == 4) *reinterpret_cast<uint32_t *>(dst) = jd_rs_conv4(reinterpret_cast<const uint32_t *>(row) + xmin, 1, taps, w, r.dst_w);
-        else *dst = (uint8_t)jd_rs_conv1(row + xmin, 1, taps, w, r.dst_w);
+        const bool fill = VFIRST && (x < r.wx0 || x >= r.wx1 || y < r.wy0 || y >= r.wy1);   /* the last pass: window pad */
+        if (BPP == 4) *reinterpret_cast<uint32_t *>(dst) = fill ? jd_rs_fill(4) : jd_rs_conv4(reinterpret_cast<const uint32_t *>(row) + xmin, 1, taps, w, r.dst_w);
+        else *dst = fill ? (uint8_t)jd_rs_fill(1) : (uint8_t)jd_rs_conv1(row + xmin, 1, taps, w, r.dst_w);
         return;
     }
     __shared__ uint32_t span[JD_RS_SPAN_WORDS];
@@ -2039,9 +2050,12 @@ __global__ void __launch_bounds__(JD_RS_THREADS) jdk_resize_v(const JDResizeDesc
     if (item >= (uint64_t)q * r.dst_h) return;
     const uint32_t y = (uint32_t)(item / q), x0 = (uint32_t)(item % q) * PX;
     const bool from_mid = hpass && !vfirst;
-    const uint8_t *src = scratch + (from_mid ? r.mid_off : r.src_off);     /* width pixels wide */
-    const int64_t spitch = (int64_t)width * BPP;
-    int32_t ymin = (int32_t)y, taps = 1;
+    const uint8_t *src = scratch + (from_mid ? r.mid_off : r.src_off);
+    /* the source is the window wide (the horizontal pass's intermediate) or S wide; a window's column x reads S's column
+     * x + win_x - sx without a horizontal pass, and its row y row y + win_y - sy without a vertical pass */
+    const int64_t spitch = (int64_t)(from_mid ? r.dst_w : r.src_w) * BPP;
+    const int64_t coff = (hpass || vfirst) ? 0 : (int64_t)r.win_x - r.sx;
+    int32_t ymin = (int32_t)((int64_t)y + r.win_y - r.sy), taps = 1;
     const int32_t *w = coef;
     if (vpass) {
         const int32_t *tab = coef + r.coef_v + (uint64_t)y * (r.ksize_v + 2);
@@ -2049,15 +2063,18 @@ __global__ void __launch_bounds__(JD_RS_THREADS) jdk_resize_v(const JDResizeDesc
         taps = tab[1];
         w = tab + 2;
     }
-    const uint8_t *col = src + (int64_t)ymin * spitch + (int64_t)x0 * BPP;
+    /* the last pass stores fill outside R (vfirst: jdk_resize_h<_, 1> does) */
+    const bool row_fill = !vfirst && (y < r.wy0 || y >= r.wy1);
+    const uint8_t *col = src + (int64_t)ymin * spitch + ((int64_t)x0 + coff) * BPP;
     const uint32_t npx = width - x0 < PX ? width - x0 : PX;
     uint32_t wv[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
     for (uint32_t p = 0; p < PX; p++) {
         if (p < npx) {
             uint32_t v;
-            if (BPP == 4) v = vpass ? jd_rs_conv4(reinterpret_cast<const uint32_t *>(col) + p, spitch / 4, taps, w, 1)
-                                    : reinterpret_cast<const uint32_t *>(col)[p];
+            if (!vfirst && (row_fill || x0 + p < r.wx0 || x0 + p >= r.wx1)) v = jd_rs_fill(BPP);
+            else if (BPP == 4) v = vpass ? jd_rs_conv4(reinterpret_cast<const uint32_t *>(col) + p, spitch / 4, taps, w, 1)
+                                         : reinterpret_cast<const uint32_t *>(col)[p];
             else v = vpass ? jd_rs_conv1(col + p, spitch, taps, w, 1) : col[p];
             if (BPP == 4) wv[p & 3u] = v; else wv[(p >> 2) & 3u] |= v << (8 * (p & 3));
         }
@@ -2114,17 +2131,23 @@ __global__ void __launch_bounds__(JD_RS_THREADS) jdk_resize_coeffs_box(const JDR
     const JDBoxDesc &x = bd[v];
     const uint32_t item = (blockIdx.x - x.blk_c) * JD_RS_THREADS + threadIdx.x;
     const uint32_t nh = (r.flags & 1u) ? r.dst_w : 0u, nv = (r.flags & 2u) ? r.dst_h : 0u;
-    int32_t xmin;
+    int32_t xmin;   /* a window as in jdk_resize_coeffs; the support is the whole resize source (sx = sy = 0) */
     if (item < nh) {
         int32_t *tab = coef + r.coef_h;
-        const int taps = jd_rs_coeffs_box((int)r.src_w, x.box[0], x.box[2], (int)r.dst_w, filter, (int)item, &xmin,
-                                          tab + 2 * (uint64_t)r.dst_w + item, r.dst_w);
+        int taps = 0;
+        xmin = item < r.wx0 ? 0 : (int32_t)r.src_w;
+        if (item >= r.wx0 && item < r.wx1)
+            taps = jd_rs_coeffs_box((int)r.src_w, x.box[0], x.box[2], (int)r.full_w, filter, (int)((int64_t)r.win_x + item), &xmin,
+                                    tab + 2 * (uint64_t)r.dst_w + item, r.dst_w);
         tab[2 * item] = xmin;
         tab[2 * item + 1] = taps;
     } else if (item < nh + nv) {
         const uint32_t yy = item - nh;
         int32_t *tab = coef + r.coef_v + (uint64_t)yy * (r.ksize_v + 2);
-        const int taps = jd_rs_coeffs_box((int)r.src_h, x.box[1], x.box[3], (int)r.dst_h, filter, (int)yy, &xmin, tab + 2, 1);
+        int taps = 0;
+        xmin = yy < r.wy0 ? 0 : (int32_t)r.src_h;
+        if (yy >= r.wy0 && yy < r.wy1)
+            taps = jd_rs_coeffs_box((int)r.src_h, x.box[1], x.box[3], (int)r.full_h, filter, (int)((int64_t)r.win_y + yy), &xmin, tab + 2, 1);
         tab[0] = xmin;
         tab[1] = taps;
     }

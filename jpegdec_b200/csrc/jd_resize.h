@@ -113,6 +113,23 @@ JD_RS_HD int jd_rs_coeffs(int in, int out, int filter, int xx, int32_t *xmin, in
     return taps;
 }
 
+/* A window (JPEGB200_batchCreateWindow) along one axis: its sample i is output win + i of the full in -> out resize.
+ * Coefficients of window sample i with xmin relative to the support's origin sup.  Outside the window's in-image span
+ * [i0, i1): no taps, xmin 0 before it and sup_len (the support's length) after it, so that the first and last taps of a
+ * run of samples still bound the taps of every sample between them.  Returns taps. */
+JD_RS_HD int jd_rs_win_coeffs(int in, int out, int filter, int64_t win, uint32_t i, uint32_t i0, uint32_t i1, int32_t sup,
+                              int32_t sup_len, int32_t *xmin, int32_t *k, int64_t kstride)
+{
+    if (i < i0) { *xmin = 0; return 0; }
+    if (i >= i1) { *xmin = sup_len; return 0; }
+    const int taps = jd_rs_coeffs(in, out, filter, (int)(win + i), xmin, k, kstride);
+    *xmin -= sup;
+    return taps;
+}
+
+/* a window pixel outside the resized image: R = G = B = 0 and alpha 0xFF (either RGB8888 byte order), gray 0 */
+JD_RS_HD uint32_t jd_rs_fill(int bpp) { return bpp == 4 ? 0xFF000000u : 0u; }
+
 JD_RS_HD uint32_t jd_rs_clip8(int32_t ss)
 {
     if (ss >= (1 << (JD_RS_PRECISION + 8))) return 255u;
